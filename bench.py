@@ -2,9 +2,11 @@
 """bench.py -- the driver-facing benchmark of the fused ABFT-SGEMM hot path.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--size n] [--id KERNEL_ID] [--sweep]
+                  [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one batch of synthetic input: one fused fault-tolerant SGEMM
-C = alpha*A*B^T + beta*C (encode pre-pass + tcgen05 kernel with checksum tile-columns, per-tile detect/correct) at
+C = alpha*A*B^T + beta*C (operand transposes + encode front phase + wgmma kernel with checksum tile-columns, per-tile
+detect/correct) at
 BASELINE.json configs[1]: M=N=K=4096, alpha=1, beta=-1.5 (the reference's timing phase, sgemm.cu:22,234), reference
 input distribution (utils/utils.cu:23-31).  Inputs are resident in HBM for `value`; `e2e` runs the same step through
 the host-buffer C-ABI call (ftsgemm_run_host) with H2D/D2H inside the timed region.  At N>1 every rank (one process per
@@ -16,6 +18,13 @@ The JSON line also carries: `sweep` (N=1: fused ABFT / own plain kernel / cuBLAS
 number of launches per cell, engines interleaved), `strong` (BASELINE.json configs[4]: ONE 32768^3 product on the P x Q
 rank grid, incl. the verdict exchange), `id16` (configs[1] literally: the 128x128x8 tile), `parity` (sampled rows of the
 bench's own result against the CPU oracle, outside the timed regions).
+
+--dump-outputs DIR writes what the timed path computed in its last timed step: C.npy (float32, a fixed seeded sample of
+at most 512 rows of the M x N result, as [row, n]) with C_rows.npy (int64, the sampled rows) and stats.npy (float64, the
+fault verdict of the timed region: tiles, rows_checked, detected, corrected, uncorrectable, checksum_faults,
+max_abs_residual, max_rel_residual); at N > 1 every rank writes its own block's files with a _rank<r> suffix, the row count
+chosen so that all files together stay within 64 MB.  With --impl reference it writes the whole 1024 x 1024 C of the last
+step.  The inputs are seeded, so two builds run with the same arguments can be compared output for output.
 
 --impl reference times the reference's own CPU SGEMM (cpu_gemm, utils/utils.cu:79-89, compiled unmodified into
 oracle/_ref/libref_utils.so; falls back to the OpenMP oracle port) on the host cores; rank 0 only.
@@ -45,7 +54,8 @@ def _peaks():
         d = json.loads(p.read_text())
         return {"bf16_tflops": float(d["bf16_tflops"]), "bf16_tflops_sustained": float(d.get("bf16_tflops_sustained", d["bf16_tflops"])),
                 "hbm_gbs": float(d["hbm_gbs"]), "src": "measured (MEASURED_PEAKS.json)"}
-    return {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "hbm_gbs": 6650.0, "src": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet (dense, at up to 700 W): BF16 989 TFLOP/s, HBM3 3.35 TB/s -- not measured
+    return {"bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "hbm_gbs": 3350.0, "src": "H100 SXM data sheet (not measured)"}
 
 
 class ClockSampler:
@@ -79,6 +89,14 @@ class ClockSampler:
                 self.how = "NVML index = CUDA index (UUID lookup unavailable)"
 
             self.max_sm = pynvml.nvmlDeviceGetMaxClockInfo(self.h, pynvml.NVML_CLOCK_SM)
+            # the card and its power limit are part of every number measured on it
+            self.gpu_name, self.power_limit_w = None, None
+            try:
+                name = pynvml.nvmlDeviceGetName(self.h)
+                self.gpu_name = name.decode() if isinstance(name, bytes) else str(name)
+                self.power_limit_w = pynvml.nvmlDeviceGetPowerManagementLimit(self.h) / 1000.0
+            except Exception:
+                pass
         except Exception:
             self.nvml = None
             return
@@ -111,7 +129,8 @@ class ClockSampler:
                 if rs & bit:
                     reasons.add(name)
         sm = [x[1] for x in inside]
-        return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": self.max_sm,
+        return {"gpu": self.gpu_name, "power_limit_w": self.power_limit_w,
+                "sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": self.max_sm,
                 "power_w_max": max((x[2] for x in inside), default=None), "samples": len(inside),
                 "reasons": sorted(reasons), "how": "pynvml polled from a thread during the timed region; device " + getattr(self, "how", "?")}
 
@@ -154,8 +173,9 @@ def run_reference_arm(args):
     r = O.ref_utils()
     A, B, C = O.make_inputs(n_ref)
     X = np.ascontiguousarray(B.reshape(n_ref, n_ref).T).reshape(-1)
-    steps, warm = max(1, min(args.steps, 6)), min(args.warmup, 1)
+    steps, warm = args.steps, args.warmup
     times = []
+    last = None  # C of the last timed step
     if r is not None:
         # cpu_gemm itself is single-threaded: one independent instance per host thread (ctypes releases the GIL), all on
         # the same inputs, each into its own output; the step's throughput is the aggregate over the instances
@@ -169,10 +189,7 @@ def run_reference_arm(args):
         def one(z):
             r.ref_cpu_gemm(1.0, -1.5, O._p(X), O._p(A), n_ref, O._p(z))
 
-        t_begin = time.time()
         for i in range(warm + steps):
-            if times and time.time() - t_begin > 120.0:
-                break  # 128 instances take ~38 s per step on the pool's hosts: keep the whole arm within a few minutes
             for z in outs:
                 z.fill(0.0)
             ths = [threading.Thread(target=one, args=(z,)) for z in outs]
@@ -183,6 +200,7 @@ def run_reference_arm(args):
                 t.join()
             if i >= warm:
                 times.append(time.time() - t0)
+        last = outs[0]
     else:
         kind, cores = "port", O.num_threads()
         sample = f"oracle_sgemm_nt (OpenMP port of cpu_gemm) n={n_ref} per step"
@@ -192,6 +210,13 @@ def run_reference_arm(args):
             O.sgemm_nt(n_ref, n_ref, n_ref, 1.0, A, B, -1.5, Z)
             if i >= warm:
                 times.append(time.time() - t0)
+        last = Z
+    if args.dump_outputs:
+        # the whole n_ref x n_ref result (4 MiB), column-major buffer -> [m, n]
+        d = Path(args.dump_outputs)
+        d.mkdir(parents=True, exist_ok=True)
+        np.save(d / "C.npy", np.ascontiguousarray(last.reshape(n_ref, n_ref).T))
+        np.save(d / "C_rows.npy", np.arange(n_ref, dtype=np.int64))
     dt = sum(times) / len(times)
     instances = cores if kind == "reference" else 1
     gf = instances * 2.0 * n_ref ** 3 / dt / 1e9
@@ -242,13 +267,34 @@ def fill_ref_dist(t, gen):
     return t
 
 
+DUMP_BUDGET_BYTES = 64_000_000  # --dump-outputs writes at most this much in all, over all ranks
+
+
+def dump_outputs(out_dir, prob, st, suffix, world):
+    """C of the last timed step -- a fixed seeded sample of rows, as many as this rank's share of DUMP_BUDGET_BYTES holds
+    (at most 512: 8 MiB at M = N = 4096) -- and the timed region's verdict."""
+    import numpy as np
+    d = Path(out_dir)
+    d.mkdir(parents=True, exist_ok=True)
+    M, N = prob.M, prob.N
+    share = DUMP_BUDGET_BYTES // world - 4096  # (.npy headers, the verdict)
+    n_rows = max(1, min(M, 512, share // (4 * N + 8)))
+    rows = np.sort(np.random.default_rng(2024).choice(M, size=n_rows, replace=False)).astype(np.int64)
+    C = prob.dC.view(N, M).t()  # column-major M x N -> [m, n]
+    import torch
+    sample = C[torch.from_numpy(rows).to(prob.dC.device)].cpu().numpy().astype(np.float32)
+    np.save(d / f"C{suffix}.npy", sample)
+    np.save(d / f"C_rows{suffix}.npy", rows)
+    keys = ("tiles", "rows_checked", "detected", "corrected", "uncorrectable", "checksum_faults", "max_abs_residual", "max_rel_residual")
+    np.save(d / f"stats{suffix}.npy", np.array([float(st[k]) for k in keys], dtype=np.float64))
+
+
 def main():
     _claim_stdout()
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    # defaults = the regime every number in DESIGN.md / profiles is quoted in (and the driver's): 20 back-to-back launches at
-    # boost clocks.  Hundreds of steps heat the chip: the comparator measured after the headline then reads 15-20 % lower than
-    # the one before, and averaged "overhead" figures are meaningless (VERDICT r1).
+    # defaults = the regime every number in DESIGN.md is quoted in: 20 back-to-back launches.  Hundreds of steps heat the
+    # chip: the comparator measured after the headline then reads lower than the one before.
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="ours")
@@ -257,10 +303,14 @@ def main():
                     help="G > 0: the headline itself is ONE G^3 product sharded over the P x Q rank grid (strong scaling)")
     ap.add_argument("--strong-size", type=int, default=32768,
                     help="G of the `strong` sub-record (BASELINE.json configs[4]; 0 = skip)")
-    ap.add_argument("--id", type=int, default=31, help="fused ABFT kernel id (31 = 256x256 CTA-pair tile, 16 = literal huge 128x128)")
+    ap.add_argument("--id", type=int, default=31, help="fused ABFT kernel id (31 = 256x256 two-CTA tile, 16 = literal huge 128x128)")
     ap.add_argument("--no-sweep", action="store_true", help="skip the 1024..16384 sweep (N=1)")
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the timed path computed in its last step to DIR/<name>.npy (see the module docstring)")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     if args.impl == "reference":
         return run_reference_arm(args)
 
@@ -284,7 +334,7 @@ def main():
     P, Q = sharding.shard_grid(world)
     alpha, beta = 1.0, -1.5
     W = max(args.warmup, 3)
-    steps = max(1, args.steps)
+    steps = args.steps
     g = torch.Generator(device="cuda").manual_seed(1234 + rank)
     ft = pkg.FtSgemm()
     stream = torch.cuda.current_stream().cuda_stream
@@ -396,6 +446,8 @@ def main():
     clocks = sampler.stop(t_wall0, t_wall1) if rank == 0 else None
     verdict = exch.verdict() if exch is not None else (peer.verdict() if peer is not None else None)
     st = ft.stats()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, prob, st, "" if world == 1 else f"_rank{rank}", world)
     ms_step = ms_total / steps
     value = world * flops_per_step / (ms_step * 1e-3) / 1e9
     comp["plain"] = prob.time_engine(plain_id, steps)
@@ -419,7 +471,7 @@ def main():
         s16 = min(steps, 50)
         id16 = {"abft_kernel_huge_gflops": round(prob.time_engine(16, s16, o=opts), 1),
                 "kernel_sgemm_huge_gflops": round(prob.time_engine(6, s16), 1), "steps": s16,
-                "note": "BASELINE.json configs[1] literally (tile 128x128, one CTA per tile); the headline uses the CTA-pair tile 256x256"}
+                "note": "BASELINE.json configs[1] literally (tile 128x128, one CTA per tile); the headline uses the two-CTA tile 256x256"}
         id16["overhead_pct_vs_cublas_tf32"] = round(100.0 * (comp["cublas_tf32"] / id16["abft_kernel_huge_gflops"] - 1.0), 2)
         ft.stats()
 
@@ -549,7 +601,7 @@ def main():
             dist.destroy_process_group()
         return
     peaks = _peaks()
-    tf32_peak = peaks["bf16_tflops"] / 2.0  # kind::tf32 issues at half the kind::f16 rate on tcgen05
+    tf32_peak = peaks["bf16_tflops"] / 2.0  # dense TF32 runs at half the BF16 rate (495 of 989 TFLOP/s on the data sheet)
     achieved = flops_per_step / (k_ms * 1e-3) / 1e12
     info = names[args.id]
     region_ms = ms_total
@@ -571,8 +623,8 @@ def main():
                                                    "memory, no collective launch)" if peer is not None else
                                                    "snapshot kernel + asynchronous NCCL all-gather, joined inside the timed region"))
                                if world > 1 else "single GPU",
-                   "l2": (f"inputs {4 * (M * K + N * K + M * N) / 2**20:.0f} MiB per step vs 126 MB L2: larger than L2, no flush needed"
-                          if 4 * (M * K + N * K + M * N) > 160e6 else "L2-resident working set (small size)"),
+                   "l2": (f"inputs {4 * (M * K + N * K + M * N) / 2**20:.0f} MiB per step vs 50 MB L2: larger than L2, no flush needed"
+                          if 4 * (M * K + N * K + M * N) > 64e6 else "L2-resident working set (small size)"),
                    "baseline_note": "vs_baseline = per-GPU value / 4005 GFLOPS (README.md:53 abft_kernel_huge @4096, GPU unspecified)"},
         "abft": {"overhead_pct_vs_cublas_tf32": round(100.0 * (comp["cublas_tf32"] / (value / world) - 1.0), 2),
                  "overhead_pct_vs_own_plain_kernel": round(100.0 * (comp["plain"] / (value / world) - 1.0), 2),
@@ -584,12 +636,13 @@ def main():
                  "encode_us_per_step": round((ms_step - k_ms) * 1e3, 2),
                  "tiles_checked": st["tiles"], "rows_checked": st["rows_checked"], "detected": st["detected"],
                  "max_abs_residual": st["max_abs_residual"], "max_rel_residual": st["max_rel_residual"]},
+        # traffic: the bytes the algorithm needs per step, from the shapes (A and B read once, C written, and read when beta != 0)
         "roofline": {"bound": "tensor", "achieved": round(achieved, 1), "peak": round(tf32_peak, 1), "unit": "TFLOP/s",
-                     "frac": round(achieved / tf32_peak, 4), "traffic": None,
+                     "frac": round(achieved / tf32_peak, 4), "traffic": 4 * (M * K + N * K + M * N * (2 if beta != 0.0 else 1)),
                      "regime": regime, "timed_region_ms": round(region_ms, 3),
-                     "note": f"kernel ftsgemm_tc_kernel alone (checksum vectors reused: no encode launch), 2*M*N*K per launch / "
-                             f"CUDA-event mean over {steps} back-to-back launches; peak = bf16 burst {peaks['bf16_tflops']} / 2 "
-                             f"(kind::tf32 issues at half the kind::f16 rate; no TF32 peak is measured), {peaks['src']}; "
+                     "note": f"kernel ftsgemm_tc_kernel alone (checksum vectors reused: no encode), 2*M*N*K per launch / "
+                             f"CUDA-event mean over {steps} back-to-back launches; peak = bf16 {peaks['bf16_tflops']} / 2 "
+                             f"(dense TF32 is half the BF16 rate; no TF32 peak is measured), {peaks['src']}; "
                              f"clocks during the headline region: {regime}"},
         "e2e": {"value": round(e2e_val, 1), "unit": "GFLOPS", "h2d_bytes_per_step": 4 * (M * K + N * K + M * N), "d2h_bytes_per_step": 4 * M * N,
                 "steps": e2e_steps, "finite": result_ok},
@@ -611,13 +664,6 @@ def main():
         out["sweep"] = sweep
     if strong is not None:
         out["strong"] = strong
-    tp = ROOT / "profiles" / "traffic.json"
-    if tp.exists():
-        try:
-            t = json.loads(tp.read_text()).get(str(args.id))
-            out["roofline"]["traffic"] = t.get(str(n)) if isinstance(t, dict) else (t if n == 4096 else None)
-        except Exception:
-            pass
     if not args.no_cpu and world == 1:  # (rank 0 at N = 1 only: torchrun pins OMP_NUM_THREADS=1)
         out["cpu_baseline"] = _cpu_port_baseline(n if n <= 4096 else 4096)
     _emit(out)

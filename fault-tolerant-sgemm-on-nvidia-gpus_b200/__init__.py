@@ -7,7 +7,7 @@ The reference (shixun404/Fault-Tolerant-SGEMM-on-NVIDIA-GPUs) has no Python API;
   * verify_matrix(...)      (utils/utils.cu:61-77),
   * the CLI  ft_sgemm START END GAP ST_KERNEL END_KERNEL  (sgemm.cu:13-19).
 This module mirrors exactly those, binding the shared library with ctypes (plain pointers and sizes; torch is only
-used by callers to own device memory).  There is NO CPU fallback: if the library or an sm_100 device is missing,
+used by callers to own device memory).  There is NO CPU fallback: if the library or an sm_90 device is missing,
 every call raises.
 """
 from __future__ import annotations
@@ -26,7 +26,7 @@ MAX_EVENTS = 16
 
 # kernel ids (include/ftsgemm.h; reference sgemm.cu:235-237)
 ID_CUBLAS, ID_CUBLAS_TF32, ID_ABFT_BASELINE, ID_ABFT_BASELINE_TF32 = 0, 7, 10, 30
-ID_SGEMM_AUTO, ID_ABFT_AUTO = 20, 40  # per-shape choice among the tcgen05 variants (select_kernel)
+ID_SGEMM_AUTO, ID_ABFT_AUTO = 20, 40  # per-shape choice among the wgmma variants (select_kernel)
 SGEMM_IDS = {"small": 1, "medium": 2, "large": 3, "tall": 4, "wide": 5, "huge": 6, "giant": 21, "pair128": 22}
 ABFT_IDS = {"small": 11, "medium": 12, "large": 13, "tall": 14, "wide": 15, "huge": 16, "giant": 31, "pair128": 32}
 
@@ -199,7 +199,7 @@ def make_opts(stream=None, selftest=None, faults=None, tau_abs=0.0, tau_rel=0.0,
     return o
 
 
-def debug_schedule(kernel_id: int, M: int, N: int, K: int, num_sms: int = 148):
+def debug_schedule(kernel_id: int, M: int, N: int, K: int, num_sms: int = 132):
     """Work decomposition of one launch, enumerated on the host (no GPU needed): (header dict, list of segment dicts)."""
     hdr = (C.c_int * 8)()
     n = lib().ftsgemm_debug_schedule(kernel_id, M, N, K, num_sms, hdr, None, 0)

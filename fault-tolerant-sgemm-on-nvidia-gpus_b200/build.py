@@ -1,4 +1,4 @@
-"""In-tree build of libftsgemm.so and the ft_sgemm driver for sm_100a (nvcc cross-compiles without a GPU)."""
+"""In-tree build of libftsgemm.so and the ft_sgemm driver for sm_90a (nvcc cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os
@@ -10,7 +10,7 @@ HERE = Path(__file__).resolve().parent
 CSRC = HERE / "csrc"
 ROOT = HERE.parent
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-ccbin", "/usr/bin/g++"]
 
 LIB = HERE / "libftsgemm.so"

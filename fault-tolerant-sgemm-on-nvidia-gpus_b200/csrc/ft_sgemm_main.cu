@@ -126,7 +126,7 @@ int main(int argc, char **argv) {
   ftsgemm_opts opts;
   ftsgemm_default_opts(&opts);
   if (inject) opts.inject_mode = 1;  // +10000 into one accumulator of every CTA tile (ft_sgemm_huge.cuh:324-327)
-  // optional modes of the tcgen05 engines (not in the reference's argv: environment only)
+  // optional modes of the wgmma engines (not in the reference's argv: environment only)
   if (getenv("FTSGEMM_PRECISION") && !strcmp(getenv("FTSGEMM_PRECISION"), "x3")) opts.precision = 1;  // 3xTF32, FP32-grade
   opts.check_segments = env_int("FTSGEMM_CHECK_SEGMENTS", 0);  // S > 1: intra-K checking, S verified K-segments
   opts.protect_epilogue = env_int("FTSGEMM_PROTECT_EPILOGUE", 0) ? 1 : 0;  // checked store pass (stats.epilogue_faults)
@@ -160,7 +160,7 @@ int main(int argc, char **argv) {
     // near-zero elements outside the element-wise 1 %/0.01 rule (1e-5 at K = 1024, a few 1e-4 at K = 16384; cuBLAS-TF32
     // does too), so for the TF32 engines the verdict has two parts: (1) norm-wise, the tolerance this build is specified
     // to -- Frobenius-norm relative error vs FP32 cuBLAS <= 1e-3 (DESIGN.md section 4) -- and (2) ELEMENT-wise with the
-    // reference's own rule against a TF32 reference with the same operand rounding (the plain tcgen05 kernel id 21, or
+    // reference's own rule against a TF32 reference with the same operand rounding (the plain wgmma kernel id 21, or
     // id 6 when id 21 itself is under test; cuBLAS-TF32 rounds its operands differently and is therefore only judged
     // norm-wise), so that a single wrong element (e.g. a mis-corrected fault) fails the run although it is invisible in
     // the norm.  The element count vs FP32 goes to stderr.
@@ -182,7 +182,7 @@ int main(int argc, char **argv) {
     }
     const bool failed = tf32_engine ? (rel > 1e-3 || tf_bad != 0) : (vrc != FTSGEMM_OK);
     if (tf32_engine && tf_bad != 0)
-      fprintf(stderr, "[verify] kernel %d: %lld elements outside 1%%/0.01 of the TF32 reference (plain tcgen05 kernel)\n", id, tf_bad);
+      fprintf(stderr, "[verify] kernel %d: %lld elements outside 1%%/0.01 of the TF32 reference (plain wgmma kernel)\n", id, tf_bad);
     if (failed)
       printf("kernel %d failed to pass the correctness verification against NVIDIA cuBLAS. Exited.\n", id);
     if (vrc != FTSGEMM_OK && !failed)
@@ -223,7 +223,7 @@ int main(int argc, char **argv) {
   for (int id : list) {
     if (id < st_kernel) continue;
     if (id > end_kernel) break;
-    if ((id == 7 || id > 16) && end_kernel <= 16) continue;  // B200 extras only when asked for
+    if ((id == 7 || id > 16) && end_kernel <= 16) continue;  // this library's extras only when asked for
     ftsgemm_kernel_info info;
     ftsgemm_kernel_lookup(id, &info);
     printf("%-20s|", info.name);

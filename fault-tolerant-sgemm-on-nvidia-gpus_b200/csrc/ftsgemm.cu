@@ -4,7 +4,7 @@
 // launch dispatch (reference: sgemm.cu:110-199, 256-430), TMA tensor-map construction, the encode pre-pass launch,
 // the cuBLAS comparator rows (sgemm.cu:108,198,260), the non-fused ABFT baseline
 // (include/baseline_ft_sgemm.cuh:1-33) and the device-side comparator (utils/utils.cu:61-77).
-// There is NO CPU fallback: without an sm_100 device every compute entry point returns FTSGEMM_ERR_NO_DEVICE.
+// There is NO CPU fallback: without an sm_90 device every compute entry point returns FTSGEMM_ERR_NO_DEVICE.
 #include <cublas_v2.h>
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -29,16 +29,16 @@ using namespace ftsgemm;
 // ------------------------------------------------------------------------------------------- variant table
 struct Variant {
   ftsgemm_kernel_info info;
-  int bn;  // CTA(-pair) tile N of the tcgen05 kernel (0 for library rows)
-  int cg;  // 1 = one CTA per tile (UMMA M = 128), 2 = CTA pair per tile (cta_group::2, UMMA M = 256)
+  int bn;  // tile N of the wgmma kernel (0 for library rows)
+  int cg;  // CTAs per tile: 1 = 128 rows, 2 = 256 rows
 };
 
-// Reference tiles from code_gen/main.py:8-16.  sm_100a tiles: UMMA M is 128 per CTA (256 for a CTA pair), so the
+// Reference tiles from code_gen/main.py:8-16.  sm_90a tiles: 128 rows per CTA (256 for a two-CTA unit), so the
 // reference's "tall" (128x32) and "huge" (128x128) shapes are literal; the four others map, in the reference's order of
-// size, onto the remaining UMMA-legal shapes -- six names, six DISTINCT binaries (round 1 aliased small = tall and
+// size, onto the remaining tile shapes -- six names, six DISTINCT binaries (round 1 aliased small = tall and
 // large = huge):   small 128x64   medium 256x64 (pair)   large 256x128 (pair)   tall 128x32   wide 128x256   huge 128x128.
-// "giant" (ids 21/31) is the B200-only CTA-pair tile 256x256, "pair128" (22/32) an alias of large kept for round-1
-// callers; ids 20 / 40 pick per shape (select_variant).  tile_k = K extent of one shared-memory stage (4 UMMA k-steps).
+// "giant" (ids 21/31) is the two-CTA tile 256x256, "pair128" (22/32) an alias of large kept for round-1
+// callers; ids 20 / 40 pick per shape (select_variant).  tile_k = K extent of one shared-memory stage (4 wgmma k-steps).
 const Variant kVariants[] = {
     {{0, "cublas", 0, 0, 0, 0, 0, 0, 0, 0}, 0, 0},
     {{1, "kernel_sgemm_small", 0, 1, 16, 16, 16, 128, 64, 32}, 64, 1},
@@ -72,11 +72,9 @@ const Variant *find_variant(int id) {
   return nullptr;
 }
 
-// Per-shape choice of the tcgen05 variant (replaces the reference's manual id choice, sgemm.cu:110-199; SURVEY 8 f2).
-// Measured on B200 (profiles/r02_sweep_small_all_variants.jsonl, r02_small_slices_*.jsonl; 20-launch bursts, us per
-// launch): with few tiles the 74 CTA pairs are mostly idle with 256x256 tiles and the 256x128 pair tile ("large") is ahead --
-//   plain: 1024^3 12.4 vs 17.0, 1536^3 16.4 vs 21.9, 2048^3 32.7 vs 27.8  -> giant from 49 tiles of 256x256 on;
-//   ABFT:  1024^3 18.6 vs 22.2, 1536^3 33.8 vs 28.2                          -> giant from 25 tiles on.
+// Per-shape choice of the wgmma variant (replaces the reference's manual id choice, sgemm.cu:110-199; SURVEY 8 f2):
+// with few tiles most units idle with 256x256 tiles, so the 256x128 tile ("large") is used below a tile-count threshold
+// (49 tiles of 256x256 plain, 25 ABFT; thresholds not re-tuned for H100).
 int select_variant(int M, int N, bool ft) {
   const long long tiles256 = (static_cast<long long>(M) + 255) / 256 * ((static_cast<long long>(N) + 255) / 256);
   if (tiles256 >= (ft ? 25 : 49)) return ft ? FTSGEMM_ID_ABFT_GIANT : FTSGEMM_ID_SGEMM_GIANT;
@@ -86,6 +84,9 @@ int select_variant(int M, int N, bool ft) {
 // slab flags of the checksum tile-columns live in front of the expected-checksum matrix (one int per 32-row slab and
 // checksum tile-column: 128 KiB for the 128 x 32 tile at 16384^2)
 constexpr size_t kChkFlagBytes = 1u << 20;
+
+// L2 size assumed by the device-free schedule enumeration (ftsgemm_debug_schedule): H100's 50 MiB
+constexpr long long kDefaultL2Bytes = 50ll << 20;
 
 // ------------------------------------------------------------------------------------------- debug knobs
 std::mutex g_dbg_mu;
@@ -106,6 +107,7 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t
 struct ftsgemm_handle_s {
   int device = 0;
   int num_sms = 0;
+  long long l2_bytes = 0;
   cublasHandle_t cublas = nullptr;
   EncodeTiledFn encode_tiled = nullptr;
   DeviceStats *d_stats = nullptr;
@@ -123,8 +125,10 @@ struct ftsgemm_handle_s {
   int peer_world = 0, peer_rank = 0;
   unsigned long long peer_seq = 0;
   unsigned int *d_exit_count = nullptr;
-  int *d_enc_done = nullptr;    // front-phase encode: warps done, monotonic over launches
-  int enc_done_value = 0;
+  int *d_front_done = nullptr;  // kernel front phase (operand transposes, encode): warps done, monotonic over launches
+  int front_done_value = 0;
+  float *d_at = nullptr, *d_bt = nullptr;  // K-major copies of A and B
+  size_t at_bytes = 0, bt_bytes = 0;
   float *d_lo = nullptr;        // 3xTF32: A_lo | B_lo
   size_t lo_bytes = 0;
   float *d_aux = nullptr;       // baseline vectors
@@ -152,7 +156,7 @@ struct ftsgemm_handle_s {
   cudaStream_t s_in = nullptr, s_out = nullptr;     // run_host: upload / download streams of the panel pipeline
   cudaEvent_t ev_in[16] = {}, ev_done[16] = {};
   double *d_verify = nullptr;   // {first_bad (as long long), num, den}
-  std::map<int, int> max_units;     // per kernel instantiation (BN * 8 + FT * 4 + CG): co-resident CTAs / CTA pairs
+  std::map<int, int> max_units;     // per kernel instantiation (BN * 8 + FT * 4 + CG): co-resident work units
   cudaStream_t last_stream = nullptr;
   unsigned long long launch_count = 0;  // kernels of THIS library launched through the handle (ftsgemm_launch_count)
   int last_cuda_error = 0;
@@ -201,16 +205,16 @@ int check_abort_flag(ftsgemm_handle_t h) {
   return FTSGEMM_ERR_TIMEOUT;
 }
 
-int make_tmap_2d(ftsgemm_handle_t h, CUtensorMap *tm, const float *base, uint64_t inner, uint64_t outer,
-                 uint64_t ld_elems, uint32_t box_inner, uint32_t box_outer) {
-  cuuint64_t dims[2] = {inner, outer};
-  cuuint64_t strides[1] = {ld_elems * sizeof(float)};
-  cuuint32_t box[2] = {box_inner, box_outer};
+// K-major operand copy (rows x K, row stride ldk floats): one box = 32 k (128 bytes, 128B-swizzled) x box_rows rows, the
+// layout the wgmma descriptors describe (ptx::make_smem_desc_k128).  Rows and k beyond the operand are zero-filled.
+int make_tmap_kmajor(ftsgemm_handle_t h, CUtensorMap *tm, const float *base, uint64_t rows, uint64_t K, uint64_t ldk,
+                     uint32_t box_rows) {
+  cuuint64_t dims[2] = {K, rows};
+  cuuint64_t strides[1] = {ldk * sizeof(float)};
+  cuuint32_t box[2] = {kBK, box_rows};
   cuuint32_t estr[2] = {1, 1};
-  const CUtensorMapSwizzle sw =
-      static_cast<CUtensorMapSwizzle>(dbg("tma_swizzle", static_cast<long long>(CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B)));
   CUresult r = h->encode_tiled(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(base), dims, strides, box,
-                               estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                               estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     h->last_cuda_error = static_cast<int>(r);
@@ -219,31 +223,12 @@ int make_tmap_2d(ftsgemm_handle_t h, CUtensorMap *tm, const float *base, uint64_
   return FTSGEMM_OK;
 }
 
-// 3-D view {32, K, rows/32} of a column-major rows x K operand (rows % 32 == 0): element (i, k, a) = base[(a*32+i) + k*ld].
-// One box {32, kBK, atoms} lands in shared memory as [atom][k][32 floats] -- exactly the canonical MN-major layout the
-// UMMA descriptors describe -- with a single TMA instruction.
-int make_tmap_3d(ftsgemm_handle_t h, CUtensorMap *tm, const float *base, uint64_t rows, uint64_t kdim, uint64_t ld_elems,
-                 uint32_t atoms_per_box) {
-  cuuint64_t dims[3] = {kAtomMN, kdim, rows / kAtomMN};
-  cuuint64_t strides[2] = {ld_elems * sizeof(float), kAtomMN * sizeof(float)};
-  cuuint32_t box[3] = {kAtomMN, kBK, atoms_per_box};
-  cuuint32_t estr[3] = {1, 1, 1};
-  const CUtensorMapSwizzle sw =
-      static_cast<CUtensorMapSwizzle>(dbg("tma_swizzle", static_cast<long long>(CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B)));
-  CUresult r = h->encode_tiled(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float *>(base), dims, strides, box,
-                               estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    h->last_cuda_error = static_cast<int>(r);
-    return FTSGEMM_ERR_CUDA;
-  }
-  return FTSGEMM_OK;
-}
-
-// Largest grid (in work units = CTAs or CTA pairs) of this instantiation whose CTAs are all resident at once.  The
-// persistent kernel's inter-CTA waits (checksum flags, parked accumulators, wave counters) are only deadlock-free for
-// such a grid, so the planner never gets more units than this -- on a device partition (MPS active-thread percentage,
-// green context) that is fewer than multiProcessorCount / CG.  Cached per handle (= per device).
+// Largest grid (in work units of CG CTAs) of this instantiation whose CTAs can all be resident at once: one CTA per SM the
+// device reports (multiProcessorCount, which an MPS active-thread percentage reduces), or none when a CTA does not fit.
+// The persistent kernel's inter-CTA waits (front phase, checksum flags, parked accumulators, wave counters) are only
+// deadlock-free for such a grid, so the planner never gets more units than this.  If SMs are nevertheless held by other
+// work so that the grid cannot become resident, the waits' watchdog (ptx.cuh) ends the launch with FTSGEMM_ERR_TIMEOUT
+// instead of hanging.  Cached per handle (= per device).
 template <int BN, bool FT, int CG, bool PROT = false>
 int query_max_units(ftsgemm_handle_t h, int *out) {
   using Cfg = TileCfg<BN, FT, CG>;
@@ -255,55 +240,32 @@ int query_max_units(ftsgemm_handle_t h, int *out) {
   }
   auto kern = ftsgemm_tc_kernel<BN, FT, CG, PROT>;
   FT_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-  int units = 0;
-  if (CG > 1) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(h->num_sms / CG * CG);
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = Cfg::kSmemBytes;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CG;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    FT_CUDA(h, cudaOccupancyMaxActiveClusters(&units, kern, &cfg));
-  } else {
-    int per_sm = 0;
-    FT_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, Cfg::kSmemBytes));
-    units = (per_sm > 0 ? 1 : 0) * h->num_sms;  // one persistent CTA per SM
-  }
-  if (units > h->num_sms / CG) units = h->num_sms / CG;
+  int per_sm = 0;
+  FT_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, Cfg::kSmemBytes));
+  const int units = per_sm > 0 ? h->num_sms / CG : 0;  // one persistent CTA per SM
   h->max_units[key] = units;
   *out = units;
   return FTSGEMM_OK;
 }
 
-template <int BN, bool FT, int CG, bool PROT = false>
+template <int BN, bool FT, int CG, bool PROT, bool SEED>
 int launch_tc(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
               const KernelParams &p, int units, cudaStream_t stream) {
   // p.pdl_wait: the launch may overlap the tail of its predecessor in the stream (KernelParams::pdl_wait)
   using Cfg = TileCfg<BN, FT, CG>;
-  auto kern = ftsgemm_tc_kernel<BN, FT, CG, PROT>;
+  auto kern = ftsgemm_tc_kernel<BN, FT, CG, PROT, SEED>;
   int resident = 0;
-  const int qrc = query_max_units<BN, FT, CG, PROT>(h, &resident);  // (also sets the shared-memory attribute, once per handle)
+  const int qrc = query_max_units<BN, FT, CG, PROT>(h, &resident);
   if (qrc) return qrc;
   if (units > resident) return FTSGEMM_ERR_UNSUPPORTED;  // the plan was built for more units than can be co-resident
+  FT_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(units * CG);
   cfg.blockDim = dim3(kThreads);
   cfg.dynamicSmemBytes = Cfg::kSmemBytes;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
+  cudaLaunchAttribute attr[1];
   int na = 0;
-  if (CG > 1) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = CG;
-    attr[na].val.clusterDim.y = 1;
-    attr[na].val.clusterDim.z = 1;
-    ++na;
-  }
   if (p.pdl_wait) {
     attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[na].val.programmaticStreamSerializationAllowed = 1;
@@ -315,38 +277,42 @@ int launch_tc(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB
   return FTSGEMM_OK;
 }
 
+template <int BN, int CG, bool SEED>
+int launch_variant(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
+                   const KernelParams &p, int units, cudaStream_t stream, bool ft, bool prot) {
+  if (!ft) return launch_tc<BN, false, CG, false, SEED>(h, tmA, tmB, tmC, p, units, stream);
+  if (prot) return launch_tc<BN, true, CG, true, SEED>(h, tmA, tmB, tmC, p, units, stream);
+  return launch_tc<BN, true, CG, false, SEED>(h, tmA, tmB, tmC, p, units, stream);
+}
+
 // Planner input for one launch (tile grid already set by plan_tiles).
-// Measured on B200 (device timeline, profiles/r01_trace_*): a checksum tile's main loop takes 0.57-0.58 of a data tile's
-// whatever its UMMA N (it is bound by the A-operand feed, L2 -> shared memory), one k-block of a 256x256 CTA-pair tile
-// takes ~0.33 us, an item costs ~1.5 us of pipeline fill + drain, and a parked accumulator is back in the next owner's
-// tensor memory ~8 us after the piece's last UMMA.
+// Cost model in tile-times: a checksum tile's main loop costs a fixed fraction of a data tile's whatever its N (it is
+// bound by the A-operand feed), an item costs a fixed pipeline fill + drain, and a parked accumulator reaches the next
+// owner a fixed latency after the piece's last k-block.  (Constants carried over from the previous target, not re-tuned
+// for H100.)
 template <int BNv, int CGv>
 void chk_costs(const KernelParams &p, double floor_cost, std::vector<double> *out) {
   for (int c = 0; c < p.tiles_c; ++c)
     out->push_back(std::max(floor_cost, static_cast<double>(chk_tile_width<BNv, CGv>(p, c)) / BNv));
 }
 
-int carrier_tile_index(const KernelParams &p, int m_blk);
-
-PlanInput make_plan_input(int max_units, int CG, int BN, int K, const KernelParams &p) {
+// l2_bytes: the device's L2 size (cudaDevAttrL2CacheSize)
+PlanInput make_plan_input(int max_units, int CG, int BN, int K, const KernelParams &p, long long l2_bytes) {
   PlanInput in;
   long long units = dbg("grid", 0);
   in.units = (units > 0 && units <= max_units) ? static_cast<int>(units) : max_units;
   in.chk_slices = p.chk_slices > 1 ? p.chk_slices : 1;
-  in.n_chk_tiles = p.chk_in_carriers ? 0 : p.tiles_c * p.tiles_m * in.chk_slices;
-  if (p.chk_in_carriers) {
-    for (int m = 0; m < p.tiles_m; ++m) in.carriers.push_back(carrier_tile_index(p, m));
-    in.carrier_cost = static_cast<double>(dbg("carrier_cost_permille", 1400)) * 1e-3;
-  }
+  in.n_chk_tiles = p.tiles_c * p.tiles_m * in.chk_slices;
   in.n_data_tiles = p.tiles_m * p.tiles_n;
   in.num_kb = (K + kBK - 1) / kBK;
   in.tiles_m = p.tiles_m;
-  // operands larger than ~3/4 of the 126 MB L2: keep the units in k-lockstep (plan.h)
+  // operands larger than ~3/4 of the L2 (A and B panels cannot stay resident while the units stream them): keep the units
+  // in k-lockstep (plan.h)
   const long long lock = dbg("lockstep", -2);
   in.lockstep = lock >= 0 ? static_cast<int>(lock)
-                          : (4.0 * K * (static_cast<double>(p.M) + p.N) > 96.0 * 1024 * 1024 ? 1 : 0);
-  // a checksum item's main loop runs at 0.22 us per k-block whatever the size (round 2 timelines: 0.67-0.69 of a data
-  // tile at 2048 .. 4096, where data tiles take 0.33 us per k-block out of L2; 0.58 where they are HBM-bound)
+                          : (4.0 * K * (static_cast<double>(p.M) + p.N) > 0.75 * static_cast<double>(l2_bytes) ? 1 : 0);
+  // a checksum item's main loop costs a fixed fraction of a data tile's: larger where data tiles run out of L2, smaller
+  // where they are HBM-bound
   const double chk_floor = static_cast<double>(dbg("chk_cost_permille", in.lockstep ? 580 : 680)) * 1e-3;
   if (BN == 32) chk_costs<32, 1>(p, chk_floor, &in.chk_col_cost);
   else if (BN == 64 && CG == 1) chk_costs<64, 1>(p, chk_floor, &in.chk_col_cost);
@@ -367,31 +333,9 @@ PlanInput make_plan_input(int max_units, int CG, int BN, int K, const KernelPara
   return in;
 }
 
-// Carrier tiles or checksum items?  Legal when the whole checksum-operand box fits the 4 KiB slot of a stage
-// (n_chk_cols <= 32 * CG, i.e. N <= 4096 with 256-wide pair tiles), every operand goes through 3-D tensor maps and there is
-// at most one carrier per unit (a carrier must be the FIRST item of its unit: tensor-memory stage 1 is only free then).
-// Measured (profiles/r02_carriers_on_off.jsonl, us per launch, carriers vs checksum items): a carrier's main loop takes 1.39
-// tile-times (59.8 vs 42.9 us at 4096^3) against 0.68 + epilogue for a checksum item, but it is a longer CHAIN: with fewer
-// than ~2.3 waves of tiles the carrier + its unit's next tile set the makespan -- 2304^3 58.4 vs 53.8, 2560^3 67.5 vs 60.5,
-// then 3328^3 111.9 vs 113.3, 3584^3 137.4 vs 144.8, 3840^3 172.0 vs 171.9, 4096^3 199.8 vs 202.3.
-bool use_carriers(const KernelParams &p, int units, int CG) {
-  const long long c = dbg("carriers", -2);
-  if (c == 0) return false;
-  const bool legal = p.tiles_c == 1 && p.n_chk_cols <= kAtomMN * CG && (p.tma3d & 7) == 7 && p.tiles_m <= units;
-  if (!legal) return false;
-  if (c > 0) return true;
-  return 4ll * p.tiles_m * p.tiles_n >= 9ll * units;  // from 2.25 waves of data tiles on
-}
-
-// raster index (among the data tiles) of tile (m_blk, n_blk = 0): inverse of decode_tile
-int carrier_tile_index(const KernelParams &p, int m_blk) {
-  const int gsz = p.group_n < p.tiles_n ? p.group_n : p.tiles_n;
-  return m_blk * gsz;
-}
-
 // K-slices of the checksum items (KernelParams::chk_slices): only where units would otherwise idle -- all data tiles and
-// all slices run concurrently in one wave -- and a slice keeps at least 8 k-blocks.  Measured at 1024^3 (id 13): the
-// checksum item's K loop (7 us, after the encode) + its epilogue were the critical path of a 19.5 us step.
+// all slices run concurrently in one wave -- and a slice keeps at least 8 k-blocks: in such small problems the checksum
+// item's K loop (after the encode) + its epilogue are the critical path.
 int choose_chk_slices(const KernelParams &p, int units, int K) {
   const long long forced = dbg("chk_slices", -2);
   const int num_kb = (K + kBK - 1) / kBK;
@@ -450,15 +394,8 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const floa
   p.C = dC; p.ldc = M;
   p.alpha = alpha; p.beta = beta;
   plan_tiles(M, N, BN, CG, ft, &p);
-  // MN-major fp32 operands: 128B swizzle with 32B atoms.  One TMA box = 32 (M|N) x 32 (K) floats = 32 rows of
-  // 128 bytes, so successive M|N atoms are kBK*128 bytes apart (LBO), successive groups of 4 K-rows 512 bytes (SBO),
-  // and one UMMA k-step (8 K-rows) advances the start address by 1024 bytes.
-  p.lbo_bytes = static_cast<unsigned>(dbg("lbo", kBK * 128));
-  p.sbo_bytes = static_cast<unsigned>(dbg("sbo", 512));
-  p.layout_type = static_cast<unsigned>(dbg("layout_type", 1));
-  p.kstep_bytes = static_cast<unsigned>(dbg("kstep", 1024));
   p.tau_abs = o.tau_abs > 0 ? o.tau_abs : 1e-3f;
-  p.tau_rel = o.tau_rel > 0 ? o.tau_rel : 1e-5f;  // 13x the measured fault-free floor at K = 8192 (7.6e-7)
+  p.tau_rel = o.tau_rel > 0 ? o.tau_rel : 1e-5f;  // DESIGN.md section 5
   p.detect_only = o.detect_only;
   p.recompute = o.no_recompute ? 0 : 1;
   p.A = dA;
@@ -486,33 +423,30 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const floa
     p.exit_count = h->d_exit_count;
   }
 
+  // K-major copies of A and B (written by the kernel's front phase), row stride ldk: TMA needs 16-byte row strides
   CUtensorMap tmA, tmB, tmC;
   bool enc_front = false;
-  const bool allow3d = dbg("tma3d", 1) != 0;
   int rc;
-  if (allow3d && M % kAtomMN == 0) {
-    rc = make_tmap_3d(h, &tmA, dA, M, K, M, kBM / kAtomMN);
-    p.tma3d |= 1;
-  } else {
-    rc = make_tmap_2d(h, &tmA, dA, M, K, M, kAtomMN, kBK);
-  }
+  p.ldk = (K + 3) / 4 * 4;
+  rc = ensure_buf(h, &h->d_at, &h->at_bytes, static_cast<size_t>(M) * p.ldk * sizeof(float));
   if (rc) return rc;
-  if (allow3d && N % kAtomMN == 0) {
-    rc = make_tmap_3d(h, &tmB, dB, N, K, N, BN / CG / kAtomMN);
-    p.tma3d |= 2;
-  } else {
-    rc = make_tmap_2d(h, &tmB, dB, N, K, N, kAtomMN, kBK);
-  }
+  rc = ensure_buf(h, &h->d_bt, &h->bt_bytes, static_cast<size_t>(N) * p.ldk * sizeof(float));
+  if (rc) return rc;
+  p.At = h->d_at;
+  p.Bt = h->d_bt;
+  rc = make_tmap_kmajor(h, &tmA, p.At, M, K, p.ldk, kBM);
+  if (rc) return rc;
+  rc = make_tmap_kmajor(h, &tmB, p.Bt, N, K, p.ldk, BN);
   if (rc) return rc;
   tmC = tmB;
   if (ft) {
     // checksum vectors of B: 8 columns per N-tile, appended to B as extra tile-columns of the same GEMM
     p.dbg_flags = static_cast<int>(dbg("ft_dbg", 0)) & 1;
-    const int chk_ld = (p.n_chk_cols + kAtomMN - 1) / kAtomMN * kAtomMN;  // padded so the 3-D TMA view is exact; pad
-                                                                          // columns are never stored (n_chk_cols mask)
+    // the checksum operand is K-major like B^T: n_chk_cols rows of K (row stride ldk)
+    const int chk_ld = p.ldk;
     const int n_slabs = p.tiles_m * CG * (kBM / 32);
     const float *chk_before = h->d_chk;
-    rc = ensure_buf(h, &h->d_chk, &h->chk_bytes, static_cast<size_t>(K) * chk_ld * sizeof(float));
+    rc = ensure_buf(h, &h->d_chk, &h->chk_bytes, static_cast<size_t>(p.n_chk_cols) * chk_ld * sizeof(float));
     if (rc) return rc;
     if (h->d_chk != chk_before) h->chk_for_b = nullptr;  // reallocated: the cached encode is gone
     const size_t out_floats = static_cast<size_t>(M) * p.n_chk_cols;
@@ -530,10 +464,8 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const floa
     p.chk_epoch = ++h->chk_epoch;
     p.dbg_flags = static_cast<int>(dbg("ft_dbg", 0)) & 1;
     const bool reuse = o.reuse_b_checksums && h->chk_for_b == dB && h->chk_n == N && h->chk_k == K && h->chk_bn == BN;
-    // Default: the encode is a FRONT PHASE of the GEMM kernel (KernelParams::enc_front) -- one launch per fused GEMM, like
-    // the reference (sgemm.cu:191-192).  Measured equal to the stand-alone pre-pass within noise from 2048^3 to 12288^3
-    // (profiles/r02_front_phase_vs_prepass.jsonl: 200.0 vs 200.6 us at 4096^3, 1437 vs 1442 at 8192^3, -2.6 us at 2560^3);
-    // only below ~8 MB of B (1024^3: 23.0 vs 22.1 us) the two-launch form is kept.
+    // Default: the encode is part of the FRONT PHASE of the GEMM kernel (KernelParams::enc_front) -- one launch per fused
+    // GEMM, like the reference (sgemm.cu:191-192); only below ~8 MB of B the stand-alone pre-pass is used.
     const long long ef = dbg("enc_front", -2);
     enc_front = !reuse && (ef >= 0 ? ef != 0 : 4.0 * N * static_cast<double>(K) >= static_cast<double>(dbg("enc_front_min_mb", 8)) * 1048576.0);
     if (enc_front) {
@@ -544,15 +476,13 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const floa
     if (!reuse && !enc_front) {
       // stand-alone pre-pass in the caller's stream
       const int rounding = static_cast<int>(dbg("enc_rounding", 0));
-      // grid-stride over (column block, k-row group) items.  Item size (8 / 4 KiB) and grid (2 / 4 blocks per SM) make no
-      // measurable difference (profiles/r01_probe22_*: 695-698 TFLOP/s at 4096^3 for all four): the pass is HBM time.
+      // grid-stride over (column block, k-row group) items; the pass is HBM time.
       const int grid = static_cast<int>(dbg("enc_blocks_per_sm", 4)) * h->num_sms;
       const bool small_items = dbg("enc_kr", 8) == 4;
       const bool chain = dbg("pdl_chain", 1) != 0;
       // B larger than ~half of L2: read it with evict-first loads (it cannot stay resident for the GEMM anyway)
       const long long sb = dbg("enc_stream", -2);
-      const bool stream_b = sb > 0;  // measured at 8192^3: 1550 vs 1480 us per step -- the tail of B the pre-pass leaves in L2 is
-                                     // worth more to the GEMM's first wave than the residue it evicts: off by default
+      const bool stream_b = sb > 0;  // off by default: the tail of B the pre-pass leaves in L2 serves the GEMM's first wave
 #define FT_ENC(bn)                                                                                                          \
   if (BN == bn) {                                                                                                           \
     cudaLaunchConfig_t ec = {};                                                                                             \
@@ -575,28 +505,9 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const floa
       ++h->launch_count;
 #undef FT_ENC
       FT_CUDA(h, cudaGetLastError());
-      // The GEMM launch below becomes a programmatic dependent of this kernel: its CTAs start on SMs as they drain, and
-      // only its checksum items wait for the pre-pass to complete.  Measured: +7.8 % at 2048^3, +1.2 % at 4096^3, but
-      // -1.4 % at 8192^3 (CTAs that start early fall out of k-lockstep with the others), hence the size limit.
-      const long long pdl = dbg("pdl", -2);
-      p.pdl_wait = pdl >= 0 ? (pdl != 0) : (4.0 * K * (static_cast<double>(M) + N) <= 160.0 * 1024 * 1024);
     }
     if (!reuse) { h->chk_for_b = dB; h->chk_n = N; h->chk_k = K; h->chk_bn = BN; }
-    p.chk_box_bytes = BN / CG * kBK * static_cast<int>(sizeof(float));
-    if (allow3d) {
-      // the checksum operand's box only spans the atoms that exist (e.g. 128 of 256 columns at N = 8192), so a
-      // checksum item moves A plus a small B box per stage
-      int atoms = BN / CG / kAtomMN;
-      if (p.tiles_c == 1) {
-        const int w = (p.n_chk_cols + 32 * CG - 1) / (32 * CG) * (32 * CG);
-        atoms = (w < BN ? w : BN) / CG / kAtomMN;
-      }
-      p.chk_box_bytes = atoms * kAtomMN * kBK * static_cast<int>(sizeof(float));
-      rc = make_tmap_3d(h, &tmC, h->d_chk, chk_ld, K, chk_ld, atoms);
-      p.tma3d |= 4;
-    } else {
-      rc = make_tmap_2d(h, &tmC, h->d_chk, chk_ld, K, chk_ld, kAtomMN, kBK);
-    }
+    rc = make_tmap_kmajor(h, &tmC, h->d_chk, p.n_chk_cols, K, chk_ld, BN);
     if (rc) return rc;
   }
   // ---- work plan (plan.h), cached per shape on the handle
@@ -611,9 +522,7 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const floa
     if (max_units < 1) return FTSGEMM_ERR_UNSUPPORTED;  // not a single CTA (pair) of this kernel fits on the device partition
   }
   if (ft) {
-    // Carrier tiles instead of checksum items (KernelParams::chk_in_carriers, use_carriers)
-    p.chk_in_carriers = use_carriers(p, max_units, CG) ? 1 : 0;
-    p.chk_slices = p.chk_in_carriers ? 1 : choose_chk_slices(p, max_units, K);
+    p.chk_slices = choose_chk_slices(p, max_units, K);
     const size_t n_flags_s = static_cast<size_t>(p.tiles_m) * CG * (kBM / 32) * p.tiles_c * p.chk_slices;
     if (p.chk_slices > 1 && n_flags_s * sizeof(int) > kChkFlagBytes) p.chk_slices = 1;
     if (p.chk_slices > 1) {
@@ -631,9 +540,9 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const floa
       p.chk_out = h->d_chk_out + kChkFlagBytes / sizeof(float);
     }
   }
-  const PlanInput pin = make_plan_input(max_units, CG, BN, K, p);
+  const PlanInput pin = make_plan_input(max_units, CG, BN, K, p, h->l2_bytes);
   const std::array<long long, 6> key = {v.info.id, M, N, K, pin.units,
-                                        pin.force_slices * 16 + pin.max_slices + pin.lockstep * 8192 + pin.full_search * 16384 + pin.chk_slices * 65536 + (p.chk_in_carriers ? 1048576 : 0)};
+                                        pin.force_slices * 16 + pin.max_slices + pin.lockstep * 8192 + pin.full_search * 16384 + pin.chk_slices * 65536};
   ftsgemm_handle_s::CachedPlan &cp = h->plans[key];
   if (!cp.uploaded) {
     if (h->plans.size() > 64) {  // bound the cache: drop everything but this entry
@@ -672,19 +581,19 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const floa
     cp.uploaded = true;
   }
   const int units = cp.plan.units;
-  if (enc_front) {
+  {
     const int inc = units * CG * (kThreads / 32);
-    if (h->d_enc_done == nullptr) {
-      FT_CUDA(h, cudaMalloc(&h->d_enc_done, sizeof(int)));
-      FT_CUDA(h, cudaMemsetAsync(h->d_enc_done, 0, sizeof(int), stream));
-      h->enc_done_value = 0;
-    } else if (h->enc_done_value > (1 << 30) - inc) {
-      FT_CUDA(h, cudaMemsetAsync(h->d_enc_done, 0, sizeof(int), stream));
-      h->enc_done_value = 0;
+    if (h->d_front_done == nullptr) {
+      FT_CUDA(h, cudaMalloc(&h->d_front_done, sizeof(int)));
+      FT_CUDA(h, cudaMemsetAsync(h->d_front_done, 0, sizeof(int), stream));
+      h->front_done_value = 0;
+    } else if (h->front_done_value > (1 << 30) - inc) {
+      FT_CUDA(h, cudaMemsetAsync(h->d_front_done, 0, sizeof(int), stream));
+      h->front_done_value = 0;
     }
-    h->enc_done_value += inc;
-    p.enc_done = h->d_enc_done;
-    p.enc_target = h->enc_done_value;
+    h->front_done_value += inc;
+    p.front_done = h->d_front_done;
+    p.front_target = h->front_done_value;
   }
   p.plan = cp.d_items;
   p.plan_off = cp.d_off;
@@ -705,19 +614,14 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const floa
     p.sk_epoch = ++h->sk_epoch;
   }
   {
-    // Helper-assisted final epilogues (the helper warp of each TMEM lane quadrant takes the upper half of the columns).
-    // Measured (profiles/r01_probe24_*, beta = -1.5): ABFT +2.4 % at 1024^3, +5 % at 2048^3, +2 % at 3072^3, +0.8 % at
-    // 4096^3, +0.5 % at 8192^3; plain kernel +10.6 % at 1024^3 (one wave: the whole epilogue is exposed), neutral in
-    // between, -0.7 % at 8192^3 (the pair barriers cost more than the 3.6 us tail they shorten) -- hence the rule.
+    // Helper-assisted final epilogues (the helper warp of each 32-row quadrant takes the upper half of the columns): on
+    // for ABFT kernels and for plain kernels with at most three items per unit, where the epilogue is most exposed.
     const long long ea = dbg("epi_assist", -2);
     p.epi_assist = ea >= 0 ? (ea != 0) : (ft || cp.plan.items.size() <= 3 * static_cast<size_t>(units));
   }
   {
-    // Wave re-synchronisation for problems that run many waves over operands that do not fit L2.  Measured
-    // (profiles/r01_probe21_*, r01_trace_16384_per_wave.txt): without it the units' start times drift apart by ~2 us per
-    // wave and the tile time grows from 178 to 209 us over the 56 waves of 16384^3; with it the spread stays below 6 us:
-    // 16384^3 plain 750 -> 811 TFLOP/s (cuBLAS-TF32 831), ABFT 571-695 -> 721-821; 14336^3 +2-7 % / +3-12 %; neutral
-    // between 6144 and 12288, -2 % at 4096 (3 waves) -- hence the wave-count limit.
+    // Wave re-synchronisation for problems that run many waves (>= 24) over operands that do not fit L2: without it the
+    // units' start times drift apart wave by wave and stop sharing the A / B panels in L2.
     const long long ws = dbg("wave_sync", -2);
     const bool on = ws >= 0 ? (ws != 0) : (pin.lockstep && static_cast<int>(cp.wave_target.size()) >= 24);
     if (on && cp.wave_target.size() > 1) {
@@ -746,17 +650,15 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const floa
     p.trace_cap = cap;
   }
   // Programmatic dependent launch by default: the kernel's launch latency and prologue overlap the tail of whatever
-  // precedes it in the stream; unless it follows its own pre-pass (pdl_wait = 1: only the checksum items wait) every
-  // thread executes griddepcontrol.wait before the first global access.
-  if (p.pdl_wait == 0 && dbg("pdl_chain", 1) != 0) p.pdl_wait = 2;
+  // precedes it in the stream; every thread executes griddepcontrol.wait before the first global access.
+  p.pdl_wait = dbg("pdl_chain", 1) != 0 ? 1 : 0;
   h->last_stream = stream;
   ++h->launch_count;
   int lrc = FTSGEMM_ERR_UNSUPPORTED;
-#define FT_DISPATCH(bn, cg)                                                          \
-  if (BN == bn && CG == cg)                                                          \
-    lrc = !ft ? launch_tc<bn, false, cg>(h, tmA, tmB, tmC, p, units, stream)         \
-              : (o.protect_epilogue ? launch_tc<bn, true, cg, true>(h, tmA, tmB, tmC, p, units, stream) \
-                                    : launch_tc<bn, true, cg>(h, tmA, tmB, tmC, p, units, stream));
+#define FT_DISPATCH(bn, cg)                                                                                    \
+  if (BN == bn && CG == cg)                                                                                    \
+    lrc = p.sk_tiles > 0 ? launch_variant<bn, cg, true>(h, tmA, tmB, tmC, p, units, stream, ft, o.protect_epilogue) \
+                         : launch_variant<bn, cg, false>(h, tmA, tmB, tmC, p, units, stream, ft, o.protect_epilogue);
   FT_DISPATCH(32, 1)
   FT_DISPATCH(64, 1)
   FT_DISPATCH(128, 1)
@@ -856,7 +758,7 @@ const char *ftsgemm_error_string(int code) {
     case FTSGEMM_ERR_INVALID_ARG: return "invalid argument";
     case FTSGEMM_ERR_UNSUPPORTED: return "unsupported shape or kernel id";
     case FTSGEMM_ERR_CUDA: return "CUDA error (see ftsgemm_last_cuda_error)";
-    case FTSGEMM_ERR_NO_DEVICE: return "no sm_100 CUDA device available (libftsgemm has no CPU fallback)";
+    case FTSGEMM_ERR_NO_DEVICE: return "no sm_90 CUDA device available (libftsgemm has no CPU fallback)";
     case FTSGEMM_ERR_CUBLAS: return "cuBLAS error";
     case FTSGEMM_ERR_VERIFY: return "verification failed";
     case FTSGEMM_ERR_TIMEOUT: return "device-side wait timed out (grid not co-resident or protocol error): the launch's result is undefined";
@@ -904,11 +806,9 @@ int ftsgemm_debug_schedule(int kernel_id, int M, int N, int K, int num_sms, int 
   p.M = M; p.N = N; p.K = K;
   plan_tiles(M, N, v->bn, v->cg, v->info.fault_tolerant != 0, &p);
   if (v->info.fault_tolerant) {
-    if (M % kAtomMN == 0 && N % kAtomMN == 0 && dbg("tma3d", 1) != 0) p.tma3d = 7;
-    p.chk_in_carriers = use_carriers(p, num_sms / v->cg, v->cg) ? 1 : 0;
-    p.chk_slices = p.chk_in_carriers ? 1 : choose_chk_slices(p, num_sms / v->cg, K);
+    p.chk_slices = choose_chk_slices(p, num_sms / v->cg, K);
   }
-  const PlanInput pin = make_plan_input(num_sms / v->cg, v->cg, v->bn, K, p);
+  const PlanInput pin = make_plan_input(num_sms / v->cg, v->cg, v->bn, K, p, kDefaultL2Bytes);
   const Plan plan = build_plan(pin);
   if (hdr) {
     hdr[0] = plan.units; hdr[1] = pin.n_chk_tiles + pin.n_data_tiles; hdr[2] = pin.n_chk_tiles; hdr[3] = plan.sk_tiles;
@@ -956,11 +856,12 @@ int ftsgemm_create(ftsgemm_handle_t *out) {
   ftsgemm_handle_t h = new ftsgemm_handle_s();
   cudaDeviceProp prop;
   if (cudaGetDevice(&h->device) != cudaSuccess || cudaGetDeviceProperties(&prop, h->device) != cudaSuccess ||
-      prop.major != 10) {
+      prop.major != 9) {
     delete h;
     return FTSGEMM_ERR_NO_DEVICE;
   }
   h->num_sms = prop.multiProcessorCount;
+  h->l2_bytes = prop.l2CacheSize;
   void *fn = nullptr;
   cudaDriverEntryPointQueryResult qres;
   if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || !fn) {
@@ -1000,7 +901,9 @@ int ftsgemm_destroy(ftsgemm_handle_t h) {
   }
   cudaFree(h->d_aux);
   cudaFree(h->d_lo);
-  cudaFree(h->d_enc_done);
+  cudaFree(h->d_front_done);
+  cudaFree(h->d_at);
+  cudaFree(h->d_bt);
   for (int r = 0; r < kMaxPeers; ++r)
     if (h->peer_opened[r]) cudaIpcCloseMemHandle(h->peer_box[r]);
   cudaFree(h->d_mailbox);

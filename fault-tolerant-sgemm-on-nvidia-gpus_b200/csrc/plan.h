@@ -1,17 +1,16 @@
 // plan.h -- host-side work planner for the persistent fused ABFT-SGEMM kernel.
 //
 // The reference launches one CTA per output tile and lets the hardware scheduler deal them out
-// (/root/reference/kernel/ft_sgemm/sgemm.cu:110-199: grid = (M/ms, N/ns)).  A persistent tcgen05 kernel with one CTA
-// (pair) per SM has to do that job itself, and with 256x256 tiles a 4096^3 problem is only 256 tiles on 74 CTA pairs:
-// dealing whole tiles round-robin leaves 13.5 % of the machine idle in the last wave (measured with the device timeline,
-// profiles/r01_trace_*: units finish between 135 and 180 us).  The planner therefore cuts the last H data tiles of the
-// raster along K into pieces and levels the units with a list scheduler.
+// (kernel/ft_sgemm/sgemm.cu:110-199 of the reference: grid = (M/ms, N/ns)).  A persistent kernel with one CTA per SM has
+// to do that job itself, and with 256x256 tiles a 3072^3 problem is only 144 tiles on 66 two-CTA units: dealing whole
+// tiles round-robin leaves the machine 27 % idle in the last of 3 waves.  The planner therefore cuts the last H data
+// tiles of the raster along K into pieces and levels the units with a list scheduler.
 //
 // A cut tile is computed as a CHAIN: the unit that owns piece p+1 first loads the raw accumulator its predecessor
-// parked ("seeds" tensor memory with it) and then keeps accumulating, so the sum is formed in exactly the k order of an
+// parked ("seeds" its accumulator with it) and then keeps accumulating, so the sum is formed in exactly the k order of an
 // uncut tile -- bit-identical results, and (what matters for ABFT) the tensor core's accumulation bias stays the same
-// as in the checksum tile-columns.  (Adding independently accumulated partial sums, the usual split-K, raised the
-// fault-free ABFT residual 6x, profiles/r01_probe8_residual_vs_splitk.jsonl.)
+// as in the checksum tile-columns.  (Adding independently accumulated partial sums, the usual split-K, raises the
+// fault-free ABFT residual.)
 //
 // Global item order:  [early first pieces][checksum tiles][whole data tiles, raster order]
 //                     [late first pieces][2nd pieces][3rd pieces]...
@@ -31,8 +30,7 @@ namespace ftsgemm {
 struct PlanItem {
   int tile;        // decode order: checksum tiles first, then data tiles
   int kb_begin, kb_end;
-  int kind;        // 0 whole tile, 1 first piece (park), 3 middle piece (seed + park), 2 last piece (seed + finish),
-                   // 6 carrier (a whole data tile that also computes its tile-row's checksum product; first in its unit's list)
+  int kind;        // 0 whole tile, 1 first piece (park), 3 middle piece (seed + park), 2 last piece (seed + finish)
   int slice;       // piece index within its tile
   int split_idx;   // index among the cut tiles (workspace slot), -1 otherwise
 };
@@ -47,7 +45,7 @@ struct Plan {
 };
 
 struct PlanInput {
-  int units;            // CTAs or CTA pairs
+  int units;            // work units of CG CTAs
   int n_chk_tiles;      // checksum tile-columns x tiles_m x chk_slices (first tiles in decode order)
   int chk_slices = 1;   // K-slices per checksum tile (tile t belongs to slice t / (n_chk_tiles / chk_slices))
   int n_data_tiles;
@@ -55,19 +53,16 @@ struct PlanInput {
   int tiles_m;          // checksum tile t belongs to checksum tile-column t / tiles_m
   std::vector<double> chk_col_cost;  // tile-times of one tile of each checksum tile-column
   double chk_release = 0.0;          // tile-times before checksum items can start (their operand comes from the pre-pass)
-  std::vector<int> carriers;         // raster indices of the data tiles that carry their tile-row's checksum product
-                                     // (then n_chk_tiles == 0); given first, one per unit
-  double carrier_cost = 1.4;         // tile-times of a carrier (second UMMA per k-step on the same A slab; measured 59.8 vs 42.9 us)
   double item_overhead = 0.0;        // tile-times per item (pipeline fill + drain)
   double park_latency = 0.0;         // tile-times between the end of a piece's main loop and its successor's start
-  double seed_overhead = 0.0;        // extra tile-times of a seeded piece (its accumulator stage is loaded before the first UMMA)
+  double seed_overhead = 0.0;        // extra tile-times of a seeded piece (its accumulator is loaded before the first MMA)
   int max_slices = 2;   // 1 disables cutting
   int force_slices = 0; // > 1: cut into exactly this many equal pieces (tests)
   int full_search = 0;  // 1: always try the full candidate menu (default: a reduced menu from 8 waves up, where a cut
                         //    can only buy a few per cent and the simulation of thousands of items is what costs)
   int lockstep = 0;     // 1: the operands do not fit in L2, so the units must keep streaming the SAME k range of the
-                        //    panels they share (measured at 8192^3: first pieces of mixed lengths put the units out of
-                        //    phase and every whole tile got 10 % slower, HBM-bound): one cut fraction for all cut tiles
+                        //    panels they share (first pieces of mixed lengths put the units out of phase and every
+                        //    whole tile gets slower, HBM-bound): one cut fraction for all cut tiles
   size_t slab_bytes = 0;// bytes of one parked accumulator tile x CTAs per unit (workspace sizing)
 };
 
@@ -135,11 +130,6 @@ inline double schedule(const PlanInput &in, const Cut &c, Plan *out) {
                             len + (p > 0 ? in.seed_overhead : 0.0), ready[i], false);
     ready[i] = end + in.park_latency;
   };
-  std::vector<char> is_carrier(static_cast<size_t>(in.n_data_tiles), 0);
-  for (int d : in.carriers) {
-    is_carrier[static_cast<size_t>(d)] = 1;
-    give(PlanItem{in.n_chk_tiles + d, 0, in.num_kb, 6, 0, -1}, in.carrier_cost, 0.0, true);
-  }
   for (int i = 0; i < c.He; ++i) piece(i, 0);
   {
     const int S = in.chk_slices > 1 ? in.chk_slices : 1, per_slice = in.n_chk_tiles / S;
@@ -151,7 +141,7 @@ inline double schedule(const PlanInput &in, const Cut &c, Plan *out) {
     }
   }
   for (int d = 0; d < whole; ++d)
-    if (!is_carrier[static_cast<size_t>(d)]) give(PlanItem{in.n_chk_tiles + d, 0, in.num_kb, 0, 0, -1}, 1.0, 0.0, true);
+    give(PlanItem{in.n_chk_tiles + d, 0, in.num_kb, 0, 0, -1}, 1.0, 0.0, true);
   for (int i = c.He; i < H; ++i) piece(i, 0);
   for (int p = 1; p < max_pieces; ++p) {
     std::vector<int> order;
@@ -163,8 +153,7 @@ inline double schedule(const PlanInput &in, const Cut &c, Plan *out) {
     for (int i : order) piece(i, p);
   }
   // Operands that do not fit in L2: units that share A / B panels must stream the same k range at the same time.
-  // Measured at 8192^3 (profiles/r01_trace_*): with the checksum units 0.58 tile-times out of phase every whole tile is
-  // 2-3 % slower, with first pieces of mixed lengths 10 %.
+  // (Units out of phase -- behind checksum items or first pieces of mixed lengths -- make every whole tile slower.)
   if (in.lockstep) {
     double lo = 1e30, hi = -1.0;
     for (int u = 0; u < in.units; ++u)
@@ -210,11 +199,8 @@ inline Plan build_plan(const PlanInput &in) {
     const size_t slab_cap = std::min<size_t>((static_cast<size_t>(256) << 20) / std::max<size_t>(1, in.slab_bytes * (pieces - 1)),
                                              65536 / (8 * sizeof(int) * (pieces - 1)));
     const int hcap = static_cast<int>(std::min<size_t>(slab_cap, static_cast<size_t>(T)));
-    int max_carrier = -1;
-    for (int d : in.carriers) max_carrier = std::max(max_carrier, d);
     auto consider = [&](const Cut &c) {
       if (c.He + c.Hl <= 0 || c.He + c.Hl > hcap) return;
-      if (T - (c.He + c.Hl) <= max_carrier) return;  // the cut tiles are the last ones of the raster: no carrier among them
       const double t = schedule(in, c, nullptr);
       if (best < 0.0 || t < best) {
         best = t;

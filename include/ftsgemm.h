@@ -1,5 +1,5 @@
 /*
- * ftsgemm.h -- C ABI of libftsgemm.so: fused fault-tolerant (ABFT) SGEMM for NVIDIA B200 (sm_100a).
+ * ftsgemm.h -- C ABI of libftsgemm.so: fused fault-tolerant (ABFT) SGEMM for NVIDIA H100 (sm_90a).
  *
  * This is the drop-in boundary for the ONE hot path of
  * shixun404/Fault-Tolerant-SGEMM-on-NVIDIA-GPUs.  The reference exposes no library API; its boundary is
@@ -34,7 +34,7 @@ enum {
   FTSGEMM_ERR_INVALID_ARG = -1,  /* bad pointer / size / id */
   FTSGEMM_ERR_UNSUPPORTED = -2,  /* shape not supported by the selected variant */
   FTSGEMM_ERR_CUDA = -3,         /* a CUDA runtime/driver call failed; see ftsgemm_last_cuda_error */
-  FTSGEMM_ERR_NO_DEVICE = -4,    /* no sm_100 device / driver (the product has NO CPU fallback) */
+  FTSGEMM_ERR_NO_DEVICE = -4,    /* no sm_90 device / driver (the product has NO CPU fallback) */
   FTSGEMM_ERR_CUBLAS = -5,
   FTSGEMM_ERR_VERIFY = -6,       /* used by the driver helpers only */
   FTSGEMM_ERR_TIMEOUT = -7       /* a device-side wait of the persistent kernel timed out (its CTAs were not all resident,
@@ -45,7 +45,7 @@ enum {
 
 /* Kernel ids: the reference's table (sgemm.cu:235-237) is kept verbatim for ids 0,1-6,10,11-16.
  * ids 7-9 fall through to cuBLAS in the reference (sgemm.cu:197-199); here 7 = cuBLAS with TF32 tensor-op math
- * (the "fault-free cuBLAS TF32" bar), 8-9 = cuBLAS FP32.  ids >= 20 are B200-only extras. */
+ * (the "fault-free cuBLAS TF32" bar), 8-9 = cuBLAS FP32.  ids >= 20 are extras of this library. */
 enum {
   FTSGEMM_ID_CUBLAS = 0,
   FTSGEMM_ID_SGEMM_SMALL = 1, FTSGEMM_ID_SGEMM_MEDIUM = 2, FTSGEMM_ID_SGEMM_LARGE = 3,
@@ -54,13 +54,13 @@ enum {
   FTSGEMM_ID_ABFT_BASELINE = 10,
   FTSGEMM_ID_ABFT_SMALL = 11, FTSGEMM_ID_ABFT_MEDIUM = 12, FTSGEMM_ID_ABFT_LARGE = 13,
   FTSGEMM_ID_ABFT_TALL = 14, FTSGEMM_ID_ABFT_WIDE = 15, FTSGEMM_ID_ABFT_HUGE = 16,
-  FTSGEMM_ID_SGEMM_AUTO = 20,        /* plain tcgen05 kernel, variant chosen per shape (ftsgemm_select_kernel)  (B200 extra) */
-  FTSGEMM_ID_SGEMM_GIANT = 21,       /* 256 x 256 tile on a CTA pair (cta_group::2), plain  (B200 extra) */
-  FTSGEMM_ID_SGEMM_PAIR128 = 22,     /* 256 x 128 tile on a CTA pair, plain: alias of "large" (id 3) */
+  FTSGEMM_ID_SGEMM_AUTO = 20,        /* plain wgmma kernel, variant chosen per shape (ftsgemm_select_kernel)  (extra) */
+  FTSGEMM_ID_SGEMM_GIANT = 21,       /* 256 x 256 tile on two CTAs, plain  (extra) */
+  FTSGEMM_ID_SGEMM_PAIR128 = 22,     /* 256 x 128 tile on two CTAs, plain: alias of "large" (id 3) */
   FTSGEMM_ID_ABFT_BASELINE_TF32 = 30,/* non-fused baseline with TF32 tensor-op math */
-  FTSGEMM_ID_ABFT_GIANT = 31,        /* 256 x 256 CTA-pair tile, fused ABFT: the bench configuration (B200 extra) */
-  FTSGEMM_ID_ABFT_PAIR128 = 32,      /* 256 x 128 CTA-pair tile, fused ABFT: alias of "large" (id 13) */
-  FTSGEMM_ID_ABFT_AUTO = 40          /* fused ABFT, variant chosen per shape (ftsgemm_select_kernel)  (B200 extra) */
+  FTSGEMM_ID_ABFT_GIANT = 31,        /* 256 x 256 two-CTA tile, fused ABFT: the bench configuration (extra) */
+  FTSGEMM_ID_ABFT_PAIR128 = 32,      /* 256 x 128 two-CTA tile, fused ABFT: alias of "large" (id 13) */
+  FTSGEMM_ID_ABFT_AUTO = 40          /* fused ABFT, variant chosen per shape (ftsgemm_select_kernel)  (extra) */
 };
 
 typedef struct ftsgemm_handle_s *ftsgemm_handle_t;
@@ -71,18 +71,18 @@ typedef struct ftsgemm_kernel_info {
   int id;
   char name[24];         /* reference row label, e.g. "abft_kernel_huge" */
   int fault_tolerant;    /* 1 = online ABFT fused into the kernel */
-  int engine;            /* 0 = cuBLAS, 1 = tcgen05 fused kernel, 2 = cuBLAS call sequence (baseline) */
+  int engine;            /* 0 = cuBLAS, 1 = wgmma fused kernel, 2 = cuBLAS call sequence (baseline) */
   int ref_tile_m, ref_tile_n, ref_tile_k; /* the reference's CUDA-core CTA tile (0 for library rows) */
-  int tile_m, tile_n, tile_k;             /* this build's sm_100a CTA tile (UMMA M x N, K per smem stage) */
+  int tile_m, tile_n, tile_k;             /* this build's sm_90a tile (M x N of a work unit, K per smem stage) */
 } ftsgemm_kernel_info;
 
-/* Fault to inject into the FP32 accumulator tile in tensor memory, before the checksum test
+/* Fault to inject into the FP32 accumulator tile, before the checksum test
  * (generalises the reference's always-on injector, ft_sgemm_huge.cuh:49-51,324-327). */
 typedef struct ftsgemm_fault {
   int row, col;          /* global element (m, n) of C */
   int mode;              /* 0: acc += add_value      1: acc bits ^= xor_mask (single/multi bit flip)
                           * epilogue upsets (what opts.protect_epilogue detects; the accumulator check has already passed):
-                          * 2: acc bits ^= xor_mask in tensor memory AFTER the check, before the store pass re-reads it
+                          * 2: acc bits ^= xor_mask in the accumulator AFTER the check, before the store pass re-reads it
                           * 3: the value alpha*acc + beta*c about to be stored has its bits ^= xor_mask (injected by the
                           *    protected store pass only: ignored without opts.protect_epilogue) */
   float add_value;
@@ -133,9 +133,8 @@ typedef struct ftsgemm_opts {
                             old values within rounding).  A row segment that fails is counted in stats.epilogue_faults
                             and, when beta == 0, recomputed from A and B; with beta != 0 the old values are gone: it is
                             counted in stats.uncorrectable.  Tiles that are ragged in N are not covered; Inf / NaN already in the old C are
-                            not verifiable and not flagged.  A separate kernel instantiation (the default one has no register to
-                            spare); measured cost, id 31: +6 % at 8192^3, +18 % at 4096^3, +52 % at 2048^3
-                            (profiles/r02_protect_epilogue_cost.jsonl). */
+                            not verifiable and not flagged.  A separate kernel instantiation (the opt-in path costs the
+                            default one no registers); bench.py reports its rate as modes.protect_epilogue_gflops. */
 } ftsgemm_opts;
 /* sizeof(ftsgemm_opts) of ABI version 1: the smallest struct_size the library accepts (a zero-initialised struct is
  * rejected with FTSGEMM_ERR_INVALID_ARG instead of silently meaning "all defaults on the default stream"). */
@@ -183,7 +182,7 @@ void ftsgemm_default_opts(ftsgemm_opts *o);
 /* ---- kernel-variant table  (replaces sgemm.cu:235-237 + code_gen/main.py:8-16) --------------------------- */
 int ftsgemm_kernel_table(ftsgemm_kernel_info *out, int cap); /* returns number of rows (fills min(cap, rows)) */
 int ftsgemm_kernel_lookup(int kernel_id, ftsgemm_kernel_info *out);
-/* The concrete tcgen05 kernel id that ids 20 / 40 (AUTO) resolve to for this shape (replaces the reference's manual
+/* The concrete wgmma kernel id that ids 20 / 40 (AUTO) resolve to for this shape (replaces the reference's manual
  * choice of a variant per run, sgemm.cu:110-199).  Returns the id (> 0) or a negative error code. */
 int ftsgemm_select_kernel(int M, int N, int K, int fault_tolerant);
 
@@ -250,8 +249,8 @@ long long ftsgemm_verify_bad_count(ftsgemm_handle_t h);
 int ftsgemm_debug_set(const char *key, long long value);
 /* Host-side enumeration of the work decomposition of one launch (split-K head + data-parallel body), for tests:
  * rows of 9 ints {unit, tile, is_chk, m_blk, n_blk, kb_begin, kb_end, kind(0 whole,1 contributor,2 finisher), slice};
- * hdr[8] = {units, num_tiles, n_chk_tiles, sk_tiles, num_kb, cta_group, sk_slices, chk_slices}; checksum tiles carry
- * their K-slice index in the `slice` column.  Needs no GPU. */
+ * hdr[8] = {units, num_tiles, n_chk_tiles, sk_tiles, num_kb, CTAs per unit, sk_slices, chk_slices}; checksum tiles carry
+ * their K-slice index in the `slice` column.  Needs no GPU (assumes an L2 of 50 MiB, as on H100). */
 int ftsgemm_debug_schedule(int kernel_id, int M, int N, int K, int num_sms, int *hdr, int *rows, int cap);
 /* Device timeline of the last tensor-core launch made with ftsgemm_debug_set("trace", 1): per work unit 64 items x 8
  * u64 = %globaltimer ns {producer start, producer end, MMA start, MMA issue end, accumulator complete, check done,

@@ -194,8 +194,8 @@ def num_threads() -> int:
 
 
 # ----------------------------------------------------------------------------------------------
-# TF32 model of the B200 kernel (used only to explain/bound the kernel's deviation from the fp32
-# oracle; the parity target remains oracle_sgemm_nt).  tcgen05 kind::tf32 consumes fp32 bit patterns
+# TF32 model of the kernel (used only to explain/bound the kernel's deviation from the fp32
+# oracle; the parity target remains oracle_sgemm_nt).  wgmma with TF32 inputs consumes fp32 bit patterns
 # and ignores the 13 low mantissa bits.
 # ----------------------------------------------------------------------------------------------
 def tf32_trunc(x: np.ndarray) -> np.ndarray:

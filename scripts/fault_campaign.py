@@ -1,6 +1,6 @@
-"""BASELINE.json config 4: single-bit fault injection into the FP32 accumulator tile (tensor memory) of the fused
+"""BASELINE.json config 4: single-bit fault injection into the FP32 accumulator tile of the fused
 ABFT kernel, M=N=K=8192 by default; detection / location / correction rate per flipped bit position, plus the
-run-time overhead of the always-on self-test.  Writes gpurun_out/fault_campaign_<n>_id<k>.json (copied to profiles/ afterwards).
+run-time overhead of the always-on self-test.  Writes out/fault_campaign_<n>_id<k>.json.
 
 usage: python scripts/fault_campaign.py [n=8192] [kernel_id=31] [trials_per_bit=6]
 """
@@ -91,7 +91,7 @@ st = ft.stats()
 out["timing_ms"] = {"fault_free": t_clean, "selftest_every_tile": t_self,
                     "selftest_overhead_pct": 100.0 * (t_self / t_clean - 1.0)}
 out["maxC"] = scale
-(ROOT / "gpurun_out").mkdir(exist_ok=True)
-p = ROOT / "gpurun_out" / f"fault_campaign_{n}_id{kid}.json"
+(ROOT / "out").mkdir(exist_ok=True)
+p = ROOT / "out" / f"fault_campaign_{n}_id{kid}.json"
 p.write_text(json.dumps(out, indent=1))
 print("wrote", p)

@@ -1,6 +1,6 @@
 """Device timeline of the persistent kernel (ftsgemm_debug_trace): per-item main-loop / epilogue durations and stalls.
 
-usage: gpu_trace.py [ID N [key=value ...]] ...   writes gpurun_out/trace_<id>_<n>[_tag].json (summary + raw timeline)
+usage: gpu_trace.py [ID N [key=value ...]] ...   writes out/trace_<id>_<n>[_tag].json (summary + raw timeline)
 """
 import json
 import sys
@@ -14,7 +14,7 @@ sys.path.insert(0, str(ROOT / "scripts"))
 import __graft_entry__ as ge  # noqa: E402
 import cuda_rt as cu  # noqa: E402
 
-OUT = ROOT / "gpurun_out"
+OUT = ROOT / "out"
 OUT.mkdir(exist_ok=True)
 
 

@@ -1,5 +1,6 @@
 import sys, time
-sys.path.insert(0, '/root/repo')
+from pathlib import Path
+sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 import torch
 import __graft_entry__ as ge
 pkg = ge.load_package()

@@ -1,6 +1,6 @@
 """Burst-regime comparison of debug-knob settings inside ONE process (same box, same clock state).
 
-usage: knob_matrix.py sizes=2048,4096 id=31 steps=20 rounds=3 -- "carriers=0" "carriers=0,enc_units=16" ...
+usage: knob_matrix.py sizes=2048,4096 id=31 steps=20 rounds=3 -- "splitk=0" "splitk=0,epi_assist=0" ...
 Every setting is a comma-separated list of key=value debug knobs ("" = defaults); per size and round the settings (and
 cuBLAS-TF32, id 7) are interleaved.  One JSON line per size: median us per launch per setting, overhead vs id 7, and whether
 each setting's C (beta = 0) is bit-identical to the first setting's.

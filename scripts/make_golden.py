@@ -1,6 +1,6 @@
-"""Generate tests/golden/*.json from the reference's OWN host code (oracle/_ref/libref_utils.so =
-/root/reference/utils/utils.cu compiled unmodified).  Run in the build container, where
-/root/reference exists; the JSON travels to the GPU box, /root/reference does not.
+"""Generate tests/golden/* from the reference's OWN code (oracle/_ref/libref_utils.so = the reference's utils/utils.cu
+compiled unmodified, oracle/_ref/libref_kernels_cpu.so = its generated kernels under a CPU thread shim).  Run where the
+reference checkout exists (`make -C oracle REF=<path>`); the fixtures are committed, so the tests need neither.
 
 For END in {64,128,256,512,1024}: srand(10); A,B,C = generate_random_matrix(END); C=0 (sgemm.cu:12,52-56);
 C = cpu_gemm(1, 0, B^T-buffer, A-buffer) which is the kernels' column-major NT result
@@ -36,3 +36,33 @@ for n in (64, 128, 256, 512, 1024):
     }
     print(n, gold[str(n)]["C_sel"], gold[str(n)]["C_sum"], gold[str(n)]["C_abs_sum"])
 (out_dir / "ref_cpu_gemm.json").write_text(json.dumps(gold, indent=1))
+
+# Host-code pins at END = 160 (tests/test_oracle.py::test_oracle_equals_reference_host_code): the reference's inputs, its
+# cpu_gemm result and its verify_matrix verdicts on an exact and a perturbed copy.
+n = 160
+A, B, _ = O.ref_make_inputs(n)
+X = np.ascontiguousarray(B.reshape(n, n).T).reshape(-1)
+Z = np.zeros(n * n, np.float32)
+r.ref_cpu_gemm(1.0, 0.0, O._p(X), O._p(A), n, O._p(Z))
+bad = Z.copy(); bad[77] += 5.0
+host = {"n": n, "sha256": {"A": hashlib.sha256(A.tobytes()).hexdigest(), "B": hashlib.sha256(B.tobytes()).hexdigest(),
+                           "C": hashlib.sha256(Z.tobytes()).hexdigest()},
+        "verify_exact": int(r.ref_verify_matrix(O._p(Z), O._p(Z.copy()), n, n)),
+        "verify_perturbed_77": int(r.ref_verify_matrix(O._p(Z), O._p(bad), n, n))}
+(out_dir / "ref_host_code.json").write_text(json.dumps(host, indent=1))
+
+# The reference's generated kernels executed on the CPU (oracle/_ref/libref_kernels_cpu.so): their C for the inputs
+# tests/test_oracle.py::test_reference_kernels_on_cpu builds (seed 2), one .npy per case (<= 64 KiB each).
+rk = O.ref_kernels()
+assert rk is not None, "needs oracle/_ref/libref_kernels_cpu.so"
+for kid, variant, K in ((6, "huge", 160), (16, "huge", 160), (13, "large", 160), (11, "small", 480)):
+    ms, ns, _, _, _ = O.VARIANTS[variant]
+    M, N = ms, ns
+    rng = np.random.default_rng(2)
+    pad = 4096
+    A = np.zeros(M * K + pad, np.float32); B = np.zeros(N * K + pad, np.float32)
+    A[:M * K] = (rng.integers(-9, 10, M * K) * 0.1).astype(np.float32)
+    B[:N * K] = (rng.integers(-9, 10, N * K) * 0.1).astype(np.float32)
+    C = np.zeros(M * N, np.float32)
+    assert rk.ref_kernel_run(kid, M, N, K, O._p(A), O._p(B), O._p(C), 1.0, 0.0) == 0
+    np.save(out_dir / f"ref_kernel_{kid}_{variant}_K{K}.npy", C)

@@ -1,4 +1,4 @@
-"""Per-wave main-loop times from a device timeline (gpurun_out/trace_<id>_<n>.json): does the tile time grow with the wave?"""
+"""Per-wave main-loop times from a device timeline (out/trace_<id>_<n>.json): does the tile time grow with the wave?"""
 import json, sys
 import numpy as np
 for path in sys.argv[1:]:

@@ -44,14 +44,14 @@ def test_kernel_table_matches_reference_ids(ft):
     for nm, tile in ref_tiles.items():
         assert tab[ft.SGEMM_IDS[nm]]["ref_tile"] == tile and tab[ft.ABFT_IDS[nm]]["ref_tile"] == tile
         assert tab[ft.SGEMM_IDS[nm]]["tile"] == tab[ft.ABFT_IDS[nm]]["tile"]  # FT and non-FT share the tiling
-    # config 2 of BASELINE.json: the huge tile is literally 128 x 128 with UMMA K = 8 steps
+    # config 2 of BASELINE.json: the huge tile is literally 128 x 128 with MMA K = 8 steps
     assert tab[16]["tile"][:2] == (128, 128) and tab[14]["tile"][:2] == (128, 32)
-    # six names, six DISTINCT sm_100a tiles (round 1 aliased small = tall and large = huge)
+    # six names, six DISTINCT sm_90a tiles (round 1 aliased small = tall and large = huge)
     tiles = {nm: tab[ft.SGEMM_IDS[nm]]["tile"][:2] for nm in ref_tiles}
     assert len(set(tiles.values())) == 6, tiles
     assert tiles == {"small": (128, 64), "medium": (256, 64), "large": (256, 128), "tall": (128, 32), "wide": (128, 256),
                      "huge": (128, 128)}
-    # UMMA legality of every tcgen05 tile: M = 128 (cta_group::1) or 256 (cta_group::2), N % 16 == 0, 16 <= N <= 256
+    # legality of every wgmma tile: M = 128 (one CTA) or 256 (two CTAs), N % 16 == 0, 16 <= N <= 256
     for k in tab.values():
         if k["engine"] == 1 and k["id"] not in (ft.ID_SGEMM_AUTO, ft.ID_ABFT_AUTO):
             m, n, kk = k["tile"]

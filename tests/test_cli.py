@@ -46,4 +46,4 @@ def test_cli_refuses_without_gpu(ft):
     if torch.cuda.is_available():
         pytest.skip("GPU present")
     p = ft.run_cli([64, 64, 0, 0, 0], timeout=60)
-    assert p.returncode == 1 and "no sm_100 CUDA device" in p.stderr
+    assert p.returncode == 1 and "no sm_90 CUDA device" in p.stderr

@@ -1,11 +1,11 @@
-"""GPU parity tests proper (run on the B200 box with -m gpu): the CUDA path, called through the C ABI, against the
+"""GPU parity tests proper (run on an H100 with -m gpu): the CUDA path, called through the C ABI, against the
 CPU oracle on the same seeded inputs, against the committed golden fixtures, and -- at BASELINE.json's full sizes --
 through size-independent properties.
 
 Tolerances (stated once, used everywhere):
   * TOL_NORM = 1e-3: Frobenius-norm relative error against the FP32 sequential-k oracle -- the north_star's
     "within 1e-3 rel of the reference's CPU SGEMM".  The main contraction is single-pass TF32 (operands truncated to
-    10 mantissa bits by the tensor core, FP32 accumulate), measured 6.1e-4 .. 7.8e-4 on B200.
+    10 mantissa bits by the tensor core, FP32 accumulate).
   * TOL_MODEL = 5e-5: norm-wise against a float64 product of TF32-TRUNCATED operands (what the tensor core computes up
     to FP32 accumulation order); measured 1.5e-7 (K=64) .. 2e-5 (K=8192).
   * the reference comparator verify_matrix (utils/utils.cu:61-77; fail iff rel>1e-2 AND abs>1e-2) is applied too; with
@@ -155,7 +155,7 @@ def test_random_shapes_and_knobs(cuda, ft, dev, oracle, seed):
     beta = float(rng.choice([0.0, -1.5, 1.0]))
     knobs = {"splitk": int(rng.choice([-1, 0, 2, 3])), 
              "wave_sync": int(rng.choice([0, 1])), "pdl": int(rng.choice([0, 1])), "epi_assist": int(rng.choice([0, 1])),
-             "carriers": int(rng.choice([0, 1])), "chk_slices": int(rng.choice([1, 2, 3])), "enc_front": int(rng.choice([0, 1]))}
+             "chk_slices": int(rng.choice([1, 2, 3])), "enc_front": int(rng.choice([0, 1]))}
     A, B = rng.standard_normal(M * K).astype(np.float32), rng.standard_normal(N * K).astype(np.float32)
     C0 = rng.standard_normal(M * N).astype(np.float32)
     model = oracle.sgemm_nt_tf32_model(M, N, K, alpha, A, B, beta, C0, "trunc")
@@ -182,46 +182,9 @@ def test_random_shapes_and_knobs(cuda, ft, dev, oracle, seed):
             ft.debug_set(k, -1)
 
 
-def test_carrier_tiles_equal_checksum_items(cuda, ft, dev, oracle):
-    """Carrier tiles (the first data tile of every tile-row also accumulates the row's checksum product in tensor-memory
-    stage 1, plan kind 6) against checksum items: the same UMMA sequence produces the same expected checksums, so results
-    and verdicts are bit-identical -- fault-free, with faults inside and outside carrier tiles, with every cut plan (a seeded
-    piece right behind a carrier must wait for the carrier's epilogue before its seed goes into stage 1)."""
-    rng = np.random.default_rng(31)
-    for (kid, M, N, K) in ((31, 1536, 1024, 640), (31, 768, 2048, 352), (15, 512, 512, 256), (12, 1024, 512, 300)):
-        A, B = _rand(rng, M * K), _rand(rng, N * K)
-        C0 = rng.standard_normal(M * N).astype(np.float32)
-        faults = [{"row": 5, "col": 3, "xor": 1 << 29}, {"row": M - 1, "col": N - 1, "add": 77.0},
-                  {"row": M // 2, "col": 200, "xor": 1 << 30}, {"row": 300, "col": N // 2 + 7, "add": -9.0}]
-        for splitk in (-1, 0, 2, 3):
-            outs, sts = [], []
-            for carriers in (1, 0):
-                try:
-                    ft.debug_set("carriers", carriers)
-                    ft.debug_set("splitk", splitk)
-                    ft.debug_set("chk_slices", 1)  # (K-slices of checksum items add their partial sums in another order)
-                    if carriers:  # (the plan really contains carriers: one per tile-row)
-                        hdr, segs = ft.debug_schedule(kid, M, N, K, cuda.cuda.get_device_properties(0).multi_processor_count)
-                        assert sum(1 for s_ in segs if s_["kind"] == 6) > 0 and hdr["n_chk_tiles"] == 0
-                    dev.stats()
-                    clean = _run(cuda, dev, kid, M, N, K, A, B, C0, 0.75, -1.5)
-                    assert dev.stats()["detected"] == 0
-                    outs.append((clean, _run(cuda, dev, kid, M, N, K, A, B, C0, 0.75, -1.5, opts=ft.make_opts(faults=faults))))
-                    st = dev.stats()
-                    sts.append((st["detected"], st["corrected"], st["recomputed"], st["uncorrectable"]))
-                finally:
-                    ft.debug_set("carriers", -1)
-                    ft.debug_set("splitk", -1)
-                    ft.debug_set("chk_slices", -1)
-            assert sts[0] == sts[1] and sts[0][0] == 4 and sts[0][3] == 0, (kid, splitk, sts)
-            assert np.array_equal(outs[0][0], outs[1][0]) and np.array_equal(outs[0][1], outs[1][1]), (kid, splitk)
-    model = oracle.sgemm_nt_tf32_model(M, N, K, 0.75, A, B, -1.5, C0, "trunc")
-    assert oracle.error_metrics(model, outs[0][0])["rel_fro"] < TOL_MODEL
-
-
 def test_epilogue_assist_is_neutral(cuda, ft, dev):
     """The helper-assisted epilogue splits the columns of a final data-tile epilogue between the epilogue warp and the helper
-    warp of the same TMEM lane quadrant (row sums exchanged through shared memory): results bit-identical with it on and
+    warp of the same 32-row quadrant (row sums exchanged through shared memory): results bit-identical with it on and
     off, injected faults in both column halves and on the split corrected."""
     rng = np.random.default_rng(13)
     M, N, K = 640, 1024, 352
@@ -253,7 +216,7 @@ def test_wave_sync_is_bitwise_neutral(cuda, ft, dev):
     """The wave re-synchronisation of large problems (a barrier among the leader producers at whole-tile boundaries) only
     delays loads: forced on a multi-wave shape, with and without cut tiles / ABFT, the results must not change a bit."""
     rng = np.random.default_rng(11)
-    M, N, K = 2048, 2304, 288   # 72 tiles of 256x256 on 74 CTA pairs is one wave: use the 128-wide pair tile as well
+    M, N, K = 2048, 2304, 288   # 72 tiles of 256x256 on 66 two-CTA units is just over one wave: use the 128-wide two-CTA tile as well
     A, B = _rand(rng, M * K), _rand(rng, N * K)
     C0 = rng.standard_normal(M * N).astype(np.float32)
     for kid in (6, 16, 22, 32, 21, 31):
@@ -273,7 +236,7 @@ def test_wave_sync_is_bitwise_neutral(cuda, ft, dev):
 
 @pytest.mark.parametrize("slices", [2, 3, 5])
 def test_split_k_head_forced(cuda, ft, dev, oracle, slices):
-    """Force cut tiles (pieces park their accumulator, the next piece seeds tensor memory with it) on shapes where the
+    """Force cut tiles (pieces park their accumulator, the next piece seeds its accumulator with it) on shapes where the
     planner would not cut, with and without ABFT + injected faults."""
     rng = np.random.default_rng(slices)
     M, N, K = 768, 1024, 1600
@@ -411,7 +374,7 @@ def test_reference_selftest_every_tile_corrected(cuda, ft, dev, oracle):
 
 @pytest.mark.parametrize("bit", [31, 30, 27, 23, 22, 21, 20])
 def test_single_bit_flips_detected_and_corrected(cuda, ft, dev, bit):
-    """Config 4 of BASELINE.json in miniature: flip one bit of one FP32 accumulator in tensor memory.  Elements with
+    """Config 4 of BASELINE.json in miniature: flip one bit of one FP32 accumulator.  Elements with
     |value| in [8, 64) are chosen so that every listed bit moves the value by >= 1 (bit 20 of an element in [8,16));
     the per-bit detection/correction RATES over random elements are measured by scripts/fault_campaign.py."""
     rng = np.random.default_rng(bit)
@@ -486,9 +449,9 @@ def test_two_faults_in_one_row_are_recomputed(cuda, ft, dev):
 
 def test_protected_epilogue(cuda, ft, dev):
     """opts.protect_epilogue (the reference's epilogue, ft_sgemm_huge.cuh:573-690, and the window between its last check and
-    the store are unprotected): the store pass re-derives the verified row sums from what it re-reads out of tensor memory
+    the store are unprotected): the store pass re-derives the verified row sums from what it re-reads out of the accumulator
     and checks the sum of what it stores.  Fault-free: bit-identical to the unprotected kernel, nothing flagged.  An upset of
-    tensor memory AFTER the accumulator check (fault mode 2) or of the value being stored (mode 3) goes unnoticed without
+    the accumulator AFTER the accumulator check (fault mode 2) or of the value being stored (mode 3) goes unnoticed without
     the option, is detected with it, and with beta == 0 the row segment is recomputed."""
     rng = np.random.default_rng(17)
     M, N, K = 640, 1024, 352

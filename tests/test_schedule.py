@@ -2,7 +2,7 @@
 tile-columns), using the host-side enumeration of the SAME inline code the device runs (ftsgemm_debug_schedule):
   * every (tile, k-block) is computed exactly once, the pieces of a cut tile are contiguous and ordered first/middle/last;
   * every unit's list follows the global order [early first pieces][checksum][whole][late first pieces][2nd pieces]...;
-  * no circular wait: with in-order roles, 2 TMEM accumulator stages per unit, a piece's main loop waiting for the
+  * no circular wait: with in-order roles, one accumulator per unit, a piece's main loop waiting for the
     previous piece's parked accumulator and ABFT data tiles waiting for their checksum tile-columns in the epilogue,
     every item completes."""
 import itertools
@@ -11,7 +11,7 @@ import pytest
 
 TILE_N = {1: 64, 2: 64, 3: 128, 4: 32, 6: 128, 5: 256, 21: 256, 22: 128, 11: 64, 12: 64, 13: 128, 14: 32, 16: 128, 15: 256, 31: 256,
           32: 128}
-PAIR_IDS = (2, 3, 12, 13, 21, 22, 31, 32)  # CTA-pair tiles (cta_group::2)
+PAIR_IDS = (2, 3, 12, 13, 21, 22, 31, 32)  # 256-row tiles (two CTAs per work unit)
 
 
 def _simulate(hdr, segs, acc_stages):
@@ -29,8 +29,6 @@ def _simulate(hdr, segs, acc_stages):
                 tiles_c = max(tiles_c, s["n_blk"] + 1)
             if s["kind"] in (1, 2, 3):
                 piece_at[(s["tile"], s["slice"])] = (u, i)
-    carrier_rows = {s["m_blk"] for s in segs if s["kind"] == 6}  # rows whose checksum product rides on their first data tile
-    row_done = {m: False for m in carrier_rows}
     mma_done = [0] * units   # number of items whose main loop finished
     epi_done = [0] * units
     done_epi = set()         # (unit, idx)
@@ -52,16 +50,12 @@ def _simulate(hdr, segs, acc_stages):
                 ok = True
                 if hdr["n_chk_tiles"] and not s["is_chk"] and s["kind"] in (0, 2):  # parking pieces are not checked
                     ok = all(chk_done[(s["m_blk"], c, sl)] for c in range(tiles_c) for sl in range(max(1, hdr.get("chk_slices", 1))))
-                if carrier_rows and s["kind"] in (0, 2):  # waits for the carrier of its tile-row (a carrier publishes, then checks itself)
-                    ok = row_done[s["m_blk"]]
                 if not ok:
                     break
                 epi_done[u] += 1
                 done_epi.add((u, i))
                 if s["is_chk"]:
                     chk_done[(s["m_blk"], s["n_blk"], s["slice"])] = True
-                if s["kind"] == 6:
-                    row_done[s["m_blk"]] = True
                 progress = True
     return all(epi_done[u] == len(per_unit[u]) for u in range(units))
 
@@ -70,7 +64,7 @@ def _simulate(hdr, segs, acc_stages):
 @pytest.mark.parametrize("shape", [(4096, 4096, 4096), (2048, 2048, 2048), (1024, 1024, 1024), (8192, 8192, 512),
                                    (1536, 2560, 1000), (256, 256, 64), (128, 4096, 32), (5120, 384, 4096),
                                    (16384, 16384, 1024), (32768, 1024, 256)])
-@pytest.mark.parametrize("num_sms", [148, 16, 6])
+@pytest.mark.parametrize("num_sms", [148, 132, 16, 6])
 def test_decomposition_covers_and_cannot_deadlock(ft, kid, shape, num_sms):
     M, N, K = shape
     hdr, segs = ft.debug_schedule(kid, M, N, K, num_sms)
@@ -110,8 +104,8 @@ def test_decomposition_covers_and_cannot_deadlock(ft, kid, shape, num_sms):
     for s_ in segs:
         per_unit.setdefault(s_["unit"], []).append(s_)
     for lst in per_unit.values():
-        word = "".join("C" if s_["is_chk"] else "WPFM__K"[s_["kind"]] for s_ in lst)
-        assert re.fullmatch(r"K?P*C*W*P*[FM]*", word), word  # (a carrier is always the first item of its unit)
+        word = "".join("C" if s_["is_chk"] else "WPFM"[s_["kind"]] for s_ in lst)
+        assert re.fullmatch(r"P*C*W*P*[FM]*", word), word
         later = [s_["slice"] for s_ in lst if s_["kind"] in (2, 3)]
         assert later == sorted(later)
         for cls in ("C", "W"):
@@ -123,32 +117,29 @@ def test_decomposition_covers_and_cannot_deadlock(ft, kid, shape, num_sms):
     # checksum tiles: n_chk_tiles of them, 8 columns per N-tile
     chk = {(s["m_blk"], s["n_blk"], s["slice"]) for s in segs if s["is_chk"]}
     assert len(chk) == hdr["n_chk_tiles"]
-    carriers = [s_ for s_ in segs if s_["kind"] == 6]
-    if carriers:  # one per tile-row, the row's first tile, and no checksum tiles at all
-        assert hdr["n_chk_tiles"] == 0 and sorted(s_["m_blk"] for s_ in carriers) == list(range(-(-M // (128 * hdr["cta_group"]))))
-        assert all(s_["n_blk"] == 0 for s_ in carriers) and 4 * -(-N // TILE_N[kid]) <= 32 * hdr["cta_group"]
-    elif kid in (11, 12, 13, 14, 16, 15, 31, 32):
+    assert all(s_["kind"] in (0, 1, 2, 3) for s_ in segs)
+    if kid in (11, 12, 13, 14, 16, 15, 31, 32):
         tiles_n = -(-N // TILE_N[kid])
         assert hdr["n_chk_tiles"] == -(-M // (128 * hdr["cta_group"])) * -(-(tiles_n * 4) // TILE_N[kid]) * S_chk
         if S_chk > 1:  # slices only where every data tile and every slice get a unit of their own
             assert hdr["num_tiles"] <= units and num_kb // S_chk >= 8
-    acc_stages = 2 if 2 * TILE_N[kid] <= 512 else 1
+    acc_stages = 1  # the next main loop of a unit starts once the previous epilogue has freed the ring
     assert _simulate(hdr, segs, acc_stages), "circular wait in the schedule"
 
 
 def test_planner_levels_the_units(ft):
     """The list scheduler + cut tiles remove the wave-quantisation loss where that pays."""
     def makespan(kid, n):
-        hdr, segs = ft.debug_schedule(kid, n, n, n, 148)
+        hdr, segs = ft.debug_schedule(kid, n, n, n, 132)
         work = [0.0] * hdr["units"]
         for s in segs:
             work[s["unit"]] += (0.58 if s["is_chk"] else 1.25 if s["kind"] == 6 else 1.0) * (s["kb_end"] - s["kb_begin"]) / hdr["num_kb"]
         return hdr, max(work), sum(work) / hdr["units"]
-    hdr, t, ideal = makespan(21, 4096)   # 256 tiles on 74 pairs: 3.46 waves -> 4 waves uncut
-    assert hdr["sk_tiles"] > 0 and hdr["sk_slices"] == 2 and t <= 3.7
-    hdr, t, ideal = makespan(21, 1024)   # 16 tiles on 74 pairs: nothing to level
+    hdr, t, ideal = makespan(21, 3072)   # 144 tiles on 66 units: 2.18 waves -> 3 waves uncut
+    assert hdr["sk_tiles"] > 0 and hdr["sk_slices"] == 2 and t <= 2.5
+    hdr, t, ideal = makespan(21, 1024)   # 16 tiles on 66 units: nothing to level
     assert hdr["sk_tiles"] == 0 and t == 1.0
     hdr, t, ideal = makespan(31, 4096)   # ABFT tiles are cut as well (seeded chains keep the checksum algebra exact); the
-    assert hdr["sk_tiles"] > 0 and hdr["n_chk_tiles"] == 0 and t <= ideal * 1.05  # checksum product rides on 16 carrier tiles
+    assert hdr["sk_tiles"] > 0 and hdr["n_chk_tiles"] == 16 and t <= ideal * 1.05  # checksum product: one item per tile-row
     hdr, t, ideal = makespan(31, 8192)
     assert hdr["n_chk_tiles"] == 32 and t <= ideal * 1.03

@@ -142,7 +142,7 @@ def _nccl_worker(rank, world, port, q):
 def test_world2_nccl_device_verdict_exchange(cuda, ft):
     """The multi-GPU exchange step on real GPUs: two ranks, NCCL all-gather of the device-side verdict vectors."""
     if cuda.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
