@@ -224,7 +224,8 @@ int make_tmap_kmajor(ftsgemm_handle_t h, CUtensorMap *tm, const float *base, uin
 }
 
 // Largest grid (in work units of CG CTAs) of this instantiation whose CTAs can all be resident at once: one CTA per SM the
-// device reports (multiProcessorCount, which an MPS active-thread percentage reduces), or none when a CTA does not fit.
+// device reports (multiProcessorCount, which an MPS active-thread percentage reduces), at most as many two-CTA clusters as
+// the device can hold at once (CG = 2), or none when a CTA does not fit.
 // The persistent kernel's inter-CTA waits (front phase, checksum flags, parked accumulators, wave counters) are only
 // deadlock-free for such a grid, so the planner never gets more units than this.  If SMs are nevertheless held by other
 // work so that the grid cannot become resident, the waits' watchdog (ptx.cuh) ends the launch with FTSGEMM_ERR_TIMEOUT
@@ -242,7 +243,24 @@ int query_max_units(ftsgemm_handle_t h, int *out) {
   FT_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
   int per_sm = 0;
   FT_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, Cfg::kSmemBytes));
-  const int units = per_sm > 0 ? h->num_sms / CG : 0;  // one persistent CTA per SM
+  int units = per_sm > 0 ? h->num_sms / CG : 0;  // one persistent CTA per SM
+  if (CG == 2 && units > 0) {
+    // a unit is a cluster of two CTAs, placed on two SMs of one GPC: fewer may fit than half the SMs
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(units * CG);
+    cfg.blockDim = dim3(kThreads);
+    cfg.dynamicSmemBytes = Cfg::kSmemBytes;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = CG;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    int clusters = 0;
+    FT_CUDA(h, cudaOccupancyMaxActiveClusters(&clusters, kern, &cfg));
+    units = std::min(units, clusters);
+  }
   h->max_units[key] = units;
   *out = units;
   return FTSGEMM_OK;
@@ -264,11 +282,18 @@ int launch_tc(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB
   cfg.blockDim = dim3(kThreads);
   cfg.dynamicSmemBytes = Cfg::kSmemBytes;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
+  cudaLaunchAttribute attr[2];
   int na = 0;
   if (p.pdl_wait) {
     attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[na].val.programmaticStreamSerializationAllowed = 1;
+    ++na;
+  }
+  if (CG == 2) {  // a work unit is a cluster: its CTAs share the B tile through TMA multicast
+    attr[na].id = cudaLaunchAttributeClusterDimension;
+    attr[na].val.clusterDim.x = CG;
+    attr[na].val.clusterDim.y = 1;
+    attr[na].val.clusterDim.z = 1;
     ++na;
   }
   cfg.attrs = attr;
@@ -436,7 +461,8 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const floa
   p.Bt = h->d_bt;
   rc = make_tmap_kmajor(h, &tmA, p.At, M, K, p.ldk, kBM);
   if (rc) return rc;
-  rc = make_tmap_kmajor(h, &tmB, p.Bt, N, K, p.ldk, BN);
+  // CG = 2: each CTA of a unit loads BN/2 rows of the B tile and multicasts them to both
+  rc = make_tmap_kmajor(h, &tmB, p.Bt, N, K, p.ldk, BN / CG);
   if (rc) return rc;
   tmC = tmB;
   if (ft) {
@@ -507,7 +533,7 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const floa
       FT_CUDA(h, cudaGetLastError());
     }
     if (!reuse) { h->chk_for_b = dB; h->chk_n = N; h->chk_k = K; h->chk_bn = BN; }
-    rc = make_tmap_kmajor(h, &tmC, h->d_chk, p.n_chk_cols, K, chk_ld, BN);
+    rc = make_tmap_kmajor(h, &tmC, h->d_chk, p.n_chk_cols, K, chk_ld, BN / CG);
     if (rc) return rc;
   }
   // ---- work plan (plan.h), cached per shape on the handle

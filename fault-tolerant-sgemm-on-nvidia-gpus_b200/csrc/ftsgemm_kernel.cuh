@@ -9,7 +9,8 @@
 //   front phase   : every warp of the grid transposes its share of A and B into K-major copies (wgmma takes TF32
 //                   operands K-major only; the caller's operands are MN-major) and, for large B, encodes B (below)
 //   warp 0        : TMA producer: cp.async.bulk.tensor 32(K) x 128(M) and 32(K) x BN(N) fp32 boxes, 128B swizzle, into a
-//                   STAGES-deep shared-memory ring (full/empty mbarriers)
+//                   STAGES-deep shared-memory ring (full/empty mbarriers); CG = 2: a unit is a cluster, each CTA loads
+//                   BN/2 rows of B and multicasts them into the ring of both CTAs
 //   warps 4-11    : two consumer warpgroups (64 rows each): wgmma.m64nBNk8 TF32, FP32 accumulate in registers; after the
 //                   main loop the accumulator is written over the (then idle) ring, and
 //                   warps 4-7  epilogue  (lane = row): per-row ABFT detect / locate / correct, C = alpha*acc + beta*C
@@ -980,8 +981,8 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t a_desc, 
 // ------------------------------------------------------------------------------------------------------------
 // PROT: the instantiation with the protected store pass (opts.protect_epilogue) -- a separate binary, so that the opt-in
 // path costs the common epilogue no registers.
-// SEED: the instantiation for plans with cut tiles.  Loading a parked accumulator into the wgmma accumulator registers
-// makes ptxas serialise every wgmma of the function, so plans without cut tiles run a kernel that has no such path.
+// SEED: the instantiation for plans with cut tiles, which load a parked accumulator into the wgmma accumulator registers;
+// plans without cut tiles run a kernel that has no such path.
 template <int BN, bool FT, int CG, bool PROT = false, bool SEED = false>
 __global__ void __launch_bounds__(kThreads, 1)
 ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -1002,7 +1003,8 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int cta_rank = (CG == 2) ? static_cast<int>(blockIdx.x % CG) : 0;
+  // CG = 2: a work unit is a cluster of two CTAs (launched with cluster dimension 2, consecutive blockIdx.x)
+  const int cta_rank = (CG == 2) ? static_cast<int>(ptx::cluster_ctarank()) : 0;
   const int unit = blockIdx.x / CG;  // persistent work unit = CG CTAs
 
   // the next kernel in the stream (if it was launched as a programmatic dependent) may be scheduled as soon as this
@@ -1014,14 +1016,20 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     if (FT) ptx::tma_prefetch_desc(&tmChk);
   }
   if (warp == 1 && lane == 0) {
+    // CG = 2: each producer multicasts its half of the B tile into the same stage of both CTAs, so a stage (and, since the
+    // accumulator is written over the ring, the ring after an item) may only be refilled once the consumers of BOTH CTAs
+    // have released it: every consumer warp arrives on its own and on the peer's empty barrier, every epilogue on both
+    // ring-free barriers
     for (int s = 0; s < kStages; ++s) {
-      ptx::mbar_init(full_bar(s), 1);   // the producer's arrive.expect_tx
-      ptx::mbar_init(empty_bar(s), 8);  // one arrive per consumer warp once its wgmma reading the stage is complete
+      ptx::mbar_init(full_bar(s), 1);        // the producer's arrive.expect_tx
+      ptx::mbar_init(empty_bar(s), 8 * CG);  // one arrive per consumer warp (of each CTA) once its wgmma reading the stage is complete
     }
-    ptx::mbar_init(ring_free_bar, 1);
+    ptx::mbar_init(ring_free_bar, CG);
     ptx::fence_mbar_init();
   }
-  __syncthreads();
+  // (CG = 2: the peer's barriers are initialised before any remote arrive or multicast reaches them)
+  if constexpr (CG == 2) ptx::cluster_sync();
+  else __syncthreads();
   if (p.pdl_wait) ptx::pdl_wait();  // everything before this line touched no global memory
 
   {
@@ -1085,9 +1093,13 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           const uint32_t sB = sA + Cfg::kABytes;
           const int k0 = kb * kBK;
           if (ptx::elect_one()) {
+            // (CG = 2: own A box + own B half + the peer's B half = kStageBytes as well)
             ptx::mbar_arrive_expect_tx(full_bar(stage), static_cast<uint32_t>(Cfg::kStageBytes));
             ptx::tma_load_2d(sA, &tmA, full_bar(stage), k0, m0);
-            ptx::tma_load_2d(sB, tmb, full_bar(stage), k0, nb0);
+            if constexpr (CG == 2)  // B box = BN/2 rows; the 1 KiB-aligned halves give the layout of one BN-row box
+              ptx::tma_load_2d_multicast(sB + cta_rank * (Cfg::kBBytes / 2), tmb, full_bar(stage), k0, nb0 + cta_rank * (BN / 2), 0x3);
+            else
+              ptx::tma_load_2d(sB, tmb, full_bar(stage), k0, nb0);
           }
           __syncwarp();
           if (++stage == kStages) {
@@ -1117,6 +1129,10 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     const uint32_t taddr = static_cast<uint32_t>(q * 32) << 16;
     const bool tracer = p.trace != nullptr && cta_rank == 0 && warp == 4 && lane == 0;
     const bool assist_on = p.epi_assist != 0 && BN >= 64;
+    auto release_stage = [&](int s) {
+      ptx::mbar_arrive(empty_bar(s));
+      if constexpr (CG == 2) ptx::mbar_arrive_cluster(empty_bar(s), cta_rank ^ 1);
+    };
     int stage = 0;
     uint32_t phase = 0;
     SegIter it(p, unit);
@@ -1131,6 +1147,9 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const int m = m0_cta + row;
       // the first wgmma of a tile overwrites the accumulator ...
       uint32_t scale_d = 0u;
+      // (nothing is in flight here -- the previous item ended with wait_group 0 -- but ptxas only sees that through this
+      // wait: without it, the seed loads below make it serialise every wgmma of the function)
+      if (SEED) ptx::wgmma_wait<0>();
       if (SEED && (sg.kind == 2 || sg.kind == 3)) {
         // ... unless it continues a cut tile: seed: the previous piece's parked accumulator (its 32-row quadrant is complete once its flag is raised)
         const int slot = ((sg.slice - 1) * p.sk_tiles + sg.split_idx) * CG + cta_rank;
@@ -1169,7 +1188,7 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         ptx::wgmma_commit();
         // one k-block stays in flight; the one before it is complete and its stage goes back to the producer
         ptx::wgmma_wait<1>();
-        if (prev_stage >= 0 && lane == 0) ptx::mbar_arrive(empty_bar(prev_stage));
+        if (prev_stage >= 0 && lane == 0) release_stage(prev_stage);
         prev_stage = stage;
         if (++stage == kStages) {
           stage = 0;
@@ -1178,7 +1197,7 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       }
       ptx::wgmma_wait<0>();
       ptx::fence_regs(acc);
-      if (prev_stage >= 0 && lane == 0) ptx::mbar_arrive(empty_bar(prev_stage));
+      if (prev_stage >= 0 && lane == 0) release_stage(prev_stage);
       if (tracer) trace_put(p, unit, item_idx, 3, globaltimer_ns());
       // every consumer warp's MMAs are complete, so the ring is idle: the accumulator goes over it
       ptx::named_bar_sync(1, 256);
@@ -1296,12 +1315,17 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (tracer) trace_put(p, unit, item_idx, 6, globaltimer_ns());
       ptx::fence_proxy_async();  // generic accesses of the ring before the next TMA writes into it
       ptx::named_bar_sync(1, 256);
-      if (warp == 4 && lane == 0) ptx::mbar_arrive(ring_free_bar);
+      if (warp == 4 && lane == 0) {
+        ptx::mbar_arrive(ring_free_bar);
+        if constexpr (CG == 2) ptx::mbar_arrive_cluster(ring_free_bar, cta_rank ^ 1);  // the peer's producer writes B here too
+      }
     }
   }
 
   __syncwarp();  // reconverge the single-lane roles before the barrier below
-  __syncthreads();
+  // (CG = 2: neither CTA exits while the peer may still arrive on its barriers)
+  if constexpr (CG == 2) ptx::cluster_sync();
+  else __syncthreads();
   if (FT && p.peer_world > 0 && threadIdx.x == 0) {
     // fused verdict push: every CTA's counter updates are ordered before its arrival; the last arrival publishes
     __threadfence();

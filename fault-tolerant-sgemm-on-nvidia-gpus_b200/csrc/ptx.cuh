@@ -38,6 +38,30 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t byt
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
+// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster.  Default semantics (release at CTA
+// scope): the callers only hand back shared memory whose reads have completed (wgmma after wait_group, accumulator
+// loads whose values are consumed); .release.cluster would put MEMBAR.ALL.GPU in front of every arrive, which made the
+// main loop ~40 % slower.
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}" ::"r"(bar),
+      "r"(cta)
+      : "memory");
+}
+
+// ----------------------------------------------------------------------------- cluster
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster (not .aligned: see named_bar_sync)
+__device__ __forceinline__ void cluster_sync() {
+  __syncwarp();
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
 // FTSGEMM_TRYWAIT_HINT_NS > 0 passes a suspend-time hint: the waiting warp is parked by the hardware (and woken by the
 // phase completion) instead of re-issuing try_wait, which leaves the issue slots of its SM sub-partition to the warps
 // that have work.
@@ -145,6 +169,14 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *tm,
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
       "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1)
+      : "memory");
+}
+// The same, written to the same shared-memory offset in every CTA of `cta_mask`, each signalling its own mbarrier at `bar`.
+__device__ __forceinline__ void tma_load_2d_multicast(uint32_t dst, const CUtensorMap *tm, uint32_t bar, int c0, int c1,
+                                                      uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(dst),
+      "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
 __device__ __forceinline__ float ld_shared_f1(uint32_t addr) {
