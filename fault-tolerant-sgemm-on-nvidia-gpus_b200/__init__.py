@@ -30,6 +30,10 @@ ID_SGEMM_AUTO, ID_ABFT_AUTO = 20, 40  # per-shape choice among the wgmma variant
 SGEMM_IDS = {"small": 1, "medium": 2, "large": 3, "tall": 4, "wide": 5, "huge": 6, "giant": 21, "pair128": 22}
 ABFT_IDS = {"small": 11, "medium": 12, "large": 13, "tall": 14, "wide": 15, "huge": 16, "giant": 31, "pair128": 32}
 
+# operand layouts of run_ex (include/ftsgemm.h): MN-major A(m,k) at A[m + k*lda], B(n,k) at B[n + k*ldb] (the reference's);
+# K-major A(m,k) at A[k + m*lda], B(n,k) at B[k + n*ldb]
+LAYOUT_MN_MAJOR, LAYOUT_K_MAJOR = 0, 1
+
 
 class FtsgemmError(RuntimeError):
     def __init__(self, code: int, msg: str):
@@ -82,7 +86,7 @@ class Stats(C.Structure):
 # every symbol include/ftsgemm.h declares (checked by tests/test_abi.py without a GPU)
 EXPORTED_SYMBOLS = [
     "ftsgemm_create", "ftsgemm_destroy", "ftsgemm_abi_version", "ftsgemm_error_string", "ftsgemm_last_cuda_error",
-    "ftsgemm_default_opts", "ftsgemm_kernel_table", "ftsgemm_kernel_lookup", "ftsgemm_run", "ftsgemm_get_stats",
+    "ftsgemm_default_opts", "ftsgemm_kernel_table", "ftsgemm_kernel_lookup", "ftsgemm_run", "ftsgemm_run_ex", "ftsgemm_get_stats",
     "ftsgemm_run_host", "ftsgemm_baseline", "ftsgemm_verify", "ftsgemm_debug_set", "ftsgemm_debug_schedule",
     "ftsgemm_verify_bad_count", "ftsgemm_debug_trace", "ftsgemm_stats_device", "ftsgemm_select_kernel", "ftsgemm_launch_count", "ftsgemm_peer_export", "ftsgemm_peer_connect",
     "ftsgemm_peer_verdict",
@@ -118,6 +122,7 @@ def lib():
         L.ftsgemm_kernel_table.argtypes = [C.POINTER(KernelInfo), ip]
         L.ftsgemm_kernel_lookup.argtypes = [ip, C.POINTER(KernelInfo)]
         L.ftsgemm_run.argtypes = [vp, ip, ip, ip, ip, vp, vp, vp, fp, fp, C.POINTER(Opts)]
+        L.ftsgemm_run_ex.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, vp, ip, ip, vp, ip, fp, fp, C.POINTER(Opts)]
         L.ftsgemm_get_stats.argtypes = [vp, C.POINTER(Stats)]
         L.ftsgemm_run_host.argtypes = [vp, ip, ip, ip, ip, vp, vp, vp, fp, fp, C.POINTER(Opts)]
         L.ftsgemm_stats_device.argtypes = [vp, vp, vp]
@@ -216,6 +221,60 @@ def debug_set(key: str, value: int) -> None:
     _check(lib().ftsgemm_debug_set(key.encode(), int(value)))
 
 
+def _pad4(n: int) -> int:
+    return (n + 3) // 4 * 4
+
+
+def _view(shape, stride, ptr: int, ld4: bool):
+    """("row", ld) or ("col", ld) of a 2-D matrix the library can read in place, None if it cannot: it needs a unit
+    stride, a leading stride of at least the row length, a 16-byte aligned base and -- for A and B (ld4) -- 16-byte rows."""
+    R, Cn = shape
+    s0, s1 = stride
+    if ptr % 16:
+        return None
+    if s1 == 1 or Cn == 1:  # row-major (a one-column matrix is both)
+        ld = s0 if R > 1 else _pad4(Cn)
+        if ld >= Cn and (not ld4 or ld % 4 == 0):
+            return ("row", ld)
+    if s0 == 1 or R == 1:  # column-major
+        ld = s1 if Cn > 1 else _pad4(R)
+        if ld >= R and (not ld4 or ld % 4 == 0):
+            return ("col", ld)
+    return None
+
+
+def matmul_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0, b_ptr: int = 0, out_ptr: int = 0) -> dict:
+    """run_ex arguments for out = a @ b with a: (M, K), b: (K, N), out: (M, N), from shapes, element strides and addresses.
+
+    Column-major out: C = out, kernel A = a, kernel B = b^T.  Row-major out: C = out^T = b^T a^T (swap = True), so the
+    kernel's M and N are N and M, kernel A = b^T and kernel B = a; for x @ W.T with row-major x, W and out both kernel
+    operands are then K-major and no transpose runs.  copy_a / copy_b / copy_out mark matrices that cannot be read in
+    place (see _view); the arguments returned describe the copies matmul makes of them: a as row-major and b as
+    column-major with the row length padded to a multiple of 4 (both K-major for the kernel), out as a contiguous
+    row-major matrix."""
+    M, K = a_shape
+    K2, N = b_shape
+    if K != K2:
+        raise ValueError(f"inner dimensions differ: {tuple(a_shape)} @ {tuple(b_shape)}")
+    va = _view(a_shape, a_stride, a_ptr, True)
+    vb = _view(b_shape, b_stride, b_ptr, True)
+    vo = _view((M, N), out_stride, out_ptr, False)
+    copies = {"copy_a": va is None, "copy_b": vb is None, "copy_out": vo is None}
+    va = va or ("row", _pad4(K))
+    vb = vb or ("col", _pad4(K))
+    vo = vo or ("row", N)
+    a_kmajor, b_kmajor = va[0] == "row", vb[0] == "col"  # a(m, k) along k / b(k, n) along k
+    lay = {True: LAYOUT_K_MAJOR, False: LAYOUT_MN_MAJOR}
+    if vo[0] == "col":
+        args = {"M": M, "N": N, "K": K, "layout_a": lay[a_kmajor], "lda": va[1], "layout_b": lay[b_kmajor], "ldb": vb[1],
+                "ldc": vo[1], "swap": False}
+    else:
+        args = {"M": N, "N": M, "K": K, "layout_a": lay[b_kmajor], "lda": vb[1], "layout_b": lay[a_kmajor], "ldb": va[1],
+                "ldc": vo[1], "swap": True}
+    args.update(copies)
+    return args
+
+
 def _ptr(x) -> int:
     """Device/host address of a torch tensor, numpy array or raw int."""
     if isinstance(x, int):
@@ -255,6 +314,61 @@ class FtSgemm:
             opts: Opts | None = None) -> None:
         self._run_checked(lib().ftsgemm_run(self._h, kernel_id, M, N, K, _ptr(dA), _ptr(dB), _ptr(dC), alpha, beta,
                                             C.byref(opts) if opts is not None else None))
+
+    def run_ex(self, kernel_id: int, M: int, N: int, K: int, dA, layout_a: int, lda: int, dB, layout_b: int, ldb: int, dC,
+               ldc: int, alpha: float = 1.0, beta: float = 0.0, opts: Opts | None = None) -> None:
+        """C = alpha * A * B^T + beta * C with a layout (LAYOUT_MN_MAJOR / LAYOUT_K_MAJOR) and a leading dimension per
+        operand; C column-major with ldc >= M (include/ftsgemm.h: ftsgemm_run_ex)."""
+        self._run_checked(lib().ftsgemm_run_ex(self._h, kernel_id, M, N, K, _ptr(dA), layout_a, lda, _ptr(dB), layout_b, ldb,
+                                               _ptr(dC), ldc, alpha, beta, C.byref(opts) if opts is not None else None))
+
+    def matmul(self, a, b, out=None, *, kernel_id: int = ID_ABFT_AUTO, alpha: float = 1.0, beta: float = 0.0,
+               opts: Opts | None = None):
+        """out = alpha * (a @ b) + beta * out for 2-D float32 CUDA tensors a: (M, K), b: (K, N); returns out.
+
+        a, b and out may each be row-major or column-major (a .t() view is the other layout) with any leading stride that
+        keeps 16-byte rows; they are read and written in place -- x @ W.T (F.linear without bias) on row-major tensors
+        copies nothing.  An operand that cannot be read in place (no unit stride, a base address or, for a and b, a
+        leading stride that is not a multiple of 16 bytes) is copied once into an aligned buffer first; an out that cannot
+        be written in place is computed in a contiguous buffer and copied back.  With out=None a new row-major out is
+        returned and beta must be 0.  The mapping onto run_ex is matmul_plan: a row-major out is computed as
+        out^T = b^T a^T, so the kernel's (row, col) is out's (col, row) -- the coordinates of injected faults (opts) and
+        of stats() events are the kernel's, transposed against out in that case.  A kernel M or N (after the mapping)
+        that is not a multiple of 4 raises FtsgemmError(-2) for the tensor-core ids, as run does.  Runs on the current
+        torch stream unless opts.stream says otherwise.  No autograd."""
+        import torch
+        for name, t in (("a", a), ("b", b)):
+            if t.dim() != 2 or t.dtype != torch.float32 or not t.is_cuda:
+                raise TypeError(f"{name} must be a 2-D float32 CUDA tensor")
+        M, K = a.shape
+        N = b.shape[1]
+        if out is None:
+            if beta != 0.0:
+                raise ValueError("beta != 0 needs an out tensor")
+            out = torch.empty(M, N, device=a.device, dtype=torch.float32)
+        if out.shape != (M, N) or out.dtype != torch.float32 or out.device != a.device or b.device != a.device:
+            raise ValueError(f"out must be a float32 ({M}, {N}) tensor on {a.device}")
+        plan = matmul_plan(tuple(a.shape), a.stride(), tuple(b.shape), b.stride(), out.stride(), a.data_ptr(), b.data_ptr(),
+                           out.data_ptr())
+        if plan["copy_a"]:  # row-major, rows padded to 16 bytes: K-major for the kernel
+            a = torch.empty(M, _pad4(K), device=a.device, dtype=torch.float32)[:, :K].copy_(a)
+        if plan["copy_b"]:  # column-major, columns padded to 16 bytes: K-major for the kernel
+            b = torch.empty(N, _pad4(K), device=a.device, dtype=torch.float32)[:, :K].copy_(b.t()).t()
+        dst = out
+        if plan["copy_out"]:
+            dst = (out.clone(memory_format=torch.contiguous_format) if beta != 0.0
+                   else torch.empty(M, N, device=a.device, dtype=torch.float32))
+        if plan["copy_a"] or plan["copy_b"] or plan["copy_out"]:
+            plan = matmul_plan(tuple(a.shape), a.stride(), tuple(b.shape), b.stride(), dst.stride(), a.data_ptr(),
+                               b.data_ptr(), dst.data_ptr())
+        if opts is None:
+            opts = make_opts(stream=torch.cuda.current_stream(a.device).cuda_stream)
+        kA, kB = (b, a) if plan["swap"] else (a, b)
+        self.run_ex(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], kB, plan["layout_b"],
+                    plan["ldb"], dst, plan["ldc"], alpha, beta, opts)
+        if dst is not out:
+            out.copy_(dst)
+        return out
 
     def run_host(self, kernel_id: int, M: int, N: int, K: int, hA, hB, hC, alpha: float = 1.0, beta: float = 0.0,
                  opts: Opts | None = None) -> None:

@@ -115,8 +115,10 @@ struct ftsgemm_handle_s {
   size_t chk_bytes = 0;
   float *d_chk_out = nullptr;   // expected checksums M x (tiles_n*8), column-major, + slab flags behind it
   size_t chk_out_bytes = 0;
-  const float *chk_for_b = nullptr;  // B pointer / shape the panel was encoded from
+  const float *chk_for_b = nullptr;  // B pointer / shape / layout the panel was encoded from
   int chk_n = 0, chk_k = 0, chk_bn = 0;
+  bool chk_b_kmajor = false;
+  int chk_ldb = 0;
   // fused verdict exchange (ftsgemm_peer_*): this rank's mailbox (kMaxPeers slots), the peers' mailboxes mapped through
   // CUDA IPC, the exit counter of the publishing launches and their sequence number
   double *d_mailbox = nullptr;
@@ -127,7 +129,7 @@ struct ftsgemm_handle_s {
   unsigned int *d_exit_count = nullptr;
   int *d_front_done = nullptr;  // kernel front phase (operand transposes, encode): warps done, monotonic over launches
   int front_done_value = 0;
-  float *d_at = nullptr, *d_bt = nullptr;  // K-major copies of A and B
+  float *d_at = nullptr, *d_bt = nullptr;  // K-major copies of MN-major A and B (never allocated for a K-major operand)
   size_t at_bytes = 0, bt_bytes = 0;
   float *d_lo = nullptr;        // 3xTF32: A_lo | B_lo
   size_t lo_bytes = 0;
@@ -402,11 +404,20 @@ int ensure_buf(ftsgemm_handle_t h, float **buf, size_t *have, size_t bytes) {
   return FTSGEMM_OK;
 }
 
-int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const float *dA, const float *dB, float *dC,
+// One operand of ftsgemm_run_ex: MN-major (the reference's: element (r, k) at p[r + k*ld]) or K-major (p[k + r*ld]).
+struct Operand {
+  const float *p;
+  bool kmajor;
+  int ld;
+};
+
+int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC, int ldc,
            float alpha, float beta, const ftsgemm_opts &o, cudaStream_t stream) {
   const int BN = v.bn, CG = v.cg;
   const bool ft = v.info.fault_tolerant != 0;
+  const float *dA = A.p, *dB = B.p;
   if ((M % 4) || (N % 4)) return FTSGEMM_ERR_UNSUPPORTED;  // TMA global strides must be multiples of 16 bytes
+  if ((A.ld % 4) || (B.ld % 4)) return FTSGEMM_ERR_INVALID_ARG;  // (the same for the rows of an operand)
   // work-plan items carry k-block indices in 16 bits and tile indices in 31; the trace / wave tables are sized per unit
   if ((K + kBK - 1) / kBK > 65535) return FTSGEMM_ERR_UNSUPPORTED;
   if ((static_cast<long long>(M + kBM * CG - 1) / (kBM * CG)) * ((N + BN - 1) / BN) > (1ll << 28)) return FTSGEMM_ERR_UNSUPPORTED;
@@ -416,7 +427,7 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const floa
   KernelParams p;
   memset(&p, 0, sizeof(p));
   p.M = M; p.N = N; p.K = K;
-  p.C = dC; p.ldc = M;
+  p.C = dC; p.ldc = ldc;
   p.alpha = alpha; p.beta = beta;
   plan_tiles(M, N, BN, CG, ft, &p);
   p.tau_abs = o.tau_abs > 0 ? o.tau_abs : 1e-3f;
@@ -425,8 +436,10 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const floa
   p.recompute = o.no_recompute ? 0 : 1;
   p.A = dA;
   p.B = dB;
-  p.lda = M;
-  p.ldb = N;
+  p.lda = A.ld;
+  p.ldb = B.ld;
+  p.a_kmajor = A.kmajor ? 1 : 0;
+  p.b_kmajor = B.kmajor ? 1 : 0;
   p.inject_mode = ft ? o.inject_mode : 0;
   p.selftest_value = o.selftest_value;
   p.selftest_row = o.selftest_row & (kBM - 1);  // (>= 0: validated by load_opts)
@@ -448,21 +461,30 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const floa
     p.exit_count = h->d_exit_count;
   }
 
-  // K-major copies of A and B (written by the kernel's front phase), row stride ldk: TMA needs 16-byte row strides
+  // The tensor maps read K-major operands: a K-major operand in place, an MN-major one through its K-major copy (written by
+  // the kernel's front phase, row stride ldk: TMA needs 16-byte row strides).  The main loop is the same either way.
   CUtensorMap tmA, tmB, tmC;
   bool enc_front = false;
   int rc;
   p.ldk = (K + 3) / 4 * 4;
-  rc = ensure_buf(h, &h->d_at, &h->at_bytes, static_cast<size_t>(M) * p.ldk * sizeof(float));
-  if (rc) return rc;
-  rc = ensure_buf(h, &h->d_bt, &h->bt_bytes, static_cast<size_t>(N) * p.ldk * sizeof(float));
-  if (rc) return rc;
-  p.At = h->d_at;
-  p.Bt = h->d_bt;
-  rc = make_tmap_kmajor(h, &tmA, p.At, M, K, p.ldk, kBM);
+  if (A.kmajor) {
+    rc = make_tmap_kmajor(h, &tmA, dA, M, K, A.ld, kBM);
+  } else {
+    rc = ensure_buf(h, &h->d_at, &h->at_bytes, static_cast<size_t>(M) * p.ldk * sizeof(float));
+    if (rc) return rc;
+    p.At = h->d_at;
+    rc = make_tmap_kmajor(h, &tmA, p.At, M, K, p.ldk, kBM);
+  }
   if (rc) return rc;
   // CG = 2: each CTA of a unit loads BN/2 rows of the B tile and multicasts them to both
-  rc = make_tmap_kmajor(h, &tmB, p.Bt, N, K, p.ldk, BN / CG);
+  if (B.kmajor) {
+    rc = make_tmap_kmajor(h, &tmB, dB, N, K, B.ld, BN / CG);
+  } else {
+    rc = ensure_buf(h, &h->d_bt, &h->bt_bytes, static_cast<size_t>(N) * p.ldk * sizeof(float));
+    if (rc) return rc;
+    p.Bt = h->d_bt;
+    rc = make_tmap_kmajor(h, &tmB, p.Bt, N, K, p.ldk, BN / CG);
+  }
   if (rc) return rc;
   tmC = tmB;
   if (ft) {
@@ -489,7 +511,9 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const floa
     }
     p.chk_epoch = ++h->chk_epoch;
     p.dbg_flags = static_cast<int>(dbg("ft_dbg", 0)) & 1;
-    const bool reuse = o.reuse_b_checksums && h->chk_for_b == dB && h->chk_n == N && h->chk_k == K && h->chk_bn == BN;
+    // (the same pointer read in another layout or with another row stride is another B)
+    const bool reuse = o.reuse_b_checksums && h->chk_for_b == dB && h->chk_n == N && h->chk_k == K && h->chk_bn == BN &&
+                       h->chk_b_kmajor == B.kmajor && h->chk_ldb == B.ld;
     // Default: the encode is part of the FRONT PHASE of the GEMM kernel (KernelParams::enc_front) -- one launch per fused
     // GEMM, like the reference (sgemm.cu:191-192); only below ~8 MB of B the stand-alone pre-pass is used.
     const long long ef = dbg("enc_front", -2);
@@ -522,17 +546,18 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const floa
     ec.numAttrs = chain ? 1 : 0;                                                                                            \
     const float *eb = dB;                                                                                                   \
     float *eo = h->d_chk;                                                                                                   \
-    int en = N, ek = K, el = chk_ld, er = rounding, et = p.tiles_n;                                                         \
-    if (small_items) FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_b_kernel<bn, 4, false>, eb, en, ek, en, eo, el, er, et));    \
-    else if (stream_b) FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_b_kernel<bn, 8, true>, eb, en, ek, en, eo, el, er, et));   \
-    else FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_b_kernel<bn, 8, false>, eb, en, ek, en, eo, el, er, et));                \
+    int en = N, ek = K, eld = B.ld, el = chk_ld, er = rounding, et = p.tiles_n;                                             \
+    if (B.kmajor) FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_bk_kernel<bn>, eb, en, ek, eld, eo, el, er, et));               \
+    else if (small_items) FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_b_kernel<bn, 4, false>, eb, en, ek, eld, eo, el, er, et)); \
+    else if (stream_b) FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_b_kernel<bn, 8, true>, eb, en, ek, eld, eo, el, er, et));  \
+    else FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_b_kernel<bn, 8, false>, eb, en, ek, eld, eo, el, er, et));               \
   }
       FT_ENC(32) FT_ENC(64) FT_ENC(128) FT_ENC(256)
       ++h->launch_count;
 #undef FT_ENC
       FT_CUDA(h, cudaGetLastError());
     }
-    if (!reuse) { h->chk_for_b = dB; h->chk_n = N; h->chk_k = K; h->chk_bn = BN; }
+    if (!reuse) { h->chk_for_b = dB; h->chk_n = N; h->chk_k = K; h->chk_bn = BN; h->chk_b_kmajor = B.kmajor; h->chk_ldb = B.ld; }
     rc = make_tmap_kmajor(h, &tmC, h->d_chk, p.n_chk_cols, K, chk_ld, BN / CG);
     if (rc) return rc;
   }
@@ -696,13 +721,15 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const floa
   return lrc;
 }
 
-int run_cublas(ftsgemm_handle_t h, bool tf32, int M, int N, int K, const float *dA, const float *dB, float *dC,
+int run_cublas(ftsgemm_handle_t h, bool tf32, int M, int N, int K, const Operand &A, const Operand &B, float *dC, int ldc,
                float alpha, float beta, cudaStream_t stream) {
   FT_CUBLAS(h, cublasSetStream(h->cublas, stream));
   FT_CUBLAS(h, cublasSetPointerMode(h->cublas, CUBLAS_POINTER_MODE_HOST));
   FT_CUBLAS(h, cublasSetMathMode(h->cublas, tf32 ? CUBLAS_TF32_TENSOR_OP_MATH : CUBLAS_DEFAULT_MATH));
-  // NT on column-major buffers, as the reference's verification call (sgemm.cu:108)
-  FT_CUBLAS(h, cublasSgemm(h->cublas, CUBLAS_OP_N, CUBLAS_OP_T, M, N, K, &alpha, dA, M, dB, N, &beta, dC, M));
+  // C = A B^T on column-major buffers: the reference layout is NT, as the reference's verification call (sgemm.cu:108); a
+  // K-major A is an M x K matrix stored transposed (OP_T), a K-major B is the K x N matrix B^T itself (OP_N)
+  FT_CUBLAS(h, cublasSgemm(h->cublas, A.kmajor ? CUBLAS_OP_T : CUBLAS_OP_N, B.kmajor ? CUBLAS_OP_N : CUBLAS_OP_T, M, N, K, &alpha,
+                           A.p, A.ld, B.p, B.ld, &beta, dC, ldc));
   h->last_stream = stream;
   return FTSGEMM_OK;
 }
@@ -722,6 +749,16 @@ __global__ void split_lo_kernel(const float4 *__restrict__ x, float4 *__restrict
     r.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u);
     r.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
     lo[i] = r;
+  }
+}
+// the same for an operand with padded rows: `outer` rows of `inner` elements, row stride ldx in, ldlo out
+__global__ void split_lo_strided_kernel(const float *__restrict__ x, size_t ldx, float *__restrict__ lo, size_t ldlo, int inner,
+                                        size_t outer) {
+  const size_t n = outer * inner;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const size_t o = i / inner, r = i - o * inner;
+    const float v = __ldg(x + o * ldx + r);
+    lo[o * ldlo + r] = v - __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
   }
 }
 
@@ -968,10 +1005,21 @@ static int load_opts(const ftsgemm_opts *opts, ftsgemm_opts *o) {
 
 int ftsgemm_run(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, const float *dB, float *dC,
                 float alpha, float beta, const ftsgemm_opts *opts) {
+  return ftsgemm_run_ex(h, kernel_id, M, N, K, dA, FTSGEMM_LAYOUT_MN_MAJOR, M, dB, FTSGEMM_LAYOUT_MN_MAJOR, N, dC, M, alpha, beta,
+                        opts);
+}
+
+int ftsgemm_run_ex(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda, const float *dB,
+                   int layout_b, int ldb, float *dC, int ldc, float alpha, float beta, const ftsgemm_opts *opts) {
   if (!h) return FTSGEMM_ERR_NO_DEVICE;
   if (!dA || !dB || !dC || M <= 0 || N <= 0 || K <= 0) return FTSGEMM_ERR_INVALID_ARG;
   const Variant *v = find_variant(kernel_id);
   if (!v) return FTSGEMM_ERR_INVALID_ARG;
+  if ((layout_a != FTSGEMM_LAYOUT_MN_MAJOR && layout_a != FTSGEMM_LAYOUT_K_MAJOR) ||
+      (layout_b != FTSGEMM_LAYOUT_MN_MAJOR && layout_b != FTSGEMM_LAYOUT_K_MAJOR))
+    return FTSGEMM_ERR_INVALID_ARG;
+  const Operand A = {dA, layout_a == FTSGEMM_LAYOUT_K_MAJOR, lda}, B = {dB, layout_b == FTSGEMM_LAYOUT_K_MAJOR, ldb};
+  if (lda < (A.kmajor ? K : M) || ldb < (B.kmajor ? K : N) || ldc < M) return FTSGEMM_ERR_INVALID_ARG;
   ftsgemm_opts o;
   const int orc = load_opts(opts, &o);
   if (orc) return orc;
@@ -982,9 +1030,10 @@ int ftsgemm_run(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const fl
     if (!v) return FTSGEMM_ERR_UNSUPPORTED;
   }
   if (v->info.engine == 1 && o.check_segments > 1 && v->info.fault_tolerant) {
-    // Intra-K checking (ftsgemm_opts::check_segments): S consecutive K-segments, each a complete fault-tolerant GEMM.  A and
-    // B are column-major with k the slow index, so a segment is a pointer offset; segment boundaries are multiples of the
-    // stage depth (32 k-rows).  Injected faults (tests) go to the first segment only.
+    // Intra-K checking (ftsgemm_opts::check_segments): S consecutive K-segments, each a complete fault-tolerant GEMM.  A
+    // segment of an operand is a pointer offset: k0 * ld for an MN-major operand (k is the slow index), k0 for a K-major one;
+    // segment boundaries are multiples of the stage depth (32 k-rows), so the offsets keep 16-byte alignment.  Injected
+    // faults (tests) go to the first segment only.
     int S = o.check_segments;
     const int num_kb = (K + kBK - 1) / kBK;
     if (S > num_kb) S = num_kb;
@@ -997,8 +1046,10 @@ int ftsgemm_run(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const fl
       int k1 = static_cast<int>(static_cast<long long>(num_kb) * (sg + 1) / S) * kBK;
       if (k1 > K) k1 = K;
       if (sg > 0) os.inject_mode = 0;
-      rc = ftsgemm_run(h, v->info.id, M, N, k1 - k0, dA + static_cast<size_t>(k0) * M, dB + static_cast<size_t>(k0) * N, dC, alpha,
-                       sg == 0 ? beta : 1.0f, &os);
+      const size_t oa = A.kmajor ? static_cast<size_t>(k0) : static_cast<size_t>(k0) * lda;
+      const size_t ob = B.kmajor ? static_cast<size_t>(k0) : static_cast<size_t>(k0) * ldb;
+      rc = ftsgemm_run_ex(h, v->info.id, M, N, k1 - k0, dA + oa, layout_a, lda, dB + ob, layout_b, ldb, dC, ldc, alpha,
+                          sg == 0 ? beta : 1.0f, &os);
     }
     return rc;
   }
@@ -1009,14 +1060,33 @@ int ftsgemm_run(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const fl
     // as three launches of the same kernel, smallest terms first, each accumulating into C -- every one of them a
     // complete fault-tolerant GEMM with its own checksum vectors, so ABFT covers the whole 3-pass product.
     if ((static_cast<size_t>(M) * K) % 4 || (static_cast<size_t>(N) * K) % 4) return FTSGEMM_ERR_UNSUPPORTED;
-    const size_t need = (static_cast<size_t>(M) + N) * K * sizeof(float);
-    int rc = ensure_buf(h, &h->d_lo, &h->lo_bytes, need);
+    // (run_tc's argument checks, before the split kernels read the operands with 16-byte loads)
+    if ((M % 4) || (N % 4)) return FTSGEMM_ERR_UNSUPPORTED;
+    if ((lda % 4) || (ldb % 4) || ((reinterpret_cast<uintptr_t>(dA) | reinterpret_cast<uintptr_t>(dB)) & 15))
+      return FTSGEMM_ERR_INVALID_ARG;
+    // The lo parts are written dense in the operand's own layout: ld = rows (MN-major) or K rounded up to 4 (K-major).
+    auto lo_of = [K](const Operand &x, int rows) {
+      return Operand{nullptr, x.kmajor, x.kmajor ? (K + 3) / 4 * 4 : rows};
+    };
+    Operand Alo = lo_of(A, M), Blo = lo_of(B, N);
+    const size_t a_floats = static_cast<size_t>(Alo.ld) * (Alo.kmajor ? M : K);
+    const size_t b_floats = static_cast<size_t>(Blo.ld) * (Blo.kmajor ? N : K);
+    int rc = ensure_buf(h, &h->d_lo, &h->lo_bytes, (a_floats + b_floats) * sizeof(float));
     if (rc) return rc;
-    float *dAlo = h->d_lo, *dBlo = h->d_lo + static_cast<size_t>(M) * K;
-    split_lo_kernel<<<h->num_sms * 8, 256, 0, stream>>>(reinterpret_cast<const float4 *>(dA), reinterpret_cast<float4 *>(dAlo),
-                                                        static_cast<size_t>(M) * K / 4);
-    split_lo_kernel<<<h->num_sms * 8, 256, 0, stream>>>(reinterpret_cast<const float4 *>(dB), reinterpret_cast<float4 *>(dBlo),
-                                                        static_cast<size_t>(N) * K / 4);
+    float *dAlo = h->d_lo, *dBlo = h->d_lo + a_floats;
+    Alo.p = dAlo;
+    Blo.p = dBlo;
+    auto split = [&](const Operand &x, const Operand &lo, int rows, float *dst) {
+      const int inner = x.kmajor ? K : rows;  // elements per stored row of the operand
+      const size_t outer = x.kmajor ? rows : K;
+      if (x.ld == inner && lo.ld == inner)  // dense: one flat array (x % 4 == 0 elements, see above)
+        split_lo_kernel<<<h->num_sms * 8, 256, 0, stream>>>(reinterpret_cast<const float4 *>(x.p), reinterpret_cast<float4 *>(dst),
+                                                            outer * inner / 4);
+      else  // padded rows: nothing outside the operand's rows is read
+        split_lo_strided_kernel<<<h->num_sms * 8, 256, 0, stream>>>(x.p, x.ld, dst, lo.ld, inner, outer);
+    };
+    split(A, Alo, M, dAlo);
+    split(B, Blo, N, dBlo);
     FT_CUDA(h, cudaGetLastError());
     h->launch_count += 2;
     ftsgemm_opts o3 = o;
@@ -1024,15 +1094,18 @@ int ftsgemm_run(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const fl
     o3.precision = 0;
     ftsgemm_opts o_quiet = o3;  // injected faults belong to the main product only
     o_quiet.inject_mode = 0;
-    rc = run_tc(h, *v, M, N, K, dAlo, dB, dC, alpha, beta, o_quiet, stream);
-    if (!rc) rc = run_tc(h, *v, M, N, K, dA, dBlo, dC, alpha, 1.0f, o_quiet, stream);
-    if (!rc) rc = run_tc(h, *v, M, N, K, dA, dB, dC, alpha, 1.0f, o3, stream);
+    rc = run_tc(h, *v, M, N, K, Alo, B, dC, ldc, alpha, beta, o_quiet, stream);
+    if (!rc) rc = run_tc(h, *v, M, N, K, A, Blo, dC, ldc, alpha, 1.0f, o_quiet, stream);
+    if (!rc) rc = run_tc(h, *v, M, N, K, A, B, dC, ldc, alpha, 1.0f, o3, stream);
     return rc;
   }
   switch (v->info.engine) {
-    case 0: return run_cublas(h, v->info.id == 7, M, N, K, dA, dB, dC, alpha, beta, stream);
-    case 1: return run_tc(h, *v, M, N, K, dA, dB, dC, alpha, beta, o, stream);
-    case 2: return ftsgemm_baseline(h, M, N, K, dA, dB, dC, alpha, beta, v->info.id == 30 ? 1 : 0, &o, nullptr);
+    case 0: return run_cublas(h, v->info.id == 7, M, N, K, A, B, dC, ldc, alpha, beta, stream);
+    case 1: return run_tc(h, *v, M, N, K, A, B, dC, ldc, alpha, beta, o, stream);
+    case 2:
+      // the non-fused baseline keeps the reference's call sequence, on the reference layout only
+      if (A.kmajor || B.kmajor || lda != M || ldb != N || ldc != M) return FTSGEMM_ERR_UNSUPPORTED;
+      return ftsgemm_baseline(h, M, N, K, dA, dB, dC, alpha, beta, v->info.id == 30 ? 1 : 0, &o, nullptr);
   }
   return FTSGEMM_ERR_UNSUPPORTED;
 }

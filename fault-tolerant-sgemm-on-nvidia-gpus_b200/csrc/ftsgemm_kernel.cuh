@@ -6,8 +6,8 @@
 // with ONE warp-specialised, persistent wgmma kernel template <BN, FT, CG>; a CTA computes 128 x BN of C, and a work
 // unit is CG CTAs that together cover a 128*CG x BN tile.
 //
-//   front phase   : every warp of the grid transposes its share of A and B into K-major copies (wgmma takes TF32
-//                   operands K-major only; the caller's operands are MN-major) and, for large B, encodes B (below)
+//   front phase   : every warp of the grid transposes its share of the MN-major operands into K-major copies (wgmma
+//                   takes TF32 operands K-major only; a K-major operand is read in place) and, for large B, encodes B
 //   warp 0        : TMA producer: cp.async.bulk.tensor 32(K) x 128(M) and 32(K) x BN(N) fp32 boxes, 128B swizzle, into a
 //                   STAGES-deep shared-memory ring (full/empty mbarriers); CG = 2: a unit is a cluster, each CTA loads
 //                   BN/2 rows of B and multicasts them into the ring of both CTAs
@@ -76,8 +76,8 @@ struct KernelParams {
   float alpha, beta;
   // tile schedule (tiles_m counts CG*128-row blocks)
   int tiles_m, tiles_n, group_n;
-  // K-major copies of the operands written by the front phase (row stride ldk floats, ldk % 4 == 0); the tensor maps
-  // point at them
+  // K-major copies of the MN-major operands written by the front phase (row stride ldk floats, ldk % 4 == 0); the tensor
+  // maps point at them, or straight at the caller's buffer of a K-major operand (a_kmajor / b_kmajor: no copy)
   float *At, *Bt;
   int ldk;
   int dbg_flags;        // experiments only: bit 0 = skip the epilogue ABFT check of data tiles (timing breakdowns)
@@ -130,8 +130,11 @@ struct KernelParams {
   // (TF32-truncated operands, FP32 accumulate) and written straight to C; the store pass skips it.  Nothing that was
   // detected is stored as computed.  (The reference only ever adds the residual, ft_sgemm_huge.cuh:422-485.)
   int recompute;
-  const float *A, *B;   // the operands in global memory (lda = M, ldb = N)
+  // the operands in global memory: MN-major A(m, k) at A[m + k*lda], B(n, k) at B[n + k*ldb]; K-major (a_kmajor /
+  // b_kmajor) A(m, k) at A[k + m*lda], B(n, k) at B[k + n*ldb]
+  const float *A, *B;
   int lda, ldb;
+  int a_kmajor, b_kmajor;
   int inject_mode;
   float selftest_value;
   int selftest_row, selftest_col;
@@ -649,25 +652,29 @@ __device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, flo
 // ------------------------------------------------------------------------------------------------------------
 // Recompute fallback (rare): one warp recomputes row m of the tile's BN columns from global memory -- the values the
 // tensor core would have produced up to FP32 accumulation order (TF32-truncated operands: every product is exact in
-// FP32) -- and writes C = alpha * acc + beta * C directly.  K iterations of 1 broadcast + BN/32 coalesced loads.
+// FP32) -- and writes C = alpha * acc + beta * C directly.  K iterations of 1 broadcast + BN/32 loads (coalesced for an
+// MN-major B, one stride-ldb load per lane for a K-major one).  kmajor: bit 0 = A is K-major, bit 1 = B is K-major.
 // ------------------------------------------------------------------------------------------------------------
 // (scalars by value: a reference to the __grid_constant__ parameter block would force a local copy of all of it)
 template <int BN>
-__device__ __noinline__ void recompute_row(const float *A, const float *B, float *C, int lda, int ldb, int ldc, int N, int K,
-                                           float alpha, float beta, int m, int n0, int lane) {
+__device__ __noinline__ void recompute_row(const float *A, const float *B, float *C, int lda, int ldb, int kmajor, int ldc, int N,
+                                           int K, float alpha, float beta, int m, int n0, int lane) {
   constexpr int J = BN / 32;
   float acc[J];
 #pragma unroll
   for (int j = 0; j < J; ++j) acc[j] = 0.0f;
-  const float *a = A + m;
-  const float *b = B + n0 + lane;
+  // element (r, k) of an operand at base + r * rs + k * ks
+  const size_t a_ks = (kmajor & 1) ? 1 : static_cast<size_t>(lda);
+  const size_t b_ns = (kmajor & 2) ? static_cast<size_t>(ldb) : 1, b_ks = (kmajor & 2) ? 1 : static_cast<size_t>(ldb);
+  const float *a = A + static_cast<size_t>(m) * ((kmajor & 1) ? static_cast<size_t>(lda) : 1);
+  const float *b = B + static_cast<size_t>(n0 + lane) * b_ns;
 #pragma unroll 2
   for (int k = 0; k < K; ++k) {
-    const float av = u2f(f2u(__ldg(a + static_cast<size_t>(k) * lda)) & 0xFFFFE000u);
-    const float *bk = b + static_cast<size_t>(k) * ldb;
+    const float av = u2f(f2u(__ldg(a + static_cast<size_t>(k) * a_ks)) & 0xFFFFE000u);
+    const float *bk = b + static_cast<size_t>(k) * b_ks;
 #pragma unroll
     for (int j = 0; j < J; ++j) {
-      const float bv = (n0 + lane + 32 * j < N) ? u2f(f2u(__ldg(bk + 32 * j)) & 0xFFFFE000u) : 0.0f;
+      const float bv = (n0 + lane + 32 * j < N) ? u2f(f2u(__ldg(bk + 32 * j * b_ns)) & 0xFFFFE000u) : 0.0f;
       acc[j] = fmaf(av, bv, acc[j]);
     }
   }
@@ -687,8 +694,8 @@ __device__ __noinline__ void recompute_row(const float *A, const float *B, float
 // block would force a local copy of all of it.  Row segments that fail are counted and, with beta == 0, recomputed from A
 // and B (with beta != 0 the old values of C are already overwritten: reported as uncorrectable).
 template <int BN>
-__device__ __noinline__ void protected_store_pass(uint32_t taddr, const float *A, const float *B, float *C, int lda, int ldb, int ldc,
-                                                  int N, int K, float alpha, float beta, DeviceStats *stats, bool can_recompute,
+__device__ __noinline__ void protected_store_pass(uint32_t taddr, const float *A, const float *B, float *C, int lda, int ldb,
+                                                  int kmajor, int ldc, int N, int K, float alpha, float beta, DeviceStats *stats, bool can_recompute,
                                                   int m, int row0, bool row_ok, int n0, int c_begin, int c_end, float chk_s1,
                                                   bool chk_s1_valid, int bad_col, uint32_t bad_mask, int lane) {
   const StoreVerdict sv = store_tile_protected<BN>(taddr, C + m, row_ok, n0, ldc, alpha, beta, c_begin, c_end, chk_s1, chk_s1_valid,
@@ -715,9 +722,10 @@ __device__ __noinline__ void protected_store_pass(uint32_t taddr, const float *A
     const int r = __ffs(mask) - 1;
     mask &= mask - 1u;
     if (c_end - c_begin == BN / 32) {
-      recompute_row<BN>(A, B, C, lda, ldb, ldc, N, K, alpha, beta, row0 + r, n0, lane);
+      recompute_row<BN>(A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r, n0, lane);
     } else {
-      if constexpr (BN >= 64) recompute_row<BN / 2>(A, B, C, lda, ldb, ldc, N, K, alpha, beta, row0 + r, n0 + c_begin * 32, lane);
+      if constexpr (BN >= 64)
+        recompute_row<BN / 2>(A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r, n0 + c_begin * 32, lane);
     }
   }
 }
@@ -942,6 +950,82 @@ __device__ __forceinline__ void encode_b_warp(const float *__restrict__ B, int N
   }
 }
 
+// The same checksum operand from a K-major B (element (n, k) at B[k + n*ldb], ldb % 4 == 0), with the same accuracy
+// contract: TF32-truncated inputs, FP32 partial sums over groups of 8 rows, FP64 totals, 2-way TF32 split.  A warp item is
+// (column block t, 32 consecutive k): lane = (row group rg = lane / 8, k quad kq = lane % 8); every load instruction reads
+// 128 contiguous bytes of four rows (float4 along k), a lane walks the 8-row groups rg, rg + 4, ... of the block, and the
+// four row groups are added in FP64 with two butterfly steps.  Lane group rg then stores checksum row rg (e hi, e lo, w hi,
+// w lo) of the item's 32 k as one coalesced 128-byte row.  (An item of 128 k per warp, with no cross-lane sum, leaves too few
+// items for the pre-pass shapes: 4 column blocks x 8 k-items at N = K = 1024.)
+template <int BN>
+__device__ __forceinline__ void encode_bk_warp(const float *__restrict__ B, int N, int K, int ldb, float *__restrict__ chk,
+                                               int chk_ld, int rounding, int tiles_n, int gw, int nw, int lane) {
+  const int kq = lane & 7, rg = lane >> 3;
+  const int k_items = (K + 31) / 32;
+  const long long total = static_cast<long long>(tiles_n) * k_items;
+  for (long long item = gw; item < total; item += nw) {
+    const int t = static_cast<int>(item / k_items);  // k fastest: warps side by side read neighbouring 128-byte segments
+    const int k = static_cast<int>(item - static_cast<long long>(t) * k_items) * 32 + 4 * kq;
+    const int n0 = t * BN;
+    const int rows = min(BN, N - n0);
+    const float *src = B + static_cast<size_t>(n0) * ldb + k;
+    double e[4] = {0.0, 0.0, 0.0, 0.0}, w[4] = {0.0, 0.0, 0.0, 0.0};
+#pragma unroll 1
+    for (int g = 8 * rg; g < rows; g += 32) {
+      float4 x[8];
+#pragma unroll
+      for (int r = 0; r < 8; ++r) {
+        x[r] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (g + r < rows) {
+          const float *pr = src + static_cast<size_t>(g + r) * ldb;
+          if (k + 4 <= K) {
+            x[r] = __ldg(reinterpret_cast<const float4 *>(pr));
+          } else if (k < K) {  // K tail: no read past the row's last element
+            x[r].x = __ldg(pr);
+            if (k + 1 < K) x[r].y = __ldg(pr + 1);
+            if (k + 2 < K) x[r].z = __ldg(pr + 2);
+          }
+        }
+      }
+      float pe[4] = {0.0f, 0.0f, 0.0f, 0.0f}, pw[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+#pragma unroll
+      for (int r = 0; r < 8; ++r) {
+        const float wr = static_cast<float>(g + r + 1);  // (n - n0 + 1) * b is exact in FP32
+        const float b[4] = {tf32_bits(x[r].x, rounding), tf32_bits(x[r].y, rounding), tf32_bits(x[r].z, rounding),
+                            tf32_bits(x[r].w, rounding)};
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          pe[c] += b[c];
+          pw[c] = fmaf(b[c], wr, pw[c]);
+        }
+      }
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        e[c] += static_cast<double>(pe[c]);
+        w[c] += static_cast<double>(pw[c]);
+      }
+    }
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+#pragma unroll
+      for (int o = 8; o < 32; o <<= 1) {
+        e[c] += __shfl_xor_sync(0xffffffffu, e[c], o);
+        w[c] += __shfl_xor_sync(0xffffffffu, w[c], o);
+      }
+    }
+    if (k < K) {  // (k + 3 may reach past K: still inside the row stride chk_ld, and the zero-filled values are not read)
+      float o[4];
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        float h, l;
+        split2_tf32(rg < 2 ? e[c] : w[c], h, l);
+        o[c] = (rg & 1) ? l : h;
+      }
+      *reinterpret_cast<float4 *>(chk + static_cast<size_t>(t * kChkPerTile + rg) * chk_ld + k) = make_float4(o[0], o[1], o[2], o[3]);
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------------------
 // Front phase: one warp transposes 32 x 32 blocks of a column-major rows x K operand (element (r, k) at src[r + k*ld])
 // into the K-major copy dst[r * ldk + k], through a 32 x 33 shared-memory tile (conflict-free both ways); blocks
@@ -965,6 +1049,21 @@ __device__ __forceinline__ void transpose_warp(const float *__restrict__ src, in
     for (int i = 0; i < 32; ++i)
       if (r0 + i < rows && k < K) dst[static_cast<size_t>(r0 + i) * ldk + k] = tile[lane * 33 + i];
     __syncwarp();
+  }
+}
+
+// The front phase when at least one operand is K-major: transpose only the MN-major one, encode B in its own layout.  Out of
+// line, so that the GEMM kernel's register allocation sees the reference layout's front phase only (inlined, this branch
+// raised the spills of the 256-wide fault-tolerant instantiations; out of line, the plain instantiations stopped spilling).
+template <int BN, bool FT>
+__device__ __noinline__ void front_phase_kmajor(const float *A, const float *B, int M, int N, int K, int lda, int ldb,
+                                                int a_kmajor, int b_kmajor, float *At, float *Bt, int ldk, int enc_front,
+                                                float *enc_out, int enc_ld, int tiles_n, int gw, int nw, int lane, float *tile) {
+  if (!a_kmajor) transpose_warp(A, M, K, lda, At, ldk, gw, nw, lane, tile);
+  if (!b_kmajor) transpose_warp(B, N, K, ldb, Bt, ldk, gw, nw, lane, tile);
+  if (FT && enc_front) {
+    if (b_kmajor) encode_bk_warp<BN>(B, N, K, ldb, enc_out, enc_ld, 0, tiles_n, gw, nw, lane);
+    else encode_b_warp<BN, 8>(B, N, K, ldb, enc_out, enc_ld, 0, tiles_n, gw, nw, lane);
   }
 }
 
@@ -1033,12 +1132,17 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (p.pdl_wait) ptx::pdl_wait();  // everything before this line touched no global memory
 
   {
-    // front phase: operand transposes (+ the encode of B); the ring is free scratch until the producer starts
+    // front phase: transposes of the MN-major operands (+ the encode of B); the ring is free scratch until the producer starts
     const int gw = static_cast<int>(blockIdx.x) * (kThreads / 32) + warp, nw = static_cast<int>(gridDim.x) * (kThreads / 32);
     float *tile = smem_f + warp * 32 * 33;
-    transpose_warp(p.A, p.M, p.K, p.lda, p.At, p.ldk, gw, nw, lane, tile);
-    transpose_warp(p.B, p.N, p.K, p.ldb, p.Bt, p.ldk, gw, nw, lane, tile);
-    if (FT && p.enc_front) encode_b_warp<BN, 8>(p.B, p.N, p.K, p.ldb, p.enc_out, p.enc_ld, 0, p.tiles_n, gw, nw, lane);
+    if ((p.a_kmajor | p.b_kmajor) == 0) {  // the reference layout
+      transpose_warp(p.A, p.M, p.K, p.lda, p.At, p.ldk, gw, nw, lane, tile);
+      transpose_warp(p.B, p.N, p.K, p.ldb, p.Bt, p.ldk, gw, nw, lane, tile);
+      if (FT && p.enc_front) encode_b_warp<BN, 8>(p.B, p.N, p.K, p.ldb, p.enc_out, p.enc_ld, 0, p.tiles_n, gw, nw, lane);
+    } else {
+      front_phase_kmajor<BN, FT>(p.A, p.B, p.M, p.N, p.K, p.lda, p.ldb, p.a_kmajor, p.b_kmajor, p.At, p.Bt, p.ldk, p.enc_front,
+                                 p.enc_out, p.enc_ld, p.tiles_n, gw, nw, lane, tile);
+    }
     ptx::fence_proxy_async();  // this warp's shared-memory scratch accesses before the TMA writes into the ring
     __syncwarp();              // the warp's stores are ordered before lane 0's release (cumulativity)
     if (lane == 0) {
@@ -1234,8 +1338,8 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N) {
             uint32_t bad_bits = 0u;
             const int bad_col = stored_value_fault<BN>(p, q, lane, m0_cta, n0, kMid, BN / 32, bad_bits);
-            protected_store_pass<BN>(taddr, p.A, p.B, p.C, p.lda, p.ldb, p.ldc, p.N, p.K, p.alpha, p.beta, p.stats,
-                                     p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32, m < p.M && !skip, n0, kMid, BN / 32, s1,
+            protected_store_pass<BN>(taddr, p.A, p.B, p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K, p.alpha,
+                                     p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32, m < p.M && !skip, n0, kMid, BN / 32, s1,
                                      stale == 0u, bad_col, bad_bits, lane);
           } else {
             store_tile<BN>(taddr, p.C + m, m < p.M && !skip, n0, p.N, p.ldc, p.alpha, p.beta, kMid, BN / 32);
@@ -1295,8 +1399,8 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N) {
           uint32_t bad_bits = 0u;
           const int bad_col = stored_value_fault<BN>(p, q, lane, m0_cta, n0, 0, c_mid, bad_bits);
-          protected_store_pass<BN>(taddr, p.A, p.B, p.C, p.lda, p.ldb, p.ldc, p.N, p.K, p.alpha, p.beta, p.stats,
-                                   p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32, m < p.M && !redo, n0, 0, c_mid, own_s1,
+          protected_store_pass<BN>(taddr, p.A, p.B, p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K, p.alpha,
+                                   p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32, m < p.M && !redo, n0, 0, c_mid, own_s1,
                                    ((stale_mask >> lane) & 1u) == 0u, bad_col, bad_bits, lane);
         } else {
           store_tile<BN>(taddr, p.C + m, m < p.M && !redo, n0, p.N, p.ldc, p.alpha, p.beta, 0, c_mid);
@@ -1306,7 +1410,8 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           while (rm != 0u) {
             const int r = __ffs(rm) - 1;
             rm &= rm - 1u;
-            recompute_row<BN>(p.A, p.B, p.C, p.lda, p.ldb, p.ldc, p.N, p.K, p.alpha, p.beta, m0_cta + q * 32 + r, n0, lane);
+            recompute_row<BN>(p.A, p.B, p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K, p.alpha, p.beta,
+                              m0_cta + q * 32 + r, n0, lane);
           }
         }
         if (assist_on) ptx::named_bar_sync(4 + q, 64);  // both halves are out of the accumulator
@@ -1369,6 +1474,17 @@ encode_b_kernel(const float *__restrict__ B, int N, int K, int ldb, float *__res
   ptx::pdl_launch_dependents();  // the GEMM kernel may start its prologue on SMs as they drain (then waits for this grid)
   encode_b_warp<BN, KRQ, STREAM>(B, N, K, ldb, chk, chk_ld, rounding, tiles_n, blockIdx.x * kEncWarps + (threadIdx.x >> 5),
                     gridDim.x * kEncWarps, threadIdx.x & 31);
+}
+
+// The pre-pass for a K-major B.
+template <int BN>
+__global__ void __launch_bounds__(kEncWarps * 32, 2)
+encode_bk_kernel(const float *__restrict__ B, int N, int K, int ldb, float *__restrict__ chk, int chk_ld, int rounding,
+                 int tiles_n) {
+  ptx::pdl_wait();
+  ptx::pdl_launch_dependents();
+  encode_bk_warp<BN>(B, N, K, ldb, chk, chk_ld, rounding, tiles_n, blockIdx.x * kEncWarps + (threadIdx.x >> 5),
+                     gridDim.x * kEncWarps, threadIdx.x & 31);
 }
 
 }  // namespace ftsgemm

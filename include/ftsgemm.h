@@ -13,8 +13,9 @@
  * Every entry point below names the reference interface it replaces.  Plain C types only: device/host
  * pointers, ints, floats; no torch / C++ types.
  *
- * Data layout (identical to the reference kernels): A is M x K column-major (ld = M), B is N x K
- * column-major (ld = N), C is M x N column-major (ld = M);  C = alpha * A * B^T + beta * C  in place.
+ * Data layout of ftsgemm_run (identical to the reference kernels): A is M x K column-major (ld = M), B is N x K
+ * column-major (ld = N), C is M x N column-major (ld = M);  C = alpha * A * B^T + beta * C  in place.  ftsgemm_run_ex takes
+ * leading dimensions and a K-major layout per operand as well.
  * All functions return FTSGEMM_OK (0) or a negative FTSGEMM_ERR_* code; nothing calls exit().
  */
 #ifndef FTSGEMM_H_
@@ -193,6 +194,27 @@ int ftsgemm_select_kernel(int M, int N, int K, int fault_tolerant);
  * M/N/K need not be multiples of the tile (TMA zero-fills the ragged edge).  K >= 1. */
 int ftsgemm_run(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, const float *dB,
                 float *dC, float alpha, float beta, const ftsgemm_opts *opts);
+
+/* ---- operand layouts and leading dimensions  (new work: the reference's kernels take no ld and no transpose flag; their
+ *      layout is implicit in the indexing, ft_sgemm_huge.cuh:11,37-41: A column-major M x K, B column-major N x K) -----------
+ * The same product C = alpha * A * B^T + beta * C (C column-major, ldc >= M) with each operand in either layout:
+ *   FTSGEMM_LAYOUT_MN_MAJOR  A(m,k) at A[m + k*lda] (lda >= M); B(n,k) at B[n + k*ldb] (ldb >= N) -- the reference's
+ *   FTSGEMM_LAYOUT_K_MAJOR   A(m,k) at A[k + m*lda] (lda >= K); B(n,k) at B[k + n*ldb] (ldb >= K)
+ * ftsgemm_run(...) is ftsgemm_run_ex(..., MN_MAJOR, M, ..., MN_MAJOR, N, ..., M, ...).  A row-major torch tensor x (M x K) is a
+ * K-major A with lda = x.stride(0); F.linear's weight W (N x K, row-major) is a K-major B with ldb = W.stride(0).
+ * The tensor cores read TF32 operands K-major only: a K-major operand is read in place, an MN-major one is first transposed
+ * into a workspace copy by the kernel's front phase.  Results do not depend on the layouts (bit-identical C).
+ * Engines: the wgmma ids take every layout (preconditions of ftsgemm_run, plus lda % 4 == 0 and ldb % 4 == 0 -- 16-byte
+ * rows -- else FTSGEMM_ERR_INVALID_ARG); cuBLAS ids 0 / 7 map onto cublasSgemm (A: MN-major OP_N, K-major OP_T; B: MN-major
+ * OP_T, K-major OP_N); the baseline ids 10 / 30 take only the reference layout with lda = M, ldb = N, ldc = M, else
+ * FTSGEMM_ERR_UNSUPPORTED.  A layout other than 0 / 1 or an ld below its row length: FTSGEMM_ERR_INVALID_ARG. */
+enum {
+  FTSGEMM_LAYOUT_MN_MAJOR = 0,
+  FTSGEMM_LAYOUT_K_MAJOR = 1
+};
+int ftsgemm_run_ex(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
+                   const float *dB, int layout_b, int ldb, float *dC, int ldc, float alpha, float beta,
+                   const ftsgemm_opts *opts);
 
 /* Counters of all FT launches since the previous call (synchronises the handle's last stream, then resets). */
 int ftsgemm_get_stats(ftsgemm_handle_t h, ftsgemm_stats *out);
