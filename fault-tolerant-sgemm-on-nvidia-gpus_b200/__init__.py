@@ -34,6 +34,9 @@ ABFT_IDS = {"small": 11, "medium": 12, "large": 13, "tall": 14, "wide": 15, "hug
 # K-major A(m,k) at A[k + m*lda], B(n,k) at B[k + n*ldb]
 LAYOUT_MN_MAJOR, LAYOUT_K_MAJOR = 0, 1
 
+# bias of run_bias (include/ftsgemm.h): ROW adds bias[m] to row m of C (length M), COL adds bias[n] to column n (length N)
+BIAS_NONE, BIAS_ROW, BIAS_COL = 0, 1, 2
+
 
 class FtsgemmError(RuntimeError):
     def __init__(self, code: int, msg: str):
@@ -86,7 +89,7 @@ class Stats(C.Structure):
 # every symbol include/ftsgemm.h declares (checked by tests/test_abi.py without a GPU)
 EXPORTED_SYMBOLS = [
     "ftsgemm_create", "ftsgemm_destroy", "ftsgemm_abi_version", "ftsgemm_error_string", "ftsgemm_last_cuda_error",
-    "ftsgemm_default_opts", "ftsgemm_kernel_table", "ftsgemm_kernel_lookup", "ftsgemm_run", "ftsgemm_run_ex", "ftsgemm_get_stats",
+    "ftsgemm_default_opts", "ftsgemm_kernel_table", "ftsgemm_kernel_lookup", "ftsgemm_run", "ftsgemm_run_ex", "ftsgemm_run_bias", "ftsgemm_get_stats",
     "ftsgemm_run_host", "ftsgemm_baseline", "ftsgemm_verify", "ftsgemm_debug_set", "ftsgemm_debug_schedule",
     "ftsgemm_verify_bad_count", "ftsgemm_debug_trace", "ftsgemm_stats_device", "ftsgemm_select_kernel", "ftsgemm_launch_count", "ftsgemm_peer_export", "ftsgemm_peer_connect",
     "ftsgemm_peer_verdict",
@@ -123,6 +126,7 @@ def lib():
         L.ftsgemm_kernel_lookup.argtypes = [ip, C.POINTER(KernelInfo)]
         L.ftsgemm_run.argtypes = [vp, ip, ip, ip, ip, vp, vp, vp, fp, fp, C.POINTER(Opts)]
         L.ftsgemm_run_ex.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, vp, ip, ip, vp, ip, fp, fp, C.POINTER(Opts)]
+        L.ftsgemm_run_bias.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, vp, ip, ip, vp, ip, fp, fp, vp, ip, C.POINTER(Opts)]
         L.ftsgemm_get_stats.argtypes = [vp, C.POINTER(Stats)]
         L.ftsgemm_run_host.argtypes = [vp, ip, ip, ip, ip, vp, vp, vp, fp, fp, C.POINTER(Opts)]
         L.ftsgemm_stats_device.argtypes = [vp, vp, vp]
@@ -243,7 +247,8 @@ def _view(shape, stride, ptr: int, ld4: bool):
     return None
 
 
-def matmul_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0, b_ptr: int = 0, out_ptr: int = 0) -> dict:
+def matmul_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0, b_ptr: int = 0, out_ptr: int = 0,
+                bias_stride=None, bias_ptr: int = 0) -> dict:
     """run_ex arguments for out = a @ b with a: (M, K), b: (K, N), out: (M, N), from shapes, element strides and addresses.
 
     Column-major out: C = out, kernel A = a, kernel B = b^T.  Row-major out: C = out^T = b^T a^T (swap = True), so the
@@ -251,7 +256,9 @@ def matmul_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0
     operands are then K-major and no transpose runs.  copy_a / copy_b / copy_out mark matrices that cannot be read in
     place (see _view); the arguments returned describe the copies matmul makes of them: a as row-major and b as
     column-major with the row length padded to a multiple of 4 (both K-major for the kernel), out as a contiguous
-    row-major matrix."""
+    row-major matrix.  bias_stride (the element stride of a length-N bias, None without a bias) gives bias_mode: a bias
+    over out's columns is one per kernel column (BIAS_COL), or per kernel row (BIAS_ROW) when swapped; copy_bias marks a
+    bias without unit stride or with a base that is not 4-byte aligned."""
     M, K = a_shape
     K2, N = b_shape
     if K != K2:
@@ -272,7 +279,28 @@ def matmul_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0
         args = {"M": N, "N": M, "K": K, "layout_a": lay[b_kmajor], "lda": vb[1], "layout_b": lay[a_kmajor], "ldb": va[1],
                 "ldc": vo[1], "swap": True}
     args.update(copies)
+    args["bias_mode"] = BIAS_NONE if bias_stride is None else (BIAS_ROW if args["swap"] else BIAS_COL)
+    args["copy_bias"] = bias_stride is not None and ((bias_stride != 1 and N > 1) or bias_ptr % 4 != 0)
     return args
+
+
+def linear_plan(x_shape, x_stride, w_shape) -> dict:
+    """Shapes of linear(x, weight) with x: (..., K), weight: (N, K): the product runs on x flattened to (M, K); view is
+    (M, K) element strides of that flattening when x's leading dimensions collapse into one stride (a view, no copy),
+    None when x has to be copied first."""
+    *lead, K = x_shape
+    N, K2 = w_shape
+    if K != K2:
+        raise ValueError(f"x has {K} features, weight expects {K2}")
+    M = 1
+    for d in lead:
+        M *= d
+    # the leading dimensions of size > 1 must nest: stride[i] = stride[i+1] * shape[i+1]
+    dims = [(d, s) for d, s in zip(lead, x_stride[:-1]) if d > 1]
+    view = None
+    if all(dims[i][1] == dims[i + 1][1] * dims[i + 1][0] for i in range(len(dims) - 1)):
+        view = (dims[-1][1] if dims else max(K, 1), x_stride[-1])
+    return {"M": M, "K": K, "N": N, "out_shape": (*lead, N), "view": view}
 
 
 def _ptr(x) -> int:
@@ -322,20 +350,32 @@ class FtSgemm:
         self._run_checked(lib().ftsgemm_run_ex(self._h, kernel_id, M, N, K, _ptr(dA), layout_a, lda, _ptr(dB), layout_b, ldb,
                                                _ptr(dC), ldc, alpha, beta, C.byref(opts) if opts is not None else None))
 
-    def matmul(self, a, b, out=None, *, kernel_id: int = ID_ABFT_AUTO, alpha: float = 1.0, beta: float = 0.0,
+    def run_bias(self, kernel_id: int, M: int, N: int, K: int, dA, layout_a: int, lda: int, dB, layout_b: int, ldb: int, dC,
+                 ldc: int, alpha: float = 1.0, beta: float = 0.0, bias=None, bias_mode: int = BIAS_NONE,
+                 opts: Opts | None = None) -> None:
+        """C = (alpha * A * B^T + beta * C) + bias, the bias added in the store pass under the same ABFT protection:
+        bias[m] per row (BIAS_ROW, length M) or bias[n] per column (BIAS_COL, length N) (include/ftsgemm.h:
+        ftsgemm_run_bias).  The value in parentheses is bit for bit what run_ex stores."""
+        self._run_checked(lib().ftsgemm_run_bias(self._h, kernel_id, M, N, K, _ptr(dA), layout_a, lda, _ptr(dB), layout_b, ldb,
+                                                 _ptr(dC), ldc, alpha, beta, _ptr(bias) if bias is not None else None, bias_mode,
+                                                 C.byref(opts) if opts is not None else None))
+
+    def matmul(self, a, b, out=None, *, bias=None, kernel_id: int = ID_ABFT_AUTO, alpha: float = 1.0, beta: float = 0.0,
                opts: Opts | None = None):
-        """out = alpha * (a @ b) + beta * out for 2-D float32 CUDA tensors a: (M, K), b: (K, N); returns out.
+        """out = alpha * (a @ b) + beta * out + bias for 2-D float32 CUDA tensors a: (M, K), b: (K, N) and an optional 1-D
+        float32 bias of length N (one value per column of out, added in the fused store pass); returns out.
 
         a, b and out may each be row-major or column-major (a .t() view is the other layout) with any leading stride that
-        keeps 16-byte rows; they are read and written in place -- x @ W.T (F.linear without bias) on row-major tensors
-        copies nothing.  An operand that cannot be read in place (no unit stride, a base address or, for a and b, a
+        keeps 16-byte rows; they are read and written in place -- x @ W.T + b (F.linear) on row-major tensors copies
+        nothing.  An operand that cannot be read in place (no unit stride, a base address or, for a and b, a
         leading stride that is not a multiple of 16 bytes) is copied once into an aligned buffer first; an out that cannot
-        be written in place is computed in a contiguous buffer and copied back.  With out=None a new row-major out is
-        returned and beta must be 0.  The mapping onto run_ex is matmul_plan: a row-major out is computed as
-        out^T = b^T a^T, so the kernel's (row, col) is out's (col, row) -- the coordinates of injected faults (opts) and
-        of stats() events are the kernel's, transposed against out in that case.  A kernel M or N (after the mapping)
-        that is not a multiple of 4 raises FtsgemmError(-2) for the tensor-core ids, as run does.  Runs on the current
-        torch stream unless opts.stream says otherwise.  No autograd."""
+        be written in place is computed in a contiguous buffer and copied back; a bias without unit stride is copied once.
+        With out=None a new row-major out is returned and beta must be 0.  The mapping onto run_bias is matmul_plan: a
+        row-major out is computed as out^T = b^T a^T, so the kernel's (row, col) is out's (col, row) -- the coordinates of
+        injected faults (opts) and of stats() events are the kernel's, transposed against out in that case.  A kernel M or
+        N (after the mapping) that is not a multiple of 4 raises FtsgemmError(-2) for the tensor-core ids, as run does.
+        Runs on the current torch stream unless opts.stream says otherwise.  No autograd: linear() is the differentiable
+        F.linear."""
         import torch
         for name, t in (("a", a), ("b", b)):
             if t.dim() != 2 or t.dtype != torch.float32 or not t.is_cuda:
@@ -348,8 +388,13 @@ class FtSgemm:
             out = torch.empty(M, N, device=a.device, dtype=torch.float32)
         if out.shape != (M, N) or out.dtype != torch.float32 or out.device != a.device or b.device != a.device:
             raise ValueError(f"out must be a float32 ({M}, {N}) tensor on {a.device}")
+        if bias is not None and (bias.shape != (N,) or bias.dtype != torch.float32 or bias.device != a.device):
+            raise ValueError(f"bias must be a float32 ({N},) tensor on {a.device}")
+        bias_stride = bias.stride(0) if bias is not None else None
         plan = matmul_plan(tuple(a.shape), a.stride(), tuple(b.shape), b.stride(), out.stride(), a.data_ptr(), b.data_ptr(),
-                           out.data_ptr())
+                           out.data_ptr(), bias_stride, bias.data_ptr() if bias is not None else 0)
+        if plan["copy_bias"]:
+            bias = torch.empty(N, device=a.device, dtype=torch.float32).copy_(bias)
         if plan["copy_a"]:  # row-major, rows padded to 16 bytes: K-major for the kernel
             a = torch.empty(M, _pad4(K), device=a.device, dtype=torch.float32)[:, :K].copy_(a)
         if plan["copy_b"]:  # column-major, columns padded to 16 bytes: K-major for the kernel
@@ -360,15 +405,39 @@ class FtSgemm:
                    else torch.empty(M, N, device=a.device, dtype=torch.float32))
         if plan["copy_a"] or plan["copy_b"] or plan["copy_out"]:
             plan = matmul_plan(tuple(a.shape), a.stride(), tuple(b.shape), b.stride(), dst.stride(), a.data_ptr(),
-                               b.data_ptr(), dst.data_ptr())
+                               b.data_ptr(), dst.data_ptr(), bias_stride)
         if opts is None:
             opts = make_opts(stream=torch.cuda.current_stream(a.device).cuda_stream)
         kA, kB = (b, a) if plan["swap"] else (a, b)
-        self.run_ex(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], kB, plan["layout_b"],
-                    plan["ldb"], dst, plan["ldc"], alpha, beta, opts)
+        self.run_bias(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], kB, plan["layout_b"],
+                      plan["ldb"], dst, plan["ldc"], alpha, beta, bias, plan["bias_mode"], opts)
         if dst is not out:
             out.copy_(dst)
         return out
+
+    def linear(self, x, weight, bias=None, *, kernel_id: int = ID_ABFT_AUTO, opts: Opts | None = None):
+        """F.linear(x, weight, bias) = x @ weight.T + bias under ABFT protection, differentiable: x (..., K), weight (N, K),
+        bias (N,) or None, all float32 CUDA tensors; returns (..., N).
+
+        The forward is one matmul with the bias fused into the store pass; x's leading dimensions are flattened as a view
+        where the strides allow it (linear_plan) and copied otherwise.  Backward: grad_x = grad_y @ weight and
+        grad_weight = grad_y^T @ x through matmul with the same kernel id and opts (both read in place), grad_bias =
+        grad_y.sum(0) in torch.  Faults injected through opts land in the forward product only; faults detected in any of
+        the three products are counted in stats().  The forward runs on the current torch stream unless opts.stream names
+        one; the backward runs on the stream autograd runs it on."""
+        import torch
+        if x.dtype != torch.float32 or not x.is_cuda or x.dim() < 1:
+            raise TypeError("x must be a float32 CUDA tensor with at least one dimension")
+        if weight.dim() != 2:
+            raise TypeError("weight must be 2-D (out_features, in_features)")
+        lp = linear_plan(tuple(x.shape), x.stride(), tuple(weight.shape))
+        x2 = (x.as_strided((lp["M"], lp["K"]), lp["view"], x.storage_offset()) if lp["view"] is not None
+              else x.reshape(lp["M"], lp["K"]).contiguous())
+        fwd = Opts.from_buffer_copy(opts) if opts is not None else make_opts()
+        if not fwd.stream:
+            fwd.stream = torch.cuda.current_stream(x.device).cuda_stream
+        y = _linear_fn().apply(x2, weight, bias, self, kernel_id, fwd)
+        return y.view(lp["out_shape"])
 
     def run_host(self, kernel_id: int, M: int, N: int, K: int, hA, hB, hC, alpha: float = 1.0, beta: float = 0.0,
                  opts: Opts | None = None) -> None:
@@ -444,6 +513,41 @@ class FtSgemm:
         if code not in (0, -6):
             self._run_checked(code)
         return code == 0, int(bad.value), float(rel.value)
+
+
+_LINEAR_FN = None
+
+
+def _linear_fn():
+    """The torch.autograd.Function behind FtSgemm.linear (built on first use: torch is imported lazily)."""
+    global _LINEAR_FN
+    if _LINEAR_FN is None:
+        import torch
+
+        class LinearFn(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, x2, weight, bias, dev, kernel_id, opts):
+                ctx.save_for_backward(x2, weight)
+                ctx.dev, ctx.kernel_id, ctx.opts = dev, kernel_id, opts
+                return dev.matmul(x2, weight.t(), bias=bias, kernel_id=kernel_id, opts=opts)
+
+            @staticmethod
+            def backward(ctx, gy):
+                x2, weight = ctx.saved_tensors
+                bwd = Opts.from_buffer_copy(ctx.opts)
+                bwd.inject_mode, bwd.n_faults = 0, 0
+                bwd.stream = torch.cuda.current_stream(gy.device).cuda_stream
+                gx = gw = gb = None
+                if ctx.needs_input_grad[0]:
+                    gx = ctx.dev.matmul(gy, weight, kernel_id=ctx.kernel_id, opts=bwd)
+                if ctx.needs_input_grad[1]:
+                    gw = ctx.dev.matmul(gy.t(), x2, kernel_id=ctx.kernel_id, opts=bwd)
+                if ctx.needs_input_grad[2]:
+                    gb = gy.sum(0)
+                return gx, gw, gb, None, None, None
+
+        _LINEAR_FN = LinearFn
+    return _LINEAR_FN
 
 
 def run_cli(args, timeout=None) -> subprocess.CompletedProcess:

@@ -25,6 +25,7 @@
 namespace {
 
 using namespace ftsgemm;
+static_assert(kBiasNone == FTSGEMM_BIAS_NONE && kBiasRow == FTSGEMM_BIAS_ROW && kBiasCol == FTSGEMM_BIAS_COL, "bias modes");
 
 // ------------------------------------------------------------------------------------------- variant table
 struct Variant {
@@ -190,7 +191,11 @@ struct DeviceGuard {
   int prev = -1;
   bool switched = false;
   explicit DeviceGuard(ftsgemm_handle_t h) {
-    if (h && cudaGetDevice(&prev) == cudaSuccess && prev != h->device) switched = cudaSetDevice(h->device) == cudaSuccess;
+    if (!h || cudaGetDevice(&prev) != cudaSuccess) return;
+    if (prev != h->device) switched = cudaSetDevice(h->device) == cudaSuccess;
+    // (on a thread that has made no runtime call yet -- autograd's backward thread -- this makes the device's primary context
+    // current, which the driver entry point cuTensorMapEncodeTiled needs: it fails with CUDA_ERROR_INVALID_CONTEXT otherwise)
+    else cudaSetDevice(prev);
   }
   ~DeviceGuard() {
     if (switched) cudaSetDevice(prev);
@@ -268,12 +273,12 @@ int query_max_units(ftsgemm_handle_t h, int *out) {
   return FTSGEMM_OK;
 }
 
-template <int BN, bool FT, int CG, bool PROT, bool SEED>
+template <int BN, bool FT, int CG, bool PROT, bool SEED, bool BIAS>
 int launch_tc(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
               const KernelParams &p, int units, cudaStream_t stream) {
   // p.pdl_wait: the launch may overlap the tail of its predecessor in the stream (KernelParams::pdl_wait)
   using Cfg = TileCfg<BN, FT, CG>;
-  auto kern = ftsgemm_tc_kernel<BN, FT, CG, PROT, SEED>;
+  auto kern = ftsgemm_tc_kernel<BN, FT, CG, PROT, SEED, BIAS>;
   int resident = 0;
   const int qrc = query_max_units<BN, FT, CG, PROT>(h, &resident);
   if (qrc) return qrc;
@@ -304,12 +309,20 @@ int launch_tc(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB
   return FTSGEMM_OK;
 }
 
+template <int BN, int CG, bool SEED, bool BIAS>
+int launch_ft(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
+              const KernelParams &p, int units, cudaStream_t stream, bool ft, bool prot) {
+  if (!ft) return launch_tc<BN, false, CG, false, SEED, BIAS>(h, tmA, tmB, tmC, p, units, stream);
+  if (prot) return launch_tc<BN, true, CG, true, SEED, BIAS>(h, tmA, tmB, tmC, p, units, stream);
+  return launch_tc<BN, true, CG, false, SEED, BIAS>(h, tmA, tmB, tmC, p, units, stream);
+}
+
+// (a bias selects the BIAS instantiation: KernelParams::bias, ftsgemm_tc_kernel)
 template <int BN, int CG, bool SEED>
 int launch_variant(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
                    const KernelParams &p, int units, cudaStream_t stream, bool ft, bool prot) {
-  if (!ft) return launch_tc<BN, false, CG, false, SEED>(h, tmA, tmB, tmC, p, units, stream);
-  if (prot) return launch_tc<BN, true, CG, true, SEED>(h, tmA, tmB, tmC, p, units, stream);
-  return launch_tc<BN, true, CG, false, SEED>(h, tmA, tmB, tmC, p, units, stream);
+  if (p.bias_mode != kBiasNone) return launch_ft<BN, CG, SEED, true>(h, tmA, tmB, tmC, p, units, stream, ft, prot);
+  return launch_ft<BN, CG, SEED, false>(h, tmA, tmB, tmC, p, units, stream, ft, prot);
 }
 
 // Planner input for one launch (tile grid already set by plan_tiles).
@@ -412,7 +425,7 @@ struct Operand {
 };
 
 int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC, int ldc,
-           float alpha, float beta, const ftsgemm_opts &o, cudaStream_t stream) {
+           float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o, cudaStream_t stream) {
   const int BN = v.bn, CG = v.cg;
   const bool ft = v.info.fault_tolerant != 0;
   const float *dA = A.p, *dB = B.p;
@@ -429,6 +442,7 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
   p.M = M; p.N = N; p.K = K;
   p.C = dC; p.ldc = ldc;
   p.alpha = alpha; p.beta = beta;
+  p.bias = bias; p.bias_mode = bias_mode;
   plan_tiles(M, N, BN, CG, ft, &p);
   p.tau_abs = o.tau_abs > 0 ? o.tau_abs : 1e-3f;
   p.tau_rel = o.tau_rel > 0 ? o.tau_rel : 1e-5f;  // DESIGN.md section 5
@@ -1011,6 +1025,13 @@ int ftsgemm_run(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const fl
 
 int ftsgemm_run_ex(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda, const float *dB,
                    int layout_b, int ldb, float *dC, int ldc, float alpha, float beta, const ftsgemm_opts *opts) {
+  return ftsgemm_run_bias(h, kernel_id, M, N, K, dA, layout_a, lda, dB, layout_b, ldb, dC, ldc, alpha, beta, nullptr,
+                          FTSGEMM_BIAS_NONE, opts);
+}
+
+int ftsgemm_run_bias(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
+                     const float *dB, int layout_b, int ldb, float *dC, int ldc, float alpha, float beta, const float *bias,
+                     int bias_mode, const ftsgemm_opts *opts) {
   if (!h) return FTSGEMM_ERR_NO_DEVICE;
   if (!dA || !dB || !dC || M <= 0 || N <= 0 || K <= 0) return FTSGEMM_ERR_INVALID_ARG;
   const Variant *v = find_variant(kernel_id);
@@ -1020,6 +1041,10 @@ int ftsgemm_run_ex(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const
     return FTSGEMM_ERR_INVALID_ARG;
   const Operand A = {dA, layout_a == FTSGEMM_LAYOUT_K_MAJOR, lda}, B = {dB, layout_b == FTSGEMM_LAYOUT_K_MAJOR, ldb};
   if (lda < (A.kmajor ? K : M) || ldb < (B.kmajor ? K : N) || ldc < M) return FTSGEMM_ERR_INVALID_ARG;
+  if (bias_mode < FTSGEMM_BIAS_NONE || bias_mode > FTSGEMM_BIAS_COL) return FTSGEMM_ERR_INVALID_ARG;
+  if (bias_mode == FTSGEMM_BIAS_NONE) bias = nullptr;
+  else if (!bias || (reinterpret_cast<uintptr_t>(bias) & 3)) return FTSGEMM_ERR_INVALID_ARG;
+  if (bias && v->info.engine != 1) return FTSGEMM_ERR_UNSUPPORTED;  // the bias is fused into the wgmma kernels' store pass only
   ftsgemm_opts o;
   const int orc = load_opts(opts, &o);
   if (orc) return orc;
@@ -1033,7 +1058,7 @@ int ftsgemm_run_ex(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const
     // Intra-K checking (ftsgemm_opts::check_segments): S consecutive K-segments, each a complete fault-tolerant GEMM.  A
     // segment of an operand is a pointer offset: k0 * ld for an MN-major operand (k is the slow index), k0 for a K-major one;
     // segment boundaries are multiples of the stage depth (32 k-rows), so the offsets keep 16-byte alignment.  Injected
-    // faults (tests) go to the first segment only.
+    // faults (tests) go to the first segment only, the bias to the last one (added once, after the final alpha*acc + C).
     int S = o.check_segments;
     const int num_kb = (K + kBK - 1) / kBK;
     if (S > num_kb) S = num_kb;
@@ -1048,8 +1073,9 @@ int ftsgemm_run_ex(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const
       if (sg > 0) os.inject_mode = 0;
       const size_t oa = A.kmajor ? static_cast<size_t>(k0) : static_cast<size_t>(k0) * lda;
       const size_t ob = B.kmajor ? static_cast<size_t>(k0) : static_cast<size_t>(k0) * ldb;
-      rc = ftsgemm_run_ex(h, v->info.id, M, N, k1 - k0, dA + oa, layout_a, lda, dB + ob, layout_b, ldb, dC, ldc, alpha,
-                          sg == 0 ? beta : 1.0f, &os);
+      const bool last = sg == S - 1;
+      rc = ftsgemm_run_bias(h, v->info.id, M, N, k1 - k0, dA + oa, layout_a, lda, dB + ob, layout_b, ldb, dC, ldc, alpha,
+                            sg == 0 ? beta : 1.0f, last ? bias : nullptr, last ? bias_mode : FTSGEMM_BIAS_NONE, &os);
     }
     return rc;
   }
@@ -1094,14 +1120,15 @@ int ftsgemm_run_ex(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const
     o3.precision = 0;
     ftsgemm_opts o_quiet = o3;  // injected faults belong to the main product only
     o_quiet.inject_mode = 0;
-    rc = run_tc(h, *v, M, N, K, Alo, B, dC, ldc, alpha, beta, o_quiet, stream);
-    if (!rc) rc = run_tc(h, *v, M, N, K, A, Blo, dC, ldc, alpha, 1.0f, o_quiet, stream);
-    if (!rc) rc = run_tc(h, *v, M, N, K, A, B, dC, ldc, alpha, 1.0f, o3, stream);
+    // (the bias goes to the last pass only: added once, after the final alpha*acc + C)
+    rc = run_tc(h, *v, M, N, K, Alo, B, dC, ldc, alpha, beta, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream);
+    if (!rc) rc = run_tc(h, *v, M, N, K, A, Blo, dC, ldc, alpha, 1.0f, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream);
+    if (!rc) rc = run_tc(h, *v, M, N, K, A, B, dC, ldc, alpha, 1.0f, bias, bias_mode, o3, stream);
     return rc;
   }
   switch (v->info.engine) {
     case 0: return run_cublas(h, v->info.id == 7, M, N, K, A, B, dC, ldc, alpha, beta, stream);
-    case 1: return run_tc(h, *v, M, N, K, A, B, dC, ldc, alpha, beta, o, stream);
+    case 1: return run_tc(h, *v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream);
     case 2:
       // the non-fused baseline keeps the reference's call sequence, on the reference layout only
       if (A.kmajor || B.kmajor || lda != M || ldb != N || ldc != M) return FTSGEMM_ERR_UNSUPPORTED;

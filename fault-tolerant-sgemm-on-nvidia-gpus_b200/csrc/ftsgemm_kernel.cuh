@@ -74,6 +74,10 @@ struct KernelParams {
   float *C;
   int ldc;
   float alpha, beta;
+  // bias added where a data tile's final value is stored (ftsgemm_run_bias): kBiasRow bias[m], kBiasCol bias[n]; never in
+  // checksum tile-columns, parked pieces or the accumulator check
+  const float *bias;
+  int bias_mode;
   // tile schedule (tiles_m counts CG*128-row blocks)
   int tiles_m, tiles_n, group_n;
   // K-major copies of the MN-major operands written by the front phase (row stride ldk floats, ldk % 4 == 0); the tensor
@@ -280,10 +284,29 @@ __device__ __forceinline__ int ld_acquire(const int *p) {
 
 // ------------------------------------------------------------------------------------------------------------
 // Epilogue store pass: out = alpha*acc + beta*out, column-major, lane = consecutive rows -> 128-byte coalesced.
+// BIAS: out = (alpha*acc + beta*out) + b with one more FP32 rounding (__fadd_rn: never contracted into the product, so the
+// parenthesised value is bit for bit the unbiased one).  b = bias[m] (kBiasRow: lane = row, loaded once) or bias[n]
+// (kBiasCol: the same address in every lane -- broadcast loads, which unlike shuffles need no converged warp inside the
+// row_ok branches).
 // ------------------------------------------------------------------------------------------------------------
-template <int BN>
+constexpr int kBiasNone = 0, kBiasRow = 1, kBiasCol = 2;
+struct BiasRef {
+  const float *p;
+  int mode;
+  float row_value;  // bias[m] of this lane (kBiasRow)
+  __device__ __forceinline__ float at(int n) const { return mode == kBiasRow ? row_value : __ldg(p + n); }
+};
+__device__ __forceinline__ BiasRef make_bias(const float *p, int mode, int m, bool row_ok) {
+  BiasRef b;
+  b.p = p;
+  b.mode = mode;
+  b.row_value = (mode == kBiasRow && row_ok) ? __ldg(p + m) : 0.0f;
+  return b;
+}
+
+template <int BN, bool BIAS = false>
 __device__ __forceinline__ void store_tile(uint32_t taddr, float *crow, bool row_ok, int n0, int n_limit, int ldc,
-                                           float alpha, float beta, int c_begin = 0, int c_end = BN / 32) {
+                                           float alpha, float beta, int c_begin = 0, int c_end = BN / 32, BiasRef bias = {}) {
   const bool full_n = (n0 + BN <= n_limit);
   if (full_n && beta != 0.0f) {
     // Software pipeline: the old values of chunk c + 1 are fetched while chunk c is stored (a chunk's 32 loads would
@@ -301,7 +324,10 @@ __device__ __forceinline__ void store_tile(uint32_t taddr, float *crow, bool row
       const int nb = n0 + c * 32;
       if (row_ok) {
 #pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = f2u(alpha * u2f(v[i]) + beta * old[i]);
+        for (int i = 0; i < 32; ++i) {
+          v[i] = f2u(alpha * u2f(v[i]) + beta * old[i]);
+          if constexpr (BIAS) v[i] = f2u(__fadd_rn(u2f(v[i]), bias.at(nb + i)));
+        }
         if (c + 1 < c_end) {
 #pragma unroll
           for (int i = 0; i < 32; ++i) old[i] = crow[static_cast<size_t>(nb + 32 + i) * ldc];
@@ -320,14 +346,20 @@ __device__ __forceinline__ void store_tile(uint32_t taddr, float *crow, bool row
     if (!row_ok) continue;
     if (full_n) {
 #pragma unroll
-      for (int i = 0; i < 32; ++i) crow[static_cast<size_t>(nb + i) * ldc] = alpha * u2f(v[i]);
+      for (int i = 0; i < 32; ++i) {
+        float x = alpha * u2f(v[i]);
+        if constexpr (BIAS) x = __fadd_rn(x, bias.at(nb + i));
+        crow[static_cast<size_t>(nb + i) * ldc] = x;
+      }
     } else {
 #pragma unroll
       for (int i = 0; i < 32; ++i) {
         if (nb + i < n_limit) {
           float *dst = crow + static_cast<size_t>(nb + i) * ldc;
           const float o = (beta == 0.0f) ? 0.0f : beta * (*dst);
-          *dst = alpha * u2f(v[i]) + o;
+          float x = alpha * u2f(v[i]) + o;
+          if constexpr (BIAS) x = __fadd_rn(x, bias.at(nb + i));
+          *dst = x;
         }
       }
     }
@@ -583,16 +615,22 @@ __device__ __forceinline__ void abft_check(const KernelParams &p, uint32_t taddr
 // memory or of the read path after the check -- and sums what it stores: sum(out) must equal alpha * sum(acc) + beta *
 // sum(old) within the rounding of n_cols fused multiply-adds (2 * 128 * 2^-24 of the magnitudes).  Returns true in the
 // lanes (= rows) whose segment failed.  bad_col / bad_mask: test injector (ftsgemm_fault.mode 3), -1 = none.
+// With a bias the stored value is fl(x + b) with x = alpha * acc + beta * old: the reference gains sum(b) over the segment
+// (bias[m] * n_cols for kBiasRow, the segment's column sum for kBiasCol), and since |fl(x + b) - (x + b)| <= 2^-24 (|x| + |b|)
+// the one extra rounding per element and the summation of the b's are bounded by the same per-element budget with |b|
+// added to the magnitudes: tol = 1.6e-5 * (|alpha| sum|acc| + |beta| sum|old| + sum|b|).  Detection itself (the accumulator
+// check) runs before alpha, beta and the bias and is unchanged.
 // ------------------------------------------------------------------------------------------------------------
 struct StoreVerdict {
   float resid;
   bool bad;
 };
-template <int BN>
+template <int BN, bool BIAS>
 __device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, float *crow, bool row_ok, int n0, int ldc, float alpha,
                                                           float beta, int c_begin, int c_end, float chk_s1, bool chk_s1_valid,
-                                                          int bad_col, uint32_t bad_mask) {
+                                                          int bad_col, uint32_t bad_mask, const BiasRef &bias) {
   float s1 = 0.0f, s2 = 0.0f, sabs = 0.0f, so0 = 0.0f, so1 = 0.0f, sold0 = 0.0f, sold1 = 0.0f, aold0 = 0.0f, aold1 = 0.0f;
+  float sb = 0.0f, ab = 0.0f;  // sum(b), sum|b| of the segment
   const bool rmw = beta != 0.0f;
   float old[32];
   if (row_ok && rmw) {
@@ -625,6 +663,15 @@ __device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, flo
 #pragma unroll
         for (int i = 0; i < 32; ++i) v[i] = f2u(alpha * u2f(v[i]));
       }
+      if constexpr (BIAS) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          const float b = bias.at(nb + i);
+          v[i] = f2u(__fadd_rn(u2f(v[i]), b));
+          sb += b;
+          ab += fabsf(b);
+        }
+      }
       if (bad_col >= c * 32 && bad_col < c * 32 + 32) {
 #pragma unroll
         for (int i = 0; i < 32; ++i)
@@ -639,8 +686,12 @@ __device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, flo
       for (int i = 0; i < 32; ++i) crow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
     }
   }
-  const float ref = alpha * s1 + beta * (sold0 + sold1);
-  const float tol = 1.6e-5f * (fabsf(alpha) * sabs + fabsf(beta) * (aold0 + aold1)) + 1e-30f;
+  float ref = alpha * s1 + beta * (sold0 + sold1);
+  float tol = 1.6e-5f * (fabsf(alpha) * sabs + fabsf(beta) * (aold0 + aold1)) + 1e-30f;
+  if constexpr (BIAS) {
+    ref += sb;
+    tol = 1.6e-5f * (fabsf(alpha) * sabs + fabsf(beta) * (aold0 + aold1) + ab) + 1e-30f;
+  }
   StoreVerdict out;
   out.resid = (so0 + so1) - ref;
   const bool reread_differs = chk_s1_valid && f2u(s1) != f2u(chk_s1);
@@ -652,13 +703,15 @@ __device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, flo
 // ------------------------------------------------------------------------------------------------------------
 // Recompute fallback (rare): one warp recomputes row m of the tile's BN columns from global memory -- the values the
 // tensor core would have produced up to FP32 accumulation order (TF32-truncated operands: every product is exact in
-// FP32) -- and writes C = alpha * acc + beta * C directly.  K iterations of 1 broadcast + BN/32 loads (coalesced for an
-// MN-major B, one stride-ldb load per lane for a K-major one).  kmajor: bit 0 = A is K-major, bit 1 = B is K-major.
+// FP32) -- and writes C = alpha * acc + beta * C (+ the bias: an input, so a row stays repairable with beta = 0) directly.
+// K iterations of 1 broadcast + BN/32 loads (coalesced for an MN-major B, one stride-ldb load per lane for a K-major one).
+// kmajor: bit 0 = A is K-major, bit 1 = B is K-major.
 // ------------------------------------------------------------------------------------------------------------
 // (scalars by value: a reference to the __grid_constant__ parameter block would force a local copy of all of it)
-template <int BN>
-__device__ __noinline__ void recompute_row(const float *A, const float *B, float *C, int lda, int ldb, int kmajor, int ldc, int N,
-                                           int K, float alpha, float beta, int m, int n0, int lane) {
+template <int BN, bool BIAS>
+__device__ __forceinline__ void recompute_row_body(const float *A, const float *B, float *C, int lda, int ldb, int kmajor, int ldc,
+                                                   int N, int K, float alpha, float beta, int m, int n0, int lane, const float *bias,
+                                                   int bias_mode) {
   constexpr int J = BN / 32;
   float acc[J];
 #pragma unroll
@@ -684,22 +737,43 @@ __device__ __noinline__ void recompute_row(const float *A, const float *B, float
     if (n < N) {
       float *dst = C + m + static_cast<size_t>(n) * ldc;
       const float o = (beta == 0.0f) ? 0.0f : beta * (*dst);
-      *dst = alpha * acc[j] + o;
+      float x = alpha * acc[j] + o;
+      if constexpr (BIAS) x = __fadd_rn(x, __ldg(bias + (bias_mode == kBiasRow ? m : n)));
+      *dst = x;
     }
   }
+}
+// Out-of-line entries without and with a bias (the one without keeps its parameter list: the callers' register allocation
+// depends on it, see protected_store_pass)
+template <int BN>
+__device__ __noinline__ void recompute_row(const float *A, const float *B, float *C, int lda, int ldb, int kmajor, int ldc, int N,
+                                           int K, float alpha, float beta, int m, int n0, int lane) {
+  recompute_row_body<BN, false>(A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, m, n0, lane, nullptr, kBiasNone);
+}
+template <int BN>
+__device__ __noinline__ void recompute_row_bias(const float *A, const float *B, float *C, int lda, int ldb, int kmajor, int ldc,
+                                                int N, int K, float alpha, float beta, int m, int n0, int lane, const float *bias,
+                                                int bias_mode) {
+  recompute_row_body<BN, true>(A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, m, n0, lane, bias, bias_mode);
+}
+template <int BN, bool BIAS, typename... Args>
+__device__ __forceinline__ void recompute(const float *bias, int bias_mode, Args... args) {
+  if constexpr (BIAS) recompute_row_bias<BN>(args..., bias, bias_mode);
+  else recompute_row<BN>(args...);
 }
 
 // The whole protected store pass of one warp, out of line and with scalars by value: an opt-in path must not cost the
 // common epilogue registers (inlined it pushed the kernel into spills), and a reference to the __grid_constant__ parameter
 // block would force a local copy of all of it.  Row segments that fail are counted and, with beta == 0, recomputed from A
 // and B (with beta != 0 the old values of C are already overwritten: reported as uncorrectable).
-template <int BN>
-__device__ __noinline__ void protected_store_pass(uint32_t taddr, const float *A, const float *B, float *C, int lda, int ldb,
-                                                  int kmajor, int ldc, int N, int K, float alpha, float beta, DeviceStats *stats, bool can_recompute,
-                                                  int m, int row0, bool row_ok, int n0, int c_begin, int c_end, float chk_s1,
-                                                  bool chk_s1_valid, int bad_col, uint32_t bad_mask, int lane) {
-  const StoreVerdict sv = store_tile_protected<BN>(taddr, C + m, row_ok, n0, ldc, alpha, beta, c_begin, c_end, chk_s1, chk_s1_valid,
-                                                   bad_col, bad_mask);
+template <int BN, bool BIAS>
+__device__ __forceinline__ void protected_store_body(uint32_t taddr, const float *A, const float *B, float *C, int lda, int ldb,
+                                                     int kmajor, int ldc, int N, int K, float alpha, float beta, DeviceStats *stats,
+                                                     bool can_recompute, int m, int row0, bool row_ok, int n0, int c_begin, int c_end,
+                                                     float chk_s1, bool chk_s1_valid, int bad_col, uint32_t bad_mask, int lane,
+                                                     const float *bias, int bias_mode) {
+  const StoreVerdict sv = store_tile_protected<BN, BIAS>(taddr, C + m, row_ok, n0, ldc, alpha, beta, c_begin, c_end, chk_s1, chk_s1_valid,
+                                                         bad_col, bad_mask, make_bias(bias, bias_mode, m, BIAS && row_ok));
   unsigned mask = __ballot_sync(0xffffffffu, sv.bad);
   if (mask == 0u) return;
   const bool can_fix = beta == 0.0f && can_recompute;
@@ -722,12 +796,36 @@ __device__ __noinline__ void protected_store_pass(uint32_t taddr, const float *A
     const int r = __ffs(mask) - 1;
     mask &= mask - 1u;
     if (c_end - c_begin == BN / 32) {
-      recompute_row<BN>(A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r, n0, lane);
+      recompute<BN, BIAS>(bias, bias_mode, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r, n0, lane);
     } else {
       if constexpr (BN >= 64)
-        recompute_row<BN / 2>(A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r, n0 + c_begin * 32, lane);
+        recompute<BN / 2, BIAS>(bias, bias_mode, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r, n0 + c_begin * 32, lane);
     }
   }
+}
+#define FT_PROT_PARAMS                                                                                                        \
+  uint32_t taddr, const float *A, const float *B, float *C, int lda, int ldb, int kmajor, int ldc, int N, int K, float alpha, \
+      float beta, DeviceStats *stats, bool can_recompute, int m, int row0, bool row_ok, int n0, int c_begin, int c_end,        \
+      float chk_s1, bool chk_s1_valid, int bad_col, uint32_t bad_mask, int lane
+#define FT_PROT_ARGS                                                                                                            \
+  taddr, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, stats, can_recompute, m, row0, row_ok, n0, c_begin, c_end, chk_s1, \
+      chk_s1_valid, bad_col, bad_mask, lane
+// Two out-of-line entries, so that the pass without a bias is the same function as before the bias existed (ptxas allocates
+// the caller's registers around what a callee clobbers: a changed callee moved the spills of the protected instantiations).
+template <int BN>
+__device__ __noinline__ void protected_store_pass(FT_PROT_PARAMS) {
+  protected_store_body<BN, false>(FT_PROT_ARGS, nullptr, kBiasNone);
+}
+template <int BN>
+__device__ __noinline__ void protected_store_pass_bias(FT_PROT_PARAMS, const float *bias, int bias_mode) {
+  protected_store_body<BN, true>(FT_PROT_ARGS, bias, bias_mode);
+}
+#undef FT_PROT_PARAMS
+#undef FT_PROT_ARGS
+template <int BN, bool BIAS, typename... Args>
+__device__ __forceinline__ void protected_store(const float *bias, int bias_mode, Args... args) {
+  if constexpr (BIAS) protected_store_pass_bias<BN>(args..., bias, bias_mode);
+  else protected_store_pass<BN>(args...);
 }
 
 // Test injectors for upsets AFTER the accumulator check (ftsgemm_fault.mode 2: into the accumulator before the store pass
@@ -1082,7 +1180,10 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t a_desc, 
 // path costs the common epilogue no registers.
 // SEED: the instantiation for plans with cut tiles, which load a parked accumulator into the wgmma accumulator registers;
 // plans without cut tiles run a kernel that has no such path.
-template <int BN, bool FT, int CG, bool PROT = false, bool SEED = false>
+// BIAS: the instantiation for calls with a bias (ftsgemm_run_bias).  A warp-uniform branch into an out-of-line biased store
+// pass raised the spills of every instantiation (the call alone, even where it is never taken), so a bias selects its own
+// binary and the default kernels are compiled exactly as without the feature.
+template <int BN, bool FT, int CG, bool PROT = false, bool SEED = false, bool BIAS = false>
 __global__ void __launch_bounds__(kThreads, 1)
 ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmChk, const KernelParams p) {
@@ -1338,11 +1439,12 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N) {
             uint32_t bad_bits = 0u;
             const int bad_col = stored_value_fault<BN>(p, q, lane, m0_cta, n0, kMid, BN / 32, bad_bits);
-            protected_store_pass<BN>(taddr, p.A, p.B, p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K, p.alpha,
-                                     p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32, m < p.M && !skip, n0, kMid, BN / 32, s1,
-                                     stale == 0u, bad_col, bad_bits, lane);
+            protected_store<BN, BIAS>(p.bias, p.bias_mode, taddr, p.A, p.B, p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
+                                      p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32,
+                                      m < p.M && !skip, n0, kMid, BN / 32, s1, stale == 0u, bad_col, bad_bits, lane);
           } else {
-            store_tile<BN>(taddr, p.C + m, m < p.M && !skip, n0, p.N, p.ldc, p.alpha, p.beta, kMid, BN / 32);
+            store_tile<BN, BIAS>(taddr, p.C + m, m < p.M && !skip, n0, p.N, p.ldc, p.alpha, p.beta, kMid, BN / 32,
+                                 make_bias(p.bias, p.bias_mode, m, BIAS && m < p.M && !skip));
           }
           ptx::named_bar_sync(4 + q, 64);  // both halves are out of the accumulator
         }
@@ -1399,19 +1501,20 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N) {
           uint32_t bad_bits = 0u;
           const int bad_col = stored_value_fault<BN>(p, q, lane, m0_cta, n0, 0, c_mid, bad_bits);
-          protected_store_pass<BN>(taddr, p.A, p.B, p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K, p.alpha,
-                                   p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32, m < p.M && !redo, n0, 0, c_mid, own_s1,
-                                   ((stale_mask >> lane) & 1u) == 0u, bad_col, bad_bits, lane);
+          protected_store<BN, BIAS>(p.bias, p.bias_mode, taddr, p.A, p.B, p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
+                                    p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32,
+                                    m < p.M && !redo, n0, 0, c_mid, own_s1, ((stale_mask >> lane) & 1u) == 0u, bad_col, bad_bits, lane);
         } else {
-          store_tile<BN>(taddr, p.C + m, m < p.M && !redo, n0, p.N, p.ldc, p.alpha, p.beta, 0, c_mid);
+          store_tile<BN, BIAS>(taddr, p.C + m, m < p.M && !redo, n0, p.N, p.ldc, p.alpha, p.beta, 0, c_mid,
+                               make_bias(p.bias, p.bias_mode, m, BIAS && m < p.M && !redo));
         }
         if (FT && redo_mask != 0u) {  // rare, warp-uniform: recompute the flagged rows from global memory
           unsigned rm = redo_mask;
           while (rm != 0u) {
             const int r = __ffs(rm) - 1;
             rm &= rm - 1u;
-            recompute_row<BN>(p.A, p.B, p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K, p.alpha, p.beta,
-                              m0_cta + q * 32 + r, n0, lane);
+            recompute<BN, BIAS>(p.bias, p.bias_mode, p.A, p.B, p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K,
+                                p.alpha, p.beta, m0_cta + q * 32 + r, n0, lane);
           }
         }
         if (assist_on) ptx::named_bar_sync(4 + q, 64);  // both halves are out of the accumulator

@@ -216,6 +216,29 @@ int ftsgemm_run_ex(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const
                    const float *dB, int layout_b, int ldb, float *dC, int ldc, float alpha, float beta,
                    const ftsgemm_opts *opts);
 
+/* ---- bias fused into the store pass  (new work: the reference's epilogue c = alpha*res + beta*c, ft_sgemm_huge.cuh:573-690,
+ *      has no bias and no protection) -------------------------------------------------------------------------------------
+ * The product of ftsgemm_run_ex plus a bias, added where the kernel stores a tile's final value:
+ *   C(m,n) = (alpha * acc(m,n) + beta * C_old(m,n)) + b      b = bias[m] (FTSGEMM_BIAS_ROW, length M)
+ *                                                            b = bias[n] (FTSGEMM_BIAS_COL, length N)
+ * The parenthesised value is bit for bit what ftsgemm_run_ex stores for the same call, and the add is one FP32 rounding.  The
+ * ABFT check runs on the accumulator before alpha, beta and the bias, so its sensitivity does not change; the recompute
+ * fallback and the protected store pass (opts.protect_epilogue) include the bias, so what is stored is what was checked.
+ * With opts.precision = 1 only the last of the three passes, with opts.check_segments = S only the last segment adds it:
+ * the bias is added exactly once.  A linear layer y = x W^T + b on row-major tensors is the swapped product
+ * y^T = W x^T: M = out_features, N = tokens, both operands K-major, FTSGEMM_BIAS_ROW.
+ * The bias is dense and 4-byte aligned.  Errors: a mode outside 0..2, or ROW / COL with a NULL or misaligned bias:
+ * FTSGEMM_ERR_INVALID_ARG; a bias with the cuBLAS ids 0 / 7 or the baseline ids 10 / 30: FTSGEMM_ERR_UNSUPPORTED (there is
+ * no unfused fallback).  With FTSGEMM_BIAS_NONE the pointer is ignored and the call is ftsgemm_run_ex. */
+enum {
+  FTSGEMM_BIAS_NONE = 0,
+  FTSGEMM_BIAS_ROW = 1,
+  FTSGEMM_BIAS_COL = 2
+};
+int ftsgemm_run_bias(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
+                     const float *dB, int layout_b, int ldb, float *dC, int ldc, float alpha, float beta,
+                     const float *bias, int bias_mode, const ftsgemm_opts *opts);
+
 /* Counters of all FT launches since the previous call (synchronises the handle's last stream, then resets). */
 int ftsgemm_get_stats(ftsgemm_handle_t h, ftsgemm_stats *out);
 
