@@ -92,7 +92,7 @@ EXPORTED_SYMBOLS = [
     "ftsgemm_default_opts", "ftsgemm_kernel_table", "ftsgemm_kernel_lookup", "ftsgemm_run", "ftsgemm_run_ex", "ftsgemm_run_bias", "ftsgemm_get_stats",
     "ftsgemm_run_host", "ftsgemm_baseline", "ftsgemm_verify", "ftsgemm_debug_set", "ftsgemm_debug_schedule",
     "ftsgemm_verify_bad_count", "ftsgemm_debug_trace", "ftsgemm_stats_device", "ftsgemm_select_kernel", "ftsgemm_launch_count", "ftsgemm_peer_export", "ftsgemm_peer_connect",
-    "ftsgemm_peer_verdict",
+    "ftsgemm_peer_verdict", "ftsgemm_run_batched", "ftsgemm_debug_schedule_batched",
 ]
 
 _lib = None
@@ -127,6 +127,9 @@ def lib():
         L.ftsgemm_run.argtypes = [vp, ip, ip, ip, ip, vp, vp, vp, fp, fp, C.POINTER(Opts)]
         L.ftsgemm_run_ex.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, vp, ip, ip, vp, ip, fp, fp, C.POINTER(Opts)]
         L.ftsgemm_run_bias.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, vp, ip, ip, vp, ip, fp, fp, vp, ip, C.POINTER(Opts)]
+        ll = C.c_longlong
+        L.ftsgemm_run_batched.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, ll, vp, ip, ip, ll, vp, ip, ll, ip, fp, fp, vp, ip,
+                                          C.POINTER(Opts)]
         L.ftsgemm_get_stats.argtypes = [vp, C.POINTER(Stats)]
         L.ftsgemm_run_host.argtypes = [vp, ip, ip, ip, ip, vp, vp, vp, fp, fp, C.POINTER(Opts)]
         L.ftsgemm_stats_device.argtypes = [vp, vp, vp]
@@ -142,6 +145,7 @@ def lib():
         L.ftsgemm_verify_bad_count.argtypes = [vp]
         L.ftsgemm_verify_bad_count.restype = C.c_longlong
         L.ftsgemm_debug_schedule.argtypes = [ip, ip, ip, ip, ip, C.POINTER(C.c_int), C.POINTER(C.c_int), ip]
+        L.ftsgemm_debug_schedule_batched.argtypes = [ip, ip, ip, ip, ip, ip, C.POINTER(C.c_int), C.POINTER(C.c_int), ip]
         L.ftsgemm_debug_trace.argtypes = [vp, C.POINTER(C.c_ulonglong), ip]
         _lib = L
     return _lib
@@ -221,6 +225,19 @@ def debug_schedule(kernel_id: int, M: int, N: int, K: int, num_sms: int = 132):
     return dict(zip(("units", "num_tiles", "n_chk_tiles", "sk_tiles", "num_kb", "cta_group", "sk_slices", "chk_slices"), hdr)), segs
 
 
+def debug_schedule_batched(kernel_id: int, M: int, N: int, K: int, batch: int, num_sms: int = 132):
+    """debug_schedule for a strided batch of `batch` entries: every segment dict carries its entry as well."""
+    hdr = (C.c_int * 8)()
+    n = lib().ftsgemm_debug_schedule_batched(kernel_id, M, N, K, batch, num_sms, hdr, None, 0)
+    if n < 0:
+        _check(n)
+    rows = (C.c_int * (10 * max(n, 1)))()
+    lib().ftsgemm_debug_schedule_batched(kernel_id, M, N, K, batch, num_sms, hdr, rows, n)
+    keys = ("unit", "tile", "is_chk", "m_blk", "n_blk", "kb_begin", "kb_end", "kind", "slice", "batch")
+    segs = [dict(zip(keys, rows[10 * i:10 * i + 10])) for i in range(n)]
+    return dict(zip(("units", "num_tiles", "n_chk_tiles", "sk_tiles", "num_kb", "cta_group", "sk_slices", "chk_slices"), hdr)), segs
+
+
 def debug_set(key: str, value: int) -> None:
     _check(lib().ftsgemm_debug_set(key.encode(), int(value)))
 
@@ -282,6 +299,43 @@ def matmul_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0
     args["bias_mode"] = BIAS_NONE if bias_stride is None else (BIAS_ROW if args["swap"] else BIAS_COL)
     args["copy_bias"] = bias_stride is not None and ((bias_stride != 1 and N > 1) or bias_ptr % 4 != 0)
     return args
+
+
+def bmm_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0, b_ptr: int = 0, out_ptr: int = 0,
+             bias_stride=None, bias_ptr: int = 0) -> dict:
+    """run_batched arguments for out = a @ b with a: (Bt, M, K), b: (Bt, K, N), out: (Bt, M, N), from shapes, element strides
+    and addresses.  Each matrix is mapped as in matmul_plan (layouts, lds, swap, bias_mode); stride_a / stride_b / stride_c
+    are the batch strides of the kernel's A, B and C (b's and a's when swapped).  With more than one entry a tensor is also
+    marked for copying when its batch stride is not a positive multiple of 4 floats (an expanded operand has stride 0), and
+    out when its entries would overlap; the arguments returned then describe the dense copies bmm makes (a row-major and b
+    column-major with rows padded to a multiple of 4, out contiguous row-major)."""
+    Bt, M, K = a_shape
+    Bt2, K2, N = b_shape
+    if Bt != Bt2:
+        raise ValueError(f"batch sizes differ: {tuple(a_shape)} @ {tuple(b_shape)}")
+    mp = matmul_plan((M, K), tuple(a_stride[1:]), (K2, N), tuple(b_stride[1:]), tuple(out_stride[1:]), a_ptr, b_ptr, out_ptr,
+                     bias_stride, bias_ptr)
+    sa, sb, so = a_stride[0], b_stride[0], out_stride[0]
+    if Bt > 1:
+        def bad(st):
+            return st <= 0 or st % 4 != 0
+        mp["copy_a"] = mp["copy_a"] or bad(sa)
+        mp["copy_b"] = mp["copy_b"] or bad(sb)
+        mp["copy_out"] = mp["copy_out"] or bad(so) or so < mp["ldc"] * mp["N"]
+    if mp["copy_a"] or mp["copy_b"] or mp["copy_out"]:
+        # the copies: a (Bt, M, pad4(K)) row-major, b as (Bt, N, pad4(K)) transposed, out (Bt, M, N) contiguous
+        a_st = (M * _pad4(K), _pad4(K), 1) if mp["copy_a"] else tuple(a_stride)
+        b_st = (N * _pad4(K), 1, _pad4(K)) if mp["copy_b"] else tuple(b_stride)
+        o_st = (M * N, N, 1) if mp["copy_out"] else tuple(out_stride)
+        copies = {k: mp[k] for k in ("copy_a", "copy_b", "copy_out", "copy_bias")}
+        mp = matmul_plan((M, K), a_st[1:], (K, N), b_st[1:], o_st[1:], 0 if copies["copy_a"] else a_ptr,
+                         0 if copies["copy_b"] else b_ptr, 0 if copies["copy_out"] else out_ptr, bias_stride, bias_ptr)
+        mp.update(copies)
+        sa, sb, so = a_st[0], b_st[0], o_st[0]
+    mp["batch"] = Bt
+    mp["stride_a"], mp["stride_b"] = (sb, sa) if mp["swap"] else (sa, sb)
+    mp["stride_c"] = so
+    return mp
 
 
 def linear_plan(x_shape, x_stride, w_shape) -> dict:
@@ -359,6 +413,70 @@ class FtSgemm:
         self._run_checked(lib().ftsgemm_run_bias(self._h, kernel_id, M, N, K, _ptr(dA), layout_a, lda, _ptr(dB), layout_b, ldb,
                                                  _ptr(dC), ldc, alpha, beta, _ptr(bias) if bias is not None else None, bias_mode,
                                                  C.byref(opts) if opts is not None else None))
+
+    def run_batched(self, kernel_id: int, M: int, N: int, K: int, dA, layout_a: int, lda: int, stride_a: int, dB, layout_b: int,
+                    ldb: int, stride_b: int, dC, ldc: int, stride_c: int, batch: int, alpha: float = 1.0, beta: float = 0.0,
+                    bias=None, bias_mode: int = BIAS_NONE, opts: Opts | None = None) -> None:
+        """`batch` run_bias products in one launch: entry i on dA + i*stride_a, dB + i*stride_b, dC + i*stride_c (element
+        strides), one bias shared by all entries (include/ftsgemm.h: ftsgemm_run_batched).  Fault and event rows are stacked
+        rows i*M + m."""
+        self._run_checked(lib().ftsgemm_run_batched(self._h, kernel_id, M, N, K, _ptr(dA), layout_a, lda, stride_a, _ptr(dB),
+                                                    layout_b, ldb, stride_b, _ptr(dC), ldc, stride_c, batch, alpha, beta,
+                                                    _ptr(bias) if bias is not None else None, bias_mode,
+                                                    C.byref(opts) if opts is not None else None))
+
+    def bmm(self, a, b, out=None, *, bias=None, kernel_id: int = ID_ABFT_AUTO, alpha: float = 1.0, beta: float = 0.0,
+            opts: Opts | None = None):
+        """out = alpha * (a @ b) + beta * out + bias for 3-D float32 CUDA tensors a: (Bt, M, K), b: (Bt, K, N), out: (Bt, M, N)
+        and an optional bias (N,) shared by all entries -- torch.baddbmm plus a bias -- as ONE run_batched call; returns out.
+
+        Every matrix may be row- or column-major with any leading stride that keeps 16-byte rows, and is read in place when
+        its batch stride is a multiple of 4 floats: contiguous bmm operands and q @ k.transpose(-1, -2) copy nothing.  An
+        expanded operand (batch stride 0), a batch stride that is not a multiple of 4, or a matrix matmul could not read in
+        place is copied once (bmm_plan); an out that cannot be written in place is computed in a contiguous buffer and copied
+        back.  Fault and event coordinates (opts, stats()) are stacked kernel rows entry * kernel_M + row, transposed against
+        out when the call is swapped (a row-major out: the kernel's rows are out's columns).  No autograd."""
+        import torch
+        for name, t in (("a", a), ("b", b)):
+            if t.dim() != 3 or t.dtype != torch.float32 or not t.is_cuda:
+                raise TypeError(f"{name} must be a 3-D float32 CUDA tensor")
+        Bt, M, K = a.shape
+        N = b.shape[2]
+        if b.shape[0] != Bt or b.shape[1] != K or b.device != a.device:
+            raise ValueError(f"b must be a ({Bt}, {K}, N) tensor on {a.device}")
+        if out is None:
+            if beta != 0.0:
+                raise ValueError("beta != 0 needs an out tensor")
+            out = torch.empty(Bt, M, N, device=a.device, dtype=torch.float32)
+        if out.shape != (Bt, M, N) or out.dtype != torch.float32 or out.device != a.device:
+            raise ValueError(f"out must be a float32 ({Bt}, {M}, {N}) tensor on {a.device}")
+        if bias is not None and (bias.shape != (N,) or bias.dtype != torch.float32 or bias.device != a.device):
+            raise ValueError(f"bias must be a float32 ({N},) tensor on {a.device}")
+        if Bt == 0:  # an empty batch (torch.bmm accepts it): nothing to compute
+            return out
+        bias_stride = bias.stride(0) if bias is not None else None
+        plan = bmm_plan(tuple(a.shape), a.stride(), tuple(b.shape), b.stride(), out.stride(), a.data_ptr(), b.data_ptr(),
+                        out.data_ptr(), bias_stride, bias.data_ptr() if bias is not None else 0)
+        if plan["copy_bias"]:
+            bias = torch.empty(N, device=a.device, dtype=torch.float32).copy_(bias)
+        if plan["copy_a"]:
+            a = torch.empty(Bt, M, _pad4(K), device=a.device, dtype=torch.float32)[:, :, :K].copy_(a)
+        if plan["copy_b"]:
+            b = torch.empty(Bt, N, _pad4(K), device=a.device, dtype=torch.float32)[:, :, :K].copy_(b.transpose(1, 2)).transpose(1, 2)
+        dst = out
+        if plan["copy_out"]:
+            dst = (out.contiguous() if beta != 0.0 else torch.empty(Bt, M, N, device=a.device, dtype=torch.float32))
+            if dst is out:
+                dst = out.clone()
+        if opts is None:
+            opts = make_opts(stream=torch.cuda.current_stream(a.device).cuda_stream)
+        kA, kB = (b, a) if plan["swap"] else (a, b)
+        self.run_batched(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], plan["stride_a"], kB,
+                         plan["layout_b"], plan["ldb"], plan["stride_b"], dst, plan["ldc"], plan["stride_c"], Bt, alpha, beta,
+                         bias, plan["bias_mode"], opts)
+        if dst is not out:
+            out.copy_(dst)
+        return out
 
     def matmul(self, a, b, out=None, *, bias=None, kernel_id: int = ID_ABFT_AUTO, alpha: float = 1.0, beta: float = 0.0,
                opts: Opts | None = None):

@@ -76,14 +76,16 @@ const Variant *find_variant(int id) {
 // Per-shape choice of the wgmma variant (replaces the reference's manual id choice, sgemm.cu:110-199; SURVEY 8 f2):
 // with few tiles most units idle with 256x256 tiles, so the 256x128 tile ("large") is used below a tile-count threshold
 // (49 tiles of 256x256 plain, 25 ABFT; thresholds not re-tuned for H100).
-int select_variant(int M, int N, bool ft) {
-  const long long tiles256 = (static_cast<long long>(M) + 255) / 256 * ((static_cast<long long>(N) + 255) / 256);
+// (batch: the tiles of all entries of a strided batch count)
+int select_variant(int M, int N, bool ft, int batch = 1) {
+  const long long tiles256 = (static_cast<long long>(M) + 255) / 256 * ((static_cast<long long>(N) + 255) / 256) * batch;
   if (tiles256 >= (ft ? 25 : 49)) return ft ? FTSGEMM_ID_ABFT_GIANT : FTSGEMM_ID_SGEMM_GIANT;
   return ft ? FTSGEMM_ID_ABFT_LARGE : FTSGEMM_ID_SGEMM_LARGE;
 }
 
 // slab flags of the checksum tile-columns live in front of the expected-checksum matrix (one int per 32-row slab and
-// checksum tile-column: 128 KiB for the 128 x 32 tile at 16384^2)
+// checksum tile-column: 128 KiB for the 128 x 32 tile at 16384^2); the region grows (in steps of this size) for batches
+// that need more
 constexpr size_t kChkFlagBytes = 1u << 20;
 
 // L2 size assumed by the device-free schedule enumeration (ftsgemm_debug_schedule): H100's 50 MiB
@@ -116,10 +118,13 @@ struct ftsgemm_handle_s {
   size_t chk_bytes = 0;
   float *d_chk_out = nullptr;   // expected checksums M x (tiles_n*8), column-major, + slab flags behind it
   size_t chk_out_bytes = 0;
-  const float *chk_for_b = nullptr;  // B pointer / shape / layout the panel was encoded from
+  size_t chk_flag_bytes = kChkFlagBytes;  // bytes of d_chk_out in front of the expected checksums: the slab flags
+  const float *chk_for_b = nullptr;  // B pointer / shape / layout / batch the panel was encoded from
   int chk_n = 0, chk_k = 0, chk_bn = 0;
   bool chk_b_kmajor = false;
   int chk_ldb = 0;
+  int chk_batch = 1;
+  long long chk_stride_b = 0;
   // fused verdict exchange (ftsgemm_peer_*): this rank's mailbox (kMaxPeers slots), the peers' mailboxes mapped through
   // CUDA IPC, the exit counter of the publishing launches and their sequence number
   double *d_mailbox = nullptr;
@@ -145,7 +150,7 @@ struct ftsgemm_handle_s {
     int *d_off = nullptr;
     bool uploaded = false;
   };
-  std::map<std::array<long long, 6>, CachedPlan> plans;  // key: kernel id, M, N, K, units, forced slices
+  std::map<std::array<long long, 7>, CachedPlan> plans;  // key: kernel id, M, N, K, units, forced slices, batch
   int *d_wave_cnt = nullptr;    // wave re-synchronisation counters (cleared per launch)
   size_t wave_cnt_cap = 0;
   int chk_epoch = 0;
@@ -229,6 +234,23 @@ int make_tmap_kmajor(ftsgemm_handle_t h, CUtensorMap *tm, const float *base, uin
   }
   return FTSGEMM_OK;
 }
+// The same for a strided batch: a third dimension of `batch` entries, entry_stride floats apart (a multiple of 4), and a box of
+// one entry -- so that rows or k beyond one entry's operand are zero-filled, not read from the next entry.
+int make_tmap_kmajor_batched(ftsgemm_handle_t h, CUtensorMap *tm, const float *base, uint64_t rows, uint64_t K, uint64_t ldk,
+                             uint64_t entry_stride, uint64_t batch, uint32_t box_rows) {
+  cuuint64_t dims[3] = {K, rows, batch};
+  cuuint64_t strides[2] = {ldk * sizeof(float), entry_stride * sizeof(float)};
+  cuuint32_t box[3] = {kBK, box_rows, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = h->encode_tiled(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float *>(base), dims, strides, box,
+                               estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    h->last_cuda_error = static_cast<int>(r);
+    return FTSGEMM_ERR_CUDA;
+  }
+  return FTSGEMM_OK;
+}
 
 // Largest grid (in work units of CG CTAs) of this instantiation whose CTAs can all be resident at once: one CTA per SM the
 // device reports (multiProcessorCount, which an MPS active-thread percentage reduces), at most as many two-CTA clusters as
@@ -273,12 +295,12 @@ int query_max_units(ftsgemm_handle_t h, int *out) {
   return FTSGEMM_OK;
 }
 
-template <int BN, bool FT, int CG, bool PROT, bool SEED, bool BIAS>
+template <int BN, bool FT, int CG, bool PROT, bool SEED, bool BIAS, bool BATCH>
 int launch_tc(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
               const KernelParams &p, int units, cudaStream_t stream) {
   // p.pdl_wait: the launch may overlap the tail of its predecessor in the stream (KernelParams::pdl_wait)
   using Cfg = TileCfg<BN, FT, CG>;
-  auto kern = ftsgemm_tc_kernel<BN, FT, CG, PROT, SEED, BIAS>;
+  auto kern = ftsgemm_tc_kernel<BN, FT, CG, PROT, SEED, BIAS, BATCH>;
   int resident = 0;
   const int qrc = query_max_units<BN, FT, CG, PROT>(h, &resident);
   if (qrc) return qrc;
@@ -309,20 +331,24 @@ int launch_tc(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB
   return FTSGEMM_OK;
 }
 
-template <int BN, int CG, bool SEED, bool BIAS>
+template <int BN, int CG, bool SEED, bool BIAS, bool BATCH>
 int launch_ft(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
               const KernelParams &p, int units, cudaStream_t stream, bool ft, bool prot) {
-  if (!ft) return launch_tc<BN, false, CG, false, SEED, BIAS>(h, tmA, tmB, tmC, p, units, stream);
-  if (prot) return launch_tc<BN, true, CG, true, SEED, BIAS>(h, tmA, tmB, tmC, p, units, stream);
-  return launch_tc<BN, true, CG, false, SEED, BIAS>(h, tmA, tmB, tmC, p, units, stream);
+  if (!ft) return launch_tc<BN, false, CG, false, SEED, BIAS, BATCH>(h, tmA, tmB, tmC, p, units, stream);
+  if (prot) return launch_tc<BN, true, CG, true, SEED, BIAS, BATCH>(h, tmA, tmB, tmC, p, units, stream);
+  return launch_tc<BN, true, CG, false, SEED, BIAS, BATCH>(h, tmA, tmB, tmC, p, units, stream);
 }
 
-// (a bias selects the BIAS instantiation: KernelParams::bias, ftsgemm_tc_kernel)
+// (a bias selects the BIAS instantiation: KernelParams::bias, ftsgemm_tc_kernel; a batch of more than one entry the BATCH one)
 template <int BN, int CG, bool SEED>
 int launch_variant(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
                    const KernelParams &p, int units, cudaStream_t stream, bool ft, bool prot) {
-  if (p.bias_mode != kBiasNone) return launch_ft<BN, CG, SEED, true>(h, tmA, tmB, tmC, p, units, stream, ft, prot);
-  return launch_ft<BN, CG, SEED, false>(h, tmA, tmB, tmC, p, units, stream, ft, prot);
+  if (p.batch > 1) {
+    if (p.bias_mode != kBiasNone) return launch_ft<BN, CG, SEED, true, true>(h, tmA, tmB, tmC, p, units, stream, ft, prot);
+    return launch_ft<BN, CG, SEED, false, true>(h, tmA, tmB, tmC, p, units, stream, ft, prot);
+  }
+  if (p.bias_mode != kBiasNone) return launch_ft<BN, CG, SEED, true, false>(h, tmA, tmB, tmC, p, units, stream, ft, prot);
+  return launch_ft<BN, CG, SEED, false, false>(h, tmA, tmB, tmC, p, units, stream, ft, prot);
 }
 
 // Planner input for one launch (tile grid already set by plan_tiles).
@@ -342,12 +368,14 @@ PlanInput make_plan_input(int max_units, int CG, int BN, int K, const KernelPara
   long long units = dbg("grid", 0);
   in.units = (units > 0 && units <= max_units) ? static_cast<int>(units) : max_units;
   in.chk_slices = p.chk_slices > 1 ? p.chk_slices : 1;
-  in.n_chk_tiles = p.tiles_c * p.tiles_m * in.chk_slices;
-  in.n_data_tiles = p.tiles_m * p.tiles_n;
+  // a strided batch is one tile space: its checksum tile-columns stack the row blocks of all entries (decode_tile_batched)
+  in.n_chk_tiles = p.tiles_c * p.tiles_m * p.batch * in.chk_slices;
+  in.n_data_tiles = p.tiles_m * p.tiles_n * p.batch;
   in.num_kb = (K + kBK - 1) / kBK;
-  in.tiles_m = p.tiles_m;
+  in.tiles_m = p.tiles_m * p.batch;
   // operands larger than ~3/4 of the L2 (A and B panels cannot stay resident while the units stream them): keep the units
-  // in k-lockstep (plan.h)
+  // in k-lockstep (plan.h).  In a batch one entry's footprint counts: units running at the same time work on neighbouring
+  // entries.
   const long long lock = dbg("lockstep", -2);
   in.lockstep = lock >= 0 ? static_cast<int>(lock)
                           : (4.0 * K * (static_cast<double>(p.M) + p.N) > 0.75 * static_cast<double>(l2_bytes) ? 1 : 0);
@@ -383,8 +411,9 @@ int choose_chk_slices(const KernelParams &p, int units, int K) {
   int s = 1;
   if (forced >= 1) s = static_cast<int>(forced);
   else {
-    const int spare = units - p.tiles_m * p.tiles_n;
-    if (spare >= 2 * p.tiles_m) s = spare / p.tiles_m;
+    const long long rows = static_cast<long long>(p.tiles_m) * p.batch;  // (the tiles of all entries of a batch)
+    const long long spare = units - rows * p.tiles_n;
+    if (spare >= 2 * rows) s = static_cast<int>(spare / rows);
     if (s > 4) s = 4;
   }
   while (s > 1 && num_kb / s < 8) --s;
@@ -424,16 +453,26 @@ struct Operand {
   int ld;
 };
 
+// The entries of a strided batch (ftsgemm_run_batched): their number and the element strides of A, B and C between them.
+struct BatchArg {
+  int count;
+  long long sa, sb, sc;
+};
+const BatchArg kSingle = {1, 0, 0, 0};
+
 int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC, int ldc,
-           float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o, cudaStream_t stream) {
+           float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o, cudaStream_t stream,
+           const BatchArg &bt = kSingle) {
   const int BN = v.bn, CG = v.cg;
   const bool ft = v.info.fault_tolerant != 0;
   const float *dA = A.p, *dB = B.p;
+  const bool batched = bt.count > 1;  // (one entry runs the kernels without BATCH, on 2-D tensor maps)
   if ((M % 4) || (N % 4)) return FTSGEMM_ERR_UNSUPPORTED;  // TMA global strides must be multiples of 16 bytes
   if ((A.ld % 4) || (B.ld % 4)) return FTSGEMM_ERR_INVALID_ARG;  // (the same for the rows of an operand)
   // work-plan items carry k-block indices in 16 bits and tile indices in 31; the trace / wave tables are sized per unit
   if ((K + kBK - 1) / kBK > 65535) return FTSGEMM_ERR_UNSUPPORTED;
-  if ((static_cast<long long>(M + kBM * CG - 1) / (kBM * CG)) * ((N + BN - 1) / BN) > (1ll << 28)) return FTSGEMM_ERR_UNSUPPORTED;
+  if ((static_cast<long long>(M + kBM * CG - 1) / (kBM * CG)) * ((N + BN - 1) / BN) * bt.count > (1ll << 28)) return FTSGEMM_ERR_UNSUPPORTED;
+  if (static_cast<long long>(M) * bt.count > 0x7fffffffll) return FTSGEMM_ERR_UNSUPPORTED;  // stacked rows are ints
   if ((reinterpret_cast<uintptr_t>(dA) | reinterpret_cast<uintptr_t>(dB) | reinterpret_cast<uintptr_t>(dC)) & 15)
     return FTSGEMM_ERR_INVALID_ARG;
 
@@ -443,6 +482,12 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
   p.C = dC; p.ldc = ldc;
   p.alpha = alpha; p.beta = beta;
   p.bias = bias; p.bias_mode = bias_mode;
+  p.batch = bt.count;
+  if (batched) {
+    p.stride_a = bt.sa;
+    p.stride_b = bt.sb;
+    p.stride_c = bt.sc;
+  }
   plan_tiles(M, N, BN, CG, ft, &p);
   p.tau_abs = o.tau_abs > 0 ? o.tau_abs : 1e-3f;
   p.tau_rel = o.tau_rel > 0 ? o.tau_rel : 1e-5f;  // DESIGN.md section 5
@@ -481,23 +526,29 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
   bool enc_front = false;
   int rc;
   p.ldk = (K + 3) / 4 * 4;
+  // (a batch: 3-D maps with the entry as the outer dimension; the copies hold one dense rows x ldk block per entry)
+  auto tmap = [&](CUtensorMap *tm, const float *base, int rows, int ld, long long entry_stride, int box_rows) {
+    if (!batched) return make_tmap_kmajor(h, tm, base, rows, K, ld, box_rows);
+    return make_tmap_kmajor_batched(h, tm, base, rows, K, ld, entry_stride, bt.count, box_rows);
+  };
+  const long long a_copy = static_cast<long long>(M) * p.ldk, b_copy = static_cast<long long>(N) * p.ldk;
   if (A.kmajor) {
-    rc = make_tmap_kmajor(h, &tmA, dA, M, K, A.ld, kBM);
+    rc = tmap(&tmA, dA, M, A.ld, bt.sa, kBM);
   } else {
-    rc = ensure_buf(h, &h->d_at, &h->at_bytes, static_cast<size_t>(M) * p.ldk * sizeof(float));
+    rc = ensure_buf(h, &h->d_at, &h->at_bytes, static_cast<size_t>(a_copy) * bt.count * sizeof(float));
     if (rc) return rc;
     p.At = h->d_at;
-    rc = make_tmap_kmajor(h, &tmA, p.At, M, K, p.ldk, kBM);
+    rc = tmap(&tmA, p.At, M, p.ldk, a_copy, kBM);
   }
   if (rc) return rc;
   // CG = 2: each CTA of a unit loads BN/2 rows of the B tile and multicasts them to both
   if (B.kmajor) {
-    rc = make_tmap_kmajor(h, &tmB, dB, N, K, B.ld, BN / CG);
+    rc = tmap(&tmB, dB, N, B.ld, bt.sb, BN / CG);
   } else {
-    rc = ensure_buf(h, &h->d_bt, &h->bt_bytes, static_cast<size_t>(N) * p.ldk * sizeof(float));
+    rc = ensure_buf(h, &h->d_bt, &h->bt_bytes, static_cast<size_t>(b_copy) * bt.count * sizeof(float));
     if (rc) return rc;
     p.Bt = h->d_bt;
-    rc = make_tmap_kmajor(h, &tmB, p.Bt, N, K, p.ldk, BN / CG);
+    rc = tmap(&tmB, p.Bt, N, p.ldk, b_copy, BN / CG);
   }
   if (rc) return rc;
   tmC = tmB;
@@ -506,32 +557,42 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
     p.dbg_flags = static_cast<int>(dbg("ft_dbg", 0)) & 1;
     // the checksum operand is K-major like B^T: n_chk_cols rows of K (row stride ldk)
     const int chk_ld = p.ldk;
-    const int n_slabs = p.tiles_m * CG * (kBM / 32);
+    // (a batch: one checksum operand, one block of expected checksums and one run of slab flags per entry)
+    const int n_slabs = p.tiles_m * CG * (kBM / 32) * bt.count;
+    const long long chk_entry = static_cast<long long>(p.n_chk_cols) * chk_ld;
     const float *chk_before = h->d_chk;
-    rc = ensure_buf(h, &h->d_chk, &h->chk_bytes, static_cast<size_t>(p.n_chk_cols) * chk_ld * sizeof(float));
+    rc = ensure_buf(h, &h->d_chk, &h->chk_bytes, static_cast<size_t>(chk_entry) * bt.count * sizeof(float));
     if (rc) return rc;
     if (h->d_chk != chk_before) h->chk_for_b = nullptr;  // reallocated: the cached encode is gone
-    const size_t out_floats = static_cast<size_t>(M) * p.n_chk_cols;
+    const size_t out_floats = static_cast<size_t>(M) * p.n_chk_cols * bt.count;
     const size_t n_flags = static_cast<size_t>(n_slabs) * p.tiles_c;
+    if (n_flags * sizeof(int) > h->chk_flag_bytes) {
+      // grow the flag region: a new buffer, so that its flags are cleared and the epoch restarts below
+      h->chk_flag_bytes = (n_flags * sizeof(int) + kChkFlagBytes - 1) / kChkFlagBytes * kChkFlagBytes;
+      FT_CUDA(h, cudaFree(h->d_chk_out));
+      h->d_chk_out = nullptr;
+      h->chk_out_bytes = 0;
+    }
+    const size_t flag_bytes = h->chk_flag_bytes;
     const float *out_before = h->d_chk_out;
-    rc = ensure_buf(h, &h->d_chk_out, &h->chk_out_bytes, kChkFlagBytes + out_floats * sizeof(float));
+    rc = ensure_buf(h, &h->d_chk_out, &h->chk_out_bytes, flag_bytes + out_floats * sizeof(float));
     if (rc) return rc;
-    if (n_flags * sizeof(int) > kChkFlagBytes) return FTSGEMM_ERR_UNSUPPORTED;
     p.chk_flags = reinterpret_cast<int *>(h->d_chk_out);  // fixed location: stale flags never equal a new epoch
-    p.chk_out = h->d_chk_out + kChkFlagBytes / sizeof(float);
+    p.chk_out = h->d_chk_out + flag_bytes / sizeof(float);
     if (h->d_chk_out != out_before || h->chk_epoch > (1 << 30)) {
-      FT_CUDA(h, cudaMemsetAsync(p.chk_flags, 0, kChkFlagBytes, stream));
+      FT_CUDA(h, cudaMemsetAsync(p.chk_flags, 0, flag_bytes, stream));
       h->chk_epoch = 0;
     }
     p.chk_epoch = ++h->chk_epoch;
     p.dbg_flags = static_cast<int>(dbg("ft_dbg", 0)) & 1;
     // (the same pointer read in another layout or with another row stride is another B)
     const bool reuse = o.reuse_b_checksums && h->chk_for_b == dB && h->chk_n == N && h->chk_k == K && h->chk_bn == BN &&
-                       h->chk_b_kmajor == B.kmajor && h->chk_ldb == B.ld;
+                       h->chk_b_kmajor == B.kmajor && h->chk_ldb == B.ld && h->chk_batch == bt.count &&
+                       h->chk_stride_b == (batched ? bt.sb : 0);
     // Default: the encode is part of the FRONT PHASE of the GEMM kernel (KernelParams::enc_front) -- one launch per fused
     // GEMM, like the reference (sgemm.cu:191-192); only below ~8 MB of B the stand-alone pre-pass is used.
     const long long ef = dbg("enc_front", -2);
-    enc_front = !reuse && (ef >= 0 ? ef != 0 : 4.0 * N * static_cast<double>(K) >= static_cast<double>(dbg("enc_front_min_mb", 8)) * 1048576.0);
+    enc_front = !reuse && (ef >= 0 ? ef != 0 : 4.0 * N * static_cast<double>(K) * bt.count >= static_cast<double>(dbg("enc_front_min_mb", 8)) * 1048576.0);
     if (enc_front) {
       p.enc_front = 1;
       p.enc_out = h->d_chk;
@@ -566,13 +627,46 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
     else if (stream_b) FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_b_kernel<bn, 8, true>, eb, en, ek, eld, eo, el, er, et));  \
     else FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_b_kernel<bn, 8, false>, eb, en, ek, eld, eo, el, er, et));               \
   }
-      FT_ENC(32) FT_ENC(64) FT_ENC(128) FT_ENC(256)
+#define FT_ENC_BATCHED(bn)                                                                                                  \
+  if (BN == bn) {                                                                                                           \
+    cudaLaunchConfig_t ec = {};                                                                                             \
+    ec.gridDim = dim3(std::max(1, grid / bt.count), std::min(bt.count, 65535));                                             \
+    ec.blockDim = dim3(kEncWarps * 32);                                                                                     \
+    ec.stream = stream;                                                                                                     \
+    cudaLaunchAttribute ea[1];                                                                                              \
+    ea[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                                                          \
+    ea[0].val.programmaticStreamSerializationAllowed = 1;                                                                   \
+    ec.attrs = ea;                                                                                                          \
+    ec.numAttrs = chain ? 1 : 0;                                                                                            \
+    const float *eb = dB;                                                                                                   \
+    float *eo = h->d_chk;                                                                                                   \
+    int en = N, ek = K, eld = B.ld, el = chk_ld, er = rounding, et = p.tiles_n, ebt = bt.count;                             \
+    long long esb = bt.sb, ecs = chk_entry;                                                                                 \
+    if (B.kmajor)                                                                                                           \
+      FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_batched_kernel<bn, true>, eb, en, ek, eld, esb, ebt, eo, el, ecs, er, et));  \
+    else if (small_items)                                                                                                   \
+      FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_batched_kernel<bn, false, 4, false>, eb, en, ek, eld, esb, ebt, eo, el, ecs, er, et)); \
+    else if (stream_b)                                                                                                      \
+      FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_batched_kernel<bn, false, 8, true>, eb, en, ek, eld, esb, ebt, eo, el, ecs, er, et)); \
+    else                                                                                                                    \
+      FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_batched_kernel<bn, false>, eb, en, ek, eld, esb, ebt, eo, el, ecs, er, et)); \
+  }
+      // (a batch: one launch for all entries, 2-D grid)
+      if (batched) {
+        FT_ENC_BATCHED(32) FT_ENC_BATCHED(64) FT_ENC_BATCHED(128) FT_ENC_BATCHED(256)
+      } else {
+        FT_ENC(32) FT_ENC(64) FT_ENC(128) FT_ENC(256)
+      }
       ++h->launch_count;
 #undef FT_ENC
+#undef FT_ENC_BATCHED
       FT_CUDA(h, cudaGetLastError());
     }
-    if (!reuse) { h->chk_for_b = dB; h->chk_n = N; h->chk_k = K; h->chk_bn = BN; h->chk_b_kmajor = B.kmajor; h->chk_ldb = B.ld; }
-    rc = make_tmap_kmajor(h, &tmC, h->d_chk, p.n_chk_cols, K, chk_ld, BN / CG);
+    if (!reuse) {
+      h->chk_for_b = dB; h->chk_n = N; h->chk_k = K; h->chk_bn = BN; h->chk_b_kmajor = B.kmajor; h->chk_ldb = B.ld;
+      h->chk_batch = bt.count; h->chk_stride_b = batched ? bt.sb : 0;
+    }
+    rc = tmap(&tmC, h->d_chk, p.n_chk_cols, chk_ld, chk_entry, BN / CG);
     if (rc) return rc;
   }
   // ---- work plan (plan.h), cached per shape on the handle
@@ -588,26 +682,28 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
   }
   if (ft) {
     p.chk_slices = choose_chk_slices(p, max_units, K);
-    const size_t n_flags_s = static_cast<size_t>(p.tiles_m) * CG * (kBM / 32) * p.tiles_c * p.chk_slices;
-    if (p.chk_slices > 1 && n_flags_s * sizeof(int) > kChkFlagBytes) p.chk_slices = 1;
+    const size_t flag_bytes = h->chk_flag_bytes;
+    const size_t n_flags_s = static_cast<size_t>(p.tiles_m) * CG * (kBM / 32) * p.tiles_c * p.chk_slices * bt.count;
+    if (p.chk_slices > 1 && n_flags_s * sizeof(int) > flag_bytes) p.chk_slices = 1;
     if (p.chk_slices > 1) {
-      // one plane of expected checksums per slice
-      const size_t out_floats = static_cast<size_t>(M) * p.n_chk_cols * p.chk_slices;
+      // one plane of expected checksums per slice (and entry)
+      const size_t out_floats = static_cast<size_t>(M) * p.n_chk_cols * p.chk_slices * bt.count;
       const float *out_before = h->d_chk_out;
-      rc = ensure_buf(h, &h->d_chk_out, &h->chk_out_bytes, kChkFlagBytes + out_floats * sizeof(float));
+      rc = ensure_buf(h, &h->d_chk_out, &h->chk_out_bytes, flag_bytes + out_floats * sizeof(float));
       if (rc) return rc;
       if (h->d_chk_out != out_before) {  // reallocated: fresh flags, restart the epoch
-        FT_CUDA(h, cudaMemsetAsync(h->d_chk_out, 0, kChkFlagBytes, stream));
+        FT_CUDA(h, cudaMemsetAsync(h->d_chk_out, 0, flag_bytes, stream));
         h->chk_epoch = 1;
         p.chk_epoch = 1;
       }
       p.chk_flags = reinterpret_cast<int *>(h->d_chk_out);
-      p.chk_out = h->d_chk_out + kChkFlagBytes / sizeof(float);
+      p.chk_out = h->d_chk_out + flag_bytes / sizeof(float);
     }
   }
   const PlanInput pin = make_plan_input(max_units, CG, BN, K, p, h->l2_bytes);
-  const std::array<long long, 6> key = {v.info.id, M, N, K, pin.units,
-                                        pin.force_slices * 16 + pin.max_slices + pin.lockstep * 8192 + pin.full_search * 16384 + pin.chk_slices * 65536};
+  const std::array<long long, 7> key = {v.info.id, M, N, K, pin.units,
+                                        pin.force_slices * 16 + pin.max_slices + pin.lockstep * 8192 + pin.full_search * 16384 + pin.chk_slices * 65536,
+                                        bt.count};
   ftsgemm_handle_s::CachedPlan &cp = h->plans[key];
   if (!cp.uploaded) {
     if (h->plans.size() > 64) {  // bound the cache: drop everything but this entry
@@ -736,14 +832,18 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
 }
 
 int run_cublas(ftsgemm_handle_t h, bool tf32, int M, int N, int K, const Operand &A, const Operand &B, float *dC, int ldc,
-               float alpha, float beta, cudaStream_t stream) {
+               float alpha, float beta, cudaStream_t stream, const BatchArg &bt = kSingle) {
   FT_CUBLAS(h, cublasSetStream(h->cublas, stream));
   FT_CUBLAS(h, cublasSetPointerMode(h->cublas, CUBLAS_POINTER_MODE_HOST));
   FT_CUBLAS(h, cublasSetMathMode(h->cublas, tf32 ? CUBLAS_TF32_TENSOR_OP_MATH : CUBLAS_DEFAULT_MATH));
   // C = A B^T on column-major buffers: the reference layout is NT, as the reference's verification call (sgemm.cu:108); a
   // K-major A is an M x K matrix stored transposed (OP_T), a K-major B is the K x N matrix B^T itself (OP_N)
-  FT_CUBLAS(h, cublasSgemm(h->cublas, A.kmajor ? CUBLAS_OP_T : CUBLAS_OP_N, B.kmajor ? CUBLAS_OP_N : CUBLAS_OP_T, M, N, K, &alpha,
-                           A.p, A.ld, B.p, B.ld, &beta, dC, ldc));
+  if (bt.count > 1)  // the same transpose flags, one strided-batched call
+    FT_CUBLAS(h, cublasSgemmStridedBatched(h->cublas, A.kmajor ? CUBLAS_OP_T : CUBLAS_OP_N, B.kmajor ? CUBLAS_OP_N : CUBLAS_OP_T, M, N,
+                                           K, &alpha, A.p, A.ld, bt.sa, B.p, B.ld, bt.sb, &beta, dC, ldc, bt.sc, bt.count));
+  else
+    FT_CUBLAS(h, cublasSgemm(h->cublas, A.kmajor ? CUBLAS_OP_T : CUBLAS_OP_N, B.kmajor ? CUBLAS_OP_N : CUBLAS_OP_T, M, N, K, &alpha,
+                             A.p, A.ld, B.p, B.ld, &beta, dC, ldc));
   h->last_stream = stream;
   return FTSGEMM_OK;
 }
@@ -773,6 +873,18 @@ __global__ void split_lo_strided_kernel(const float *__restrict__ x, size_t ldx,
     const size_t o = i / inner, r = i - o * inner;
     const float v = __ldg(x + o * ldx + r);
     lo[o * ldlo + r] = v - __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
+  }
+}
+
+// 3xTF32 of a strided batch: entry e of x (`outer` rows of `inner` elements, row stride ldx, entry stride sx) -> its lo part
+// at lo + e * outer * ldlo (row stride ldlo)
+__global__ void split_lo_batched_kernel(const float *__restrict__ x, size_t ldx, long long sx, float *__restrict__ lo, size_t ldlo,
+                                        int inner, size_t outer, int batch) {
+  const size_t per = outer * inner, n = per * batch;
+  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+    const size_t e = i / per, j = i - e * per, o = j / inner, r = j - o * inner;
+    const float v = __ldg(x + static_cast<long long>(e) * sx + o * ldx + r);
+    lo[(e * outer + o) * ldlo + r] = v - __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
   }
 }
 
@@ -874,13 +986,15 @@ int ftsgemm_kernel_lookup(int kernel_id, ftsgemm_kernel_info *out) {
 // Enumerate the work decomposition of one launch on the HOST (same inline code the device runs): for every work unit,
 // in processing order, rows of 9 ints {unit, tile, is_chk, m_blk, n_blk, kb_begin, kb_end, kind, slice}.  Returns the
 // number of rows (fills min(cap, rows)); hdr[0..7] = {units, num_tiles, n_chk_tiles, sk_tiles, num_kb, cta_group, sk_slices, chk_slices}.
-int ftsgemm_debug_schedule(int kernel_id, int M, int N, int K, int num_sms, int *hdr, int *rows, int cap) {
+// rows of `width` ints: the 9 of ftsgemm_debug_schedule, then (width 10) the entry
+static int debug_schedule_rows(int kernel_id, int M, int N, int K, int batch, int num_sms, int *hdr, int *rows, int cap, int width) {
   const Variant *v = find_variant(kernel_id);
-  if (!v || v->info.engine != 1 || M <= 0 || N <= 0 || K <= 0 || num_sms <= 0) return FTSGEMM_ERR_INVALID_ARG;
-  if (v->bn == 0) v = find_variant(select_variant(M, N, v->info.fault_tolerant != 0));
+  if (!v || v->info.engine != 1 || M <= 0 || N <= 0 || K <= 0 || batch <= 0 || num_sms <= 0) return FTSGEMM_ERR_INVALID_ARG;
+  if (v->bn == 0) v = find_variant(select_variant(M, N, v->info.fault_tolerant != 0, batch));
   KernelParams p;
   memset(&p, 0, sizeof(p));
   p.M = M; p.N = N; p.K = K;
+  p.batch = batch;
   plan_tiles(M, N, v->bn, v->cg, v->info.fault_tolerant != 0, &p);
   if (v->info.fault_tolerant) {
     p.chk_slices = choose_chk_slices(p, num_sms / v->cg, K);
@@ -896,15 +1010,24 @@ int ftsgemm_debug_schedule(int kernel_id, int M, int N, int K, int num_sms, int 
     for (int i = plan.offsets[u]; i < plan.offsets[u + 1]; ++i) {
       const PlanItem &it = plan.items[i];
       if (rows && n < cap) {
-        const TileCoord tc = decode_tile(p, it.tile);
-        int *r = rows + 9 * n;
+        const TileCoord tc = width > 9 ? decode_tile_batched(p, it.tile) : decode_tile(p, it.tile);
+        int *r = rows + width * n;
         r[0] = u; r[1] = it.tile; r[2] = tc.is_chk ? 1 : 0; r[3] = tc.m_blk; r[4] = tc.n_blk;
         r[5] = it.kb_begin; r[6] = it.kb_end; r[7] = it.kind; r[8] = it.slice;
+        if (width > 9) r[9] = tc.batch;
       }
       ++n;
     }
   }
   return n;
+}
+
+int ftsgemm_debug_schedule(int kernel_id, int M, int N, int K, int num_sms, int *hdr, int *rows, int cap) {
+  return debug_schedule_rows(kernel_id, M, N, K, 1, num_sms, hdr, rows, cap, 9);
+}
+
+int ftsgemm_debug_schedule_batched(int kernel_id, int M, int N, int K, int batch, int num_sms, int *hdr, int *rows, int cap) {
+  return debug_schedule_rows(kernel_id, M, N, K, batch, num_sms, hdr, rows, cap, 10);
 }
 
 int ftsgemm_debug_trace(ftsgemm_handle_t h, unsigned long long *out, int cap_u64) {
@@ -1032,8 +1155,16 @@ int ftsgemm_run_ex(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const
 int ftsgemm_run_bias(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
                      const float *dB, int layout_b, int ldb, float *dC, int ldc, float alpha, float beta, const float *bias,
                      int bias_mode, const ftsgemm_opts *opts) {
+  return ftsgemm_run_batched(h, kernel_id, M, N, K, dA, layout_a, lda, 0, dB, layout_b, ldb, 0, dC, ldc, 0, 1, alpha, beta, bias,
+                             bias_mode, opts);
+}
+
+int ftsgemm_run_batched(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
+                        long long stride_a, const float *dB, int layout_b, int ldb, long long stride_b, float *dC, int ldc,
+                        long long stride_c, int batch, float alpha, float beta, const float *bias, int bias_mode,
+                        const ftsgemm_opts *opts) {
   if (!h) return FTSGEMM_ERR_NO_DEVICE;
-  if (!dA || !dB || !dC || M <= 0 || N <= 0 || K <= 0) return FTSGEMM_ERR_INVALID_ARG;
+  if (!dA || !dB || !dC || M <= 0 || N <= 0 || K <= 0 || batch < 1) return FTSGEMM_ERR_INVALID_ARG;
   const Variant *v = find_variant(kernel_id);
   if (!v) return FTSGEMM_ERR_INVALID_ARG;
   if ((layout_a != FTSGEMM_LAYOUT_MN_MAJOR && layout_a != FTSGEMM_LAYOUT_K_MAJOR) ||
@@ -1045,13 +1176,22 @@ int ftsgemm_run_bias(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, con
   if (bias_mode == FTSGEMM_BIAS_NONE) bias = nullptr;
   else if (!bias || (reinterpret_cast<uintptr_t>(bias) & 3)) return FTSGEMM_ERR_INVALID_ARG;
   if (bias && v->info.engine != 1) return FTSGEMM_ERR_UNSUPPORTED;  // the bias is fused into the wgmma kernels' store pass only
+  // A batch of one entry is the single product (strides ignored).  Otherwise the wgmma kernels need 16-byte entry strides
+  // (TMA global strides, the 16-byte aligned C of the store passes), C entries that do not overlap, and no broadcast entry.
+  const BatchArg bt = batch > 1 ? BatchArg{batch, stride_a, stride_b, stride_c} : kSingle;
+  if (batch > 1 && v->info.engine == 2) return FTSGEMM_ERR_UNSUPPORTED;  // the baseline has no batched form
+  if (batch > 1 && v->info.engine == 1) {
+    if (stride_a <= 0 || stride_b <= 0 || stride_c <= 0 || (stride_a % 4) || (stride_b % 4) || (stride_c % 4))
+      return FTSGEMM_ERR_INVALID_ARG;
+    if (stride_c < static_cast<long long>(ldc) * N) return FTSGEMM_ERR_INVALID_ARG;
+  }
   ftsgemm_opts o;
   const int orc = load_opts(opts, &o);
   if (orc) return orc;
   DeviceGuard guard(h);
   cudaStream_t stream = static_cast<cudaStream_t>(o.stream);
-  if (v->info.engine == 1 && v->bn == 0) {  // ids 20 / 40: per-shape choice
-    v = find_variant(select_variant(M, N, v->info.fault_tolerant != 0));
+  if (v->info.engine == 1 && v->bn == 0) {  // ids 20 / 40: per-shape choice (over the tiles of all entries)
+    v = find_variant(select_variant(M, N, v->info.fault_tolerant != 0, bt.count));
     if (!v) return FTSGEMM_ERR_UNSUPPORTED;
   }
   if (v->info.engine == 1 && o.check_segments > 1 && v->info.fault_tolerant) {
@@ -1074,8 +1214,10 @@ int ftsgemm_run_bias(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, con
       const size_t oa = A.kmajor ? static_cast<size_t>(k0) : static_cast<size_t>(k0) * lda;
       const size_t ob = B.kmajor ? static_cast<size_t>(k0) : static_cast<size_t>(k0) * ldb;
       const bool last = sg == S - 1;
-      rc = ftsgemm_run_bias(h, v->info.id, M, N, k1 - k0, dA + oa, layout_a, lda, dB + ob, layout_b, ldb, dC, ldc, alpha,
-                            sg == 0 ? beta : 1.0f, last ? bias : nullptr, last ? bias_mode : FTSGEMM_BIAS_NONE, &os);
+      // (a batch: the offsets apply to the base pointers, the entry strides are unchanged)
+      rc = ftsgemm_run_batched(h, v->info.id, M, N, k1 - k0, dA + oa, layout_a, lda, stride_a, dB + ob, layout_b, ldb, stride_b, dC,
+                               ldc, stride_c, batch, alpha, sg == 0 ? beta : 1.0f, last ? bias : nullptr,
+                               last ? bias_mode : FTSGEMM_BIAS_NONE, &os);
     }
     return rc;
   }
@@ -1097,6 +1239,35 @@ int ftsgemm_run_bias(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, con
     Operand Alo = lo_of(A, M), Blo = lo_of(B, N);
     const size_t a_floats = static_cast<size_t>(Alo.ld) * (Alo.kmajor ? M : K);
     const size_t b_floats = static_cast<size_t>(Blo.ld) * (Blo.kmajor ? N : K);
+    if (bt.count > 1) {
+      // a batch: the lo parts of entry e at e * a_floats (e * b_floats), dense in the operand's own layout, from one launch per
+      // operand; then the three passes as batches
+      int rc = ensure_buf(h, &h->d_lo, &h->lo_bytes, (a_floats + b_floats) * bt.count * sizeof(float));
+      if (rc) return rc;
+      float *dAlo = h->d_lo, *dBlo = h->d_lo + a_floats * bt.count;
+      Alo.p = dAlo;
+      Blo.p = dBlo;
+      auto split = [&](const Operand &x, const Operand &lo, int rows, long long sx, float *dst) {
+        const int inner = x.kmajor ? K : rows;
+        const size_t outer = x.kmajor ? rows : K;
+        split_lo_batched_kernel<<<h->num_sms * 8, 256, 0, stream>>>(x.p, x.ld, sx, dst, lo.ld, inner, outer, bt.count);
+      };
+      split(A, Alo, M, bt.sa, dAlo);
+      split(B, Blo, N, bt.sb, dBlo);
+      FT_CUDA(h, cudaGetLastError());
+      h->launch_count += 2;
+      ftsgemm_opts o3 = o;
+      o3.reuse_b_checksums = 0;
+      o3.precision = 0;
+      ftsgemm_opts o_quiet = o3;
+      o_quiet.inject_mode = 0;
+      const BatchArg lo_a = {bt.count, static_cast<long long>(a_floats), bt.sb, bt.sc};
+      const BatchArg lo_b = {bt.count, bt.sa, static_cast<long long>(b_floats), bt.sc};
+      rc = run_tc(h, *v, M, N, K, Alo, B, dC, ldc, alpha, beta, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo_a);
+      if (!rc) rc = run_tc(h, *v, M, N, K, A, Blo, dC, ldc, alpha, 1.0f, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo_b);
+      if (!rc) rc = run_tc(h, *v, M, N, K, A, B, dC, ldc, alpha, 1.0f, bias, bias_mode, o3, stream, bt);
+      return rc;
+    }
     int rc = ensure_buf(h, &h->d_lo, &h->lo_bytes, (a_floats + b_floats) * sizeof(float));
     if (rc) return rc;
     float *dAlo = h->d_lo, *dBlo = h->d_lo + a_floats;
@@ -1127,8 +1298,8 @@ int ftsgemm_run_bias(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, con
     return rc;
   }
   switch (v->info.engine) {
-    case 0: return run_cublas(h, v->info.id == 7, M, N, K, A, B, dC, ldc, alpha, beta, stream);
-    case 1: return run_tc(h, *v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream);
+    case 0: return run_cublas(h, v->info.id == 7, M, N, K, A, B, dC, ldc, alpha, beta, stream, bt);
+    case 1: return run_tc(h, *v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt);
     case 2:
       // the non-fused baseline keeps the reference's call sequence, on the reference layout only
       if (A.kmajor || B.kmajor || lda != M || ldb != N || ldc != M) return FTSGEMM_ERR_UNSUPPORTED;

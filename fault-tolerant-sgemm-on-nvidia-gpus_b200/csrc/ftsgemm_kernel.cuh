@@ -158,6 +158,12 @@ struct KernelParams {
   // MMA start, MMA issue end, epilogue start (accumulator complete), after check/fold, epilogue end}, tile | kind << 24
   unsigned long long *trace;
   int trace_cap;        // items recorded per unit
+  // Strided batch (ftsgemm_run_batched; read by the BATCH instantiations only): `batch` independent products, entry i on
+  // A + i*stride_a, B + i*stride_b, C + i*stride_c (caller's buffers, element strides).  The workspace the kernel owns holds
+  // one dense block per entry: the K-major copies (rows * ldk), the checksum operand (n_chk_cols * enc_ld), the expected
+  // checksums (M * n_chk_cols * chk_slices) and tiles_m * CG * 4 slabs of checksum flags.
+  int batch;
+  long long stride_a, stride_b, stride_c;
 };
 
 __device__ __forceinline__ unsigned long long globaltimer_ns() { return ptx::globaltimer(); }
@@ -195,6 +201,7 @@ __device__ __forceinline__ uint32_t f2u(float f) { return __float_as_uint(f); }
 struct TileCoord {
   int m_blk, n_blk;  // n_blk indexes checksum tile-columns when is_chk
   int slice;         // K-slice of a checksum tile (0 otherwise)
+  int batch;         // entry of a strided batch (decode_tile_batched; 0 otherwise)
   bool is_chk;
 };
 
@@ -203,7 +210,7 @@ struct TileCoord {
 // wave of CTAs shares few A row-panels and few B row-panels in L2.
 __host__ __device__ __forceinline__ TileCoord decode_tile(const KernelParams &p, int t) {
   TileCoord tc;
-  tc.slice = 0;
+  tc.slice = 0;  // (tc.batch is left unset: only the BATCH kernels read it, from decode_tile_batched)
   const int per_slice = p.tiles_c * p.tiles_m;
   const int n_chk_tiles = per_slice * (p.chk_slices > 1 ? p.chk_slices : 1);
   if (t < n_chk_tiles) {
@@ -216,6 +223,40 @@ __host__ __device__ __forceinline__ TileCoord decode_tile(const KernelParams &p,
   }
   t -= n_chk_tiles;
   tc.is_chk = false;
+  const int per_group = p.group_n * p.tiles_m;
+  const int g = t / per_group;
+  const int first_n = g * p.group_n;
+  const int gsz = p.group_n < p.tiles_n - first_n ? p.group_n : p.tiles_n - first_n;
+  const int local = t - g * per_group;
+  tc.n_blk = first_n + local % gsz;
+  tc.m_blk = local / gsz;
+  return tc;
+}
+
+// The tile order of a strided batch: the checksum tiles of all entries first -- per slice and checksum tile-column, the
+// row blocks of all entries stacked (entry-major) -- then the data tiles entry by entry, each entry in the order above.
+// Every wait still points to an earlier item (plan.h); with batch = 1 this is decode_tile.
+__host__ __device__ __forceinline__ TileCoord decode_tile_batched(const KernelParams &p, int t) {
+  TileCoord tc;
+  tc.slice = 0;
+  const int rows = p.batch * p.tiles_m;  // stacked row blocks
+  const int per_slice = p.tiles_c * rows;
+  const int n_chk_tiles = per_slice * (p.chk_slices > 1 ? p.chk_slices : 1);
+  if (t < n_chk_tiles) {
+    tc.is_chk = true;
+    tc.slice = t / (per_slice > 0 ? per_slice : 1);
+    t -= tc.slice * per_slice;
+    const int r = t % rows;
+    tc.n_blk = t / rows;
+    tc.batch = r / p.tiles_m;
+    tc.m_blk = r - tc.batch * p.tiles_m;
+    return tc;
+  }
+  t -= n_chk_tiles;
+  tc.is_chk = false;
+  const int per_entry = p.tiles_m * p.tiles_n;
+  tc.batch = t / per_entry;
+  t -= tc.batch * per_entry;
   const int per_group = p.group_n * p.tiles_m;
   const int g = t / per_group;
   const int first_n = g * p.group_n;
@@ -419,10 +460,11 @@ struct ExpectedChk {
   float e0, e1, w0, w1;
   bool ready;
 };
-__device__ __forceinline__ void load_expected(const KernelParams &p, int m, int n_blk, ExpectedChk &x) {
+// (chk_ofs: the entry's block of expected checksums in a strided batch)
+__device__ __forceinline__ void load_expected(const KernelParams &p, int m, int n_blk, ExpectedChk &x, size_t chk_ofs) {
   x.e0 = x.e1 = x.w0 = x.w1 = 0.0f;
   if (m < p.M) {
-    const float *cp = p.chk_out + static_cast<size_t>(n_blk) * kChkPerTile * p.M + m;
+    const float *cp = p.chk_out + chk_ofs + static_cast<size_t>(n_blk) * kChkPerTile * p.M + m;
     x.e0 = __ldcg(cp);
     x.e1 = __ldcg(cp + p.M);
     x.w0 = __ldcg(cp + 2 * static_cast<size_t>(p.M));
@@ -440,10 +482,22 @@ __device__ __forceinline__ void load_expected(const KernelParams &p, int m, int 
 // number of flags per 32-row slab: checksum tile-columns x K-slices (flag index = slice * tiles_c + c)
 __device__ __forceinline__ int chk_flags_per_slab(const KernelParams &p) { return p.tiles_c * (p.chk_slices > 1 ? p.chk_slices : 1); }
 
-template <int BN>
+// Whether a listed fault at tile row tr of the CTA tile starting at row m0_cta belongs to this entry.  In a strided batch the
+// last row tile of entry i reaches past M, where the stacked rows of entry i+1 begin: those rows are entry i's padding, not
+// the fault's element.  (A single product keeps its previous behaviour.)
+template <bool BATCH>
+__device__ __forceinline__ bool fault_in_entry(const KernelParams &p, int m0_cta, int tr) {
+  if constexpr (BATCH) return m0_cta + tr < p.M;
+  else return true;
+}
+
+template <int BN, bool BATCH = false>
 __device__ __forceinline__ void abft_check(const KernelParams &p, uint32_t taddr, int q, int lane, int m, int m0_cta,
                                            int n0, int n_blk, int &fix_col, float &fix_val, bool &redo, ExpectedChk &xp,
-                                           float &own_s1, int c_mid = BN / 32, uint32_t xchg = 0u, int pair_bar = 0) {
+                                           float &own_s1, int c_mid = BN / 32, uint32_t xchg = 0u, int pair_bar = 0,
+                                           int row_ofs = 0, int slab_ofs = 0, size_t chk_ofs = 0) {
+  // (strided batch: row_ofs = entry * M turns rows into stacked rows for the fault list and the events, slab_ofs / chk_ofs
+  // select the entry's checksum flags and expected checksums; all 0 otherwise)
   // ---- fault injection into the accumulator (reference: ft_sgemm_huge.cuh:324-327) ----
   if (p.inject_mode == 1) {
     if ((p.selftest_row >> 5) == q && p.selftest_col < BN) {
@@ -453,8 +507,9 @@ __device__ __forceinline__ void abft_check(const KernelParams &p, uint32_t taddr
     }
   } else if (p.inject_mode == 2) {
     for (int f = 0; f < p.n_faults; ++f) {
-      const int tr = p.faults[f].row - m0_cta, tc = p.faults[f].col - n0;
-      if (p.faults[f].mode <= 1 && tr >= 0 && tr < kBM && tc >= 0 && tc < BN && (tr >> 5) == q) {  // warp-uniform
+      const int tr = p.faults[f].row - (m0_cta + row_ofs), tc = p.faults[f].col - n0;
+      if (p.faults[f].mode <= 1 && tr >= 0 && tr < kBM && tc >= 0 && tc < BN && (tr >> 5) == q &&
+          fault_in_entry<BATCH>(p, m0_cta, tr)) {  // warp-uniform
         uint32_t x = ptx::acc_ld_x1(taddr + tc);
         if (lane == (tr & 31))
           x = p.faults[f].mode == 0 ? f2u(u2f(x) + p.faults[f].add_value) : (x ^ p.faults[f].xor_mask);
@@ -480,7 +535,7 @@ __device__ __forceinline__ void abft_check(const KernelParams &p, uint32_t taddr
   //      prefetch already found it raised) ----
   if (!xp.ready) {
     const int nf = chk_flags_per_slab(p);
-    const int *flag = p.chk_flags + ((m0_cta >> 5) + q) * nf;
+    const int *flag = p.chk_flags + (slab_ofs + (m0_cta >> 5) + q) * nf;
     if (lane == 0) {
       for (int c = 0; c < nf; ++c) {
         ptx::Watchdog wd;
@@ -491,7 +546,7 @@ __device__ __forceinline__ void abft_check(const KernelParams &p, uint32_t taddr
       }
     }
     __syncwarp();
-    load_expected(p, m, n_blk, xp);
+    load_expected(p, m, n_blk, xp, chk_ofs);
   }
   const float r1 = xp.e0 + xp.e1, r2 = xp.w0 + xp.w1;
   const float d1 = r1 - s1, d2 = r2 - s2;
@@ -598,7 +653,7 @@ __device__ __forceinline__ void abft_check(const KernelParams &p, uint32_t taddr
     const int slot = atomicAdd(&p.stats->n_events, 1);
     if (slot < kMaxEvents) {
       DeviceEvent ev;
-      ev.row = m;
+      ev.row = m + row_ofs;
       ev.col = j >= 0 ? n0 + j : -1;
       ev.residual = d1;
       ev.corrected_value = vc;
@@ -771,7 +826,7 @@ __device__ __forceinline__ void protected_store_body(uint32_t taddr, const float
                                                      int kmajor, int ldc, int N, int K, float alpha, float beta, DeviceStats *stats,
                                                      bool can_recompute, int m, int row0, bool row_ok, int n0, int c_begin, int c_end,
                                                      float chk_s1, bool chk_s1_valid, int bad_col, uint32_t bad_mask, int lane,
-                                                     const float *bias, int bias_mode) {
+                                                     const float *bias, int bias_mode, int row_ofs) {
   const StoreVerdict sv = store_tile_protected<BN, BIAS>(taddr, C + m, row_ok, n0, ldc, alpha, beta, c_begin, c_end, chk_s1, chk_s1_valid,
                                                          bad_col, bad_mask, make_bias(bias, bias_mode, m, BIAS && row_ok));
   unsigned mask = __ballot_sync(0xffffffffu, sv.bad);
@@ -783,7 +838,7 @@ __device__ __forceinline__ void protected_store_body(uint32_t taddr, const float
     const int slot = atomicAdd(&stats->n_events, 1);
     if (slot < kMaxEvents) {
       DeviceEvent ev;
-      ev.row = m;
+      ev.row = m + row_ofs;
       ev.col = -1;
       ev.residual = sv.resid;
       ev.corrected_value = 0.0f;
@@ -814,41 +869,51 @@ __device__ __forceinline__ void protected_store_body(uint32_t taddr, const float
 // the caller's registers around what a callee clobbers: a changed callee moved the spills of the protected instantiations).
 template <int BN>
 __device__ __noinline__ void protected_store_pass(FT_PROT_PARAMS) {
-  protected_store_body<BN, false>(FT_PROT_ARGS, nullptr, kBiasNone);
+  protected_store_body<BN, false>(FT_PROT_ARGS, nullptr, kBiasNone, 0);
 }
 template <int BN>
 __device__ __noinline__ void protected_store_pass_bias(FT_PROT_PARAMS, const float *bias, int bias_mode) {
-  protected_store_body<BN, true>(FT_PROT_ARGS, bias, bias_mode);
+  protected_store_body<BN, true>(FT_PROT_ARGS, bias, bias_mode, 0);
+}
+// strided batch: A, B, C are the entry's, row_ofs = entry * M (events carry stacked rows)
+template <int BN, bool BIAS>
+__device__ __noinline__ void protected_store_pass_batched(FT_PROT_PARAMS, const float *bias, int bias_mode, int row_ofs) {
+  protected_store_body<BN, BIAS>(FT_PROT_ARGS, bias, bias_mode, row_ofs);
 }
 #undef FT_PROT_PARAMS
 #undef FT_PROT_ARGS
-template <int BN, bool BIAS, typename... Args>
-__device__ __forceinline__ void protected_store(const float *bias, int bias_mode, Args... args) {
-  if constexpr (BIAS) protected_store_pass_bias<BN>(args..., bias, bias_mode);
+template <int BN, bool BIAS, bool BATCH, typename... Args>
+__device__ __forceinline__ void protected_store(const float *bias, int bias_mode, int row_ofs, Args... args) {
+  if constexpr (BATCH) protected_store_pass_batched<BN, BIAS>(args..., bias, bias_mode, row_ofs);
+  else if constexpr (BIAS) protected_store_pass_bias<BN>(args..., bias, bias_mode);
   else protected_store_pass<BN>(args...);
 }
 
 // Test injectors for upsets AFTER the accumulator check (ftsgemm_fault.mode 2: into the accumulator before the store pass
 // re-reads it; mode 3: into the value about to be stored -- returns the tile column for this lane, -1 if none).
-template <int BN>
-__device__ __forceinline__ void inject_after_check(const KernelParams &p, uint32_t taddr, int q, int lane, int m0_cta, int n0) {
+// (strided batch: row_ofs = entry * M, fault rows are stacked rows)
+template <int BN, bool BATCH = false>
+__device__ __forceinline__ void inject_after_check(const KernelParams &p, uint32_t taddr, int q, int lane, int m0_cta, int n0,
+                                                   int row_ofs = 0) {
   for (int f = 0; f < p.n_faults; ++f) {
-    const int tr = p.faults[f].row - m0_cta, tc = p.faults[f].col - n0;
-    if (p.faults[f].mode == 2 && tr >= 0 && tr < kBM && tc >= 0 && tc < BN && (tr >> 5) == q) {  // warp-uniform
+    const int tr = p.faults[f].row - (m0_cta + row_ofs), tc = p.faults[f].col - n0;
+    if (p.faults[f].mode == 2 && tr >= 0 && tr < kBM && tc >= 0 && tc < BN && (tr >> 5) == q &&
+        fault_in_entry<BATCH>(p, m0_cta, tr)) {  // warp-uniform
       uint32_t x = ptx::acc_ld_x1(taddr + tc);
       if (lane == (tr & 31)) x ^= p.faults[f].xor_mask;
       ptx::acc_st_x1(taddr + tc, x);
     }
   }
 }
-template <int BN>
+template <int BN, bool BATCH = false>
 __device__ __forceinline__ int stored_value_fault(const KernelParams &p, int q, int lane, int m0_cta, int n0, int c_begin, int c_end,
-                                                  uint32_t &mask) {
+                                                  uint32_t &mask, int row_ofs = 0) {
   int col = -1;
   if (p.inject_mode == 2)
     for (int f = 0; f < p.n_faults; ++f) {
-      const int tr = p.faults[f].row - m0_cta, tc = p.faults[f].col - n0;
-      if (p.faults[f].mode == 3 && tr >= 0 && tr < kBM && (tr >> 5) == q && lane == (tr & 31) && tc >= c_begin * 32 && tc < c_end * 32) {
+      const int tr = p.faults[f].row - (m0_cta + row_ofs), tc = p.faults[f].col - n0;
+      if (p.faults[f].mode == 3 && tr >= 0 && tr < kBM && (tr >> 5) == q && lane == (tr & 31) && tc >= c_begin * 32 && tc < c_end * 32 &&
+          fault_in_entry<BATCH>(p, m0_cta, tr)) {
         col = tc;
         mask = p.faults[f].xor_mask;
       }
@@ -1165,6 +1230,51 @@ __device__ __noinline__ void front_phase_kmajor(const float *A, const float *B, 
   }
 }
 
+// The front phase of a strided batch: the transposes grid-stride over (entry, 32 x 32 block) -- entry i of an MN-major
+// operand at src + i*stride into its dense K-major copy dst + i*rows*ldk -- and the encode runs entry by entry, entry i's
+// checksum operand at enc_out + i*n_chk_cols*enc_ld.  Out of line, like front_phase_kmajor.
+__device__ __forceinline__ void transpose_warp_batched(const float *__restrict__ src, int rows, int K, int ld, long long stride, int batch,
+                                                       float *__restrict__ dst, int ldk, int gw, int nw, int lane, float *tile) {
+  const int rb = (rows + 31) / 32, kb = (K + 31) / 32;
+  const long long per = static_cast<long long>(rb) * kb, total = per * batch;
+  for (long long t = gw; t < total; t += nw) {
+    const long long e = t / per, te = t - e * per;
+    const float *s = src + e * stride;
+    float *d = dst + e * static_cast<long long>(rows) * ldk;
+    const int r0 = static_cast<int>(te % rb) * 32, k0 = static_cast<int>(te / rb) * 32;
+    const int r = r0 + lane;
+#pragma unroll 8
+    for (int j = 0; j < 32; ++j) {
+      const int k = k0 + j;
+      tile[j * 33 + lane] = (r < rows && k < K) ? __ldg(s + static_cast<size_t>(k) * ld + r) : 0.0f;
+    }
+    __syncwarp();
+    const int k = k0 + lane;
+#pragma unroll 8
+    for (int i = 0; i < 32; ++i)
+      if (r0 + i < rows && k < K) d[static_cast<size_t>(r0 + i) * ldk + k] = tile[lane * 33 + i];
+    __syncwarp();
+  }
+}
+// (scalars by value: a reference to the parameter block would force a local copy of all of it)
+template <int BN, bool FT>
+__device__ __noinline__ void front_phase_batched(const float *A, const float *B, int M, int N, int K, int lda, int ldb, int a_kmajor,
+                                                 int b_kmajor, long long stride_a, long long stride_b, int batch, float *At, float *Bt,
+                                                 int ldk, int enc_front, float *enc_out, int enc_ld, int n_chk_cols, int tiles_n, int gw,
+                                                 int nw, int lane, float *tile) {
+  if (!a_kmajor) transpose_warp_batched(A, M, K, lda, stride_a, batch, At, ldk, gw, nw, lane, tile);
+  if (!b_kmajor) transpose_warp_batched(B, N, K, ldb, stride_b, batch, Bt, ldk, gw, nw, lane, tile);
+  if (FT && enc_front) {
+    const long long enc_stride = static_cast<long long>(n_chk_cols) * enc_ld;
+    for (int e = 0; e < batch; ++e) {
+      const float *Be = B + e * stride_b;
+      float *out = enc_out + e * enc_stride;
+      if (b_kmajor) encode_bk_warp<BN>(Be, N, K, ldb, out, enc_ld, 0, tiles_n, gw, nw, lane);
+      else encode_b_warp<BN, 8>(Be, N, K, ldb, out, enc_ld, 0, tiles_n, gw, nw, lane);
+    }
+  }
+}
+
 template <int BN>
 __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
   if constexpr (BN == 32) ptx::wgmma_tf32_n32(d, a_desc, b_desc, scale_d);
@@ -1183,7 +1293,10 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t a_desc, 
 // BIAS: the instantiation for calls with a bias (ftsgemm_run_bias).  A warp-uniform branch into an out-of-line biased store
 // pass raised the spills of every instantiation (the call alone, even where it is never taken), so a bias selects its own
 // binary and the default kernels are compiled exactly as without the feature.
-template <int BN, bool FT, int CG, bool PROT = false, bool SEED = false, bool BIAS = false>
+// BATCH: the instantiation for strided batches (ftsgemm_run_batched with batch > 1): 3-D tensor maps with the entry as the
+// outer coordinate, and every per-tile address offset by the item's entry.  Without it the entry is the constant 0 and
+// the code is that of the kernel before batching existed.
+template <int BN, bool FT, int CG, bool PROT = false, bool SEED = false, bool BIAS = false, bool BATCH = false>
 __global__ void __launch_bounds__(kThreads, 1)
 ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmChk, const KernelParams p) {
@@ -1236,7 +1349,10 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     // front phase: transposes of the MN-major operands (+ the encode of B); the ring is free scratch until the producer starts
     const int gw = static_cast<int>(blockIdx.x) * (kThreads / 32) + warp, nw = static_cast<int>(gridDim.x) * (kThreads / 32);
     float *tile = smem_f + warp * 32 * 33;
-    if ((p.a_kmajor | p.b_kmajor) == 0) {  // the reference layout
+    if constexpr (BATCH) {
+      front_phase_batched<BN, FT>(p.A, p.B, p.M, p.N, p.K, p.lda, p.ldb, p.a_kmajor, p.b_kmajor, p.stride_a, p.stride_b, p.batch, p.At,
+                                  p.Bt, p.ldk, p.enc_front, p.enc_out, p.enc_ld, p.n_chk_cols, p.tiles_n, gw, nw, lane, tile);
+    } else if ((p.a_kmajor | p.b_kmajor) == 0) {  // the reference layout
       transpose_warp(p.A, p.M, p.K, p.lda, p.At, p.ldk, gw, nw, lane, tile);
       transpose_warp(p.B, p.N, p.K, p.ldb, p.Bt, p.ldk, gw, nw, lane, tile);
       if (FT && p.enc_front) encode_b_warp<BN, 8>(p.B, p.N, p.K, p.ldb, p.enc_out, p.enc_ld, 0, p.tiles_n, gw, nw, lane);
@@ -1272,7 +1388,7 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     while (it.next(sg)) {
       ++item_idx;
       if (item_idx > 0) ptx::mbar_wait(ring_free_bar, static_cast<uint32_t>(item_idx - 1) & 1u);
-      const TileCoord tc = decode_tile(p, sg.tile);
+      const TileCoord tc = BATCH ? decode_tile_batched(p, sg.tile) : decode_tile(p, sg.tile);
       const int m0 = (tc.m_blk * CG + cta_rank) * kBM;  // this CTA's 128 rows of A
       const bool b_is_chk = FT && tc.is_chk;
       const bool wave_item = p.wave_cnt != nullptr && sg.kind == 0 && !b_is_chk && cta_rank == 0;
@@ -1300,11 +1416,19 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           if (ptx::elect_one()) {
             // (CG = 2: own A box + own B half + the peer's B half = kStageBytes as well)
             ptx::mbar_arrive_expect_tx(full_bar(stage), static_cast<uint32_t>(Cfg::kStageBytes));
-            ptx::tma_load_2d(sA, &tmA, full_bar(stage), k0, m0);
-            if constexpr (CG == 2)  // B box = BN/2 rows; the 1 KiB-aligned halves give the layout of one BN-row box
-              ptx::tma_load_2d_multicast(sB + cta_rank * (Cfg::kBBytes / 2), tmb, full_bar(stage), k0, nb0 + cta_rank * (BN / 2), 0x3);
-            else
-              ptx::tma_load_2d(sB, tmb, full_bar(stage), k0, nb0);
+            if constexpr (BATCH) {  // (the entry is the outer coordinate of every map, the checksum operand's too)
+              ptx::tma_load_3d(sA, &tmA, full_bar(stage), k0, m0, tc.batch);
+              if constexpr (CG == 2)
+                ptx::tma_load_3d_multicast(sB + cta_rank * (Cfg::kBBytes / 2), tmb, full_bar(stage), k0, nb0 + cta_rank * (BN / 2), tc.batch, 0x3);
+              else
+                ptx::tma_load_3d(sB, tmb, full_bar(stage), k0, nb0, tc.batch);
+            } else {
+              ptx::tma_load_2d(sA, &tmA, full_bar(stage), k0, m0);
+              if constexpr (CG == 2)  // B box = BN/2 rows; the 1 KiB-aligned halves give the layout of one BN-row box
+                ptx::tma_load_2d_multicast(sB + cta_rank * (Cfg::kBBytes / 2), tmb, full_bar(stage), k0, nb0 + cta_rank * (BN / 2), 0x3);
+              else
+                ptx::tma_load_2d(sB, tmb, full_bar(stage), k0, nb0);
+            }
           }
           __syncwarp();
           if (++stage == kStages) {
@@ -1346,10 +1470,20 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     float acc[kAccRegs];
     while (it.next(sg)) {
       ++item_idx;
-      const TileCoord tc = decode_tile(p, sg.tile);
+      const TileCoord tc = BATCH ? decode_tile_batched(p, sg.tile) : decode_tile(p, sg.tile);
       const int m0_cta = (tc.m_blk * CG + cta_rank) * kBM;
       const int n0 = (FT && tc.is_chk) ? tc.n_blk * chk_cols_per_tile(BN) : tc.n_blk * BN;
       const int m = m0_cta + row;
+      // the item's entry of a strided batch (the constant 0 without BATCH: every offset below folds away)
+      const int bt = BATCH ? tc.batch : 0;
+      // (without BATCH the call sites read p.A / p.B / p.C themselves: pointers formed up front, even equal to them, moved the
+      // register allocation of the biased fault-tolerant kernels)
+      const float *const Ab = BATCH ? p.A + bt * p.stride_a : nullptr;
+      const float *const Bb = BATCH ? p.B + bt * p.stride_b : nullptr;
+      float *const Cb = BATCH ? p.C + bt * p.stride_c : nullptr;
+      const int row_ofs = bt * p.M;                           // stacked rows: fault list and events
+      const int slab_ofs = bt * (p.tiles_m * CG * (kBM / 32));  // the entry's checksum flags
+      const size_t chk_ofs = static_cast<size_t>(bt) * p.M * p.n_chk_cols * (p.chk_slices > 1 ? p.chk_slices : 1);
       // the first wgmma of a tile overwrites the accumulator ...
       uint32_t scale_d = 0u;
       // (nothing is in flight here -- the previous item ended with wait_group 0 -- but ptxas only sees that through this
@@ -1438,12 +1572,12 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           }
           if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N) {
             uint32_t bad_bits = 0u;
-            const int bad_col = stored_value_fault<BN>(p, q, lane, m0_cta, n0, kMid, BN / 32, bad_bits);
-            protected_store<BN, BIAS>(p.bias, p.bias_mode, taddr, p.A, p.B, p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
+            const int bad_col = stored_value_fault<BN, BATCH>(p, q, lane, m0_cta, n0, kMid, BN / 32, bad_bits, row_ofs);
+            protected_store<BN, BIAS, BATCH>(p.bias, p.bias_mode, row_ofs, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
                                       p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32,
                                       m < p.M && !skip, n0, kMid, BN / 32, s1, stale == 0u, bad_col, bad_bits, lane);
           } else {
-            store_tile<BN, BIAS>(taddr, p.C + m, m < p.M && !skip, n0, p.N, p.ldc, p.alpha, p.beta, kMid, BN / 32,
+            store_tile<BN, BIAS>(taddr, (BATCH ? Cb : p.C) + m, m < p.M && !skip, n0, p.N, p.ldc, p.alpha, p.beta, kMid, BN / 32,
                                  make_bias(p.bias, p.bias_mode, m, BIAS && m < p.M && !skip));
           }
           ptx::named_bar_sync(4 + q, 64);  // both halves are out of the accumulator
@@ -1455,12 +1589,12 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       } else if (FT && tc.is_chk) {
         // checksum tile-column: publish R = A * [e, w]^T for these 128 rows, then raise the slab flag
         const int n_hi = min(p.n_chk_cols, n0 + chk_cols_per_tile(BN));  // columns beyond belong to the next item
-        store_tile<BN>(taddr, p.chk_out + static_cast<size_t>(tc.slice) * p.M * p.n_chk_cols + m, m < p.M, n0, n_hi, p.M, 1.0f, 0.0f, 0,
-                       (n_hi - n0 + 31) / 32);
+        store_tile<BN>(taddr, p.chk_out + chk_ofs + static_cast<size_t>(tc.slice) * p.M * p.n_chk_cols + m, m < p.M, n0, n_hi, p.M, 1.0f,
+                       0.0f, 0, (n_hi - n0 + 31) / 32);
         __threadfence();
         __syncwarp();
         if (lane == 0)
-          atomicExch(p.chk_flags + ((m0_cta >> 5) + q) * chk_flags_per_slab(p) + tc.slice * p.tiles_c + tc.n_blk, p.chk_epoch);
+          atomicExch(p.chk_flags + (slab_ofs + (m0_cta >> 5) + q) * chk_flags_per_slab(p) + tc.slice * p.tiles_c + tc.n_blk, p.chk_epoch);
       } else {
         // final epilogue of a data tile; with epi_assist the helper warp of this quadrant owns the chunks [kMid, BN/32)
         const int c_mid = assist_on ? kMid : BN / 32;
@@ -1471,7 +1605,8 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         ExpectedChk xp;
         xp.ready = false;
         if (FT && !(p.dbg_flags & 1))
-          abft_check<BN>(p, taddr, q, lane, m, m0_cta, n0, tc.n_blk, fix_col, fix_val, redo, xp, own_s1, c_mid, xchg_base(q), 4 + q);
+          abft_check<BN, BATCH>(p, taddr, q, lane, m, m0_cta, n0, tc.n_blk, fix_col, fix_val, redo, xp, own_s1, c_mid, xchg_base(q), 4 + q,
+                         row_ofs, slab_ofs, chk_ofs);
         // rows to recompute are skipped by both store passes (the helper reads the mask after the pair barrier below)
         const unsigned redo_mask = FT ? __ballot_sync(0xffffffffu, redo) : 0u;
         // rows repaired in the accumulator: the sums of pass 1 no longer describe what a protected store pass re-reads
@@ -1495,17 +1630,17 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             ptx::acc_st_x1(taddr + col, x);
             __syncwarp();
           }
-          if (p.inject_mode == 2) inject_after_check<BN>(p, taddr, q, lane, m0_cta, n0);
+          if (p.inject_mode == 2) inject_after_check<BN, BATCH>(p, taddr, q, lane, m0_cta, n0, row_ofs);
         }
         if (assist_on && FT && !(p.dbg_flags & 1)) ptx::named_bar_sync(4 + q, 64);  // corrections are in place
         if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N) {
           uint32_t bad_bits = 0u;
-          const int bad_col = stored_value_fault<BN>(p, q, lane, m0_cta, n0, 0, c_mid, bad_bits);
-          protected_store<BN, BIAS>(p.bias, p.bias_mode, taddr, p.A, p.B, p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
+          const int bad_col = stored_value_fault<BN, BATCH>(p, q, lane, m0_cta, n0, 0, c_mid, bad_bits, row_ofs);
+          protected_store<BN, BIAS, BATCH>(p.bias, p.bias_mode, row_ofs, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
                                     p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32,
                                     m < p.M && !redo, n0, 0, c_mid, own_s1, ((stale_mask >> lane) & 1u) == 0u, bad_col, bad_bits, lane);
         } else {
-          store_tile<BN, BIAS>(taddr, p.C + m, m < p.M && !redo, n0, p.N, p.ldc, p.alpha, p.beta, 0, c_mid,
+          store_tile<BN, BIAS>(taddr, (BATCH ? Cb : p.C) + m, m < p.M && !redo, n0, p.N, p.ldc, p.alpha, p.beta, 0, c_mid,
                                make_bias(p.bias, p.bias_mode, m, BIAS && m < p.M && !redo));
         }
         if (FT && redo_mask != 0u) {  // rare, warp-uniform: recompute the flagged rows from global memory
@@ -1513,7 +1648,7 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           while (rm != 0u) {
             const int r = __ffs(rm) - 1;
             rm &= rm - 1u;
-            recompute<BN, BIAS>(p.bias, p.bias_mode, p.A, p.B, p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K,
+            recompute<BN, BIAS>(p.bias, p.bias_mode, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K,
                                 p.alpha, p.beta, m0_cta + q * 32 + r, n0, lane);
           }
         }
@@ -1577,6 +1712,24 @@ encode_b_kernel(const float *__restrict__ B, int N, int K, int ldb, float *__res
   ptx::pdl_launch_dependents();  // the GEMM kernel may start its prologue on SMs as they drain (then waits for this grid)
   encode_b_warp<BN, KRQ, STREAM>(B, N, K, ldb, chk, chk_ld, rounding, tiles_n, blockIdx.x * kEncWarps + (threadIdx.x >> 5),
                     gridDim.x * kEncWarps, threadIdx.x & 31);
+}
+
+// The pre-pass of a strided batch (either layout of B): entry e = blockIdx.y, blockIdx.y + gridDim.y, ... reads
+// B + e*stride_b and writes its checksum operand at chk + e*chk_stride.
+// (KRQ / STREAM / rounding: the item shape, load policy and TF32 rounding of encode_b_kernel; a K-major B has one encode)
+template <int BN, bool KMAJOR, int KRQ = 8, bool STREAM = false>
+__global__ void __launch_bounds__(kEncWarps * 32, 2)
+encode_batched_kernel(const float *__restrict__ B, int N, int K, int ldb, long long stride_b, int batch, float *__restrict__ chk,
+                      int chk_ld, long long chk_stride, int rounding, int tiles_n) {
+  ptx::pdl_wait();
+  ptx::pdl_launch_dependents();
+  for (int e = blockIdx.y; e < batch; e += gridDim.y) {
+    const int gw = blockIdx.x * kEncWarps + (threadIdx.x >> 5), nw = gridDim.x * kEncWarps, lane = threadIdx.x & 31;
+    if constexpr (KMAJOR)
+      encode_bk_warp<BN>(B + e * stride_b, N, K, ldb, chk + e * chk_stride, chk_ld, rounding, tiles_n, gw, nw, lane);
+    else
+      encode_b_warp<BN, KRQ, STREAM>(B + e * stride_b, N, K, ldb, chk + e * chk_stride, chk_ld, rounding, tiles_n, gw, nw, lane);
+  }
 }
 
 // The pre-pass for a K-major B.

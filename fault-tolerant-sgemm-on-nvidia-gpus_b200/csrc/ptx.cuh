@@ -179,6 +179,21 @@ __device__ __forceinline__ void tma_load_2d_multicast(uint32_t dst, const CUtens
       "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
+// 3-D forms for strided batches (tensor map {K, rows, batch}, box {32, rows, 1}): c2 is the entry, so the out-of-bounds
+// zero-fill of rows past an entry's last one stays inside that entry.
+__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap *tm, uint32_t bar, int c0, int c1, int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];" ::"r"(dst),
+      "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
+__device__ __forceinline__ void tma_load_3d_multicast(uint32_t dst, const CUtensorMap *tm, uint32_t bar, int c0, int c1, int c2,
+                                                      uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4, %5}], [%2], %6;" ::"r"(dst),
+      "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "h"(cta_mask)
+      : "memory");
+}
 __device__ __forceinline__ float ld_shared_f1(uint32_t addr) {
   float v;
   asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));

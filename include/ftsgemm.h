@@ -80,7 +80,8 @@ typedef struct ftsgemm_kernel_info {
 /* Fault to inject into the FP32 accumulator tile, before the checksum test
  * (generalises the reference's always-on injector, ft_sgemm_huge.cuh:49-51,324-327). */
 typedef struct ftsgemm_fault {
-  int row, col;          /* global element (m, n) of C */
+  int row, col;          /* global element (m, n) of C; in a strided batch (ftsgemm_run_batched) row is the stacked row
+                            i*M + m of entry i */
   int mode;              /* 0: acc += add_value      1: acc bits ^= xor_mask (single/multi bit flip)
                           * epilogue upsets (what opts.protect_epilogue detects; the accumulator check has already passed):
                           * 2: acc bits ^= xor_mask in the accumulator AFTER the check, before the store pass re-reads it
@@ -142,7 +143,8 @@ typedef struct ftsgemm_opts {
 #define FTSGEMM_OPTS_V1_SIZE (offsetof(ftsgemm_opts, baseline_host_sync) + sizeof(int))
 
 typedef struct ftsgemm_event {
-  int row, col;          /* global element that was located (col = -1 if not locatable) */
+  int row, col;          /* global element that was located (col = -1 if not locatable); in a strided batch row is the
+                            stacked row i*M + m of entry i, col is n */
   float residual;        /* expected - actual row checksum */
   float corrected_value; /* accumulator value after correction */
   int status;            /* 1 corrected, 2 detected only (detect_only), 3 uncorrectable, 4 checksum-column fault,
@@ -239,6 +241,24 @@ int ftsgemm_run_bias(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, con
                      const float *dB, int layout_b, int ldb, float *dC, int ldc, float alpha, float beta,
                      const float *bias, int bias_mode, const ftsgemm_opts *opts);
 
+/* ---- strided batch  (new work: the reference computes one product per launch; the contract is cuBLAS's
+ *      cublasSgemmStridedBatched, with this library's layouts, ABFT options and fused bias) ---------------------------------
+ * batch independent products: entry i in [0, batch) is exactly the ftsgemm_run_bias product on A + i*stride_a, B + i*stride_b
+ * and C + i*stride_c (strides in floats).  The bias, if any, is one vector shared by all entries.  ftsgemm_run_bias is this
+ * call with batch = 1, where the strides are ignored.
+ * The wgmma ids run the whole batch in ONE launch of the persistent kernel (plus the encode pre-pass below ~8 MB of B for
+ * all entries together): the tiles of all entries form one work plan.  Every option applies per entry (3xTF32, check_segments,
+ * protect_epilogue, reuse_b_checksums -- keyed on stride_b and batch as well --, no_recompute, detect_only, injection: the
+ * self-test injector hits every CTA tile of every entry).  Fault and event rows are stacked rows i*M + m (see above).
+ * Errors (wgmma ids): batch < 1; for batch > 1 a stride that is not a positive multiple of 4 (no broadcast entries), or
+ * stride_c < ldc*N (overlapping C entries): FTSGEMM_ERR_INVALID_ARG.  batch x tiles above 2^28, or batch*M above INT_MAX:
+ * FTSGEMM_ERR_UNSUPPORTED.  cuBLAS ids 0 / 7: cublasSgemmStridedBatched with the transpose flags of ftsgemm_run_ex (a bias:
+ * FTSGEMM_ERR_UNSUPPORTED).  Baseline ids 10 / 30: batch > 1 is FTSGEMM_ERR_UNSUPPORTED. */
+int ftsgemm_run_batched(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *A, int layout_a, int lda,
+                        long long stride_a, const float *B, int layout_b, int ldb, long long stride_b, float *C, int ldc,
+                        long long stride_c, int batch, float alpha, float beta, const float *bias, int bias_mode,
+                        const ftsgemm_opts *opts);
+
 /* Counters of all FT launches since the previous call (synchronises the handle's last stream, then resets). */
 int ftsgemm_get_stats(ftsgemm_handle_t h, ftsgemm_stats *out);
 
@@ -297,6 +317,8 @@ int ftsgemm_debug_set(const char *key, long long value);
  * hdr[8] = {units, num_tiles, n_chk_tiles, sk_tiles, num_kb, CTAs per unit, sk_slices, chk_slices}; checksum tiles carry
  * their K-slice index in the `slice` column.  Needs no GPU (assumes an L2 of 50 MiB, as on H100). */
 int ftsgemm_debug_schedule(int kernel_id, int M, int N, int K, int num_sms, int *hdr, int *rows, int cap);
+/* The same for a strided batch of `batch` entries: rows of 10 ints, the 9 above (m_blk per entry) + the entry index. */
+int ftsgemm_debug_schedule_batched(int kernel_id, int M, int N, int K, int batch, int num_sms, int *hdr, int *rows, int cap);
 /* Device timeline of the last tensor-core launch made with ftsgemm_debug_set("trace", 1): per work unit 64 items x 8
  * u64 = %globaltimer ns {producer start, producer end, MMA start, MMA issue end, accumulator complete, check done,
  * epilogue end, tile | kind << 24}.  Returns the number of units (out must hold units * 512 u64), 0 if none. */
