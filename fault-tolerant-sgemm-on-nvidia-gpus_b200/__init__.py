@@ -488,18 +488,18 @@ class FtSgemm:
         nothing.  An operand that cannot be read in place (no unit stride, a base address or, for a and b, a
         leading stride that is not a multiple of 16 bytes) is copied once into an aligned buffer first; an out that cannot
         be written in place is computed in a contiguous buffer and copied back; a bias without unit stride is copied once.
-        With out=None a new row-major out is returned and beta must be 0.  The mapping onto run_bias is matmul_plan: a
+        With out=None a new row-major out is returned and beta must be 0.  The mapping onto the kernel is matmul_plan: a
         row-major out is computed as out^T = b^T a^T, so the kernel's (row, col) is out's (col, row) -- the coordinates of
         injected faults (opts) and of stats() events are the kernel's, transposed against out in that case.  A kernel M or
         N (after the mapping) that is not a multiple of 4 raises FtsgemmError(-2) for the tensor-core ids, as run does.
         Runs on the current torch stream unless opts.stream says otherwise.  No autograd: linear() is the differentiable
-        F.linear."""
+        F.linear.  This is bmm on a batch of one entry (a run_batched call with batch = 1, which is run_bias)."""
         import torch
         for name, t in (("a", a), ("b", b)):
             if t.dim() != 2 or t.dtype != torch.float32 or not t.is_cuda:
                 raise TypeError(f"{name} must be a 2-D float32 CUDA tensor")
         M, K = a.shape
-        N = b.shape[1]
+        K2, N = b.shape
         if out is None:
             if beta != 0.0:
                 raise ValueError("beta != 0 needs an out tensor")
@@ -508,29 +508,10 @@ class FtSgemm:
             raise ValueError(f"out must be a float32 ({M}, {N}) tensor on {a.device}")
         if bias is not None and (bias.shape != (N,) or bias.dtype != torch.float32 or bias.device != a.device):
             raise ValueError(f"bias must be a float32 ({N},) tensor on {a.device}")
-        bias_stride = bias.stride(0) if bias is not None else None
-        plan = matmul_plan(tuple(a.shape), a.stride(), tuple(b.shape), b.stride(), out.stride(), a.data_ptr(), b.data_ptr(),
-                           out.data_ptr(), bias_stride, bias.data_ptr() if bias is not None else 0)
-        if plan["copy_bias"]:
-            bias = torch.empty(N, device=a.device, dtype=torch.float32).copy_(bias)
-        if plan["copy_a"]:  # row-major, rows padded to 16 bytes: K-major for the kernel
-            a = torch.empty(M, _pad4(K), device=a.device, dtype=torch.float32)[:, :K].copy_(a)
-        if plan["copy_b"]:  # column-major, columns padded to 16 bytes: K-major for the kernel
-            b = torch.empty(N, _pad4(K), device=a.device, dtype=torch.float32)[:, :K].copy_(b.t()).t()
-        dst = out
-        if plan["copy_out"]:
-            dst = (out.clone(memory_format=torch.contiguous_format) if beta != 0.0
-                   else torch.empty(M, N, device=a.device, dtype=torch.float32))
-        if plan["copy_a"] or plan["copy_b"] or plan["copy_out"]:
-            plan = matmul_plan(tuple(a.shape), a.stride(), tuple(b.shape), b.stride(), dst.stride(), a.data_ptr(),
-                               b.data_ptr(), dst.data_ptr(), bias_stride)
-        if opts is None:
-            opts = make_opts(stream=torch.cuda.current_stream(a.device).cuda_stream)
-        kA, kB = (b, a) if plan["swap"] else (a, b)
-        self.run_bias(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], kB, plan["layout_b"],
-                      plan["ldb"], dst, plan["ldc"], alpha, beta, bias, plan["bias_mode"], opts)
-        if dst is not out:
-            out.copy_(dst)
+        if K != K2:
+            raise ValueError(f"inner dimensions differ: {tuple(a.shape)} @ {tuple(b.shape)}")
+        self.bmm(a.unsqueeze(0), b.unsqueeze(0), out.unsqueeze(0), bias=bias, kernel_id=kernel_id, alpha=alpha, beta=beta,
+                 opts=opts)
         return out
 
     def linear(self, x, weight, bias=None, *, kernel_id: int = ID_ABFT_AUTO, opts: Opts | None = None):

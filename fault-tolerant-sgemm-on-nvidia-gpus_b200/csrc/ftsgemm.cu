@@ -17,6 +17,7 @@
 #include <map>
 #include <mutex>
 #include <string>
+#include <type_traits>
 
 #include "../../include/ftsgemm.h"
 #include "ftsgemm_kernel.cuh"
@@ -105,6 +106,21 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t
                                   const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
+// What a checksum operand was encoded from (ftsgemm_opts::reuse_b_checksums): B pointer, shape, tile width, layout, row
+// stride and batch -- the same pointer read in another layout or with another row stride is another B.
+struct ChkKey {
+  const float *b = nullptr;  // (nullptr: nothing cached)
+  int n = 0, k = 0, bn = 0;
+  bool b_kmajor = false;
+  int ldb = 0;
+  int batch = 1;
+  long long stride_b = 0;
+  bool operator==(const ChkKey &o) const {
+    return b == o.b && n == o.n && k == o.k && bn == o.bn && b_kmajor == o.b_kmajor && ldb == o.ldb && batch == o.batch &&
+           stride_b == o.stride_b;
+  }
+};
+
 }  // namespace
 
 struct ftsgemm_handle_s {
@@ -119,12 +135,7 @@ struct ftsgemm_handle_s {
   float *d_chk_out = nullptr;   // expected checksums M x (tiles_n*8), column-major, + slab flags behind it
   size_t chk_out_bytes = 0;
   size_t chk_flag_bytes = kChkFlagBytes;  // bytes of d_chk_out in front of the expected checksums: the slab flags
-  const float *chk_for_b = nullptr;  // B pointer / shape / layout / batch the panel was encoded from
-  int chk_n = 0, chk_k = 0, chk_bn = 0;
-  bool chk_b_kmajor = false;
-  int chk_ldb = 0;
-  int chk_batch = 1;
-  long long chk_stride_b = 0;
+  ChkKey chk_key;               // what d_chk holds
   // fused verdict exchange (ftsgemm_peer_*): this rank's mailbox (kMaxPeers slots), the peers' mailboxes mapped through
   // CUDA IPC, the exit counter of the publishing launches and their sequence number
   double *d_mailbox = nullptr;
@@ -219,31 +230,17 @@ int check_abort_flag(ftsgemm_handle_t h) {
 
 // K-major operand copy (rows x K, row stride ldk floats): one box = 32 k (128 bytes, 128B-swizzled) x box_rows rows, the
 // layout the wgmma descriptors describe (ptx::make_smem_desc_k128).  Rows and k beyond the operand are zero-filled.
+// A strided batch (batch > 1) adds a third dimension of `batch` entries, entry_stride floats apart (a multiple of 4), with a
+// box of one entry -- so that rows or k beyond one entry's operand are zero-filled, not read from the next entry.  A single
+// entry gets a 2-D map: the kernels without BATCH issue 2-D loads.
 int make_tmap_kmajor(ftsgemm_handle_t h, CUtensorMap *tm, const float *base, uint64_t rows, uint64_t K, uint64_t ldk,
-                     uint32_t box_rows) {
-  cuuint64_t dims[2] = {K, rows};
-  cuuint64_t strides[1] = {ldk * sizeof(float)};
-  cuuint32_t box[2] = {kBK, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = h->encode_tiled(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(base), dims, strides, box,
-                               estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    h->last_cuda_error = static_cast<int>(r);
-    return FTSGEMM_ERR_CUDA;
-  }
-  return FTSGEMM_OK;
-}
-// The same for a strided batch: a third dimension of `batch` entries, entry_stride floats apart (a multiple of 4), and a box of
-// one entry -- so that rows or k beyond one entry's operand are zero-filled, not read from the next entry.
-int make_tmap_kmajor_batched(ftsgemm_handle_t h, CUtensorMap *tm, const float *base, uint64_t rows, uint64_t K, uint64_t ldk,
-                             uint64_t entry_stride, uint64_t batch, uint32_t box_rows) {
-  cuuint64_t dims[3] = {K, rows, batch};
-  cuuint64_t strides[2] = {ldk * sizeof(float), entry_stride * sizeof(float)};
-  cuuint32_t box[3] = {kBK, box_rows, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = h->encode_tiled(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float *>(base), dims, strides, box,
-                               estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     uint64_t entry_stride, uint64_t batch, uint32_t box_rows) {
+  const cuuint64_t dims[3] = {K, rows, batch};
+  const cuuint64_t strides[2] = {ldk * sizeof(float), entry_stride * sizeof(float)};
+  const cuuint32_t box[3] = {kBK, box_rows, 1};
+  const cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = h->encode_tiled(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, batch > 1 ? 3 : 2, const_cast<float *>(base), dims, strides,
+                               box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                                CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     h->last_cuda_error = static_cast<int>(r);
@@ -331,24 +328,41 @@ int launch_tc(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB
   return FTSGEMM_OK;
 }
 
-template <int BN, int CG, bool SEED, bool BIAS, bool BATCH>
-int launch_ft(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
-              const KernelParams &p, int units, cudaStream_t stream, bool ft, bool prot) {
-  if (!ft) return launch_tc<BN, false, CG, false, SEED, BIAS, BATCH>(h, tmA, tmB, tmC, p, units, stream);
-  if (prot) return launch_tc<BN, true, CG, true, SEED, BIAS, BATCH>(h, tmA, tmB, tmC, p, units, stream);
-  return launch_tc<BN, true, CG, false, SEED, BIAS, BATCH>(h, tmA, tmB, tmC, p, units, stream);
+// The wgmma tiles the library is built for: calls f(bn, cg) with the tile's BN and CG as compile-time constants
+// (std::integral_constant) and returns its result, or FTSGEMM_ERR_UNSUPPORTED for any other pair.
+template <int BNv, int CGv>
+struct Tile {};
+template <typename F, int... BNv, int... CGv>
+int with_tile_of(int BN, int CG, F &&f, Tile<BNv, CGv>...) {
+  int rc = FTSGEMM_ERR_UNSUPPORTED;
+  (void)((BN == BNv && CG == CGv && (rc = f(std::integral_constant<int, BNv>(), std::integral_constant<int, CGv>()), true)) || ...);
+  return rc;
+}
+template <typename F>
+int with_tile(int BN, int CG, F &&f) {
+  return with_tile_of(BN, CG, f, Tile<32, 1>(), Tile<64, 1>(), Tile<128, 1>(), Tile<256, 1>(), Tile<64, 2>(), Tile<128, 2>(),
+                      Tile<256, 2>());
+}
+// f(std::true_type()) or f(std::false_type())
+template <typename F>
+int with_flag(bool b, F &&f) {
+  return b ? f(std::true_type()) : f(std::false_type());
 }
 
-// (a bias selects the BIAS instantiation: KernelParams::bias, ftsgemm_tc_kernel; a batch of more than one entry the BATCH one)
-template <int BN, int CG, bool SEED>
+// The kernel instantiation of a launch: SEED for a plan with cut tiles, BIAS for a bias (KernelParams::bias,
+// ftsgemm_tc_kernel), BATCH for a batch of more than one entry, PROT (fault-tolerant kernels only) for opts.protect_epilogue.
+template <int BN, int CG>
 int launch_variant(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
                    const KernelParams &p, int units, cudaStream_t stream, bool ft, bool prot) {
-  if (p.batch > 1) {
-    if (p.bias_mode != kBiasNone) return launch_ft<BN, CG, SEED, true, true>(h, tmA, tmB, tmC, p, units, stream, ft, prot);
-    return launch_ft<BN, CG, SEED, false, true>(h, tmA, tmB, tmC, p, units, stream, ft, prot);
-  }
-  if (p.bias_mode != kBiasNone) return launch_ft<BN, CG, SEED, true, false>(h, tmA, tmB, tmC, p, units, stream, ft, prot);
-  return launch_ft<BN, CG, SEED, false, false>(h, tmA, tmB, tmC, p, units, stream, ft, prot);
+  return with_flag(p.sk_tiles > 0, [&](auto seed) {
+    return with_flag(p.bias_mode != kBiasNone, [&](auto bias) {
+      return with_flag(p.batch > 1, [&](auto batch) {
+        if (!ft) return launch_tc<BN, false, CG, false, seed, bias, batch>(h, tmA, tmB, tmC, p, units, stream);
+        if (prot) return launch_tc<BN, true, CG, true, seed, bias, batch>(h, tmA, tmB, tmC, p, units, stream);
+        return launch_tc<BN, true, CG, false, seed, bias, batch>(h, tmA, tmB, tmC, p, units, stream);
+      });
+    });
+  });
 }
 
 // Planner input for one launch (tile grid already set by plan_tiles).
@@ -356,12 +370,6 @@ int launch_variant(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap
 // bound by the A-operand feed), an item costs a fixed pipeline fill + drain, and a parked accumulator reaches the next
 // owner a fixed latency after the piece's last k-block.  (Constants carried over from the previous target, not re-tuned
 // for H100.)
-template <int BNv, int CGv>
-void chk_costs(const KernelParams &p, double floor_cost, std::vector<double> *out) {
-  for (int c = 0; c < p.tiles_c; ++c)
-    out->push_back(std::max(floor_cost, static_cast<double>(chk_tile_width<BNv, CGv>(p, c)) / BNv));
-}
-
 // l2_bytes: the device's L2 size (cudaDevAttrL2CacheSize)
 PlanInput make_plan_input(int max_units, int CG, int BN, int K, const KernelParams &p, long long l2_bytes) {
   PlanInput in;
@@ -382,13 +390,11 @@ PlanInput make_plan_input(int max_units, int CG, int BN, int K, const KernelPara
   // a checksum item's main loop costs a fixed fraction of a data tile's: larger where data tiles run out of L2, smaller
   // where they are HBM-bound
   const double chk_floor = static_cast<double>(dbg("chk_cost_permille", in.lockstep ? 580 : 680)) * 1e-3;
-  if (BN == 32) chk_costs<32, 1>(p, chk_floor, &in.chk_col_cost);
-  else if (BN == 64 && CG == 1) chk_costs<64, 1>(p, chk_floor, &in.chk_col_cost);
-  else if (BN == 64) chk_costs<64, 2>(p, chk_floor, &in.chk_col_cost);
-  else if (BN == 128 && CG == 1) chk_costs<128, 1>(p, chk_floor, &in.chk_col_cost);
-  else if (BN == 128) chk_costs<128, 2>(p, chk_floor, &in.chk_col_cost);
-  else if (CG == 1) chk_costs<256, 1>(p, chk_floor, &in.chk_col_cost);
-  else chk_costs<256, 2>(p, chk_floor, &in.chk_col_cost);
+  with_tile(BN, CG, [&](auto bn, auto cg) {
+    for (int c = 0; c < p.tiles_c; ++c)
+      in.chk_col_cost.push_back(std::max(chk_floor, static_cast<double>(chk_tile_width<bn, cg>(p, c)) / bn));
+    return FTSGEMM_OK;
+  });
   const double tile_us = in.num_kb * 0.333 * (static_cast<double>(BN) * CG / 512.0 < 0.25 ? 0.25 : static_cast<double>(BN) * CG / 512.0);
   in.item_overhead = static_cast<double>(dbg("item_overhead_ns", 1500)) * 1e-3 / tile_us;
   in.park_latency = static_cast<double>(dbg("park_latency_ns", 8000)) * 1e-3 / tile_us;
@@ -462,11 +468,12 @@ const BatchArg kSingle = {1, 0, 0, 0};
 
 int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC, int ldc,
            float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o, cudaStream_t stream,
-           const BatchArg &bt = kSingle) {
+           const BatchArg &batch_arg = kSingle) {
   const int BN = v.bn, CG = v.cg;
   const bool ft = v.info.fault_tolerant != 0;
   const float *dA = A.p, *dB = B.p;
-  const bool batched = bt.count > 1;  // (one entry runs the kernels without BATCH, on 2-D tensor maps)
+  // (one entry runs the kernels without BATCH, on 2-D tensor maps; its strides are ignored)
+  const BatchArg bt = batch_arg.count > 1 ? batch_arg : kSingle;
   if ((M % 4) || (N % 4)) return FTSGEMM_ERR_UNSUPPORTED;  // TMA global strides must be multiples of 16 bytes
   if ((A.ld % 4) || (B.ld % 4)) return FTSGEMM_ERR_INVALID_ARG;  // (the same for the rows of an operand)
   // work-plan items carry k-block indices in 16 bits and tile indices in 31; the trace / wave tables are sized per unit
@@ -483,11 +490,9 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
   p.alpha = alpha; p.beta = beta;
   p.bias = bias; p.bias_mode = bias_mode;
   p.batch = bt.count;
-  if (batched) {
-    p.stride_a = bt.sa;
-    p.stride_b = bt.sb;
-    p.stride_c = bt.sc;
-  }
+  p.stride_a = bt.sa;
+  p.stride_b = bt.sb;
+  p.stride_c = bt.sc;
   plan_tiles(M, N, BN, CG, ft, &p);
   p.tau_abs = o.tau_abs > 0 ? o.tau_abs : 1e-3f;
   p.tau_rel = o.tau_rel > 0 ? o.tau_rel : 1e-5f;  // DESIGN.md section 5
@@ -527,28 +532,24 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
   int rc;
   p.ldk = (K + 3) / 4 * 4;
   // (a batch: 3-D maps with the entry as the outer dimension; the copies hold one dense rows x ldk block per entry)
-  auto tmap = [&](CUtensorMap *tm, const float *base, int rows, int ld, long long entry_stride, int box_rows) {
-    if (!batched) return make_tmap_kmajor(h, tm, base, rows, K, ld, box_rows);
-    return make_tmap_kmajor_batched(h, tm, base, rows, K, ld, entry_stride, bt.count, box_rows);
-  };
   const long long a_copy = static_cast<long long>(M) * p.ldk, b_copy = static_cast<long long>(N) * p.ldk;
   if (A.kmajor) {
-    rc = tmap(&tmA, dA, M, A.ld, bt.sa, kBM);
+    rc = make_tmap_kmajor(h, &tmA, dA, M, K, A.ld, bt.sa, bt.count, kBM);
   } else {
     rc = ensure_buf(h, &h->d_at, &h->at_bytes, static_cast<size_t>(a_copy) * bt.count * sizeof(float));
     if (rc) return rc;
     p.At = h->d_at;
-    rc = tmap(&tmA, p.At, M, p.ldk, a_copy, kBM);
+    rc = make_tmap_kmajor(h, &tmA, p.At, M, K, p.ldk, a_copy, bt.count, kBM);
   }
   if (rc) return rc;
   // CG = 2: each CTA of a unit loads BN/2 rows of the B tile and multicasts them to both
   if (B.kmajor) {
-    rc = tmap(&tmB, dB, N, B.ld, bt.sb, BN / CG);
+    rc = make_tmap_kmajor(h, &tmB, dB, N, K, B.ld, bt.sb, bt.count, BN / CG);
   } else {
     rc = ensure_buf(h, &h->d_bt, &h->bt_bytes, static_cast<size_t>(b_copy) * bt.count * sizeof(float));
     if (rc) return rc;
     p.Bt = h->d_bt;
-    rc = tmap(&tmB, p.Bt, N, p.ldk, b_copy, BN / CG);
+    rc = make_tmap_kmajor(h, &tmB, p.Bt, N, K, p.ldk, b_copy, bt.count, BN / CG);
   }
   if (rc) return rc;
   tmC = tmB;
@@ -563,7 +564,7 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
     const float *chk_before = h->d_chk;
     rc = ensure_buf(h, &h->d_chk, &h->chk_bytes, static_cast<size_t>(chk_entry) * bt.count * sizeof(float));
     if (rc) return rc;
-    if (h->d_chk != chk_before) h->chk_for_b = nullptr;  // reallocated: the cached encode is gone
+    if (h->d_chk != chk_before) h->chk_key = ChkKey();  // reallocated: the cached encode is gone
     const size_t out_floats = static_cast<size_t>(M) * p.n_chk_cols * bt.count;
     const size_t n_flags = static_cast<size_t>(n_slabs) * p.tiles_c;
     if (n_flags * sizeof(int) > h->chk_flag_bytes) {
@@ -585,10 +586,8 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
     }
     p.chk_epoch = ++h->chk_epoch;
     p.dbg_flags = static_cast<int>(dbg("ft_dbg", 0)) & 1;
-    // (the same pointer read in another layout or with another row stride is another B)
-    const bool reuse = o.reuse_b_checksums && h->chk_for_b == dB && h->chk_n == N && h->chk_k == K && h->chk_bn == BN &&
-                       h->chk_b_kmajor == B.kmajor && h->chk_ldb == B.ld && h->chk_batch == bt.count &&
-                       h->chk_stride_b == (batched ? bt.sb : 0);
+    const ChkKey chk_key = {dB, N, K, BN, B.kmajor, B.ld, bt.count, bt.sb};
+    const bool reuse = o.reuse_b_checksums && h->chk_key == chk_key;
     // Default: the encode is part of the FRONT PHASE of the GEMM kernel (KernelParams::enc_front) -- one launch per fused
     // GEMM, like the reference (sgemm.cu:191-192); only below ~8 MB of B the stand-alone pre-pass is used.
     const long long ef = dbg("enc_front", -2);
@@ -599,84 +598,49 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
       p.enc_ld = chk_ld;
     }
     if (!reuse && !enc_front) {
-      // stand-alone pre-pass in the caller's stream
+      // stand-alone pre-pass in the caller's stream: grid-stride over (column block, k-row group) items, the pass is HBM
+      // time; a batch runs all entries in one launch, one grid row per entry
       const int rounding = static_cast<int>(dbg("enc_rounding", 0));
-      // grid-stride over (column block, k-row group) items; the pass is HBM time.
       const int grid = static_cast<int>(dbg("enc_blocks_per_sm", 4)) * h->num_sms;
       const bool small_items = dbg("enc_kr", 8) == 4;
       const bool chain = dbg("pdl_chain", 1) != 0;
       // B larger than ~half of L2: read it with evict-first loads (it cannot stay resident for the GEMM anyway)
       const long long sb = dbg("enc_stream", -2);
       const bool stream_b = sb > 0;  // off by default: the tail of B the pre-pass leaves in L2 serves the GEMM's first wave
-#define FT_ENC(bn)                                                                                                          \
-  if (BN == bn) {                                                                                                           \
-    cudaLaunchConfig_t ec = {};                                                                                             \
-    ec.gridDim = dim3(grid);                                                                                                \
-    ec.blockDim = dim3(kEncWarps * 32);                                                                                     \
-    ec.stream = stream;                                                                                                     \
-    cudaLaunchAttribute ea[1];                                                                                              \
-    ea[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                                                          \
-    ea[0].val.programmaticStreamSerializationAllowed = 1;                                                                   \
-    ec.attrs = ea;                                                                                                          \
-    ec.numAttrs = chain ? 1 : 0;                                                                                            \
-    const float *eb = dB;                                                                                                   \
-    float *eo = h->d_chk;                                                                                                   \
-    int en = N, ek = K, eld = B.ld, el = chk_ld, er = rounding, et = p.tiles_n;                                             \
-    if (B.kmajor) FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_bk_kernel<bn>, eb, en, ek, eld, eo, el, er, et));               \
-    else if (small_items) FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_b_kernel<bn, 4, false>, eb, en, ek, eld, eo, el, er, et)); \
-    else if (stream_b) FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_b_kernel<bn, 8, true>, eb, en, ek, eld, eo, el, er, et));  \
-    else FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_b_kernel<bn, 8, false>, eb, en, ek, eld, eo, el, er, et));               \
-  }
-#define FT_ENC_BATCHED(bn)                                                                                                  \
-  if (BN == bn) {                                                                                                           \
-    cudaLaunchConfig_t ec = {};                                                                                             \
-    ec.gridDim = dim3(std::max(1, grid / bt.count), std::min(bt.count, 65535));                                             \
-    ec.blockDim = dim3(kEncWarps * 32);                                                                                     \
-    ec.stream = stream;                                                                                                     \
-    cudaLaunchAttribute ea[1];                                                                                              \
-    ea[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                                                          \
-    ea[0].val.programmaticStreamSerializationAllowed = 1;                                                                   \
-    ec.attrs = ea;                                                                                                          \
-    ec.numAttrs = chain ? 1 : 0;                                                                                            \
-    const float *eb = dB;                                                                                                   \
-    float *eo = h->d_chk;                                                                                                   \
-    int en = N, ek = K, eld = B.ld, el = chk_ld, er = rounding, et = p.tiles_n, ebt = bt.count;                             \
-    long long esb = bt.sb, ecs = chk_entry;                                                                                 \
-    if (B.kmajor)                                                                                                           \
-      FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_batched_kernel<bn, true>, eb, en, ek, eld, esb, ebt, eo, el, ecs, er, et));  \
-    else if (small_items)                                                                                                   \
-      FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_batched_kernel<bn, false, 4, false>, eb, en, ek, eld, esb, ebt, eo, el, ecs, er, et)); \
-    else if (stream_b)                                                                                                      \
-      FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_batched_kernel<bn, false, 8, true>, eb, en, ek, eld, esb, ebt, eo, el, ecs, er, et)); \
-    else                                                                                                                    \
-      FT_CUDA(h, cudaLaunchKernelEx(&ec, encode_batched_kernel<bn, false>, eb, en, ek, eld, esb, ebt, eo, el, ecs, er, et)); \
-  }
-      // (a batch: one launch for all entries, 2-D grid)
-      if (batched) {
-        FT_ENC_BATCHED(32) FT_ENC_BATCHED(64) FT_ENC_BATCHED(128) FT_ENC_BATCHED(256)
-      } else {
-        FT_ENC(32) FT_ENC(64) FT_ENC(128) FT_ENC(256)
-      }
+      cudaLaunchConfig_t ec = {};
+      ec.gridDim = dim3(std::max(1, grid / bt.count), std::min(bt.count, 65535));
+      ec.blockDim = dim3(kEncWarps * 32);
+      ec.stream = stream;
+      cudaLaunchAttribute ea[1];
+      ea[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+      ea[0].val.programmaticStreamSerializationAllowed = 1;
+      ec.attrs = ea;
+      ec.numAttrs = chain ? 1 : 0;
+      const long long chk_stride = bt.count > 1 ? chk_entry : 0;
+      rc = with_tile(BN, CG, [&](auto bn, auto) {
+        auto launch = [&](auto kern) {
+          FT_CUDA(h, cudaLaunchKernelEx(&ec, kern, dB, N, K, B.ld, bt.sb, bt.count, h->d_chk, chk_ld, chk_stride, rounding, p.tiles_n));
+          return FTSGEMM_OK;
+        };
+        if (B.kmajor) return launch(encode_kernel<bn, true>);
+        if (small_items) return launch(encode_kernel<bn, false, 4, false>);
+        if (stream_b) return launch(encode_kernel<bn, false, 8, true>);
+        return launch(encode_kernel<bn, false, 8, false>);
+      });
+      if (rc) return rc;
       ++h->launch_count;
-#undef FT_ENC
-#undef FT_ENC_BATCHED
       FT_CUDA(h, cudaGetLastError());
     }
-    if (!reuse) {
-      h->chk_for_b = dB; h->chk_n = N; h->chk_k = K; h->chk_bn = BN; h->chk_b_kmajor = B.kmajor; h->chk_ldb = B.ld;
-      h->chk_batch = bt.count; h->chk_stride_b = batched ? bt.sb : 0;
-    }
-    rc = tmap(&tmC, h->d_chk, p.n_chk_cols, chk_ld, chk_entry, BN / CG);
+    if (!reuse) h->chk_key = chk_key;
+    rc = make_tmap_kmajor(h, &tmC, h->d_chk, p.n_chk_cols, K, chk_ld, chk_entry, bt.count, BN / CG);
     if (rc) return rc;
   }
   // ---- work plan (plan.h), cached per shape on the handle
   int max_units = 0;
   {
-    int qrc = FTSGEMM_ERR_UNSUPPORTED;
-#define FT_QUERY(bn, cg) \
-  if (BN == bn && CG == cg) qrc = ft ? query_max_units<bn, true, cg>(h, &max_units) : query_max_units<bn, false, cg>(h, &max_units);
-    FT_QUERY(32, 1) FT_QUERY(64, 1) FT_QUERY(128, 1) FT_QUERY(256, 1) FT_QUERY(64, 2) FT_QUERY(128, 2) FT_QUERY(256, 2)
-#undef FT_QUERY
+    const int qrc = with_tile(BN, CG, [&](auto bn, auto cg) {
+      return ft ? query_max_units<bn, true, cg>(h, &max_units) : query_max_units<bn, false, cg>(h, &max_units);
+    });
     if (qrc) return qrc;
     if (max_units < 1) return FTSGEMM_ERR_UNSUPPORTED;  // not a single CTA (pair) of this kernel fits on the device partition
   }
@@ -815,20 +779,9 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
   p.pdl_wait = dbg("pdl_chain", 1) != 0 ? 1 : 0;
   h->last_stream = stream;
   ++h->launch_count;
-  int lrc = FTSGEMM_ERR_UNSUPPORTED;
-#define FT_DISPATCH(bn, cg)                                                                                    \
-  if (BN == bn && CG == cg)                                                                                    \
-    lrc = p.sk_tiles > 0 ? launch_variant<bn, cg, true>(h, tmA, tmB, tmC, p, units, stream, ft, o.protect_epilogue) \
-                         : launch_variant<bn, cg, false>(h, tmA, tmB, tmC, p, units, stream, ft, o.protect_epilogue);
-  FT_DISPATCH(32, 1)
-  FT_DISPATCH(64, 1)
-  FT_DISPATCH(128, 1)
-  FT_DISPATCH(256, 1)
-  FT_DISPATCH(64, 2)
-  FT_DISPATCH(128, 2)
-  FT_DISPATCH(256, 2)
-#undef FT_DISPATCH
-  return lrc;
+  return with_tile(BN, CG, [&](auto bn, auto cg) {
+    return launch_variant<bn, cg>(h, tmA, tmB, tmC, p, units, stream, ft, o.protect_epilogue != 0);
+  });
 }
 
 int run_cublas(ftsgemm_handle_t h, bool tf32, int M, int N, int K, const Operand &A, const Operand &B, float *dC, int ldc,
@@ -865,26 +818,19 @@ __global__ void split_lo_kernel(const float4 *__restrict__ x, float4 *__restrict
     lo[i] = r;
   }
 }
-// the same for an operand with padded rows: `outer` rows of `inner` elements, row stride ldx in, ldlo out
-__global__ void split_lo_strided_kernel(const float *__restrict__ x, size_t ldx, float *__restrict__ lo, size_t ldlo, int inner,
-                                        size_t outer) {
-  const size_t n = outer * inner;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const size_t o = i / inner, r = i - o * inner;
-    const float v = __ldg(x + o * ldx + r);
-    lo[o * ldlo + r] = v - __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
-  }
-}
-
-// 3xTF32 of a strided batch: entry e of x (`outer` rows of `inner` elements, row stride ldx, entry stride sx) -> its lo part
-// at lo + e * outer * ldlo (row stride ldlo)
-__global__ void split_lo_batched_kernel(const float *__restrict__ x, size_t ldx, long long sx, float *__restrict__ lo, size_t ldlo,
+// the same for operands with padded rows: entry e = blockIdx.y, blockIdx.y + gridDim.y, ... of x (`outer` rows of `inner`
+// elements, row stride ldx, entry stride sx) -> its lo part at lo + e * outer * ldlo (row stride ldlo)
+__global__ void split_lo_strided_kernel(const float *__restrict__ x, size_t ldx, long long sx, float *__restrict__ lo, size_t ldlo,
                                         int inner, size_t outer, int batch) {
-  const size_t per = outer * inner, n = per * batch;
-  for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const size_t e = i / per, j = i - e * per, o = j / inner, r = j - o * inner;
-    const float v = __ldg(x + static_cast<long long>(e) * sx + o * ldx + r);
-    lo[(e * outer + o) * ldlo + r] = v - __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
+  const size_t n = outer * inner;
+  for (int e = blockIdx.y; e < batch; e += gridDim.y) {
+    const float *xe = x + e * sx;
+    float *le = lo + e * outer * ldlo;
+    for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
+      const size_t o = i / inner, r = i - o * inner;
+      const float v = __ldg(xe + o * ldx + r);
+      le[o * ldlo + r] = v - __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
+    }
   }
 }
 
@@ -1010,7 +956,7 @@ static int debug_schedule_rows(int kernel_id, int M, int N, int K, int batch, in
     for (int i = plan.offsets[u]; i < plan.offsets[u + 1]; ++i) {
       const PlanItem &it = plan.items[i];
       if (rows && n < cap) {
-        const TileCoord tc = width > 9 ? decode_tile_batched(p, it.tile) : decode_tile(p, it.tile);
+        const TileCoord tc = decode_tile_batched(p, it.tile);  // (batch = 1: decode_tile)
         int *r = rows + width * n;
         r[0] = u; r[1] = it.tile; r[2] = tc.is_chk ? 1 : 0; r[3] = tc.m_blk; r[4] = tc.n_blk;
         r[5] = it.kb_begin; r[6] = it.kb_end; r[7] = it.kind; r[8] = it.slice;
@@ -1239,51 +1185,26 @@ int ftsgemm_run_batched(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, 
     Operand Alo = lo_of(A, M), Blo = lo_of(B, N);
     const size_t a_floats = static_cast<size_t>(Alo.ld) * (Alo.kmajor ? M : K);
     const size_t b_floats = static_cast<size_t>(Blo.ld) * (Blo.kmajor ? N : K);
-    if (bt.count > 1) {
-      // a batch: the lo parts of entry e at e * a_floats (e * b_floats), dense in the operand's own layout, from one launch per
-      // operand; then the three passes as batches
-      int rc = ensure_buf(h, &h->d_lo, &h->lo_bytes, (a_floats + b_floats) * bt.count * sizeof(float));
-      if (rc) return rc;
-      float *dAlo = h->d_lo, *dBlo = h->d_lo + a_floats * bt.count;
-      Alo.p = dAlo;
-      Blo.p = dBlo;
-      auto split = [&](const Operand &x, const Operand &lo, int rows, long long sx, float *dst) {
-        const int inner = x.kmajor ? K : rows;
-        const size_t outer = x.kmajor ? rows : K;
-        split_lo_batched_kernel<<<h->num_sms * 8, 256, 0, stream>>>(x.p, x.ld, sx, dst, lo.ld, inner, outer, bt.count);
-      };
-      split(A, Alo, M, bt.sa, dAlo);
-      split(B, Blo, N, bt.sb, dBlo);
-      FT_CUDA(h, cudaGetLastError());
-      h->launch_count += 2;
-      ftsgemm_opts o3 = o;
-      o3.reuse_b_checksums = 0;
-      o3.precision = 0;
-      ftsgemm_opts o_quiet = o3;
-      o_quiet.inject_mode = 0;
-      const BatchArg lo_a = {bt.count, static_cast<long long>(a_floats), bt.sb, bt.sc};
-      const BatchArg lo_b = {bt.count, bt.sa, static_cast<long long>(b_floats), bt.sc};
-      rc = run_tc(h, *v, M, N, K, Alo, B, dC, ldc, alpha, beta, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo_a);
-      if (!rc) rc = run_tc(h, *v, M, N, K, A, Blo, dC, ldc, alpha, 1.0f, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo_b);
-      if (!rc) rc = run_tc(h, *v, M, N, K, A, B, dC, ldc, alpha, 1.0f, bias, bias_mode, o3, stream, bt);
-      return rc;
-    }
-    int rc = ensure_buf(h, &h->d_lo, &h->lo_bytes, (a_floats + b_floats) * sizeof(float));
+    // the lo parts of entry e at e * a_floats (e * b_floats), from one launch per operand; then the three passes
+    int rc = ensure_buf(h, &h->d_lo, &h->lo_bytes, (a_floats + b_floats) * bt.count * sizeof(float));
     if (rc) return rc;
-    float *dAlo = h->d_lo, *dBlo = h->d_lo + a_floats;
+    float *dAlo = h->d_lo, *dBlo = h->d_lo + a_floats * bt.count;
     Alo.p = dAlo;
     Blo.p = dBlo;
-    auto split = [&](const Operand &x, const Operand &lo, int rows, float *dst) {
+    auto split = [&](const Operand &x, const Operand &lo, int rows, long long sx, float *dst) {
       const int inner = x.kmajor ? K : rows;  // elements per stored row of the operand
       const size_t outer = x.kmajor ? rows : K;
-      if (x.ld == inner && lo.ld == inner)  // dense: one flat array (x % 4 == 0 elements, see above)
-        split_lo_kernel<<<h->num_sms * 8, 256, 0, stream>>>(reinterpret_cast<const float4 *>(x.p), reinterpret_cast<float4 *>(dst),
-                                                            outer * inner / 4);
-      else  // padded rows: nothing outside the operand's rows is read
-        split_lo_strided_kernel<<<h->num_sms * 8, 256, 0, stream>>>(x.p, x.ld, dst, lo.ld, inner, outer);
+      const int blocks = h->num_sms * 8;
+      if (x.ld == inner && lo.ld == inner && (bt.count == 1 || sx == static_cast<long long>(outer) * inner))
+        // dense: all entries are one flat array (a multiple of 4 elements, see above)
+        split_lo_kernel<<<blocks, 256, 0, stream>>>(reinterpret_cast<const float4 *>(x.p), reinterpret_cast<float4 *>(dst),
+                                                    outer * inner * bt.count / 4);
+      else  // padded rows or entries: nothing outside the operand's rows is read
+        split_lo_strided_kernel<<<dim3(std::max(1, blocks / bt.count), std::min(bt.count, 65535)), 256, 0, stream>>>(
+            x.p, x.ld, sx, dst, lo.ld, inner, outer, bt.count);
     };
-    split(A, Alo, M, dAlo);
-    split(B, Blo, N, dBlo);
+    split(A, Alo, M, bt.sa, dAlo);
+    split(B, Blo, N, bt.sb, dBlo);
     FT_CUDA(h, cudaGetLastError());
     h->launch_count += 2;
     ftsgemm_opts o3 = o;
@@ -1292,9 +1213,11 @@ int ftsgemm_run_batched(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, 
     ftsgemm_opts o_quiet = o3;  // injected faults belong to the main product only
     o_quiet.inject_mode = 0;
     // (the bias goes to the last pass only: added once, after the final alpha*acc + C)
-    rc = run_tc(h, *v, M, N, K, Alo, B, dC, ldc, alpha, beta, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream);
-    if (!rc) rc = run_tc(h, *v, M, N, K, A, Blo, dC, ldc, alpha, 1.0f, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream);
-    if (!rc) rc = run_tc(h, *v, M, N, K, A, B, dC, ldc, alpha, 1.0f, bias, bias_mode, o3, stream);
+    const BatchArg lo_a = {bt.count, static_cast<long long>(a_floats), bt.sb, bt.sc};
+    const BatchArg lo_b = {bt.count, bt.sa, static_cast<long long>(b_floats), bt.sc};
+    rc = run_tc(h, *v, M, N, K, Alo, B, dC, ldc, alpha, beta, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo_a);
+    if (!rc) rc = run_tc(h, *v, M, N, K, A, Blo, dC, ldc, alpha, 1.0f, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo_b);
+    if (!rc) rc = run_tc(h, *v, M, N, K, A, B, dC, ldc, alpha, 1.0f, bias, bias_mode, o3, stream, bt);
     return rc;
   }
   switch (v->info.engine) {

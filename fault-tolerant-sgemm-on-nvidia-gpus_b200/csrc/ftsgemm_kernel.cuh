@@ -20,7 +20,7 @@
 //
 // ABFT scheme (DESIGN.md section 3).  With b~ = the TF32 value the tensor core actually consumes and J_t the columns
 // of N-tile t:
-//   encode    (pre-pass encode_b_kernel; reference ENCODE ft_sgemm_huge.cuh:150-168)
+//   encode    (pre-pass encode_kernel or the kernel's front phase; reference ENCODE ft_sgemm_huge.cuh:150-168)
 //             e_t[k] = sum_{n in J_t} b~[n,k]      w_t[k] = sum_{n in J_t} (n-n0+1) b~[n,k]     (2-way TF32 split each)
 //   checksum GEMM (reference CHECKSUM-GEMV :171-213): the 4 checksum vectors of every N-tile are appended to B as extra
 //             "rows", i.e. the SAME kernel computes extra tile-columns  R = A * [e_t, w_t]^T  first (FP32 accumulate,
@@ -1194,30 +1194,34 @@ __device__ __forceinline__ void encode_bk_warp(const float *__restrict__ B, int 
 // into the K-major copy dst[r * ldk + k], through a 32 x 33 shared-memory tile (conflict-free both ways); blocks
 // rows-fastest so that warps running side by side read neighbouring segments of the same k rows.
 // ------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void transpose_block(const float *__restrict__ src, int rows, int K, int ld, float *__restrict__ dst,
+                                                int ldk, int r0, int k0, int lane, float *tile) {
+  const int r = r0 + lane;
+#pragma unroll 8
+  for (int j = 0; j < 32; ++j) {
+    const int k = k0 + j;
+    tile[j * 33 + lane] = (r < rows && k < K) ? __ldg(src + static_cast<size_t>(k) * ld + r) : 0.0f;
+  }
+  __syncwarp();
+  const int k = k0 + lane;
+#pragma unroll 8
+  for (int i = 0; i < 32; ++i)
+    if (r0 + i < rows && k < K) dst[static_cast<size_t>(r0 + i) * ldk + k] = tile[lane * 33 + i];
+  __syncwarp();
+}
 __device__ __forceinline__ void transpose_warp(const float *__restrict__ src, int rows, int K, int ld, float *__restrict__ dst,
                                                int ldk, int gw, int nw, int lane, float *tile) {
   const int rb = (rows + 31) / 32, kb = (K + 31) / 32;
   const long long total = static_cast<long long>(rb) * kb;
-  for (long long t = gw; t < total; t += nw) {
-    const int r0 = static_cast<int>(t % rb) * 32, k0 = static_cast<int>(t / rb) * 32;
-    const int r = r0 + lane;
-#pragma unroll 8
-    for (int j = 0; j < 32; ++j) {
-      const int k = k0 + j;
-      tile[j * 33 + lane] = (r < rows && k < K) ? __ldg(src + static_cast<size_t>(k) * ld + r) : 0.0f;
-    }
-    __syncwarp();
-    const int k = k0 + lane;
-#pragma unroll 8
-    for (int i = 0; i < 32; ++i)
-      if (r0 + i < rows && k < K) dst[static_cast<size_t>(r0 + i) * ldk + k] = tile[lane * 33 + i];
-    __syncwarp();
-  }
+  for (long long t = gw; t < total; t += nw)
+    transpose_block(src, rows, K, ld, dst, ldk, static_cast<int>(t % rb) * 32, static_cast<int>(t / rb) * 32, lane, tile);
 }
 
 // The front phase when at least one operand is K-major: transpose only the MN-major one, encode B in its own layout.  Out of
 // line, so that the GEMM kernel's register allocation sees the reference layout's front phase only (inlined, this branch
 // raised the spills of the 256-wide fault-tolerant instantiations; out of line, the plain instantiations stopped spilling).
+// (front_phase_batched with batch = 1 does the same work, but calling it here moved the spills of the fault-tolerant
+// 128 x 128 kernel from 664 / 448 to 668 / 452 bytes of stores / loads)
 template <int BN, bool FT>
 __device__ __noinline__ void front_phase_kmajor(const float *A, const float *B, int M, int N, int K, int lda, int ldb,
                                                 int a_kmajor, int b_kmajor, float *At, float *Bt, int ldk, int enc_front,
@@ -1239,21 +1243,8 @@ __device__ __forceinline__ void transpose_warp_batched(const float *__restrict__
   const long long per = static_cast<long long>(rb) * kb, total = per * batch;
   for (long long t = gw; t < total; t += nw) {
     const long long e = t / per, te = t - e * per;
-    const float *s = src + e * stride;
-    float *d = dst + e * static_cast<long long>(rows) * ldk;
-    const int r0 = static_cast<int>(te % rb) * 32, k0 = static_cast<int>(te / rb) * 32;
-    const int r = r0 + lane;
-#pragma unroll 8
-    for (int j = 0; j < 32; ++j) {
-      const int k = k0 + j;
-      tile[j * 33 + lane] = (r < rows && k < K) ? __ldg(s + static_cast<size_t>(k) * ld + r) : 0.0f;
-    }
-    __syncwarp();
-    const int k = k0 + lane;
-#pragma unroll 8
-    for (int i = 0; i < 32; ++i)
-      if (r0 + i < rows && k < K) d[static_cast<size_t>(r0 + i) * ldk + k] = tile[lane * 33 + i];
-    __syncwarp();
+    transpose_block(src + e * stride, rows, K, ld, dst + e * static_cast<long long>(rows) * ldk, ldk, static_cast<int>(te % rb) * 32,
+                    static_cast<int>(te / rb) * 32, lane, tile);
   }
 }
 // (scalars by value: a reference to the parameter block would force a local copy of all of it)
@@ -1704,43 +1695,27 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 // ------------------------------------------------------------------------------------------------------------
 constexpr int kEncWarps = 8;
 
-template <int BN, int KRQ, bool STREAM = false>
-__global__ void __launch_bounds__(kEncWarps * 32, 2)
-encode_b_kernel(const float *__restrict__ B, int N, int K, int ldb, float *__restrict__ chk, int chk_ld, int rounding,
-                int tiles_n) {
-  ptx::pdl_wait();               // (a programmatic dependent itself: the predecessor may still be reading the old vectors)
-  ptx::pdl_launch_dependents();  // the GEMM kernel may start its prologue on SMs as they drain (then waits for this grid)
-  encode_b_warp<BN, KRQ, STREAM>(B, N, K, ldb, chk, chk_ld, rounding, tiles_n, blockIdx.x * kEncWarps + (threadIdx.x >> 5),
-                    gridDim.x * kEncWarps, threadIdx.x & 31);
-}
-
-// The pre-pass of a strided batch (either layout of B): entry e = blockIdx.y, blockIdx.y + gridDim.y, ... reads
-// B + e*stride_b and writes its checksum operand at chk + e*chk_stride.
-// (KRQ / STREAM / rounding: the item shape, load policy and TF32 rounding of encode_b_kernel; a K-major B has one encode)
+// Either layout of B, any number of entries: entry e = blockIdx.y, blockIdx.y + gridDim.y, ... reads B + e*stride_b and
+// writes its checksum operand at chk + e*chk_stride (a single product: one entry, grid.y = 1).
+// KRQ / STREAM: the item shape and load policy of the MN-major encode (a K-major B has one encode); rounding: TF32 rounding.
 template <int BN, bool KMAJOR, int KRQ = 8, bool STREAM = false>
 __global__ void __launch_bounds__(kEncWarps * 32, 2)
-encode_batched_kernel(const float *__restrict__ B, int N, int K, int ldb, long long stride_b, int batch, float *__restrict__ chk,
-                      int chk_ld, long long chk_stride, int rounding, int tiles_n) {
-  ptx::pdl_wait();
-  ptx::pdl_launch_dependents();
-  for (int e = blockIdx.y; e < batch; e += gridDim.y) {
-    const int gw = blockIdx.x * kEncWarps + (threadIdx.x >> 5), nw = gridDim.x * kEncWarps, lane = threadIdx.x & 31;
-    if constexpr (KMAJOR)
-      encode_bk_warp<BN>(B + e * stride_b, N, K, ldb, chk + e * chk_stride, chk_ld, rounding, tiles_n, gw, nw, lane);
-    else
+encode_kernel(const float *__restrict__ B, int N, int K, int ldb, long long stride_b, int batch, float *__restrict__ chk,
+              int chk_ld, long long chk_stride, int rounding, int tiles_n) {
+  ptx::pdl_wait();               // (a programmatic dependent itself: the predecessor may still be reading the old vectors)
+  ptx::pdl_launch_dependents();  // the GEMM kernel may start its prologue on SMs as they drain (then waits for this grid)
+  const int gw = blockIdx.x * kEncWarps + (threadIdx.x >> 5), nw = gridDim.x * kEncWarps, lane = threadIdx.x & 31;
+  if constexpr (KMAJOR) {
+    // (entry pointers advanced rather than formed from e: 80 registers instead of 92, so 3 blocks per SM, not 2)
+    B += blockIdx.y * stride_b;
+    chk += blockIdx.y * chk_stride;
+    for (int e = blockIdx.y; e < batch; e += gridDim.y, B += gridDim.y * stride_b, chk += gridDim.y * chk_stride)
+      encode_bk_warp<BN>(B, N, K, ldb, chk, chk_ld, rounding, tiles_n, gw, nw, lane);
+  } else {
+    // (pointers advanced here would cost the KRQ = 4 encodes at BN = 32 / 64 their fourth block per SM)
+    for (int e = blockIdx.y; e < batch; e += gridDim.y)
       encode_b_warp<BN, KRQ, STREAM>(B + e * stride_b, N, K, ldb, chk + e * chk_stride, chk_ld, rounding, tiles_n, gw, nw, lane);
   }
-}
-
-// The pre-pass for a K-major B.
-template <int BN>
-__global__ void __launch_bounds__(kEncWarps * 32, 2)
-encode_bk_kernel(const float *__restrict__ B, int N, int K, int ldb, float *__restrict__ chk, int chk_ld, int rounding,
-                 int tiles_n) {
-  ptx::pdl_wait();
-  ptx::pdl_launch_dependents();
-  encode_bk_warp<BN>(B, N, K, ldb, chk, chk_ld, rounding, tiles_n, blockIdx.x * kEncWarps + (threadIdx.x >> 5),
-                     gridDim.x * kEncWarps, threadIdx.x & 31);
 }
 
 }  // namespace ftsgemm
