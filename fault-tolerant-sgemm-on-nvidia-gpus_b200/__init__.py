@@ -369,7 +369,15 @@ def _ptr(x) -> int:
 
 
 class FtSgemm:
-    """One handle = one device context (cuBLAS handle, checksum workspace, fault counters)."""
+    """One handle = one device context (cuBLAS handle, checksum workspace, fault counters).
+
+    CUDA graphs: matmul, bmm and linear (forward and backward) can be captured with torch.cuda.graph (its default global
+    capture mode) or torch.cuda.make_graphed_callables, first calls of a shape included.  A replay reads the tensors the
+    capture used -- copy new inputs into those same static tensors -- and writes C bit for bit as the eager call would; eager
+    calls and replays may interleave on one handle in stream order.  stats() synchronises only the stream of the handle's
+    last call, so synchronise the replay stream first; inside a capture it raises FtsgemmError(-2), as run_host, verify and
+    the baseline with host sync do.  The handle keeps what a graph uses until close(): close it after its graphs
+    (include/ftsgemm.h, "CUDA graphs")."""
 
     def __init__(self):
         self._h = C.c_void_p()
@@ -435,7 +443,8 @@ class FtSgemm:
         expanded operand (batch stride 0), a batch stride that is not a multiple of 4, or a matrix matmul could not read in
         place is copied once (bmm_plan); an out that cannot be written in place is computed in a contiguous buffer and copied
         back.  Fault and event coordinates (opts, stats()) are stacked kernel rows entry * kernel_M + row, transposed against
-        out when the call is swapped (a row-major out: the kernel's rows are out's columns).  No autograd."""
+        out when the call is swapped (a row-major out: the kernel's rows are out's columns).  No autograd.  Capturable in a
+        CUDA graph (see the class docstring); copies it makes are then graph-pool tensors, refreshed on every replay."""
         import torch
         for name, t in (("a", a), ("b", b)):
             if t.dim() != 3 or t.dtype != torch.float32 or not t.is_cuda:
@@ -493,7 +502,8 @@ class FtSgemm:
         injected faults (opts) and of stats() events are the kernel's, transposed against out in that case.  A kernel M or
         N (after the mapping) that is not a multiple of 4 raises FtsgemmError(-2) for the tensor-core ids, as run does.
         Runs on the current torch stream unless opts.stream says otherwise.  No autograd: linear() is the differentiable
-        F.linear.  This is bmm on a batch of one entry (a run_batched call with batch = 1, which is run_bias)."""
+        F.linear.  This is bmm on a batch of one entry (a run_batched call with batch = 1, which is run_bias).  Capturable in a
+        CUDA graph (see the class docstring)."""
         import torch
         for name, t in (("a", a), ("b", b)):
             if t.dim() != 2 or t.dtype != torch.float32 or not t.is_cuda:
@@ -523,7 +533,8 @@ class FtSgemm:
         grad_weight = grad_y^T @ x through matmul with the same kernel id and opts (both read in place), grad_bias =
         grad_y.sum(0) in torch.  Faults injected through opts land in the forward product only; faults detected in any of
         the three products are counted in stats().  The forward runs on the current torch stream unless opts.stream names
-        one; the backward runs on the stream autograd runs it on."""
+        one; the backward runs on the stream autograd runs it on.  Forward and backward can be captured in a CUDA graph, also
+        through torch.cuda.make_graphed_callables (see the class docstring)."""
         import torch
         if x.dtype != torch.float32 or not x.is_cuda or x.dim() < 1:
             raise TypeError("x must be a float32 CUDA tensor with at least one dimension")

@@ -16,6 +16,7 @@
 #include <array>
 #include <map>
 #include <mutex>
+#include <set>
 #include <string>
 #include <type_traits>
 
@@ -137,21 +138,25 @@ struct ftsgemm_handle_s {
   size_t chk_flag_bytes = kChkFlagBytes;  // bytes of d_chk_out in front of the expected checksums: the slab flags
   ChkKey chk_key;               // what d_chk holds
   // fused verdict exchange (ftsgemm_peer_*): this rank's mailbox (kMaxPeers slots), the peers' mailboxes mapped through
-  // CUDA IPC, the exit counter of the publishing launches and their sequence number
+  // CUDA IPC and the sequence number of the publishing launches
   double *d_mailbox = nullptr;
   double *peer_box[kMaxPeers] = {};
   bool peer_opened[kMaxPeers] = {};
   int peer_world = 0, peer_rank = 0;
   unsigned long long peer_seq = 0;
-  unsigned int *d_exit_count = nullptr;
-  int *d_front_done = nullptr;  // kernel front phase (operand transposes, encode): warps done, monotonic over launches
-  int front_done_value = 0;
+  LaunchSeq *d_seq = nullptr;   // launch sequence of the wgmma kernels: epoch, exit and front-phase counters
+  // CUDA graph capture: whether the running call is being captured; the private stream of allocations' uploads; the
+  // workspaces a captured launch references (never freed before ftsgemm_destroy) and those retired from the handle
+  bool capturing = false;
+  cudaStream_t s_up = nullptr;
+  std::set<const void *> graph_bufs;
+  std::vector<void *> retired;
   float *d_at = nullptr, *d_bt = nullptr;  // K-major copies of MN-major A and B (never allocated for a K-major operand)
   size_t at_bytes = 0, bt_bytes = 0;
   float *d_lo = nullptr;        // 3xTF32: A_lo | B_lo
   size_t lo_bytes = 0;
   float *d_aux = nullptr;       // baseline vectors
-  size_t aux_floats = 0;
+  size_t aux_bytes = 0;
   struct CachedPlan {
     std::vector<int> wave_target;   // per whole-tile ordinal: units that own more whole tiles than that
     int *d_wave_target = nullptr;
@@ -160,14 +165,13 @@ struct ftsgemm_handle_s {
     int4 *d_items = nullptr;
     int *d_off = nullptr;
     bool uploaded = false;
+    bool captured = false;      // referenced by a captured launch: never evicted
   };
   std::map<std::array<long long, 7>, CachedPlan> plans;  // key: kernel id, M, N, K, units, forced slices, batch
   int *d_wave_cnt = nullptr;    // wave re-synchronisation counters (cleared per launch)
   size_t wave_cnt_cap = 0;
-  int chk_epoch = 0;
   float *d_sk = nullptr;        // split-K partial tiles + flags
   size_t sk_bytes = 0;
-  int sk_epoch = 0;
   unsigned long long *d_trace = nullptr;  // debug timeline (ftsgemm_debug_trace), allocated on first use
   int trace_units = 0;
   float *d_stage[3] = {nullptr, nullptr, nullptr};  // run_host staging A, B, C
@@ -217,6 +221,16 @@ struct DeviceGuard {
     if (switched) cudaSetDevice(prev);
   }
 };
+
+// FTSGEMM_ERR_UNSUPPORTED when `stream` is being captured: for the entry points that synchronise a stream or copy to the
+// host, which a capture cannot hold (checked before any call that would invalidate the capture).
+#define FT_NOT_WHILE_CAPTURING(h, stream)           \
+  do {                                              \
+    bool cap__ = false;                             \
+    const int rc__ = is_capturing(h, stream, &cap__); \
+    if (rc__) return rc__;                          \
+    if (cap__) return FTSGEMM_ERR_UNSUPPORTED;      \
+  } while (0)
 
 // The kernels' watchdog (ptx.cuh) raises a device-wide flag instead of trapping; reported once, then cleared.
 int check_abort_flag(ftsgemm_handle_t h) {
@@ -442,14 +456,76 @@ void plan_tiles(int M, int N, int BN, int CG, bool ft, KernelParams *p) {
   }
 }
 
-int ensure_buf(ftsgemm_handle_t h, float **buf, size_t *have, size_t bytes) {
+// ------------------------------------------------------------------------------------------- CUDA graph capture
+// Whether work enqueued on `stream` is being captured into a graph (the legacy stream counts as capturing while a blocking
+// stream it would synchronise with is).
+int is_capturing(ftsgemm_handle_t h, cudaStream_t stream, bool *out) {
+  cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+  const cudaError_t e = cudaStreamIsCapturing(stream, &st);
+  if (e == cudaErrorStreamCaptureImplicit) {
+    cudaGetLastError();
+    *out = true;
+    return FTSGEMM_OK;
+  }
+  FT_CUDA(h, e);
+  *out = st != cudaStreamCaptureStatusNone;
+  return FTSGEMM_OK;
+}
+
+// Allocations and their uploads are not part of a captured call: for their scope the calling thread's capture mode is
+// relaxed (a capture in global mode -- torch's default -- forbids cudaMalloc and synchronous copies otherwise), and they
+// run on the handle's private stream, which is synchronised on its own.  PyTorch's caching allocator does the same.
+struct RelaxedCapture {
+  cudaStreamCaptureMode mode = cudaStreamCaptureModeRelaxed;
+  RelaxedCapture() { cudaThreadExchangeStreamCaptureMode(&mode); }
+  ~RelaxedCapture() { cudaThreadExchangeStreamCaptureMode(&mode); }
+};
+
+template <typename T>
+int dev_alloc(ftsgemm_handle_t h, T **p, size_t bytes) {
+  RelaxedCapture relaxed;
+  FT_CUDA(h, cudaMalloc(p, bytes));
+  return FTSGEMM_OK;
+}
+
+// Copies `bytes` from the host to device memory no launch is using yet (src == nullptr: zero-fills it), complete on return.
+int upload(ftsgemm_handle_t h, void *dst, const void *src, size_t bytes) {
+  RelaxedCapture relaxed;
+  if (src) FT_CUDA(h, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, h->s_up));
+  else FT_CUDA(h, cudaMemsetAsync(dst, 0, bytes, h->s_up));
+  FT_CUDA(h, cudaStreamSynchronize(h->s_up));
+  return FTSGEMM_OK;
+}
+
+// Drops a workspace from the handle.  One that a captured launch references, and any while a capture is running (cudaFree
+// synchronises the device), is retired instead: ftsgemm_destroy frees it.
+int release(ftsgemm_handle_t h, void *p) {
+  if (!p) return FTSGEMM_OK;
+  if (h->capturing || h->graph_bufs.count(p)) h->retired.push_back(p);
+  else FT_CUDA(h, cudaFree(p));
+  return FTSGEMM_OK;
+}
+
+template <typename T>
+int ensure_buf(ftsgemm_handle_t h, T **buf, size_t *have, size_t bytes) {
   if (*have >= bytes) return FTSGEMM_OK;
-  if (*buf) FT_CUDA(h, cudaFree(*buf));
+  const int rc = release(h, *buf);
+  if (rc) return rc;
   *buf = nullptr;
   *have = 0;
-  FT_CUDA(h, cudaMalloc(buf, bytes));
+  const int arc = dev_alloc(h, buf, bytes);
+  if (arc) return arc;
   *have = bytes;
   return FTSGEMM_OK;
+}
+
+// After a captured call: the workspaces it may reference stay allocated until ftsgemm_destroy.
+void pin_workspaces(ftsgemm_handle_t h) {
+  for (const void *p : {static_cast<const void *>(h->d_at), static_cast<const void *>(h->d_bt),
+                        static_cast<const void *>(h->d_chk_out), static_cast<const void *>(h->d_sk),
+                        static_cast<const void *>(h->d_lo), static_cast<const void *>(h->d_aux),
+                        static_cast<const void *>(h->d_wave_cnt), static_cast<const void *>(h->d_trace)})
+    if (p) h->graph_bufs.insert(p);
 }
 
 // One operand of ftsgemm_run_ex: MN-major (the reference's: element (r, k) at p[r + k*ld]) or K-major (p[k + r*ld]).
@@ -522,8 +598,8 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
     p.peer_world = h->peer_world;
     p.peer_rank = h->peer_rank;
     p.peer_seq = static_cast<double>(++h->peer_seq);
-    p.exit_count = h->d_exit_count;
   }
+  p.seq = h->d_seq;
 
   // The tensor maps read K-major operands: a K-major operand in place, an MN-major one through its K-major copy (written by
   // the kernel's front phase, row stride ldk: TMA needs 16-byte row strides).  The main loop is the same either way.
@@ -561,16 +637,28 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
     // (a batch: one checksum operand, one block of expected checksums and one run of slab flags per entry)
     const int n_slabs = p.tiles_m * CG * (kBM / 32) * bt.count;
     const long long chk_entry = static_cast<long long>(p.n_chk_cols) * chk_ld;
-    const float *chk_before = h->d_chk;
-    rc = ensure_buf(h, &h->d_chk, &h->chk_bytes, static_cast<size_t>(chk_entry) * bt.count * sizeof(float));
-    if (rc) return rc;
-    if (h->d_chk != chk_before) h->chk_key = ChkKey();  // reallocated: the cached encode is gone
+    const size_t chk_bytes = static_cast<size_t>(chk_entry) * bt.count * sizeof(float);
+    float *chk = nullptr;
+    if (h->capturing) {
+      // a captured call encodes on every replay, into a checksum operand of its own: replays would otherwise overwrite
+      // the one an eager call with reuse_b_checksums relies on
+      rc = dev_alloc(h, &chk, chk_bytes);
+      if (rc) return rc;
+      h->retired.push_back(chk);
+    } else {
+      const float *chk_before = h->d_chk;
+      rc = ensure_buf(h, &h->d_chk, &h->chk_bytes, chk_bytes);
+      if (rc) return rc;
+      if (h->d_chk != chk_before) h->chk_key = ChkKey();  // reallocated: the cached encode is gone
+      chk = h->d_chk;
+    }
     const size_t out_floats = static_cast<size_t>(M) * p.n_chk_cols * bt.count;
     const size_t n_flags = static_cast<size_t>(n_slabs) * p.tiles_c;
-    if (n_flags * sizeof(int) > h->chk_flag_bytes) {
-      // grow the flag region: a new buffer, so that its flags are cleared and the epoch restarts below
-      h->chk_flag_bytes = (n_flags * sizeof(int) + kChkFlagBytes - 1) / kChkFlagBytes * kChkFlagBytes;
-      FT_CUDA(h, cudaFree(h->d_chk_out));
+    if (n_flags * sizeof(SeqFlag) > h->chk_flag_bytes) {
+      // grow the flag region: a new buffer
+      h->chk_flag_bytes = (n_flags * sizeof(SeqFlag) + kChkFlagBytes - 1) / kChkFlagBytes * kChkFlagBytes;
+      rc = release(h, h->d_chk_out);
+      if (rc) return rc;
       h->d_chk_out = nullptr;
       h->chk_out_bytes = 0;
     }
@@ -578,23 +666,20 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
     const float *out_before = h->d_chk_out;
     rc = ensure_buf(h, &h->d_chk_out, &h->chk_out_bytes, flag_bytes + out_floats * sizeof(float));
     if (rc) return rc;
-    p.chk_flags = reinterpret_cast<int *>(h->d_chk_out);  // fixed location: stale flags never equal a new epoch
+    // the flags of a new buffer start at 0, below every epoch (LaunchSeq): they never need clearing again
+    if (h->d_chk_out != out_before && (rc = upload(h, h->d_chk_out, nullptr, flag_bytes))) return rc;
+    p.chk_flags = reinterpret_cast<SeqFlag *>(h->d_chk_out);
     p.chk_out = h->d_chk_out + flag_bytes / sizeof(float);
-    if (h->d_chk_out != out_before || h->chk_epoch > (1 << 30)) {
-      FT_CUDA(h, cudaMemsetAsync(p.chk_flags, 0, flag_bytes, stream));
-      h->chk_epoch = 0;
-    }
-    p.chk_epoch = ++h->chk_epoch;
     p.dbg_flags = static_cast<int>(dbg("ft_dbg", 0)) & 1;
     const ChkKey chk_key = {dB, N, K, BN, B.kmajor, B.ld, bt.count, bt.sb};
-    const bool reuse = o.reuse_b_checksums && h->chk_key == chk_key;
+    const bool reuse = !h->capturing && o.reuse_b_checksums && h->chk_key == chk_key;
     // Default: the encode is part of the FRONT PHASE of the GEMM kernel (KernelParams::enc_front) -- one launch per fused
     // GEMM, like the reference (sgemm.cu:191-192); only below ~8 MB of B the stand-alone pre-pass is used.
     const long long ef = dbg("enc_front", -2);
     enc_front = !reuse && (ef >= 0 ? ef != 0 : 4.0 * N * static_cast<double>(K) * bt.count >= static_cast<double>(dbg("enc_front_min_mb", 8)) * 1048576.0);
     if (enc_front) {
       p.enc_front = 1;
-      p.enc_out = h->d_chk;
+      p.enc_out = chk;
       p.enc_ld = chk_ld;
     }
     if (!reuse && !enc_front) {
@@ -619,7 +704,7 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
       const long long chk_stride = bt.count > 1 ? chk_entry : 0;
       rc = with_tile(BN, CG, [&](auto bn, auto) {
         auto launch = [&](auto kern) {
-          FT_CUDA(h, cudaLaunchKernelEx(&ec, kern, dB, N, K, B.ld, bt.sb, bt.count, h->d_chk, chk_ld, chk_stride, rounding, p.tiles_n));
+          FT_CUDA(h, cudaLaunchKernelEx(&ec, kern, dB, N, K, B.ld, bt.sb, bt.count, chk, chk_ld, chk_stride, rounding, p.tiles_n));
           return FTSGEMM_OK;
         };
         if (B.kmajor) return launch(encode_kernel<bn, true>);
@@ -631,8 +716,8 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
       ++h->launch_count;
       FT_CUDA(h, cudaGetLastError());
     }
-    if (!reuse) h->chk_key = chk_key;
-    rc = make_tmap_kmajor(h, &tmC, h->d_chk, p.n_chk_cols, K, chk_ld, chk_entry, bt.count, BN / CG);
+    if (!reuse && !h->capturing) h->chk_key = chk_key;
+    rc = make_tmap_kmajor(h, &tmC, chk, p.n_chk_cols, K, chk_ld, chk_entry, bt.count, BN / CG);
     if (rc) return rc;
   }
   // ---- work plan (plan.h), cached per shape on the handle
@@ -648,19 +733,15 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
     p.chk_slices = choose_chk_slices(p, max_units, K);
     const size_t flag_bytes = h->chk_flag_bytes;
     const size_t n_flags_s = static_cast<size_t>(p.tiles_m) * CG * (kBM / 32) * p.tiles_c * p.chk_slices * bt.count;
-    if (p.chk_slices > 1 && n_flags_s * sizeof(int) > flag_bytes) p.chk_slices = 1;
+    if (p.chk_slices > 1 && n_flags_s * sizeof(SeqFlag) > flag_bytes) p.chk_slices = 1;
     if (p.chk_slices > 1) {
       // one plane of expected checksums per slice (and entry)
       const size_t out_floats = static_cast<size_t>(M) * p.n_chk_cols * p.chk_slices * bt.count;
       const float *out_before = h->d_chk_out;
       rc = ensure_buf(h, &h->d_chk_out, &h->chk_out_bytes, flag_bytes + out_floats * sizeof(float));
       if (rc) return rc;
-      if (h->d_chk_out != out_before) {  // reallocated: fresh flags, restart the epoch
-        FT_CUDA(h, cudaMemsetAsync(h->d_chk_out, 0, flag_bytes, stream));
-        h->chk_epoch = 1;
-        p.chk_epoch = 1;
-      }
-      p.chk_flags = reinterpret_cast<int *>(h->d_chk_out);
+      if (h->d_chk_out != out_before && (rc = upload(h, h->d_chk_out, nullptr, flag_bytes))) return rc;  // fresh flags
+      p.chk_flags = reinterpret_cast<SeqFlag *>(h->d_chk_out);
       p.chk_out = h->d_chk_out + flag_bytes / sizeof(float);
     }
   }
@@ -670,9 +751,9 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
                                         bt.count};
   ftsgemm_handle_s::CachedPlan &cp = h->plans[key];
   if (!cp.uploaded) {
-    if (h->plans.size() > 64) {  // bound the cache: drop everything but this entry
+    if (h->plans.size() > 64 && !h->capturing) {  // bound the cache: drop everything but this entry and captured plans
       for (auto it = h->plans.begin(); it != h->plans.end();) {
-        if (&it->second == &cp) { ++it; continue; }
+        if (&it->second == &cp || it->second.captured) { ++it; continue; }
         cudaFree(it->second.d_items);
         cudaFree(it->second.d_off);
         cudaFree(it->second.d_wave_target);
@@ -685,10 +766,11 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
       const PlanItem &it = cp.plan.items[i];
       cp.packed[i] = make_int4(it.tile, it.kb_begin | (it.kb_end << 16), it.kind | (it.slice << 8), it.split_idx);
     }
-    FT_CUDA(h, cudaMalloc(&cp.d_items, std::max<size_t>(1, cp.packed.size()) * sizeof(int4)));
-    FT_CUDA(h, cudaMalloc(&cp.d_off, cp.plan.offsets.size() * sizeof(int)));
-    FT_CUDA(h, cudaMemcpyAsync(cp.d_items, cp.packed.data(), cp.packed.size() * sizeof(int4), cudaMemcpyHostToDevice, stream));
-    FT_CUDA(h, cudaMemcpyAsync(cp.d_off, cp.plan.offsets.data(), cp.plan.offsets.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
+    if ((rc = dev_alloc(h, &cp.d_items, std::max<size_t>(1, cp.packed.size()) * sizeof(int4))) ||
+        (rc = dev_alloc(h, &cp.d_off, cp.plan.offsets.size() * sizeof(int))) ||
+        (rc = upload(h, cp.d_items, cp.packed.data(), cp.packed.size() * sizeof(int4))) ||
+        (rc = upload(h, cp.d_off, cp.plan.offsets.data(), cp.plan.offsets.size() * sizeof(int))))
+      return rc;
     {  // wave targets (see KernelParams::wave_cnt)
       std::vector<int> per_unit(static_cast<size_t>(cp.plan.units), 0);
       int max_w = 0;
@@ -700,43 +782,29 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
       cp.wave_target.assign(static_cast<size_t>(max_w) + 1, 0);
       for (int u = 0; u < cp.plan.units; ++u)
         for (int w = 0; w < per_unit[u]; ++w) ++cp.wave_target[w];
-      FT_CUDA(h, cudaMalloc(&cp.d_wave_target, cp.wave_target.size() * sizeof(int)));
-      FT_CUDA(h, cudaMemcpyAsync(cp.d_wave_target, cp.wave_target.data(), cp.wave_target.size() * sizeof(int), cudaMemcpyHostToDevice, stream));
+      if ((rc = dev_alloc(h, &cp.d_wave_target, cp.wave_target.size() * sizeof(int))) ||
+          (rc = upload(h, cp.d_wave_target, cp.wave_target.data(), cp.wave_target.size() * sizeof(int))))
+        return rc;
     }
     cp.uploaded = true;
   }
+  if (h->capturing) cp.captured = true;
   const int units = cp.plan.units;
-  {
-    const int inc = units * CG * (kThreads / 32);
-    if (h->d_front_done == nullptr) {
-      FT_CUDA(h, cudaMalloc(&h->d_front_done, sizeof(int)));
-      FT_CUDA(h, cudaMemsetAsync(h->d_front_done, 0, sizeof(int), stream));
-      h->front_done_value = 0;
-    } else if (h->front_done_value > (1 << 30) - inc) {
-      FT_CUDA(h, cudaMemsetAsync(h->d_front_done, 0, sizeof(int), stream));
-      h->front_done_value = 0;
-    }
-    h->front_done_value += inc;
-    p.front_done = h->d_front_done;
-    p.front_target = h->front_done_value;
-  }
+  p.front_target = units * CG * (kThreads / 32);
   p.plan = cp.d_items;
   p.plan_off = cp.d_off;
   p.sk_tiles = cp.plan.sk_tiles;
   p.sk_slices = cp.plan.sk_slices;
   if (p.sk_tiles > 0) {
-    const size_t flag_bytes = 65536;  // fixed location at the start of the buffer
+    // fixed location at the start of the buffer: the 16384 flags build_plan allows for
+    const size_t flag_bytes = 16384 * sizeof(SeqFlag);
     const size_t ws_floats = static_cast<size_t>(p.sk_tiles) * (p.sk_slices - 1) * CG * kBM * BN;
     const float *before = h->d_sk;
     rc = ensure_buf(h, &h->d_sk, &h->sk_bytes, flag_bytes + ws_floats * sizeof(float));
     if (rc) return rc;
-    p.sk_flags = reinterpret_cast<int *>(h->d_sk);
+    if (h->d_sk != before && (rc = upload(h, h->d_sk, nullptr, flag_bytes))) return rc;  // fresh flags, below every epoch
+    p.sk_flags = reinterpret_cast<SeqFlag *>(h->d_sk);
     p.sk_ws = h->d_sk + flag_bytes / sizeof(float);
-    if (h->d_sk != before || h->sk_epoch > (1 << 30)) {  // fresh buffer (or epoch wrap): no flag may alias a live epoch
-      FT_CUDA(h, cudaMemsetAsync(p.sk_flags, 0, flag_bytes, stream));
-      h->sk_epoch = 0;
-    }
-    p.sk_epoch = ++h->sk_epoch;
   }
   {
     // Helper-assisted final epilogues (the helper warp of each 32-row quadrant takes the upper half of the columns): on
@@ -752,9 +820,9 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
     if (on && cp.wave_target.size() > 1) {
       const size_t bytes = cp.wave_target.size() * sizeof(int);
       if (h->d_wave_cnt == nullptr || h->wave_cnt_cap < cp.wave_target.size()) {
-        if (h->d_wave_cnt) FT_CUDA(h, cudaFree(h->d_wave_cnt));
+        if ((rc = release(h, h->d_wave_cnt))) return rc;
         h->d_wave_cnt = nullptr;
-        FT_CUDA(h, cudaMalloc(&h->d_wave_cnt, bytes));
+        if ((rc = dev_alloc(h, &h->d_wave_cnt, bytes))) return rc;
         h->wave_cnt_cap = cp.wave_target.size();
       }
       FT_CUDA(h, cudaMemsetAsync(h->d_wave_cnt, 0, bytes, stream));
@@ -765,9 +833,9 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
   if (dbg("trace", 0) != 0) {
     const int cap = 64;
     if (h->d_trace == nullptr || h->trace_units < units) {
-      if (h->d_trace) FT_CUDA(h, cudaFree(h->d_trace));
+      if ((rc = release(h, h->d_trace))) return rc;
       h->d_trace = nullptr;
-      FT_CUDA(h, cudaMalloc(&h->d_trace, static_cast<size_t>(units) * cap * 8 * sizeof(unsigned long long)));
+      if ((rc = dev_alloc(h, &h->d_trace, static_cast<size_t>(units) * cap * 8 * sizeof(unsigned long long)))) return rc;
       h->trace_units = units;
     }
     FT_CUDA(h, cudaMemsetAsync(h->d_trace, 0, static_cast<size_t>(units) * cap * 8 * sizeof(unsigned long long), stream));
@@ -777,6 +845,7 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
   // Programmatic dependent launch by default: the kernel's launch latency and prologue overlap the tail of whatever
   // precedes it in the stream; every thread executes griddepcontrol.wait before the first global access.
   p.pdl_wait = dbg("pdl_chain", 1) != 0 ? 1 : 0;
+  if (h->capturing) pin_workspaces(h);
   h->last_stream = stream;
   ++h->launch_count;
   return with_tile(BN, CG, [&](auto bn, auto cg) {
@@ -981,6 +1050,7 @@ int ftsgemm_debug_trace(ftsgemm_handle_t h, unsigned long long *out, int cap_u64
   if (!h->d_trace) return 0;
   const int n = h->trace_units * 64 * 8;
   if (cap_u64 < n) return FTSGEMM_ERR_INVALID_ARG;
+  FT_NOT_WHILE_CAPTURING(h, h->last_stream);
   FT_CUDA(h, cudaDeviceSynchronize());
   FT_CUDA(h, cudaMemcpy(out, h->d_trace, static_cast<size_t>(n) * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
   return h->trace_units;
@@ -1019,9 +1089,13 @@ int ftsgemm_create(ftsgemm_handle_t *out) {
     delete h;
     return FTSGEMM_ERR_CUBLAS;
   }
+  const LaunchSeq seq0 = {1ull, 0u, 0};  // epoch 1: above the 0 of fresh flag regions
   if (cudaMalloc(&h->d_stats, sizeof(DeviceStats)) != cudaSuccess ||
       cudaMemset(h->d_stats, 0, sizeof(DeviceStats)) != cudaSuccess ||
-      cudaMalloc(&h->d_verify, 4 * sizeof(double)) != cudaSuccess) {
+      cudaMalloc(&h->d_verify, 4 * sizeof(double)) != cudaSuccess ||
+      cudaMalloc(&h->d_seq, sizeof(LaunchSeq)) != cudaSuccess ||
+      cudaMemcpy(h->d_seq, &seq0, sizeof(seq0), cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaStreamCreateWithFlags(&h->s_up, cudaStreamNonBlocking) != cudaSuccess) {
     ftsgemm_destroy(h);
     return FTSGEMM_ERR_CUDA;
   }
@@ -1047,13 +1121,14 @@ int ftsgemm_destroy(ftsgemm_handle_t h) {
   }
   cudaFree(h->d_aux);
   cudaFree(h->d_lo);
-  cudaFree(h->d_front_done);
+  cudaFree(h->d_seq);
+  for (void *p : h->retired) cudaFree(p);
+  if (h->s_up) cudaStreamDestroy(h->s_up);
   cudaFree(h->d_at);
   cudaFree(h->d_bt);
   for (int r = 0; r < kMaxPeers; ++r)
     if (h->peer_opened[r]) cudaIpcCloseMemHandle(h->peer_box[r]);
   cudaFree(h->d_mailbox);
-  cudaFree(h->d_exit_count);
   cudaFree(h->d_verify);
   for (int i = 0; i < 3; ++i) cudaFree(h->d_stage[i]);
   if (h->s_in) {
@@ -1136,6 +1211,14 @@ int ftsgemm_run_batched(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, 
   if (orc) return orc;
   DeviceGuard guard(h);
   cudaStream_t stream = static_cast<cudaStream_t>(o.stream);
+  {
+    bool cap = false;
+    const int crc = is_capturing(h, stream, &cap);
+    if (crc) return crc;
+    // a peer-connected handle's verdict carries a host sequence number, which a replay cannot advance
+    if (cap && h->peer_world > 0) return FTSGEMM_ERR_UNSUPPORTED;
+    h->capturing = cap;
+  }
   if (v->info.engine == 1 && v->bn == 0) {  // ids 20 / 40: per-shape choice (over the tiles of all entries)
     v = find_variant(select_variant(M, N, v->info.fault_tolerant != 0, bt.count));
     if (!v) return FTSGEMM_ERR_UNSUPPORTED;
@@ -1235,6 +1318,7 @@ int ftsgemm_get_stats(ftsgemm_handle_t h, ftsgemm_stats *out) {
   if (!h) return FTSGEMM_ERR_NO_DEVICE;
   if (!out) return FTSGEMM_ERR_INVALID_ARG;
   DeviceGuard guard(h);
+  FT_NOT_WHILE_CAPTURING(h, h->last_stream);
   FT_CUDA(h, cudaStreamSynchronize(h->last_stream));
   const int arc = check_abort_flag(h);
   if (arc) return arc;
@@ -1272,8 +1356,6 @@ int ftsgemm_peer_export(ftsgemm_handle_t h, void *ipc_handle_64) {
     const size_t bytes = static_cast<size_t>(kMaxPeers) * kPeerSlotDoubles * sizeof(double);
     FT_CUDA(h, cudaMalloc(&h->d_mailbox, bytes));
     FT_CUDA(h, cudaMemset(h->d_mailbox, 0, bytes));
-    FT_CUDA(h, cudaMalloc(&h->d_exit_count, sizeof(unsigned int)));
-    FT_CUDA(h, cudaMemset(h->d_exit_count, 0, sizeof(unsigned int)));
   }
   cudaIpcMemHandle_t hd;
   FT_CUDA(h, cudaIpcGetMemHandle(&hd, h->d_mailbox));
@@ -1307,6 +1389,7 @@ int ftsgemm_peer_verdict(ftsgemm_handle_t h, double *out8, double *per_rank /* w
   if (!h) return FTSGEMM_ERR_NO_DEVICE;
   if (!out8 || h->peer_world < 1) return FTSGEMM_ERR_INVALID_ARG;
   DeviceGuard guard(h);
+  FT_NOT_WHILE_CAPTURING(h, h->last_stream);
   FT_CUDA(h, cudaStreamSynchronize(h->last_stream));
   const int arc = check_abort_flag(h);
   if (arc) return arc;
@@ -1366,6 +1449,7 @@ int ftsgemm_run_host(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, con
   const int orc = load_opts(opts, &o);
   if (orc) return orc;
   DeviceGuard guard(h);
+  FT_NOT_WHILE_CAPTURING(h, static_cast<cudaStream_t>(o.stream));
   const size_t bytes[3] = {sizeof(float) * M * static_cast<size_t>(K), sizeof(float) * N * static_cast<size_t>(K),
                            sizeof(float) * M * static_cast<size_t>(N)};
   for (int i = 0; i < 3; ++i)
@@ -1447,16 +1531,19 @@ int ftsgemm_baseline(ftsgemm_handle_t h, int M, int N, int K, const float *dA, c
   DeviceGuard guard(h);
   cudaStream_t stream = static_cast<cudaStream_t>(o.stream);
   const bool host_sync = o.baseline_host_sync != 0;
+  {
+    bool cap = false;
+    const int crc = is_capturing(h, stream, &cap);
+    if (crc) return crc;
+    if (cap && host_sync) return FTSGEMM_ERR_UNSUPPORTED;  // it synchronises the stream between its steps
+    h->capturing = cap;
+  }
   const int mx = M > N ? M : N;
   // aux layout: ones[mx] | c_row[M] | c_col[N] | a_col[256] | b_row[256] | acol_x_b[N] | brow_x_a[M] | res[2] | consts[3]
   const size_t need = static_cast<size_t>(mx) + M + N + 256 + 256 + N + M + 2 + 3;
-  if (h->aux_floats < need) {
-    if (h->d_aux) FT_CUDA(h, cudaFree(h->d_aux));
-    h->d_aux = nullptr;
-    h->aux_floats = 0;
-    FT_CUDA(h, cudaMalloc(&h->d_aux, need * sizeof(float)));
-    h->aux_floats = need;
-  }
+  const int arc = ensure_buf(h, &h->d_aux, &h->aux_bytes, need * sizeof(float));
+  if (arc) return arc;
+  if (h->capturing) pin_workspaces(h);
   float *ones = h->d_aux, *c_row = ones + mx, *c_col = c_row + M, *a_col = c_col + N, *b_row = a_col + 256,
         *acol_x_b = b_row + 256, *brow_x_a = acol_x_b + N, *res = brow_x_a + M;
   fill_kernel<<<(mx + 255) / 256, 256, 0, stream>>>(ones, 1.0f, mx);
@@ -1509,6 +1596,7 @@ int ftsgemm_verify(ftsgemm_handle_t h, const float *d_ref, const float *d_x, int
   if (!d_ref || !d_x || M <= 0 || N <= 0) return FTSGEMM_ERR_INVALID_ARG;
   DeviceGuard guard(h);
   cudaStream_t stream = static_cast<cudaStream_t>(stream_v);
+  FT_NOT_WHILE_CAPTURING(h, stream);
   unsigned long long init[4];
   init[0] = ~0ull;
   double z = 0.0;

@@ -69,6 +69,22 @@ struct DeviceStats {
   unsigned long long epilogue_faults;  // row segments whose store pass failed its check (protect_epilogue)
 };
 
+// The launch sequence of one handle, in device memory, shared by the CTAs of a launch and inherited by the next launch on
+// the handle.  Nothing in it is baked into the kernel parameters, so a captured launch replays correctly and eager calls
+// and graph replays can interleave on one handle:
+//   epoch       sequence number of the running launch.  Every CTA reads it after griddepcontrol.wait (stream order and PDL
+//               guarantee that the previous launch has completed); checksum and cut-tile flags are raised to it and awaited
+//               for it.  It is 64-bit and only grows, so a stale flag never equals a live epoch (2^64 launches do not wrap).
+//   exit_count  CTAs of the running launch that have finished
+//   front_done  warps of the running launch that have finished their front-phase share
+// The last CTA to finish resets exit_count and front_done and advances epoch (ftsgemm_tc_kernel's exit).
+struct LaunchSeq {
+  unsigned long long epoch;
+  unsigned int exit_count;
+  int front_done;
+};
+using SeqFlag = unsigned long long;  // a checksum or cut-tile flag: the epoch of the launch that last raised it
+
 struct KernelParams {
   int M, N, K;
   float *C;
@@ -96,8 +112,7 @@ struct KernelParams {
   const int *plan_off;
   int sk_tiles, sk_slices;
   float *sk_ws;         // per (piece < sk_slices-1, cut tile, CTA of the group): one raw 128 x BN accumulator tile
-  int *sk_flags;        // [((piece*sk_tiles + cut tile)*CG + cta_rank)*4 + quadrant] = sk_epoch once written
-  int sk_epoch;
+  SeqFlag *sk_flags;    // [((piece*sk_tiles + cut tile)*CG + cta_rank)*4 + quadrant] = epoch once written
   // fault tolerance: checksum tile-columns
   int tiles_c;          // number of BN-wide checksum tile-columns (0 when FT is off)
   int chk_slices;       // >= 1: every checksum tile is computed as chk_slices independent K-slices (one plan item each, on
@@ -106,8 +121,7 @@ struct KernelParams {
                         // checksums in plane s of chk_out / chk_flags, the check adds the planes in slice order
   int n_chk_cols;       // tiles_n * kChkPerTile
   float *chk_out;       // M x n_chk_cols, column-major (ld = M): expected checksums r1/r2 (hi, lo each)
-  int *chk_flags;       // [slab * tiles_c + c] = chk_epoch once checksum tile-column c of that 32-row slab is published
-  int chk_epoch;
+  SeqFlag *chk_flags;   // [slab * tiles_c + c] = epoch once checksum tile-column c of that 32-row slab is published
   // wave re-synchronisation (large problems): the leader producers form a barrier at every whole-tile boundary, so that
   // the units keep streaming the same k range of the A / B panels they share (without it the start times drift apart
   // wave by wave)
@@ -120,13 +134,13 @@ struct KernelParams {
                         //    pre-pass or the caller's kernels): every thread executes griddepcontrol.wait after the
                         //    barrier initialisation, so that only the launch latency overlaps the predecessor's tail
   // Front phase (every warp of the grid, before the roles start): its share of the operand transposes and, with enc_front
-  // (B larger than ~8 MB), of the encode of B -- instead of separate launches.  Each warp adds 1 to front_done when its
-  // share is stored; the producers start loading once front_done reaches front_target.
+  // (B larger than ~8 MB), of the encode of B -- instead of separate launches.  Each warp adds 1 to seq->front_done when
+  // its share is stored; the producers start loading once it reaches front_target.
   int enc_front;
   float *enc_out;       // checksum operand, K-major: [checksum column][enc_ld]
   int enc_ld;
-  int *front_done;      // monotonic counter: warps that have finished their share, over all launches
-  int front_target;
+  int front_target;     // warps of this launch: units * CG * 12, the same in every replay
+  LaunchSeq *seq;       // the handle's launch sequence (epoch, exit and front-phase counters)
   float tau_abs, tau_rel;
   int detect_only;
   // Fallback for rows that are flagged but cannot be repaired from the two checksums (upset too small to locate, two
@@ -153,7 +167,6 @@ struct KernelParams {
   double *peer_box[kMaxPeers];
   int peer_world, peer_rank;
   double peer_seq;
-  unsigned int *exit_count;  // CTAs of this launch that have finished (the last one resets it)
   // debug timeline (ftsgemm_debug_trace): per unit and item 8 x u64 = %globaltimer ns at {producer start, producer end,
   // MMA start, MMA issue end, epilogue start (accumulator complete), after check/fold, epilogue end}, tile | kind << 24
   unsigned long long *trace;
@@ -320,6 +333,18 @@ struct SegIter {
 __device__ __forceinline__ int ld_acquire(const int *p) {
   int v;
   asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
+__device__ __forceinline__ SeqFlag ld_acquire(const SeqFlag *p) {
+  SeqFlag v;
+  asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+// The epoch of the running launch (LaunchSeq): read where a flag is raised or awaited, from L2.  Constant for the whole
+// launch: only the last CTA to exit advances it.
+__device__ __forceinline__ SeqFlag live_epoch(const KernelParams &p) {
+  SeqFlag v;
+  asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(&p.seq->epoch) : "memory");
   return v;
 }
 
@@ -535,11 +560,12 @@ __device__ __forceinline__ void abft_check(const KernelParams &p, uint32_t taddr
   //      prefetch already found it raised) ----
   if (!xp.ready) {
     const int nf = chk_flags_per_slab(p);
-    const int *flag = p.chk_flags + (slab_ofs + (m0_cta >> 5) + q) * nf;
+    const SeqFlag *flag = p.chk_flags + (slab_ofs + (m0_cta >> 5) + q) * nf;
     if (lane == 0) {
+      const SeqFlag epoch = live_epoch(p);
       for (int c = 0; c < nf; ++c) {
         ptx::Watchdog wd;
-        while (ld_acquire(flag + c) != p.chk_epoch) {
+        while (ld_acquire(flag + c) != epoch) {
           __nanosleep(64);
           if (wd.tick()) break;
         }
@@ -926,7 +952,7 @@ __device__ __forceinline__ int stored_value_fault(const KernelParams &p, int q, 
 // warps of the unit that owns the next piece load it into their registers before that piece's first wgmma.
 // ------------------------------------------------------------------------------------------------------------
 template <int BN>
-__device__ __forceinline__ void sk_dump_partial(const KernelParams &p, uint32_t taddr, float *ws, int *flag, int lane) {
+__device__ __forceinline__ void sk_dump_partial(const KernelParams &p, uint32_t taddr, float *ws, SeqFlag *flag, int lane) {
 #pragma unroll 1
   for (int c = 0; c < BN / 32; ++c) {
     uint32_t v[32];
@@ -936,7 +962,7 @@ __device__ __forceinline__ void sk_dump_partial(const KernelParams &p, uint32_t 
   }
   __threadfence();
   __syncwarp();
-  if (lane == 0) atomicExch(flag, p.sk_epoch);
+  if (lane == 0) atomicExch(flag, live_epoch(p));
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1355,7 +1381,7 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     __syncwarp();              // the warp's stores are ordered before lane 0's release (cumulativity)
     if (lane == 0) {
       ptx::fence_acq_rel_gpu();
-      atomicAdd(p.front_done, 1);
+      atomicAdd(&p.seq->front_done, 1);
     }
   }
   if (warp == 0) {
@@ -1363,7 +1389,7 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     // warp-uniform loop, one elected lane issues the TMA instructions (see ptx::elect_one)
     if (lane == 0) {
       ptx::Watchdog wd;
-      while (ld_acquire(p.front_done) - p.front_target < 0) {
+      while (ld_acquire(&p.seq->front_done) < p.front_target) {
         __nanosleep(64);
         if (wd.tick()) break;
       }
@@ -1483,10 +1509,11 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (SEED && (sg.kind == 2 || sg.kind == 3)) {
         // ... unless it continues a cut tile: seed: the previous piece's parked accumulator (its 32-row quadrant is complete once its flag is raised)
         const int slot = ((sg.slice - 1) * p.sk_tiles + sg.split_idx) * CG + cta_rank;
-        const int *flag = p.sk_flags + slot * 4 + ((cw * 64 + wq * 16) >> 5);
+        const SeqFlag *flag = p.sk_flags + slot * 4 + ((cw * 64 + wq * 16) >> 5);
         if (lane == 0) {
           ptx::Watchdog wd;
-          while (ld_acquire(flag) != p.sk_epoch) {
+          const SeqFlag epoch = live_epoch(p);
+          while (ld_acquire(flag) != epoch) {
             __nanosleep(64);
             if (wd.tick()) break;
           }
@@ -1585,7 +1612,7 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         __threadfence();
         __syncwarp();
         if (lane == 0)
-          atomicExch(p.chk_flags + (slab_ofs + (m0_cta >> 5) + q) * chk_flags_per_slab(p) + tc.slice * p.tiles_c + tc.n_blk, p.chk_epoch);
+          atomicExch(p.chk_flags + (slab_ofs + (m0_cta >> 5) + q) * chk_flags_per_slab(p) + tc.slice * p.tiles_c + tc.n_blk, live_epoch(p));
       } else {
         // final epilogue of a data tile; with epi_assist the helper warp of this quadrant owns the chunks [kMid, BN/32)
         const int c_mid = assist_on ? kMid : BN / 32;
@@ -1660,31 +1687,40 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   // (CG = 2: neither CTA exits while the peer may still arrive on its barriers)
   if constexpr (CG == 2) ptx::cluster_sync();
   else __syncthreads();
-  if (FT && p.peer_world > 0 && threadIdx.x == 0) {
-    // fused verdict push: every CTA's counter updates are ordered before its arrival; the last arrival publishes
-    __threadfence();
-    const unsigned int arrived = atomicAdd(p.exit_count, 1u);
+  if (threadIdx.x == 0) {
+    // Exit.  The last CTA to arrive -- every CTA of the launch is past its front-phase wait and its flag waits by now --
+    // does the fused verdict push, resets the counters and advances the epoch for the next launch on the handle, which
+    // reads them after this grid has completed.  (Only the verdict push reads what other CTAs wrote: their counter updates
+    // are ordered before their arrival.)
+    const bool push = FT && p.peer_world > 0;
+    if (push) __threadfence();
+    const unsigned int arrived = atomicAdd(&p.seq->exit_count, 1u);
     if (arrived == gridDim.x - 1) {
-      __threadfence();
-      const volatile DeviceStats *st = p.stats;
-      double v[8];
-      v[0] = static_cast<double>(st->tiles);
-      v[1] = static_cast<double>(st->rows_checked);
-      v[2] = static_cast<double>(st->detected);
-      v[3] = static_cast<double>(st->corrected);
-      v[4] = static_cast<double>(st->uncorrectable);
-      v[5] = static_cast<double>(st->checksum_faults);
-      v[6] = static_cast<double>(__uint_as_float(st->max_abs_bits));
-      v[7] = static_cast<double>(__uint_as_float(st->max_rel_bits));
-      // every value travels with the launch's sequence number in ONE 16-byte store, so a reader can tell a complete
-      // vector (eight equal sequence numbers) without a system-scope fence between data and flag: one NVLink round trip
-      // at the end of the kernel instead of two
-      for (int r = 0; r < p.peer_world; ++r) {
-        double2 *slot = reinterpret_cast<double2 *>(p.peer_box[r] + p.peer_rank * kPeerSlotDoubles);
+      if (push) {
+        __threadfence();
+        const volatile DeviceStats *st = p.stats;
+        double v[8];
+        v[0] = static_cast<double>(st->tiles);
+        v[1] = static_cast<double>(st->rows_checked);
+        v[2] = static_cast<double>(st->detected);
+        v[3] = static_cast<double>(st->corrected);
+        v[4] = static_cast<double>(st->uncorrectable);
+        v[5] = static_cast<double>(st->checksum_faults);
+        v[6] = static_cast<double>(__uint_as_float(st->max_abs_bits));
+        v[7] = static_cast<double>(__uint_as_float(st->max_rel_bits));
+        // every value travels with the launch's sequence number in ONE 16-byte store, so a reader can tell a complete
+        // vector (eight equal sequence numbers) without a system-scope fence between data and flag: one NVLink round trip
+        // at the end of the kernel instead of two
+        for (int r = 0; r < p.peer_world; ++r) {
+          double2 *slot = reinterpret_cast<double2 *>(p.peer_box[r] + p.peer_rank * kPeerSlotDoubles);
 #pragma unroll
-        for (int i = 0; i < 8; ++i) slot[i] = make_double2(v[i], p.peer_seq);
+          for (int i = 0; i < 8; ++i) slot[i] = make_double2(v[i], p.peer_seq);
+        }
       }
-      *p.exit_count = 0u;
+      p.seq->front_done = 0;
+      p.seq->exit_count = 0u;
+      const SeqFlag next = live_epoch(p) + 1ull;
+      asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(&p.seq->epoch), "l"(next) : "memory");
     }
   }
 }

@@ -172,6 +172,23 @@ typedef struct ftsgemm_stats {
 int ftsgemm_create(ftsgemm_handle_t *out);   /* binds to the current CUDA device; owns cuBLAS handle + workspace.
                                                  A handle is one in-order context: calls on it must be issued from one
                                                  stream at a time (use one handle per concurrently used stream). */
+/* CUDA graphs.  The compute calls may be captured into a CUDA graph (stream capture in any mode, e.g. torch.cuda.graph) and
+ * replayed; a replay computes what the same call computes eagerly on the buffers' contents at replay time, bit for bit.
+ *  - Captured as they are: ftsgemm_run / _run_ex / _run_bias / _run_batched on the tensor-core ids (with every option:
+ *    3xTF32, check_segments, protect_epilogue, injected faults) and the cuBLAS ids 0 / 7, the encode pre-pass,
+ *    and ftsgemm_stats_device.  A first call of a new shape may be
+ *    captured: its workspaces and work plan are allocated and uploaded outside the capture.  reuse_b_checksums has no
+ *    effect on a captured call: it encodes B on every replay.
+ *  - Not capturable, FTSGEMM_ERR_UNSUPPORTED before any CUDA call that would invalidate the capture: ftsgemm_run_host,
+ *    ftsgemm_verify and the baseline with baseline_host_sync on a capturing stream; ftsgemm_get_stats, ftsgemm_peer_verdict
+ *    and ftsgemm_debug_trace while the stream they would synchronise (the handle's last) is capturing; any compute call of a
+ *    peer-connected handle (its verdict's sequence number cannot advance per replay).
+ *  - The workspaces and plans a captured launch uses live until ftsgemm_destroy: destroy the handle only after its graphs.
+ *  - Eager calls and replays may interleave on one handle (the kernels' launch sequence lives in device memory), in stream
+ *    order: one handle must not be replayed on two streams at once, nor replayed while it runs eager work on another stream.
+ *  - ftsgemm_launch_count counts a captured launch once, at capture, not per replay.
+ *  - ftsgemm_get_stats synchronises the handle's last stream only, which for a captured call is the capture stream:
+ *    synchronise the replay stream before reading the counters of replays. */
 int ftsgemm_destroy(ftsgemm_handle_t h);
 int ftsgemm_abi_version(void);
 const char *ftsgemm_error_string(int code);
