@@ -875,30 +875,39 @@ __global__ void fill_kernel(float *p, float v, size_t n) {
   if (i < n) p[i] = v;
 }
 
-// 3xTF32: lo = x - tf32(x) (exact in FP32; the tensor core truncates lo to its own 11 significant bits when it reads it)
-__global__ void split_lo_kernel(const float4 *__restrict__ x, float4 *__restrict__ lo, size_t n4) {
+// 3xTF32: lo = x - tf32(x) (exact in FP32; the tensor core truncates lo to its own 11 significant bits when it reads it) and
+// the sanitised operand xs = x.  For a non-finite x both are 0: the cross passes A_lo B_s and A_s B_lo then never meet an
+// Inf or NaN (Inf - Inf would put NaN in lo, and 0 * Inf in a cross pass would make NaN of a finite element), and the
+// non-finite values reach C through the A B pass alone.
+__device__ __forceinline__ void split_lo(float x, float &lo, float &xs) {
+  const bool fin = isfinite(x);
+  lo = fin ? x - __uint_as_float(__float_as_uint(x) & 0xFFFFE000u) : 0.0f;
+  xs = fin ? x : 0.0f;
+}
+__global__ void split_lo_kernel(const float4 *__restrict__ x, float4 *__restrict__ lo, float4 *__restrict__ xs, size_t n4) {
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n4; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
     const float4 v = __ldg(x + i);
-    float4 r;
-    r.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u);
-    r.y = v.y - __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u);
-    r.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u);
-    r.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
+    float4 r, s;
+    split_lo(v.x, r.x, s.x);
+    split_lo(v.y, r.y, s.y);
+    split_lo(v.z, r.z, s.z);
+    split_lo(v.w, r.w, s.w);
     lo[i] = r;
+    xs[i] = s;
   }
 }
 // the same for operands with padded rows: entry e = blockIdx.y, blockIdx.y + gridDim.y, ... of x (`outer` rows of `inner`
-// elements, row stride ldx, entry stride sx) -> its lo part at lo + e * outer * ldlo (row stride ldlo)
-__global__ void split_lo_strided_kernel(const float *__restrict__ x, size_t ldx, long long sx, float *__restrict__ lo, size_t ldlo,
-                                        int inner, size_t outer, int batch) {
+// elements, row stride ldx, entry stride sx) -> its lo part at lo + e * outer * ldlo (row stride ldlo), its sanitised copy at
+// the same offset of xs
+__global__ void split_lo_strided_kernel(const float *__restrict__ x, size_t ldx, long long sx, float *__restrict__ lo,
+                                        float *__restrict__ xs, size_t ldlo, int inner, size_t outer, int batch) {
   const size_t n = outer * inner;
   for (int e = blockIdx.y; e < batch; e += gridDim.y) {
     const float *xe = x + e * sx;
-    float *le = lo + e * outer * ldlo;
+    const size_t eo = e * outer * ldlo;
     for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
       const size_t o = i / inner, r = i - o * inner;
-      const float v = __ldg(xe + o * ldx + r);
-      le[o * ldlo + r] = v - __uint_as_float(__float_as_uint(v) & 0xFFFFE000u);
+      split_lo(__ldg(xe + o * ldx + r), lo[eo + o * ldlo + r], xs[eo + o * ldlo + r]);
     }
   }
 }
@@ -1268,12 +1277,19 @@ int ftsgemm_run_batched(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, 
     Operand Alo = lo_of(A, M), Blo = lo_of(B, N);
     const size_t a_floats = static_cast<size_t>(Alo.ld) * (Alo.kmajor ? M : K);
     const size_t b_floats = static_cast<size_t>(Blo.ld) * (Blo.kmajor ? N : K);
-    // the lo parts of entry e at e * a_floats (e * b_floats), from one launch per operand; then the three passes
-    int rc = ensure_buf(h, &h->d_lo, &h->lo_bytes, (a_floats + b_floats) * bt.count * sizeof(float));
+    // The lo parts of entry e at e * a_floats (e * b_floats), and behind them the sanitised operands A_s, B_s in the same
+    // layout (split_lo_kernel), from one launch per operand; then the three passes
+    //   A_lo B_s^T + A_s B_lo^T + A B^T
+    // so that only the last one sees a non-finite operand value.
+    const size_t lo_floats = (a_floats + b_floats) * bt.count;
+    int rc = ensure_buf(h, &h->d_lo, &h->lo_bytes, 2 * lo_floats * sizeof(float));
     if (rc) return rc;
     float *dAlo = h->d_lo, *dBlo = h->d_lo + a_floats * bt.count;
     Alo.p = dAlo;
     Blo.p = dBlo;
+    Operand As = Alo, Bs = Blo;
+    As.p = dAlo + lo_floats;
+    Bs.p = dBlo + lo_floats;
     auto split = [&](const Operand &x, const Operand &lo, int rows, long long sx, float *dst) {
       const int inner = x.kmajor ? K : rows;  // elements per stored row of the operand
       const size_t outer = x.kmajor ? rows : K;
@@ -1281,10 +1297,10 @@ int ftsgemm_run_batched(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, 
       if (x.ld == inner && lo.ld == inner && (bt.count == 1 || sx == static_cast<long long>(outer) * inner))
         // dense: all entries are one flat array (a multiple of 4 elements, see above)
         split_lo_kernel<<<blocks, 256, 0, stream>>>(reinterpret_cast<const float4 *>(x.p), reinterpret_cast<float4 *>(dst),
-                                                    outer * inner * bt.count / 4);
+                                                    reinterpret_cast<float4 *>(dst + lo_floats), outer * inner * bt.count / 4);
       else  // padded rows or entries: nothing outside the operand's rows is read
         split_lo_strided_kernel<<<dim3(std::max(1, blocks / bt.count), std::min(bt.count, 65535)), 256, 0, stream>>>(
-            x.p, x.ld, sx, dst, lo.ld, inner, outer, bt.count);
+            x.p, x.ld, sx, dst, dst + lo_floats, lo.ld, inner, outer, bt.count);
     };
     split(A, Alo, M, bt.sa, dAlo);
     split(B, Blo, N, bt.sb, dBlo);
@@ -1296,10 +1312,9 @@ int ftsgemm_run_batched(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, 
     ftsgemm_opts o_quiet = o3;  // injected faults belong to the main product only
     o_quiet.inject_mode = 0;
     // (the bias goes to the last pass only: added once, after the final alpha*acc + C)
-    const BatchArg lo_a = {bt.count, static_cast<long long>(a_floats), bt.sb, bt.sc};
-    const BatchArg lo_b = {bt.count, bt.sa, static_cast<long long>(b_floats), bt.sc};
-    rc = run_tc(h, *v, M, N, K, Alo, B, dC, ldc, alpha, beta, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo_a);
-    if (!rc) rc = run_tc(h, *v, M, N, K, A, Blo, dC, ldc, alpha, 1.0f, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo_b);
+    const BatchArg lo = {bt.count, static_cast<long long>(a_floats), static_cast<long long>(b_floats), bt.sc};
+    rc = run_tc(h, *v, M, N, K, Alo, Bs, dC, ldc, alpha, beta, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo);
+    if (!rc) rc = run_tc(h, *v, M, N, K, As, Blo, dC, ldc, alpha, 1.0f, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo);
     if (!rc) rc = run_tc(h, *v, M, N, K, A, B, dC, ldc, alpha, 1.0f, bias, bias_mode, o3, stream, bt);
     return rc;
   }

@@ -486,8 +486,11 @@ struct ExpectedChk {
   bool ready;
 };
 // (chk_ofs: the entry's block of expected checksums in a strided batch)
+// A row past M has no expected checksum: NaN, so that it is never flagged.  Its accumulator is not always 0 -- A is
+// zero-filled there, and 0 * Inf from a non-finite B is NaN -- and nothing of it is stored.
 __device__ __forceinline__ void load_expected(const KernelParams &p, int m, int n_blk, ExpectedChk &x, size_t chk_ofs) {
-  x.e0 = x.e1 = x.w0 = x.w1 = 0.0f;
+  x.e0 = CUDART_NAN_F;
+  x.e1 = x.w0 = x.w1 = 0.0f;
   if (m < p.M) {
     const float *cp = p.chk_out + chk_ofs + static_cast<size_t>(n_blk) * kChkPerTile * p.M + m;
     x.e0 = __ldcg(cp);
@@ -576,14 +579,18 @@ __device__ __forceinline__ void abft_check(const KernelParams &p, uint32_t taddr
   }
   const float r1 = xp.e0 + xp.e1, r2 = xp.w0 + xp.w1;
   const float d1 = r1 - s1, d2 = r2 - s2;
-  const float thr = p.tau_abs + p.tau_rel * sabs;
-  const bool flagged = !(fabsf(d1) <= thr);  // also true for NaN
+  // (the magnitude term is clamped so that an upset to +-Inf, which makes sabs Inf, cannot make the threshold Inf)
+  const float thr = p.tau_abs + p.tau_rel * fminf(sabs, CUDART_MAX_NORMAL_F);
+  const bool passed = fabsf(d1) <= thr;  // false for NaN
+  // A row whose expected checksum is non-finite (Inf / NaN in its operands, or a product or checksum that overflows) cannot
+  // be verified: it is not flagged and stored as computed.  With a finite r1, a non-finite row sum is an upset.
+  const bool flagged = !passed && isfinite(r1);
   const unsigned flag_mask = __ballot_sync(0xffffffffu, flagged);
 
   // fault-free residual statistics (threshold calibration, DESIGN.md section 5)
   {
-    float ra = flagged ? 0.0f : fabsf(d1);
-    float rr = flagged ? 0.0f : fabsf(d1) / fmaxf(sabs, 1e-30f);
+    float ra = passed ? fabsf(d1) : 0.0f;
+    float rr = passed ? fabsf(d1) / fmaxf(sabs, 1e-30f) : 0.0f;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
       ra = fmaxf(ra, __shfl_xor_sync(0xffffffffu, ra, o));

@@ -116,8 +116,11 @@ typedef struct ftsgemm_opts {
   /* ---- ABI version 2 ---- */
   int precision;         /* 0 (default): single-pass TF32 (operands truncated to 11 significant bits by the tensor core,
                             FP32 accumulate; norm-wise 1e-3 against FP32) | 1: 3xTF32 -- hi/lo split of A and B, three
-                            fault-tolerant passes A_lo*B + A*B_lo + A*B: FP32-grade, element-wise parity with the
-                            reference's FP32 FFMA kernels (ft_sgemm_huge.cuh:228-323) at ~1/3 of the throughput */
+                            fault-tolerant passes A_lo*B_s + A_s*B_lo + A*B: FP32-grade, element-wise parity with the
+                            reference's FP32 FFMA kernels (ft_sgemm_huge.cuh:228-323) at ~1/3 of the throughput.  A_s, B_s
+                            are the operands with Inf / NaN replaced by 0 (lo is 0 there too): the cross passes never see a
+                            non-finite value, so Inf and NaN in C sit where FP32 arithmetic on the untruncated operands
+                            puts them, Inf signs included */
   int check_segments;    /* 0 / 1 (default): one check per tile over the whole K range.  S > 1: intra-K checking -- the product is
                             formed as S consecutive K-segments (S launches, C += alpha * A[:, seg] * B[:, seg]^T), each a
                             complete fault-tolerant GEMM whose tiles are verified and repaired before the segment is
@@ -154,7 +157,11 @@ typedef struct ftsgemm_event {
 typedef struct ftsgemm_stats {
   unsigned long long tiles;        /* CTA tiles processed */
   unsigned long long rows_checked; /* row checksums tested */
-  unsigned long long detected;     /* rows whose residual exceeded the threshold */
+  unsigned long long detected;     /* rows whose residual exceeded the threshold.  A row whose expected checksum is not finite
+                                      (Inf / NaN in its operands, an overflowing product or checksum) cannot be verified:
+                                      it is never detected or counted anywhere, and is stored as the plain kernel stores it --
+                                      an upset in such a row goes undetected.  With a finite expected checksum, a non-finite
+                                      row (an upset to +-Inf or NaN) is detected and repaired like any other. */
   unsigned long long corrected;    /* single-element corrections applied */
   unsigned long long uncorrectable;/* detected, not locatable (multi-error row / ambiguous) AND left as computed
                                       (only with opts.no_recompute or detect_only) */
@@ -210,7 +217,12 @@ int ftsgemm_select_kernel(int M, int N, int K, int fault_tolerant);
  *      sgemm.cu:110-199, and cublasSgemm at sgemm.cu:108,198,260) ---------------------------------------------
  * Device pointers, caller-owned, in place on C, asynchronous on opts->stream.  Preconditions as in the
  * reference: 16-byte aligned pointers, M % 4 == 0 and N % 4 == 0 (16-byte rows for TMA); unlike the reference,
- * M/N/K need not be multiples of the tile (TMA zero-fills the ragged edge).  K >= 1. */
+ * M/N/K need not be multiples of the tile (TMA zero-fills the ragged edge).  K >= 1.
+ * Non-finite values: every tensor-core id stores what IEEE FP32 arithmetic gives on TF32-truncated operands -- the NaN
+ * positions and the +-Inf positions and signs of a float64 product of the same operands (opts.precision = 1: of FP32 on the
+ * untruncated operands); the ABFT ids store bit for bit what their plain twins store (see ftsgemm_stats.detected).
+ * beta == 0: C is not read, so Inf / NaN in the old C have no effect -- on every id and entry point (cuBLAS, the baseline,
+ * ftsgemm_run_host, batches, bias, 3xTF32, check_segments). */
 int ftsgemm_run(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, const float *dB,
                 float *dC, float alpha, float beta, const ftsgemm_opts *opts);
 
