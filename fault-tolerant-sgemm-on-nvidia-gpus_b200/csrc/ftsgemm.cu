@@ -4,6 +4,8 @@
 // launch dispatch (reference: sgemm.cu:110-199, 256-430), TMA tensor-map construction, the encode pre-pass launch,
 // the cuBLAS comparator rows (sgemm.cu:108,198,260), the non-fused ABFT baseline
 // (include/baseline_ft_sgemm.cuh:1-33) and the device-side comparator (utils/utils.cu:61-77).
+// A wgmma launch (run_tc) runs in stages, planned by plan_launch -- the same function ftsgemm_debug_schedule enumerates.
+// The handle's workspaces are DevBufs: grow replaces them, and drop decides whether a CUDA graph may still use the old one.
 // There is NO CPU fallback: without an sm_90 device every compute entry point returns FTSGEMM_ERR_NO_DEVICE.
 #include <cublas_v2.h>
 #include <cuda.h>
@@ -16,7 +18,6 @@
 #include <array>
 #include <map>
 #include <mutex>
-#include <set>
 #include <string>
 #include <type_traits>
 
@@ -122,6 +123,14 @@ struct ChkKey {
   }
 };
 
+// A device workspace of the handle, replaced by a larger one when a call needs more (grow).  pinned: a captured launch
+// references it, so it is never freed before ftsgemm_destroy.
+struct DevBuf {
+  void *ptr = nullptr;
+  size_t bytes = 0;
+  bool pinned = false;
+};
+
 }  // namespace
 
 struct ftsgemm_handle_s {
@@ -131,10 +140,8 @@ struct ftsgemm_handle_s {
   cublasHandle_t cublas = nullptr;
   EncodeTiledFn encode_tiled = nullptr;
   DeviceStats *d_stats = nullptr;
-  float *d_chk = nullptr;       // encoded checksum vectors [K][tiles_n*8]  (extra "rows" of B)
-  size_t chk_bytes = 0;
-  float *d_chk_out = nullptr;   // expected checksums M x (tiles_n*8), column-major, + slab flags behind it
-  size_t chk_out_bytes = 0;
+  DevBuf d_chk;                 // encoded checksum vectors [K][tiles_n*8]  (extra "rows" of B)
+  DevBuf d_chk_out;             // slab flags, then the expected checksums M x (tiles_n*8), column-major
   size_t chk_flag_bytes = kChkFlagBytes;  // bytes of d_chk_out in front of the expected checksums: the slab flags
   ChkKey chk_key;               // what d_chk holds
   // fused verdict exchange (ftsgemm_peer_*): this rank's mailbox (kMaxPeers slots), the peers' mailboxes mapped through
@@ -146,36 +153,31 @@ struct ftsgemm_handle_s {
   unsigned long long peer_seq = 0;
   LaunchSeq *d_seq = nullptr;   // launch sequence of the wgmma kernels: epoch, exit and front-phase counters
   // CUDA graph capture: whether the running call is being captured; the private stream of allocations' uploads; the
-  // workspaces a captured launch references (never freed before ftsgemm_destroy) and those retired from the handle
+  // workspaces retired from the handle (freed by ftsgemm_destroy)
   bool capturing = false;
   cudaStream_t s_up = nullptr;
-  std::set<const void *> graph_bufs;
   std::vector<void *> retired;
-  float *d_at = nullptr, *d_bt = nullptr;  // K-major copies of MN-major A and B (never allocated for a K-major operand)
-  size_t at_bytes = 0, bt_bytes = 0;
-  float *d_lo = nullptr;        // 3xTF32: A_lo | B_lo
-  size_t lo_bytes = 0;
-  float *d_aux = nullptr;       // baseline vectors
-  size_t aux_bytes = 0;
+  DevBuf d_at, d_bt;            // K-major copies of MN-major A and B (never allocated for a K-major operand)
+  DevBuf d_lo;                  // 3xTF32: A_lo | B_lo, then the sanitised A_s | B_s
+  DevBuf d_aux;                 // baseline vectors
   struct CachedPlan {
     std::vector<int> wave_target;   // per whole-tile ordinal: units that own more whole tiles than that
-    int *d_wave_target = nullptr;
     ftsgemm::Plan plan;
     std::vector<int4> packed;   // host copy (kept alive for the async upload)
-    int4 *d_items = nullptr;
-    int *d_off = nullptr;
+    DevBuf d_items, d_off, d_wave_target;
     bool uploaded = false;
-    bool captured = false;      // referenced by a captured launch: never evicted
+    std::array<DevBuf *, 3> bufs() { return {&d_items, &d_off, &d_wave_target}; }
   };
   std::map<std::array<long long, 7>, CachedPlan> plans;  // key: kernel id, M, N, K, units, forced slices, batch
-  int *d_wave_cnt = nullptr;    // wave re-synchronisation counters (cleared per launch)
-  size_t wave_cnt_cap = 0;
-  float *d_sk = nullptr;        // split-K partial tiles + flags
-  size_t sk_bytes = 0;
-  unsigned long long *d_trace = nullptr;  // debug timeline (ftsgemm_debug_trace), allocated on first use
-  int trace_units = 0;
-  float *d_stage[3] = {nullptr, nullptr, nullptr};  // run_host staging A, B, C
-  size_t stage_bytes[3] = {0, 0, 0};
+  DevBuf d_wave_cnt;            // wave re-synchronisation counters (cleared per launch)
+  DevBuf d_sk;                  // split-K flags + partial tiles
+  DevBuf d_trace;               // debug timeline (ftsgemm_debug_trace), allocated on first use
+  int trace_units = 0;          // units d_trace was allocated for
+  DevBuf d_stage[3];            // run_host staging A, B, C
+  // every workspace above (ftsgemm_destroy)
+  std::array<DevBuf *, 12> bufs() {
+    return {&d_chk, &d_chk_out, &d_at, &d_bt, &d_lo, &d_aux, &d_wave_cnt, &d_sk, &d_trace, &d_stage[0], &d_stage[1], &d_stage[2]};
+  }
   cudaStream_t s_in = nullptr, s_out = nullptr;     // run_host: upload / download streams of the panel pipeline
   cudaEvent_t ev_in[16] = {}, ev_done[16] = {};
   double *d_verify = nullptr;   // {first_bad (as long long), num, den}
@@ -456,6 +458,16 @@ void plan_tiles(int M, int N, int BN, int CG, bool ft, KernelParams *p) {
   }
 }
 
+// The launch plan of the product in p (M, N, K, batch) for max_units co-resident work units: sets p's tile grid and
+// checksum slices and returns the planner input.  A launch passes the device's co-residency limit, ftsgemm_debug_schedule
+// num_sms / CG -- the schedule it reports is the one a launch on such a device runs.
+PlanInput plan_launch(const Variant &v, int max_units, long long l2_bytes, KernelParams *p) {
+  const bool ft = v.info.fault_tolerant != 0;
+  plan_tiles(p->M, p->N, v.bn, v.cg, ft, p);
+  if (ft) p->chk_slices = choose_chk_slices(*p, max_units, p->K);
+  return make_plan_input(max_units, v.cg, v.bn, p->K, *p, l2_bytes);
+}
+
 // ------------------------------------------------------------------------------------------- CUDA graph capture
 // Whether work enqueued on `stream` is being captured into a graph (the legacy stream counts as capturing while a blocking
 // stream it would synchronise with is).
@@ -497,35 +509,33 @@ int upload(ftsgemm_handle_t h, void *dst, const void *src, size_t bytes) {
   return FTSGEMM_OK;
 }
 
-// Drops a workspace from the handle.  One that a captured launch references, and any while a capture is running (cudaFree
-// synchronises the device), is retired instead: ftsgemm_destroy frees it.
-int release(ftsgemm_handle_t h, void *p) {
-  if (!p) return FTSGEMM_OK;
-  if (h->capturing || h->graph_bufs.count(p)) h->retired.push_back(p);
-  else FT_CUDA(h, cudaFree(p));
+// Empties a workspace.  One that a captured launch references, and any while a capture is running (cudaFree synchronises
+// the device), is retired instead: ftsgemm_destroy frees it.
+int drop(ftsgemm_handle_t h, DevBuf &b) {
+  if (b.ptr && (h->capturing || b.pinned)) h->retired.push_back(b.ptr);
+  else if (b.ptr) FT_CUDA(h, cudaFree(b.ptr));
+  b = DevBuf();
   return FTSGEMM_OK;
 }
 
-template <typename T>
-int ensure_buf(ftsgemm_handle_t h, T **buf, size_t *have, size_t bytes) {
-  if (*have >= bytes) return FTSGEMM_OK;
-  const int rc = release(h, *buf);
+// Makes b hold at least `bytes`: a smaller allocation is dropped and replaced, and the first zero_prefix bytes of the new
+// one are zero-filled.  *changed (optional): whether b holds a new allocation.
+int grow(ftsgemm_handle_t h, DevBuf &b, size_t bytes, size_t zero_prefix = 0, bool *changed = nullptr) {
+  if (changed) *changed = false;
+  if (b.bytes >= bytes) return FTSGEMM_OK;
+  int rc = drop(h, b);
+  if (!rc) rc = dev_alloc(h, &b.ptr, bytes);
   if (rc) return rc;
-  *buf = nullptr;
-  *have = 0;
-  const int arc = dev_alloc(h, buf, bytes);
-  if (arc) return arc;
-  *have = bytes;
-  return FTSGEMM_OK;
+  b.bytes = bytes;
+  if (changed) *changed = true;
+  return zero_prefix ? upload(h, b.ptr, nullptr, zero_prefix) : FTSGEMM_OK;
 }
 
-// After a captured call: the workspaces it may reference stay allocated until ftsgemm_destroy.
-void pin_workspaces(ftsgemm_handle_t h) {
-  for (const void *p : {static_cast<const void *>(h->d_at), static_cast<const void *>(h->d_bt),
-                        static_cast<const void *>(h->d_chk_out), static_cast<const void *>(h->d_sk),
-                        static_cast<const void *>(h->d_lo), static_cast<const void *>(h->d_aux),
-                        static_cast<const void *>(h->d_wave_cnt), static_cast<const void *>(h->d_trace)})
-    if (p) h->graph_bufs.insert(p);
+// A workspace as a launch argument: pinned when the launch is being captured.
+template <typename T = float>
+T *bind(ftsgemm_handle_t h, DevBuf &b) {
+  if (h->capturing) b.pinned = true;
+  return static_cast<T *>(b.ptr);
 }
 
 // One operand of ftsgemm_run_ex: MN-major (the reference's: element (r, k) at p[r + k*ld]) or K-major (p[k + r*ld]).
@@ -542,23 +552,28 @@ struct BatchArg {
 };
 const BatchArg kSingle = {1, 0, 0, 0};
 
-int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC, int ldc,
-           float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o, cudaStream_t stream,
-           const BatchArg &batch_arg = kSingle) {
-  const int BN = v.bn, CG = v.cg;
-  const bool ft = v.info.fault_tolerant != 0;
-  const float *dA = A.p, *dB = B.p;
-  // (one entry runs the kernels without BATCH, on 2-D tensor maps; its strides are ignored)
-  const BatchArg bt = batch_arg.count > 1 ? batch_arg : kSingle;
+// Shapes and operands the wgmma kernels can run (also checked before the 3xTF32 split kernels read the operands with
+// 16-byte loads).
+int check_tc_args(const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, const float *dC, int batch) {
   if ((M % 4) || (N % 4)) return FTSGEMM_ERR_UNSUPPORTED;  // TMA global strides must be multiples of 16 bytes
   if ((A.ld % 4) || (B.ld % 4)) return FTSGEMM_ERR_INVALID_ARG;  // (the same for the rows of an operand)
   // work-plan items carry k-block indices in 16 bits and tile indices in 31; the trace / wave tables are sized per unit
   if ((K + kBK - 1) / kBK > 65535) return FTSGEMM_ERR_UNSUPPORTED;
-  if ((static_cast<long long>(M + kBM * CG - 1) / (kBM * CG)) * ((N + BN - 1) / BN) * bt.count > (1ll << 28)) return FTSGEMM_ERR_UNSUPPORTED;
-  if (static_cast<long long>(M) * bt.count > 0x7fffffffll) return FTSGEMM_ERR_UNSUPPORTED;  // stacked rows are ints
-  if ((reinterpret_cast<uintptr_t>(dA) | reinterpret_cast<uintptr_t>(dB) | reinterpret_cast<uintptr_t>(dC)) & 15)
+  if ((static_cast<long long>(M + kBM * v.cg - 1) / (kBM * v.cg)) * ((N + v.bn - 1) / v.bn) * batch > (1ll << 28))
+    return FTSGEMM_ERR_UNSUPPORTED;
+  if (static_cast<long long>(M) * batch > 0x7fffffffll) return FTSGEMM_ERR_UNSUPPORTED;  // stacked rows are ints
+  if ((reinterpret_cast<uintptr_t>(A.p) | reinterpret_cast<uintptr_t>(B.p) | reinterpret_cast<uintptr_t>(dC)) & 15)
     return FTSGEMM_ERR_INVALID_ARG;
+  return FTSGEMM_OK;
+}
 
+// The kernel parameters that follow from the call's arguments and options (the tile grid and work plan come later).
+KernelParams make_params(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B,
+                         float *dC, int ldc, float alpha, float beta, const float *bias, int bias_mode,
+                         const ftsgemm_opts &o, const BatchArg &batch_arg) {
+  const bool ft = v.info.fault_tolerant != 0;
+  // (one entry runs the kernels without BATCH, on 2-D tensor maps; its strides are ignored)
+  const BatchArg bt = batch_arg.count > 1 ? batch_arg : kSingle;
   KernelParams p;
   memset(&p, 0, sizeof(p));
   p.M = M; p.N = N; p.K = K;
@@ -569,21 +584,21 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
   p.stride_a = bt.sa;
   p.stride_b = bt.sb;
   p.stride_c = bt.sc;
-  plan_tiles(M, N, BN, CG, ft, &p);
   p.tau_abs = o.tau_abs > 0 ? o.tau_abs : 1e-3f;
   p.tau_rel = o.tau_rel > 0 ? o.tau_rel : 1e-5f;  // DESIGN.md section 5
   p.detect_only = o.detect_only;
   p.recompute = o.no_recompute ? 0 : 1;
-  p.A = dA;
-  p.B = dB;
+  p.A = A.p;
+  p.B = B.p;
   p.lda = A.ld;
   p.ldb = B.ld;
   p.a_kmajor = A.kmajor ? 1 : 0;
   p.b_kmajor = B.kmajor ? 1 : 0;
+  p.ldk = (K + 3) / 4 * 4;
   p.inject_mode = ft ? o.inject_mode : 0;
   p.selftest_value = o.selftest_value;
   p.selftest_row = o.selftest_row & (kBM - 1);  // (>= 0: validated by load_opts)
-  p.selftest_col = o.selftest_col % BN;
+  p.selftest_col = o.selftest_col % v.bn;
   p.n_faults = o.n_faults < 0 ? 0 : (o.n_faults > kMaxFaults ? kMaxFaults : o.n_faults);
   for (int i = 0; i < p.n_faults; ++i) {
     p.faults[i].row = o.faults[i].row;
@@ -600,256 +615,244 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
     p.peer_seq = static_cast<double>(++h->peer_seq);
   }
   p.seq = h->d_seq;
+  return p;
+}
 
-  // The tensor maps read K-major operands: a K-major operand in place, an MN-major one through its K-major copy (written by
-  // the kernel's front phase, row stride ldk: TMA needs 16-byte row strides).  The main loop is the same either way.
-  CUtensorMap tmA, tmB, tmC;
-  bool enc_front = false;
+// The tensor maps read K-major operands: a K-major operand in place, an MN-major one through its K-major copy (written by
+// the kernel's front phase, row stride ldk: TMA needs 16-byte row strides).  The main loop is the same either way.
+// (a batch: 3-D maps with the entry as the outer dimension; the copies hold one dense rows x ldk block per entry)
+int bind_operands(ftsgemm_handle_t h, const Variant &v, KernelParams &p, CUtensorMap *tmA, CUtensorMap *tmB) {
+  const long long a_copy = static_cast<long long>(p.M) * p.ldk, b_copy = static_cast<long long>(p.N) * p.ldk;
   int rc;
-  p.ldk = (K + 3) / 4 * 4;
-  // (a batch: 3-D maps with the entry as the outer dimension; the copies hold one dense rows x ldk block per entry)
-  const long long a_copy = static_cast<long long>(M) * p.ldk, b_copy = static_cast<long long>(N) * p.ldk;
-  if (A.kmajor) {
-    rc = make_tmap_kmajor(h, &tmA, dA, M, K, A.ld, bt.sa, bt.count, kBM);
-  } else {
-    rc = ensure_buf(h, &h->d_at, &h->at_bytes, static_cast<size_t>(a_copy) * bt.count * sizeof(float));
-    if (rc) return rc;
-    p.At = h->d_at;
-    rc = make_tmap_kmajor(h, &tmA, p.At, M, K, p.ldk, a_copy, bt.count, kBM);
+  if (p.a_kmajor) {
+    rc = make_tmap_kmajor(h, tmA, p.A, p.M, p.K, p.lda, p.stride_a, p.batch, kBM);
+  } else if (!(rc = grow(h, h->d_at, static_cast<size_t>(a_copy) * p.batch * sizeof(float)))) {
+    p.At = bind(h, h->d_at);
+    rc = make_tmap_kmajor(h, tmA, p.At, p.M, p.K, p.ldk, a_copy, p.batch, kBM);
   }
   if (rc) return rc;
   // CG = 2: each CTA of a unit loads BN/2 rows of the B tile and multicasts them to both
-  if (B.kmajor) {
-    rc = make_tmap_kmajor(h, &tmB, dB, N, K, B.ld, bt.sb, bt.count, BN / CG);
-  } else {
-    rc = ensure_buf(h, &h->d_bt, &h->bt_bytes, static_cast<size_t>(b_copy) * bt.count * sizeof(float));
-    if (rc) return rc;
-    p.Bt = h->d_bt;
-    rc = make_tmap_kmajor(h, &tmB, p.Bt, N, K, p.ldk, b_copy, bt.count, BN / CG);
-  }
-  if (rc) return rc;
-  tmC = tmB;
-  if (ft) {
-    // checksum vectors of B: 8 columns per N-tile, appended to B as extra tile-columns of the same GEMM
-    p.dbg_flags = static_cast<int>(dbg("ft_dbg", 0)) & 1;
-    // the checksum operand is K-major like B^T: n_chk_cols rows of K (row stride ldk)
-    const int chk_ld = p.ldk;
-    // (a batch: one checksum operand, one block of expected checksums and one run of slab flags per entry)
-    const int n_slabs = p.tiles_m * CG * (kBM / 32) * bt.count;
-    const long long chk_entry = static_cast<long long>(p.n_chk_cols) * chk_ld;
-    const size_t chk_bytes = static_cast<size_t>(chk_entry) * bt.count * sizeof(float);
-    float *chk = nullptr;
-    if (h->capturing) {
-      // a captured call encodes on every replay, into a checksum operand of its own: replays would otherwise overwrite
-      // the one an eager call with reuse_b_checksums relies on
-      rc = dev_alloc(h, &chk, chk_bytes);
-      if (rc) return rc;
-      h->retired.push_back(chk);
-    } else {
-      const float *chk_before = h->d_chk;
-      rc = ensure_buf(h, &h->d_chk, &h->chk_bytes, chk_bytes);
-      if (rc) return rc;
-      if (h->d_chk != chk_before) h->chk_key = ChkKey();  // reallocated: the cached encode is gone
-      chk = h->d_chk;
-    }
-    const size_t out_floats = static_cast<size_t>(M) * p.n_chk_cols * bt.count;
-    const size_t n_flags = static_cast<size_t>(n_slabs) * p.tiles_c;
-    if (n_flags * sizeof(SeqFlag) > h->chk_flag_bytes) {
-      // grow the flag region: a new buffer
-      h->chk_flag_bytes = (n_flags * sizeof(SeqFlag) + kChkFlagBytes - 1) / kChkFlagBytes * kChkFlagBytes;
-      rc = release(h, h->d_chk_out);
-      if (rc) return rc;
-      h->d_chk_out = nullptr;
-      h->chk_out_bytes = 0;
-    }
-    const size_t flag_bytes = h->chk_flag_bytes;
-    const float *out_before = h->d_chk_out;
-    rc = ensure_buf(h, &h->d_chk_out, &h->chk_out_bytes, flag_bytes + out_floats * sizeof(float));
-    if (rc) return rc;
-    // the flags of a new buffer start at 0, below every epoch (LaunchSeq): they never need clearing again
-    if (h->d_chk_out != out_before && (rc = upload(h, h->d_chk_out, nullptr, flag_bytes))) return rc;
-    p.chk_flags = reinterpret_cast<SeqFlag *>(h->d_chk_out);
-    p.chk_out = h->d_chk_out + flag_bytes / sizeof(float);
-    p.dbg_flags = static_cast<int>(dbg("ft_dbg", 0)) & 1;
-    const ChkKey chk_key = {dB, N, K, BN, B.kmajor, B.ld, bt.count, bt.sb};
-    const bool reuse = !h->capturing && o.reuse_b_checksums && h->chk_key == chk_key;
-    // Default: the encode is part of the FRONT PHASE of the GEMM kernel (KernelParams::enc_front) -- one launch per fused
-    // GEMM, like the reference (sgemm.cu:191-192); only below ~8 MB of B the stand-alone pre-pass is used.
-    const long long ef = dbg("enc_front", -2);
-    enc_front = !reuse && (ef >= 0 ? ef != 0 : 4.0 * N * static_cast<double>(K) * bt.count >= static_cast<double>(dbg("enc_front_min_mb", 8)) * 1048576.0);
-    if (enc_front) {
-      p.enc_front = 1;
-      p.enc_out = chk;
-      p.enc_ld = chk_ld;
-    }
-    if (!reuse && !enc_front) {
-      // stand-alone pre-pass in the caller's stream: grid-stride over (column block, k-row group) items, the pass is HBM
-      // time; a batch runs all entries in one launch, one grid row per entry
-      const int rounding = static_cast<int>(dbg("enc_rounding", 0));
-      const int grid = static_cast<int>(dbg("enc_blocks_per_sm", 4)) * h->num_sms;
-      const bool small_items = dbg("enc_kr", 8) == 4;
-      const bool chain = dbg("pdl_chain", 1) != 0;
-      // B larger than ~half of L2: read it with evict-first loads (it cannot stay resident for the GEMM anyway)
-      const long long sb = dbg("enc_stream", -2);
-      const bool stream_b = sb > 0;  // off by default: the tail of B the pre-pass leaves in L2 serves the GEMM's first wave
-      cudaLaunchConfig_t ec = {};
-      ec.gridDim = dim3(std::max(1, grid / bt.count), std::min(bt.count, 65535));
-      ec.blockDim = dim3(kEncWarps * 32);
-      ec.stream = stream;
-      cudaLaunchAttribute ea[1];
-      ea[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-      ea[0].val.programmaticStreamSerializationAllowed = 1;
-      ec.attrs = ea;
-      ec.numAttrs = chain ? 1 : 0;
-      const long long chk_stride = bt.count > 1 ? chk_entry : 0;
-      rc = with_tile(BN, CG, [&](auto bn, auto) {
-        auto launch = [&](auto kern) {
-          FT_CUDA(h, cudaLaunchKernelEx(&ec, kern, dB, N, K, B.ld, bt.sb, bt.count, chk, chk_ld, chk_stride, rounding, p.tiles_n));
-          return FTSGEMM_OK;
-        };
-        if (B.kmajor) return launch(encode_kernel<bn, true>);
-        if (small_items) return launch(encode_kernel<bn, false, 4, false>);
-        if (stream_b) return launch(encode_kernel<bn, false, 8, true>);
-        return launch(encode_kernel<bn, false, 8, false>);
-      });
-      if (rc) return rc;
-      ++h->launch_count;
-      FT_CUDA(h, cudaGetLastError());
-    }
-    if (!reuse && !h->capturing) h->chk_key = chk_key;
-    rc = make_tmap_kmajor(h, &tmC, chk, p.n_chk_cols, K, chk_ld, chk_entry, bt.count, BN / CG);
-    if (rc) return rc;
-  }
-  // ---- work plan (plan.h), cached per shape on the handle
+  if (p.b_kmajor) return make_tmap_kmajor(h, tmB, p.B, p.N, p.K, p.ldb, p.stride_b, p.batch, v.bn / v.cg);
+  if ((rc = grow(h, h->d_bt, static_cast<size_t>(b_copy) * p.batch * sizeof(float)))) return rc;
+  p.Bt = bind(h, h->d_bt);
+  return make_tmap_kmajor(h, tmB, p.Bt, p.N, p.K, p.ldk, b_copy, p.batch, v.bn / v.cg);
+}
+
+// The launch plan for as many work units as the device holds at once.
+int plan_on_device(ftsgemm_handle_t h, const Variant &v, KernelParams &p, PlanInput *pin) {
   int max_units = 0;
-  {
-    const int qrc = with_tile(BN, CG, [&](auto bn, auto cg) {
-      return ft ? query_max_units<bn, true, cg>(h, &max_units) : query_max_units<bn, false, cg>(h, &max_units);
-    });
-    if (qrc) return qrc;
-    if (max_units < 1) return FTSGEMM_ERR_UNSUPPORTED;  // not a single CTA (pair) of this kernel fits on the device partition
+  const int rc = with_tile(v.bn, v.cg, [&](auto bn, auto cg) {
+    return v.info.fault_tolerant ? query_max_units<bn, true, cg>(h, &max_units) : query_max_units<bn, false, cg>(h, &max_units);
+  });
+  if (rc) return rc;
+  if (max_units < 1) return FTSGEMM_ERR_UNSUPPORTED;  // not a single CTA (pair) of this kernel fits on the device partition
+  *pin = plan_launch(v, max_units, h->l2_bytes, &p);
+  return FTSGEMM_OK;
+}
+
+// Stand-alone encode pre-pass in the caller's stream: grid-stride over (column block, k-row group) items, the pass is HBM
+// time; a batch runs all entries in one launch, one grid row per entry.
+int launch_encode(ftsgemm_handle_t h, const Variant &v, const KernelParams &p, float *chk, long long chk_entry,
+                  cudaStream_t stream) {
+  const int rounding = static_cast<int>(dbg("enc_rounding", 0));
+  const int grid = static_cast<int>(dbg("enc_blocks_per_sm", 4)) * h->num_sms;
+  const bool small_items = dbg("enc_kr", 8) == 4;
+  const bool chain = dbg("pdl_chain", 1) != 0;
+  // B larger than ~half of L2: read it with evict-first loads (it cannot stay resident for the GEMM anyway)
+  const long long sb = dbg("enc_stream", -2);
+  const bool stream_b = sb > 0;  // off by default: the tail of B the pre-pass leaves in L2 serves the GEMM's first wave
+  cudaLaunchConfig_t ec = {};
+  ec.gridDim = dim3(std::max(1, grid / p.batch), std::min(p.batch, 65535));
+  ec.blockDim = dim3(kEncWarps * 32);
+  ec.stream = stream;
+  cudaLaunchAttribute ea[1];
+  ea[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  ea[0].val.programmaticStreamSerializationAllowed = 1;
+  ec.attrs = ea;
+  ec.numAttrs = chain ? 1 : 0;
+  const long long chk_stride = p.batch > 1 ? chk_entry : 0;
+  const int rc = with_tile(v.bn, v.cg, [&](auto bn, auto) {
+    auto launch = [&](auto kern) {
+      FT_CUDA(h, cudaLaunchKernelEx(&ec, kern, p.B, p.N, p.K, p.ldb, p.stride_b, p.batch, chk, p.ldk, chk_stride, rounding,
+                                    p.tiles_n));
+      return FTSGEMM_OK;
+    };
+    if (p.b_kmajor) return launch(encode_kernel<bn, true>);
+    if (small_items) return launch(encode_kernel<bn, false, 4, false>);
+    if (stream_b) return launch(encode_kernel<bn, false, 8, true>);
+    return launch(encode_kernel<bn, false, 8, false>);
+  });
+  if (rc) return rc;
+  ++h->launch_count;
+  FT_CUDA(h, cudaGetLastError());
+  return FTSGEMM_OK;
+}
+
+// The checksum operand (checksum vectors of B: 8 columns per N-tile, appended to B as extra tile-columns of the same GEMM;
+// K-major like B^T: n_chk_cols rows of K, row stride ldk), its encode, and the expected checksums with their slab flags.
+// (a batch: one checksum operand, one block of expected checksums and one run of slab flags per entry)
+int bind_checksums(ftsgemm_handle_t h, const Variant &v, KernelParams &p, const ftsgemm_opts &o, cudaStream_t stream,
+                   CUtensorMap *tmC) {
+  p.dbg_flags = static_cast<int>(dbg("ft_dbg", 0)) & 1;
+  const long long chk_entry = static_cast<long long>(p.n_chk_cols) * p.ldk;
+  const size_t chk_bytes = static_cast<size_t>(chk_entry) * p.batch * sizeof(float);
+  float *chk = nullptr;
+  int rc;
+  if (h->capturing) {
+    // a captured call encodes on every replay, into a checksum operand of its own: replays would otherwise overwrite
+    // the one an eager call with reuse_b_checksums relies on
+    if ((rc = dev_alloc(h, &chk, chk_bytes))) return rc;
+    h->retired.push_back(chk);
+  } else {
+    bool fresh = false;
+    if ((rc = grow(h, h->d_chk, chk_bytes, 0, &fresh))) return rc;
+    if (fresh) h->chk_key = ChkKey();  // reallocated: the cached encode is gone
+    chk = static_cast<float *>(h->d_chk.ptr);
   }
-  if (ft) {
-    p.chk_slices = choose_chk_slices(p, max_units, K);
-    const size_t flag_bytes = h->chk_flag_bytes;
-    const size_t n_flags_s = static_cast<size_t>(p.tiles_m) * CG * (kBM / 32) * p.tiles_c * p.chk_slices * bt.count;
-    if (p.chk_slices > 1 && n_flags_s * sizeof(SeqFlag) > flag_bytes) p.chk_slices = 1;
-    if (p.chk_slices > 1) {
-      // one plane of expected checksums per slice (and entry)
-      const size_t out_floats = static_cast<size_t>(M) * p.n_chk_cols * p.chk_slices * bt.count;
-      const float *out_before = h->d_chk_out;
-      rc = ensure_buf(h, &h->d_chk_out, &h->chk_out_bytes, flag_bytes + out_floats * sizeof(float));
-      if (rc) return rc;
-      if (h->d_chk_out != out_before && (rc = upload(h, h->d_chk_out, nullptr, flag_bytes))) return rc;  // fresh flags
-      p.chk_flags = reinterpret_cast<SeqFlag *>(h->d_chk_out);
-      p.chk_out = h->d_chk_out + flag_bytes / sizeof(float);
-    }
+  // one slab flag per 32-row slab, checksum tile-column and slice; one plane of expected checksums per slice
+  const size_t n_flags = static_cast<size_t>(p.tiles_m) * v.cg * (kBM / 32) * p.tiles_c * p.chk_slices * p.batch;
+  if (n_flags * sizeof(SeqFlag) > h->chk_flag_bytes) {  // grow the flag region: a new buffer
+    h->chk_flag_bytes = (n_flags * sizeof(SeqFlag) + kChkFlagBytes - 1) / kChkFlagBytes * kChkFlagBytes;
+    if ((rc = drop(h, h->d_chk_out))) return rc;
   }
-  const PlanInput pin = make_plan_input(max_units, CG, BN, K, p, h->l2_bytes);
-  const std::array<long long, 7> key = {v.info.id, M, N, K, pin.units,
+  const size_t flag_bytes = h->chk_flag_bytes;
+  const size_t out_floats = static_cast<size_t>(p.M) * p.n_chk_cols * p.chk_slices * p.batch;
+  // the flags of a new buffer start at 0, below every epoch (LaunchSeq): they never need clearing again
+  if ((rc = grow(h, h->d_chk_out, flag_bytes + out_floats * sizeof(float), flag_bytes))) return rc;
+  p.chk_flags = bind<SeqFlag>(h, h->d_chk_out);
+  p.chk_out = bind(h, h->d_chk_out) + flag_bytes / sizeof(float);
+  const ChkKey chk_key = {p.B, p.N, p.K, v.bn, p.b_kmajor != 0, p.ldb, p.batch, p.stride_b};
+  const bool reuse = !h->capturing && o.reuse_b_checksums && h->chk_key == chk_key;
+  // Default: the encode is part of the FRONT PHASE of the GEMM kernel (KernelParams::enc_front) -- one launch per fused
+  // GEMM, like the reference (sgemm.cu:191-192); only below ~8 MB of B the stand-alone pre-pass is used.
+  const long long ef = dbg("enc_front", -2);
+  const bool enc_front = !reuse && (ef >= 0 ? ef != 0 : 4.0 * p.N * static_cast<double>(p.K) * p.batch >= static_cast<double>(dbg("enc_front_min_mb", 8)) * 1048576.0);
+  if (enc_front) {
+    p.enc_front = 1;
+    p.enc_out = chk;
+    p.enc_ld = p.ldk;
+  }
+  if (!reuse && !enc_front && (rc = launch_encode(h, v, p, chk, chk_entry, stream))) return rc;
+  if (!reuse && !h->capturing) h->chk_key = chk_key;
+  return make_tmap_kmajor(h, tmC, chk, p.n_chk_cols, p.K, p.ldk, chk_entry, p.batch, v.bn / v.cg);
+}
+
+using CachedPlan = ftsgemm_handle_s::CachedPlan;
+
+// The work plan (plan.h), built and uploaded on first use and cached per shape on the handle.
+int cached_plan(ftsgemm_handle_t h, const Variant &v, const KernelParams &p, const PlanInput &pin, CachedPlan **out) {
+  const std::array<long long, 7> key = {v.info.id, p.M, p.N, p.K, pin.units,
                                         pin.force_slices * 16 + pin.max_slices + pin.lockstep * 8192 + pin.full_search * 16384 + pin.chk_slices * 65536,
-                                        bt.count};
-  ftsgemm_handle_s::CachedPlan &cp = h->plans[key];
-  if (!cp.uploaded) {
-    if (h->plans.size() > 64 && !h->capturing) {  // bound the cache: drop everything but this entry and captured plans
-      for (auto it = h->plans.begin(); it != h->plans.end();) {
-        if (&it->second == &cp || it->second.captured) { ++it; continue; }
-        cudaFree(it->second.d_items);
-        cudaFree(it->second.d_off);
-        cudaFree(it->second.d_wave_target);
-        it = h->plans.erase(it);
-      }
+                                        p.batch};
+  CachedPlan &cp = h->plans[key];
+  *out = &cp;
+  if (cp.uploaded) return FTSGEMM_OK;
+  int rc;
+  if (h->plans.size() > 64 && !h->capturing) {  // bound the cache: drop everything but this entry
+    for (auto it = h->plans.begin(); it != h->plans.end();) {
+      if (&it->second == &cp) { ++it; continue; }
+      for (DevBuf *b : it->second.bufs())
+        if ((rc = drop(h, *b))) return rc;
+      it = h->plans.erase(it);
     }
-    cp.plan = build_plan(pin);
-    cp.packed.resize(cp.plan.items.size());
-    for (size_t i = 0; i < cp.plan.items.size(); ++i) {
-      const PlanItem &it = cp.plan.items[i];
-      cp.packed[i] = make_int4(it.tile, it.kb_begin | (it.kb_end << 16), it.kind | (it.slice << 8), it.split_idx);
-    }
-    if ((rc = dev_alloc(h, &cp.d_items, std::max<size_t>(1, cp.packed.size()) * sizeof(int4))) ||
-        (rc = dev_alloc(h, &cp.d_off, cp.plan.offsets.size() * sizeof(int))) ||
-        (rc = upload(h, cp.d_items, cp.packed.data(), cp.packed.size() * sizeof(int4))) ||
-        (rc = upload(h, cp.d_off, cp.plan.offsets.data(), cp.plan.offsets.size() * sizeof(int))))
-      return rc;
-    {  // wave targets (see KernelParams::wave_cnt)
-      std::vector<int> per_unit(static_cast<size_t>(cp.plan.units), 0);
-      int max_w = 0;
-      for (int u = 0; u < cp.plan.units; ++u) {
-        for (int i = cp.plan.offsets[u]; i < cp.plan.offsets[u + 1]; ++i)
-          if (cp.plan.items[i].kind == 0 && cp.plan.items[i].tile >= pin.n_chk_tiles) ++per_unit[u];
-        max_w = std::max(max_w, per_unit[u]);
-      }
-      cp.wave_target.assign(static_cast<size_t>(max_w) + 1, 0);
-      for (int u = 0; u < cp.plan.units; ++u)
-        for (int w = 0; w < per_unit[u]; ++w) ++cp.wave_target[w];
-      if ((rc = dev_alloc(h, &cp.d_wave_target, cp.wave_target.size() * sizeof(int))) ||
-          (rc = upload(h, cp.d_wave_target, cp.wave_target.data(), cp.wave_target.size() * sizeof(int))))
-        return rc;
-    }
-    cp.uploaded = true;
   }
-  if (h->capturing) cp.captured = true;
+  cp.plan = build_plan(pin);
+  cp.packed.resize(cp.plan.items.size());
+  for (size_t i = 0; i < cp.plan.items.size(); ++i) {
+    const PlanItem &it = cp.plan.items[i];
+    cp.packed[i] = make_int4(it.tile, it.kb_begin | (it.kb_end << 16), it.kind | (it.slice << 8), it.split_idx);
+  }
+  // wave targets (see KernelParams::wave_cnt)
+  std::vector<int> per_unit(static_cast<size_t>(cp.plan.units), 0);
+  int max_w = 0;
+  for (int u = 0; u < cp.plan.units; ++u) {
+    for (int i = cp.plan.offsets[u]; i < cp.plan.offsets[u + 1]; ++i)
+      if (cp.plan.items[i].kind == 0 && cp.plan.items[i].tile >= pin.n_chk_tiles) ++per_unit[u];
+    max_w = std::max(max_w, per_unit[u]);
+  }
+  cp.wave_target.assign(static_cast<size_t>(max_w) + 1, 0);
+  for (int u = 0; u < cp.plan.units; ++u)
+    for (int w = 0; w < per_unit[u]; ++w) ++cp.wave_target[w];
+  const size_t item_bytes = cp.packed.size() * sizeof(int4), off_bytes = cp.plan.offsets.size() * sizeof(int),
+               wave_bytes = cp.wave_target.size() * sizeof(int);
+  if ((rc = grow(h, cp.d_items, std::max(sizeof(int4), item_bytes))) || (rc = grow(h, cp.d_off, off_bytes)) ||
+      (rc = grow(h, cp.d_wave_target, wave_bytes)) || (rc = upload(h, cp.d_items.ptr, cp.packed.data(), item_bytes)) ||
+      (rc = upload(h, cp.d_off.ptr, cp.plan.offsets.data(), off_bytes)) ||
+      (rc = upload(h, cp.d_wave_target.ptr, cp.wave_target.data(), wave_bytes)))
+    return rc;
+  cp.uploaded = true;
+  return FTSGEMM_OK;
+}
+
+// The plan's launch arguments and the workspaces that depend on it: split-K, wave re-synchronisation and trace.
+int bind_plan(ftsgemm_handle_t h, const Variant &v, KernelParams &p, const PlanInput &pin, CachedPlan &cp,
+              cudaStream_t stream) {
   const int units = cp.plan.units;
-  p.front_target = units * CG * (kThreads / 32);
-  p.plan = cp.d_items;
-  p.plan_off = cp.d_off;
+  int rc;
+  p.front_target = units * v.cg * (kThreads / 32);
+  p.plan = bind<int4>(h, cp.d_items);
+  p.plan_off = bind<int>(h, cp.d_off);
   p.sk_tiles = cp.plan.sk_tiles;
   p.sk_slices = cp.plan.sk_slices;
   if (p.sk_tiles > 0) {
-    // fixed location at the start of the buffer: the 16384 flags build_plan allows for
+    // fixed location at the start of the buffer: the 16384 flags build_plan allows for; fresh flags, below every epoch
     const size_t flag_bytes = 16384 * sizeof(SeqFlag);
-    const size_t ws_floats = static_cast<size_t>(p.sk_tiles) * (p.sk_slices - 1) * CG * kBM * BN;
-    const float *before = h->d_sk;
-    rc = ensure_buf(h, &h->d_sk, &h->sk_bytes, flag_bytes + ws_floats * sizeof(float));
-    if (rc) return rc;
-    if (h->d_sk != before && (rc = upload(h, h->d_sk, nullptr, flag_bytes))) return rc;  // fresh flags, below every epoch
-    p.sk_flags = reinterpret_cast<SeqFlag *>(h->d_sk);
-    p.sk_ws = h->d_sk + flag_bytes / sizeof(float);
+    const size_t ws_floats = static_cast<size_t>(p.sk_tiles) * (p.sk_slices - 1) * v.cg * kBM * v.bn;
+    if ((rc = grow(h, h->d_sk, flag_bytes + ws_floats * sizeof(float), flag_bytes))) return rc;
+    p.sk_flags = bind<SeqFlag>(h, h->d_sk);
+    p.sk_ws = bind(h, h->d_sk) + flag_bytes / sizeof(float);
   }
-  {
-    // Helper-assisted final epilogues (the helper warp of each 32-row quadrant takes the upper half of the columns): on
-    // for ABFT kernels and for plain kernels with at most three items per unit, where the epilogue is most exposed.
-    const long long ea = dbg("epi_assist", -2);
-    p.epi_assist = ea >= 0 ? (ea != 0) : (ft || cp.plan.items.size() <= 3 * static_cast<size_t>(units));
-  }
-  {
-    // Wave re-synchronisation for problems that run many waves (>= 24) over operands that do not fit L2: without it the
-    // units' start times drift apart wave by wave and stop sharing the A / B panels in L2.
-    const long long ws = dbg("wave_sync", -2);
-    const bool on = ws >= 0 ? (ws != 0) : (pin.lockstep && static_cast<int>(cp.wave_target.size()) >= 24);
-    if (on && cp.wave_target.size() > 1) {
-      const size_t bytes = cp.wave_target.size() * sizeof(int);
-      if (h->d_wave_cnt == nullptr || h->wave_cnt_cap < cp.wave_target.size()) {
-        if ((rc = release(h, h->d_wave_cnt))) return rc;
-        h->d_wave_cnt = nullptr;
-        if ((rc = dev_alloc(h, &h->d_wave_cnt, bytes))) return rc;
-        h->wave_cnt_cap = cp.wave_target.size();
-      }
-      FT_CUDA(h, cudaMemsetAsync(h->d_wave_cnt, 0, bytes, stream));
-      p.wave_cnt = h->d_wave_cnt;
-      p.wave_target = cp.d_wave_target;
-    }
+  // Helper-assisted final epilogues (the helper warp of each 32-row quadrant takes the upper half of the columns): on
+  // for ABFT kernels and for plain kernels with at most three items per unit, where the epilogue is most exposed.
+  const long long ea = dbg("epi_assist", -2);
+  p.epi_assist = ea >= 0 ? (ea != 0) : (v.info.fault_tolerant || cp.plan.items.size() <= 3 * static_cast<size_t>(units));
+  // Wave re-synchronisation for problems that run many waves (>= 24) over operands that do not fit L2: without it the
+  // units' start times drift apart wave by wave and stop sharing the A / B panels in L2.
+  const long long ws = dbg("wave_sync", -2);
+  const bool on = ws >= 0 ? (ws != 0) : (pin.lockstep && static_cast<int>(cp.wave_target.size()) >= 24);
+  if (on && cp.wave_target.size() > 1) {
+    const size_t bytes = cp.wave_target.size() * sizeof(int);
+    if ((rc = grow(h, h->d_wave_cnt, bytes))) return rc;
+    FT_CUDA(h, cudaMemsetAsync(h->d_wave_cnt.ptr, 0, bytes, stream));
+    p.wave_cnt = bind<int>(h, h->d_wave_cnt);
+    p.wave_target = bind<int>(h, cp.d_wave_target);
   }
   if (dbg("trace", 0) != 0) {
     const int cap = 64;
-    if (h->d_trace == nullptr || h->trace_units < units) {
-      if ((rc = release(h, h->d_trace))) return rc;
-      h->d_trace = nullptr;
-      if ((rc = dev_alloc(h, &h->d_trace, static_cast<size_t>(units) * cap * 8 * sizeof(unsigned long long)))) return rc;
-      h->trace_units = units;
-    }
-    FT_CUDA(h, cudaMemsetAsync(h->d_trace, 0, static_cast<size_t>(units) * cap * 8 * sizeof(unsigned long long), stream));
-    p.trace = h->d_trace;
+    const size_t bytes = static_cast<size_t>(units) * cap * 8 * sizeof(unsigned long long);
+    bool fresh = false;
+    if ((rc = grow(h, h->d_trace, bytes, 0, &fresh))) return rc;
+    if (fresh) h->trace_units = units;
+    FT_CUDA(h, cudaMemsetAsync(h->d_trace.ptr, 0, bytes, stream));
+    p.trace = bind<unsigned long long>(h, h->d_trace);
     p.trace_cap = cap;
   }
+  return FTSGEMM_OK;
+}
+
+// One product on the wgmma kernels, in stages: argument checks, kernel parameters, operands, launch plan, checksums, cached
+// work plan, per-plan workspaces, launch.
+int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC, int ldc,
+           float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o, cudaStream_t stream,
+           const BatchArg &bt = kSingle) {
+  int rc = check_tc_args(v, M, N, K, A, B, dC, bt.count);
+  if (rc) return rc;
+  KernelParams p = make_params(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, bt);
+  CUtensorMap tmA, tmB, tmC;
+  PlanInput pin;
+  if ((rc = bind_operands(h, v, p, &tmA, &tmB)) || (rc = plan_on_device(h, v, p, &pin))) return rc;
+  tmC = tmB;
+  if (v.info.fault_tolerant && (rc = bind_checksums(h, v, p, o, stream, &tmC))) return rc;
+  CachedPlan *cp = nullptr;
+  if ((rc = cached_plan(h, v, p, pin, &cp)) || (rc = bind_plan(h, v, p, pin, *cp, stream))) return rc;
   // Programmatic dependent launch by default: the kernel's launch latency and prologue overlap the tail of whatever
   // precedes it in the stream; every thread executes griddepcontrol.wait before the first global access.
   p.pdl_wait = dbg("pdl_chain", 1) != 0 ? 1 : 0;
-  if (h->capturing) pin_workspaces(h);
   h->last_stream = stream;
   ++h->launch_count;
-  return with_tile(BN, CG, [&](auto bn, auto cg) {
-    return launch_variant<bn, cg>(h, tmA, tmB, tmC, p, units, stream, ft, o.protect_epilogue != 0);
+  return with_tile(v.bn, v.cg, [&](auto bn, auto cg) {
+    return launch_variant<bn, cg>(h, tmA, tmB, tmC, p, cp->plan.units, stream, v.info.fault_tolerant != 0,
+                                  o.protect_epilogue != 0);
   });
 }
 
@@ -958,6 +961,173 @@ __global__ void verify_kernel(const float *ref, const float *x, size_t n, unsign
   }
 }
 
+// The non-fused ABFT baseline (ftsgemm_baseline).
+int run_baseline(ftsgemm_handle_t h, int M, int N, int K, const float *dA, const float *dB, float *dC, float alpha, float beta,
+                 int math_mode, const ftsgemm_opts &o, float *residual_out) {
+  cudaStream_t stream = static_cast<cudaStream_t>(o.stream);
+  const bool host_sync = o.baseline_host_sync != 0;
+  if (h->capturing && host_sync) return FTSGEMM_ERR_UNSUPPORTED;  // it synchronises the stream between its steps
+  const int mx = M > N ? M : N;
+  // aux layout: ones[mx] | c_row[M] | c_col[N] | a_col[256] | b_row[256] | acol_x_b[N] | brow_x_a[M] | res[2] | consts[3]
+  const size_t need = static_cast<size_t>(mx) + M + N + 256 + 256 + N + M + 2 + 3;
+  const int arc = grow(h, h->d_aux, need * sizeof(float));
+  if (arc) return arc;
+  float *ones = bind(h, h->d_aux), *c_row = ones + mx, *c_col = c_row + M, *a_col = c_col + N, *b_row = a_col + 256,
+        *acol_x_b = b_row + 256, *brow_x_a = acol_x_b + N, *res = brow_x_a + M;
+  fill_kernel<<<(mx + 255) / 256, 256, 0, stream>>>(ones, 1.0f, mx);
+  FT_CUDA(h, cudaGetLastError());
+  FT_CUBLAS(h, cublasSetStream(h->cublas, stream));
+  FT_CUBLAS(h, cublasSetMathMode(h->cublas, math_mode ? CUBLAS_TF32_TENSOR_OP_MATH : CUBLAS_DEFAULT_MATH));
+  const float one = 1.0f, zero = 0.0f, neg1 = -1.0f;
+  for (int k0 = 0; k0 < K; k0 += 256) {
+    const int kc = (K - k0) < 256 ? (K - k0) : 256;
+    const float beta_eff = (k0 == 0) ? beta : 1.0f;
+    const float *Ac = dA + static_cast<size_t>(k0) * M;
+    const float *Bc = dB + static_cast<size_t>(k0) * N;
+    FT_CUBLAS(h, cublasSetPointerMode(h->cublas, CUBLAS_POINTER_MODE_HOST));
+    // product chunk (baseline_ft_sgemm.cuh:6)
+    FT_CUBLAS(h, cublasSgemm(h->cublas, CUBLAS_OP_N, CUBLAS_OP_T, M, N, kc, &alpha, Ac, M, Bc, N, &beta_eff, dC, M));
+    if (host_sync) FT_CUDA(h, cudaStreamSynchronize(stream));
+    // row / column sums of all of C (:9,:12) -- the re-read of C the fused kernel removes
+    FT_CUBLAS(h, cublasSgemv(h->cublas, CUBLAS_OP_N, M, N, &one, dC, M, ones, 1, &zero, c_row, 1));
+    FT_CUBLAS(h, cublasSgemv(h->cublas, CUBLAS_OP_T, M, N, &one, dC, M, ones, 1, &zero, c_col, 1));
+    // encode: e^T A_chunk (:15) and B_chunk^T e (:18)
+    FT_CUBLAS(h, cublasSgemv(h->cublas, CUBLAS_OP_T, M, kc, &one, Ac, M, ones, 1, &zero, a_col, 1));
+    FT_CUBLAS(h, cublasSgemv(h->cublas, CUBLAS_OP_T, N, kc, &one, Bc, N, ones, 1, &zero, b_row, 1));
+    if (host_sync) FT_CUDA(h, cudaStreamSynchronize(stream));
+    // checksum products (:21,:24); accumulated over chunks so that, for alpha = 1 and beta = 0, the residual of
+    // the last chunk is the residual of the whole product
+    const float *acc_beta = (k0 == 0) ? &zero : &one;
+    FT_CUBLAS(h, cublasSgemv(h->cublas, CUBLAS_OP_N, N, kc, &one, Bc, N, a_col, 1, acc_beta, acol_x_b, 1));
+    FT_CUBLAS(h, cublasSgemv(h->cublas, CUBLAS_OP_N, M, kc, &one, Ac, M, b_row, 1, acc_beta, brow_x_a, 1));
+    if (host_sync) FT_CUDA(h, cudaStreamSynchronize(stream));
+    // residual + reduce (:27-31); dot results land in device memory
+    FT_CUBLAS(h, cublasSaxpy(h->cublas, N, &neg1, acol_x_b, 1, c_col, 1));
+    FT_CUBLAS(h, cublasSetPointerMode(h->cublas, CUBLAS_POINTER_MODE_DEVICE));
+    FT_CUBLAS(h, cublasSdot(h->cublas, N, c_col, 1, ones, 1, res));
+    if (host_sync) FT_CUDA(h, cudaStreamSynchronize(stream));
+    FT_CUBLAS(h, cublasSetPointerMode(h->cublas, CUBLAS_POINTER_MODE_HOST));
+    FT_CUBLAS(h, cublasSaxpy(h->cublas, M, &neg1, brow_x_a, 1, c_row, 1));
+    FT_CUBLAS(h, cublasSetPointerMode(h->cublas, CUBLAS_POINTER_MODE_DEVICE));
+    FT_CUBLAS(h, cublasSdot(h->cublas, M, c_row, 1, ones, 1, res + 1));
+  }
+  FT_CUBLAS(h, cublasSetPointerMode(h->cublas, CUBLAS_POINTER_MODE_HOST));
+  if (residual_out)
+    FT_CUDA(h, cudaMemcpyAsync(residual_out, res, 2 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
+  h->last_stream = stream;
+  return FTSGEMM_OK;
+}
+
+
+// 3xTF32 (FP32-grade accuracy, the reference's kernels are true FP32 FFMA, ft_sgemm_huge.cuh:228-323): with
+// x = hi + lo (hi = the 11 significant bits the tensor core reads, lo = x - hi exactly),
+//   A B^T ~= A_lo B_hi^T + A_hi B_lo^T + A_hi B_hi^T       (A_lo B_lo^T ~ 2^-22 relative is dropped)
+// as three launches of the same kernel, smallest terms first, each accumulating into C -- every one of them a
+// complete fault-tolerant GEMM with its own checksum vectors, so ABFT covers the whole 3-pass product.
+int run_3xtf32(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC,
+               int ldc, float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o,
+               cudaStream_t stream, const BatchArg &bt) {
+  // (before the split kernels read the operands with 16-byte loads)
+  int rc = check_tc_args(v, M, N, K, A, B, dC, bt.count);
+  if (rc) return rc;
+  // The lo parts are written dense in the operand's own layout: ld = rows (MN-major) or K rounded up to 4 (K-major).
+  auto lo_of = [K](const Operand &x, int rows) {
+    return Operand{nullptr, x.kmajor, x.kmajor ? (K + 3) / 4 * 4 : rows};
+  };
+  Operand Alo = lo_of(A, M), Blo = lo_of(B, N);
+  const size_t a_floats = static_cast<size_t>(Alo.ld) * (Alo.kmajor ? M : K);
+  const size_t b_floats = static_cast<size_t>(Blo.ld) * (Blo.kmajor ? N : K);
+  // The lo parts of entry e at e * a_floats (e * b_floats), and behind them the sanitised operands A_s, B_s in the same
+  // layout (split_lo_kernel), from one launch per operand; then the three passes
+  //   A_lo B_s^T + A_s B_lo^T + A B^T
+  // so that only the last one sees a non-finite operand value.
+  const size_t lo_floats = (a_floats + b_floats) * bt.count;
+  if ((rc = grow(h, h->d_lo, 2 * lo_floats * sizeof(float)))) return rc;
+  float *dAlo = bind(h, h->d_lo), *dBlo = dAlo + a_floats * bt.count;
+  Alo.p = dAlo;
+  Blo.p = dBlo;
+  Operand As = Alo, Bs = Blo;
+  As.p = dAlo + lo_floats;
+  Bs.p = dBlo + lo_floats;
+  auto split = [&](const Operand &x, const Operand &lo, int rows, long long sx, float *dst) {
+    const int inner = x.kmajor ? K : rows;  // elements per stored row of the operand
+    const size_t outer = x.kmajor ? rows : K;
+    const int blocks = h->num_sms * 8;
+    if (x.ld == inner && lo.ld == inner && (bt.count == 1 || sx == static_cast<long long>(outer) * inner))
+      // dense: all entries are one flat array (a multiple of 4 elements: M and N are)
+      split_lo_kernel<<<blocks, 256, 0, stream>>>(reinterpret_cast<const float4 *>(x.p), reinterpret_cast<float4 *>(dst),
+                                                  reinterpret_cast<float4 *>(dst + lo_floats), outer * inner * bt.count / 4);
+    else  // padded rows or entries: nothing outside the operand's rows is read
+      split_lo_strided_kernel<<<dim3(std::max(1, blocks / bt.count), std::min(bt.count, 65535)), 256, 0, stream>>>(
+          x.p, x.ld, sx, dst, dst + lo_floats, lo.ld, inner, outer, bt.count);
+  };
+  split(A, Alo, M, bt.sa, dAlo);
+  split(B, Blo, N, bt.sb, dBlo);
+  FT_CUDA(h, cudaGetLastError());
+  h->launch_count += 2;
+  ftsgemm_opts o3 = o;
+  o3.reuse_b_checksums = 0;
+  o3.precision = 0;
+  ftsgemm_opts o_quiet = o3;  // injected faults belong to the main product only
+  o_quiet.inject_mode = 0;
+  // (the bias goes to the last pass only: added once, after the final alpha*acc + C)
+  const BatchArg lo = {bt.count, static_cast<long long>(a_floats), static_cast<long long>(b_floats), bt.sc};
+  rc = run_tc(h, v, M, N, K, Alo, Bs, dC, ldc, alpha, beta, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo);
+  if (!rc) rc = run_tc(h, v, M, N, K, As, Blo, dC, ldc, alpha, 1.0f, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo);
+  if (!rc) rc = run_tc(h, v, M, N, K, A, B, dC, ldc, alpha, 1.0f, bias, bias_mode, o3, stream, bt);
+  return rc;
+}
+
+int run_resolved(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC,
+                 int ldc, float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o,
+                 cudaStream_t stream, const BatchArg &bt);
+
+// Intra-K checking (ftsgemm_opts::check_segments): S consecutive K-segments, each a complete fault-tolerant GEMM.  A
+// segment of an operand is a pointer offset: k0 * ld for an MN-major operand (k is the slow index), k0 for a K-major one;
+// segment boundaries are multiples of the stage depth (32 k-rows), so the offsets keep 16-byte alignment.  Injected
+// faults (tests) go to the first segment only, the bias to the last one (added once, after the final alpha*acc + C).
+int run_segments(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC,
+                 int ldc, float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o,
+                 cudaStream_t stream, const BatchArg &bt) {
+  const int num_kb = (K + kBK - 1) / kBK;
+  const int S = std::min(o.check_segments, num_kb);
+  ftsgemm_opts os = o;
+  os.check_segments = 1;
+  os.reuse_b_checksums = 0;
+  int rc = FTSGEMM_OK;
+  for (int sg = 0; sg < S && !rc; ++sg) {
+    const int k0 = static_cast<int>(static_cast<long long>(num_kb) * sg / S) * kBK;
+    const int k1 = std::min(K, static_cast<int>(static_cast<long long>(num_kb) * (sg + 1) / S) * kBK);
+    if (sg > 0) os.inject_mode = 0;
+    // (a batch: the offsets apply to the base pointers, the entry strides are unchanged)
+    const Operand As = {A.p + (A.kmajor ? static_cast<size_t>(k0) : static_cast<size_t>(k0) * A.ld), A.kmajor, A.ld};
+    const Operand Bs = {B.p + (B.kmajor ? static_cast<size_t>(k0) : static_cast<size_t>(k0) * B.ld), B.kmajor, B.ld};
+    const bool last = sg == S - 1;
+    rc = run_resolved(h, v, M, N, k1 - k0, As, Bs, dC, ldc, alpha, sg == 0 ? beta : 1.0f, last ? bias : nullptr,
+                      last ? bias_mode : FTSGEMM_BIAS_NONE, os, stream, bt);
+  }
+  return rc;
+}
+
+// One call of ftsgemm_run_batched after validation: its variant resolved (ids 20 / 40 chosen per shape), its options
+// loaded and h->capturing set.
+int run_resolved(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC,
+                 int ldc, float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o,
+                 cudaStream_t stream, const BatchArg &bt) {
+  const bool tc = v.info.engine == 1;
+  if (tc && o.check_segments > 1 && v.info.fault_tolerant)
+    return run_segments(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt);
+  if (tc && o.precision == 1) return run_3xtf32(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt);
+  switch (v.info.engine) {
+    case 0: return run_cublas(h, v.info.id == 7, M, N, K, A, B, dC, ldc, alpha, beta, stream, bt);
+    case 1: return run_tc(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt);
+    case 2:
+      // the non-fused baseline keeps the reference's call sequence, on the reference layout only
+      if (A.kmajor || B.kmajor || A.ld != M || B.ld != N || ldc != M) return FTSGEMM_ERR_UNSUPPORTED;
+      return run_baseline(h, M, N, K, A.p, B.p, dC, alpha, beta, v.info.id == 30 ? 1 : 0, o, nullptr);
+  }
+  return FTSGEMM_ERR_UNSUPPORTED;
+}
 }  // namespace
 
 // =============================================================================================== C ABI
@@ -1019,11 +1189,7 @@ static int debug_schedule_rows(int kernel_id, int M, int N, int K, int batch, in
   memset(&p, 0, sizeof(p));
   p.M = M; p.N = N; p.K = K;
   p.batch = batch;
-  plan_tiles(M, N, v->bn, v->cg, v->info.fault_tolerant != 0, &p);
-  if (v->info.fault_tolerant) {
-    p.chk_slices = choose_chk_slices(p, num_sms / v->cg, K);
-  }
-  const PlanInput pin = make_plan_input(num_sms / v->cg, v->cg, v->bn, K, p, kDefaultL2Bytes);
+  const PlanInput pin = plan_launch(*v, num_sms / v->cg, kDefaultL2Bytes, &p);
   const Plan plan = build_plan(pin);
   if (hdr) {
     hdr[0] = plan.units; hdr[1] = pin.n_chk_tiles + pin.n_data_tiles; hdr[2] = pin.n_chk_tiles; hdr[3] = plan.sk_tiles;
@@ -1056,12 +1222,12 @@ int ftsgemm_debug_schedule_batched(int kernel_id, int M, int N, int K, int batch
 
 int ftsgemm_debug_trace(ftsgemm_handle_t h, unsigned long long *out, int cap_u64) {
   if (!h || !out) return FTSGEMM_ERR_INVALID_ARG;
-  if (!h->d_trace) return 0;
+  if (!h->d_trace.ptr) return 0;
   const int n = h->trace_units * 64 * 8;
   if (cap_u64 < n) return FTSGEMM_ERR_INVALID_ARG;
   FT_NOT_WHILE_CAPTURING(h, h->last_stream);
   FT_CUDA(h, cudaDeviceSynchronize());
-  FT_CUDA(h, cudaMemcpy(out, h->d_trace, static_cast<size_t>(n) * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+  FT_CUDA(h, cudaMemcpy(out, h->d_trace.ptr, static_cast<size_t>(n) * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
   return h->trace_units;
 }
 
@@ -1118,28 +1284,16 @@ int ftsgemm_destroy(ftsgemm_handle_t h) {
   cudaDeviceSynchronize();
   if (h->cublas) cublasDestroy(h->cublas);
   cudaFree(h->d_stats);
-  cudaFree(h->d_chk);
-  cudaFree(h->d_chk_out);
-  cudaFree(h->d_sk);
-  cudaFree(h->d_trace);
-  cudaFree(h->d_wave_cnt);
-  for (auto &kv : h->plans) {
-    cudaFree(kv.second.d_items);
-    cudaFree(kv.second.d_off);
-    cudaFree(kv.second.d_wave_target);
-  }
-  cudaFree(h->d_aux);
-  cudaFree(h->d_lo);
-  cudaFree(h->d_seq);
+  for (DevBuf *b : h->bufs()) cudaFree(b->ptr);
+  for (auto &kv : h->plans)
+    for (DevBuf *b : kv.second.bufs()) cudaFree(b->ptr);
   for (void *p : h->retired) cudaFree(p);
+  cudaFree(h->d_seq);
   if (h->s_up) cudaStreamDestroy(h->s_up);
-  cudaFree(h->d_at);
-  cudaFree(h->d_bt);
   for (int r = 0; r < kMaxPeers; ++r)
     if (h->peer_opened[r]) cudaIpcCloseMemHandle(h->peer_box[r]);
   cudaFree(h->d_mailbox);
   cudaFree(h->d_verify);
-  for (int i = 0; i < 3; ++i) cudaFree(h->d_stage[i]);
   if (h->s_in) {
     cudaStreamDestroy(h->s_in);
     cudaStreamDestroy(h->s_out);
@@ -1232,101 +1386,7 @@ int ftsgemm_run_batched(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, 
     v = find_variant(select_variant(M, N, v->info.fault_tolerant != 0, bt.count));
     if (!v) return FTSGEMM_ERR_UNSUPPORTED;
   }
-  if (v->info.engine == 1 && o.check_segments > 1 && v->info.fault_tolerant) {
-    // Intra-K checking (ftsgemm_opts::check_segments): S consecutive K-segments, each a complete fault-tolerant GEMM.  A
-    // segment of an operand is a pointer offset: k0 * ld for an MN-major operand (k is the slow index), k0 for a K-major one;
-    // segment boundaries are multiples of the stage depth (32 k-rows), so the offsets keep 16-byte alignment.  Injected
-    // faults (tests) go to the first segment only, the bias to the last one (added once, after the final alpha*acc + C).
-    int S = o.check_segments;
-    const int num_kb = (K + kBK - 1) / kBK;
-    if (S > num_kb) S = num_kb;
-    ftsgemm_opts os = o;
-    os.check_segments = 1;
-    os.reuse_b_checksums = 0;
-    int rc = FTSGEMM_OK;
-    for (int sg = 0; sg < S && !rc; ++sg) {
-      const int k0 = static_cast<int>(static_cast<long long>(num_kb) * sg / S) * kBK;
-      int k1 = static_cast<int>(static_cast<long long>(num_kb) * (sg + 1) / S) * kBK;
-      if (k1 > K) k1 = K;
-      if (sg > 0) os.inject_mode = 0;
-      const size_t oa = A.kmajor ? static_cast<size_t>(k0) : static_cast<size_t>(k0) * lda;
-      const size_t ob = B.kmajor ? static_cast<size_t>(k0) : static_cast<size_t>(k0) * ldb;
-      const bool last = sg == S - 1;
-      // (a batch: the offsets apply to the base pointers, the entry strides are unchanged)
-      rc = ftsgemm_run_batched(h, v->info.id, M, N, k1 - k0, dA + oa, layout_a, lda, stride_a, dB + ob, layout_b, ldb, stride_b, dC,
-                               ldc, stride_c, batch, alpha, sg == 0 ? beta : 1.0f, last ? bias : nullptr,
-                               last ? bias_mode : FTSGEMM_BIAS_NONE, &os);
-    }
-    return rc;
-  }
-  if (v->info.engine == 1 && o.precision == 1) {
-    // 3xTF32 (FP32-grade accuracy, the reference's kernels are true FP32 FFMA, ft_sgemm_huge.cuh:228-323): with
-    // x = hi + lo (hi = the 11 significant bits the tensor core reads, lo = x - hi exactly),
-    //   A B^T ~= A_lo B_hi^T + A_hi B_lo^T + A_hi B_hi^T       (A_lo B_lo^T ~ 2^-22 relative is dropped)
-    // as three launches of the same kernel, smallest terms first, each accumulating into C -- every one of them a
-    // complete fault-tolerant GEMM with its own checksum vectors, so ABFT covers the whole 3-pass product.
-    if ((static_cast<size_t>(M) * K) % 4 || (static_cast<size_t>(N) * K) % 4) return FTSGEMM_ERR_UNSUPPORTED;
-    // (run_tc's argument checks, before the split kernels read the operands with 16-byte loads)
-    if ((M % 4) || (N % 4)) return FTSGEMM_ERR_UNSUPPORTED;
-    if ((lda % 4) || (ldb % 4) || ((reinterpret_cast<uintptr_t>(dA) | reinterpret_cast<uintptr_t>(dB)) & 15))
-      return FTSGEMM_ERR_INVALID_ARG;
-    // The lo parts are written dense in the operand's own layout: ld = rows (MN-major) or K rounded up to 4 (K-major).
-    auto lo_of = [K](const Operand &x, int rows) {
-      return Operand{nullptr, x.kmajor, x.kmajor ? (K + 3) / 4 * 4 : rows};
-    };
-    Operand Alo = lo_of(A, M), Blo = lo_of(B, N);
-    const size_t a_floats = static_cast<size_t>(Alo.ld) * (Alo.kmajor ? M : K);
-    const size_t b_floats = static_cast<size_t>(Blo.ld) * (Blo.kmajor ? N : K);
-    // The lo parts of entry e at e * a_floats (e * b_floats), and behind them the sanitised operands A_s, B_s in the same
-    // layout (split_lo_kernel), from one launch per operand; then the three passes
-    //   A_lo B_s^T + A_s B_lo^T + A B^T
-    // so that only the last one sees a non-finite operand value.
-    const size_t lo_floats = (a_floats + b_floats) * bt.count;
-    int rc = ensure_buf(h, &h->d_lo, &h->lo_bytes, 2 * lo_floats * sizeof(float));
-    if (rc) return rc;
-    float *dAlo = h->d_lo, *dBlo = h->d_lo + a_floats * bt.count;
-    Alo.p = dAlo;
-    Blo.p = dBlo;
-    Operand As = Alo, Bs = Blo;
-    As.p = dAlo + lo_floats;
-    Bs.p = dBlo + lo_floats;
-    auto split = [&](const Operand &x, const Operand &lo, int rows, long long sx, float *dst) {
-      const int inner = x.kmajor ? K : rows;  // elements per stored row of the operand
-      const size_t outer = x.kmajor ? rows : K;
-      const int blocks = h->num_sms * 8;
-      if (x.ld == inner && lo.ld == inner && (bt.count == 1 || sx == static_cast<long long>(outer) * inner))
-        // dense: all entries are one flat array (a multiple of 4 elements, see above)
-        split_lo_kernel<<<blocks, 256, 0, stream>>>(reinterpret_cast<const float4 *>(x.p), reinterpret_cast<float4 *>(dst),
-                                                    reinterpret_cast<float4 *>(dst + lo_floats), outer * inner * bt.count / 4);
-      else  // padded rows or entries: nothing outside the operand's rows is read
-        split_lo_strided_kernel<<<dim3(std::max(1, blocks / bt.count), std::min(bt.count, 65535)), 256, 0, stream>>>(
-            x.p, x.ld, sx, dst, dst + lo_floats, lo.ld, inner, outer, bt.count);
-    };
-    split(A, Alo, M, bt.sa, dAlo);
-    split(B, Blo, N, bt.sb, dBlo);
-    FT_CUDA(h, cudaGetLastError());
-    h->launch_count += 2;
-    ftsgemm_opts o3 = o;
-    o3.reuse_b_checksums = 0;
-    o3.precision = 0;
-    ftsgemm_opts o_quiet = o3;  // injected faults belong to the main product only
-    o_quiet.inject_mode = 0;
-    // (the bias goes to the last pass only: added once, after the final alpha*acc + C)
-    const BatchArg lo = {bt.count, static_cast<long long>(a_floats), static_cast<long long>(b_floats), bt.sc};
-    rc = run_tc(h, *v, M, N, K, Alo, Bs, dC, ldc, alpha, beta, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo);
-    if (!rc) rc = run_tc(h, *v, M, N, K, As, Blo, dC, ldc, alpha, 1.0f, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo);
-    if (!rc) rc = run_tc(h, *v, M, N, K, A, B, dC, ldc, alpha, 1.0f, bias, bias_mode, o3, stream, bt);
-    return rc;
-  }
-  switch (v->info.engine) {
-    case 0: return run_cublas(h, v->info.id == 7, M, N, K, A, B, dC, ldc, alpha, beta, stream, bt);
-    case 1: return run_tc(h, *v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt);
-    case 2:
-      // the non-fused baseline keeps the reference's call sequence, on the reference layout only
-      if (A.kmajor || B.kmajor || lda != M || ldb != N || ldc != M) return FTSGEMM_ERR_UNSUPPORTED;
-      return ftsgemm_baseline(h, M, N, K, dA, dB, dC, alpha, beta, v->info.id == 30 ? 1 : 0, &o, nullptr);
-  }
-  return FTSGEMM_ERR_UNSUPPORTED;
+  return run_resolved(h, *v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt);
 }
 
 int ftsgemm_get_stats(ftsgemm_handle_t h, ftsgemm_stats *out) {
@@ -1465,16 +1525,13 @@ int ftsgemm_run_host(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, con
   if (orc) return orc;
   DeviceGuard guard(h);
   FT_NOT_WHILE_CAPTURING(h, static_cast<cudaStream_t>(o.stream));
+  h->capturing = false;
   const size_t bytes[3] = {sizeof(float) * M * static_cast<size_t>(K), sizeof(float) * N * static_cast<size_t>(K),
                            sizeof(float) * M * static_cast<size_t>(N)};
-  for (int i = 0; i < 3; ++i)
-    if (h->stage_bytes[i] < bytes[i]) {
-      if (h->d_stage[i]) FT_CUDA(h, cudaFree(h->d_stage[i]));
-      h->d_stage[i] = nullptr;
-      h->stage_bytes[i] = 0;
-      FT_CUDA(h, cudaMalloc(&h->d_stage[i], bytes[i]));
-      h->stage_bytes[i] = bytes[i];
-    }
+  for (int i = 0; i < 3; ++i) {
+    const int rc = grow(h, h->d_stage[i], bytes[i]);
+    if (rc) return rc;
+  }
   cudaStream_t stream = static_cast<cudaStream_t>(o.stream);
   // Column panels of C pipeline the three phases (the PCIe link is full duplex and the GEMM of a panel takes a few per
   // cent of its transfer time): upload stream  A, B_0, C_0, B_1, C_1, ...;  compute stream  GEMM_j after (A, B_j, C_j);
@@ -1500,7 +1557,7 @@ int ftsgemm_run_host(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, con
       FT_CUDA(h, cudaEventCreateWithFlags(&h->ev_done[i], cudaEventDisableTiming));
     }
   }
-  float *dA = h->d_stage[0], *dBs = h->d_stage[1], *dC = h->d_stage[2];
+  float *dA = bind(h, h->d_stage[0]), *dBs = bind(h, h->d_stage[1]), *dC = bind(h, h->d_stage[2]);
   FT_CUDA(h, cudaMemcpyAsync(dA, hA, bytes[0], cudaMemcpyHostToDevice, h->s_in));
   for (int j = 0; j < panels; ++j) {
     const int n0 = j * pw, nj = (N - n0) < pw ? (N - n0) : pw;
@@ -1544,65 +1601,11 @@ int ftsgemm_baseline(ftsgemm_handle_t h, int M, int N, int K, const float *dA, c
   const int orc = load_opts(opts, &o);
   if (orc) return orc;
   DeviceGuard guard(h);
-  cudaStream_t stream = static_cast<cudaStream_t>(o.stream);
-  const bool host_sync = o.baseline_host_sync != 0;
-  {
-    bool cap = false;
-    const int crc = is_capturing(h, stream, &cap);
-    if (crc) return crc;
-    if (cap && host_sync) return FTSGEMM_ERR_UNSUPPORTED;  // it synchronises the stream between its steps
-    h->capturing = cap;
-  }
-  const int mx = M > N ? M : N;
-  // aux layout: ones[mx] | c_row[M] | c_col[N] | a_col[256] | b_row[256] | acol_x_b[N] | brow_x_a[M] | res[2] | consts[3]
-  const size_t need = static_cast<size_t>(mx) + M + N + 256 + 256 + N + M + 2 + 3;
-  const int arc = ensure_buf(h, &h->d_aux, &h->aux_bytes, need * sizeof(float));
-  if (arc) return arc;
-  if (h->capturing) pin_workspaces(h);
-  float *ones = h->d_aux, *c_row = ones + mx, *c_col = c_row + M, *a_col = c_col + N, *b_row = a_col + 256,
-        *acol_x_b = b_row + 256, *brow_x_a = acol_x_b + N, *res = brow_x_a + M;
-  fill_kernel<<<(mx + 255) / 256, 256, 0, stream>>>(ones, 1.0f, mx);
-  FT_CUDA(h, cudaGetLastError());
-  FT_CUBLAS(h, cublasSetStream(h->cublas, stream));
-  FT_CUBLAS(h, cublasSetMathMode(h->cublas, math_mode ? CUBLAS_TF32_TENSOR_OP_MATH : CUBLAS_DEFAULT_MATH));
-  const float one = 1.0f, zero = 0.0f, neg1 = -1.0f;
-  for (int k0 = 0; k0 < K; k0 += 256) {
-    const int kc = (K - k0) < 256 ? (K - k0) : 256;
-    const float beta_eff = (k0 == 0) ? beta : 1.0f;
-    const float *Ac = dA + static_cast<size_t>(k0) * M;
-    const float *Bc = dB + static_cast<size_t>(k0) * N;
-    FT_CUBLAS(h, cublasSetPointerMode(h->cublas, CUBLAS_POINTER_MODE_HOST));
-    // product chunk (baseline_ft_sgemm.cuh:6)
-    FT_CUBLAS(h, cublasSgemm(h->cublas, CUBLAS_OP_N, CUBLAS_OP_T, M, N, kc, &alpha, Ac, M, Bc, N, &beta_eff, dC, M));
-    if (host_sync) FT_CUDA(h, cudaStreamSynchronize(stream));
-    // row / column sums of all of C (:9,:12) -- the re-read of C the fused kernel removes
-    FT_CUBLAS(h, cublasSgemv(h->cublas, CUBLAS_OP_N, M, N, &one, dC, M, ones, 1, &zero, c_row, 1));
-    FT_CUBLAS(h, cublasSgemv(h->cublas, CUBLAS_OP_T, M, N, &one, dC, M, ones, 1, &zero, c_col, 1));
-    // encode: e^T A_chunk (:15) and B_chunk^T e (:18)
-    FT_CUBLAS(h, cublasSgemv(h->cublas, CUBLAS_OP_T, M, kc, &one, Ac, M, ones, 1, &zero, a_col, 1));
-    FT_CUBLAS(h, cublasSgemv(h->cublas, CUBLAS_OP_T, N, kc, &one, Bc, N, ones, 1, &zero, b_row, 1));
-    if (host_sync) FT_CUDA(h, cudaStreamSynchronize(stream));
-    // checksum products (:21,:24); accumulated over chunks so that, for alpha = 1 and beta = 0, the residual of
-    // the last chunk is the residual of the whole product
-    const float *acc_beta = (k0 == 0) ? &zero : &one;
-    FT_CUBLAS(h, cublasSgemv(h->cublas, CUBLAS_OP_N, N, kc, &one, Bc, N, a_col, 1, acc_beta, acol_x_b, 1));
-    FT_CUBLAS(h, cublasSgemv(h->cublas, CUBLAS_OP_N, M, kc, &one, Ac, M, b_row, 1, acc_beta, brow_x_a, 1));
-    if (host_sync) FT_CUDA(h, cudaStreamSynchronize(stream));
-    // residual + reduce (:27-31); dot results land in device memory
-    FT_CUBLAS(h, cublasSaxpy(h->cublas, N, &neg1, acol_x_b, 1, c_col, 1));
-    FT_CUBLAS(h, cublasSetPointerMode(h->cublas, CUBLAS_POINTER_MODE_DEVICE));
-    FT_CUBLAS(h, cublasSdot(h->cublas, N, c_col, 1, ones, 1, res));
-    if (host_sync) FT_CUDA(h, cudaStreamSynchronize(stream));
-    FT_CUBLAS(h, cublasSetPointerMode(h->cublas, CUBLAS_POINTER_MODE_HOST));
-    FT_CUBLAS(h, cublasSaxpy(h->cublas, M, &neg1, brow_x_a, 1, c_row, 1));
-    FT_CUBLAS(h, cublasSetPointerMode(h->cublas, CUBLAS_POINTER_MODE_DEVICE));
-    FT_CUBLAS(h, cublasSdot(h->cublas, M, c_row, 1, ones, 1, res + 1));
-  }
-  FT_CUBLAS(h, cublasSetPointerMode(h->cublas, CUBLAS_POINTER_MODE_HOST));
-  if (residual_out)
-    FT_CUDA(h, cudaMemcpyAsync(residual_out, res, 2 * sizeof(float), cudaMemcpyDeviceToDevice, stream));
-  h->last_stream = stream;
-  return FTSGEMM_OK;
+  bool cap = false;
+  const int crc = is_capturing(h, static_cast<cudaStream_t>(o.stream), &cap);
+  if (crc) return crc;
+  h->capturing = cap;
+  return run_baseline(h, M, N, K, dA, dB, dC, alpha, beta, math_mode, o, residual_out);
 }
 
 int ftsgemm_verify(ftsgemm_handle_t h, const float *d_ref, const float *d_x, int M, int N, long long *first_bad,

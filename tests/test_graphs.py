@@ -247,24 +247,47 @@ def test_replay_options(torch, ft, case):
 
 
 # ------------------------------------------------------------------ first calls inside the capture, workspaces growing
-def test_first_call_in_capture_and_workspace_growth(torch, ft):
-    """a handle that has never seen the shape: its workspaces and plan are allocated and uploaded during the capture; a
-    later, much larger eager call grows the workspaces, which must not free what the graph uses."""
+def _capture_then_grow(torch, ft, kid, kid_big=None, knobs={}, warm_up=False, **opt):
+    """a handle that has never seen the shape (warm_up: has run it once, eagerly): the captured call's workspaces and plan are
+    allocated and uploaded during the capture; a later, much larger eager call (kernel kid_big) grows the workspaces, which
+    must not free what the graph uses -- each replay gives C as an eager call on a fresh handle"""
+    kid_big = kid if kid_big is None else kid_big
     dev = ft.FtSgemm()
     try:
+        _knobs(ft, knobs)
         small = _Gemm(torch, 640, 512, 384).fill(1)
-        g = _capture(torch, lambda: small.run(dev, 40, 1.0, -1.5))
+        if warm_up:
+            small.run(dev, kid, **opt)
+            torch.cuda.synchronize()
+        g = _capture(torch, lambda: small.run(dev, kid, 1.0, -1.5, **opt))
         big = _Gemm(torch, 2048, 2048, 1536).fill(2)
-        want_big, _ = big.reference(ft, 40)
-        assert torch.equal(big.run(dev, 40).cpu(), want_big)
+        want_big, _ = big.reference(ft, kid_big, **opt)
+        assert torch.equal(big.run(dev, kid_big, **opt).cpu(), want_big)
         for r in range(2):
             small.fill(60 + r)
-            want, _ = small.reference(ft, 40, 1.0, -1.5)
+            want, _ = small.reference(ft, kid, 1.0, -1.5, **opt)
             _replay(torch, g)
             assert torch.equal(small.dC.cpu(), want), r
         assert dev.stats()["detected"] == 0
     finally:
+        _knobs(ft, {k: -1 for k in knobs})
         dev.close()
+
+
+def test_first_call_in_capture_and_workspace_growth(torch, ft):
+    """the K-major copies, the expected checksums and the work plan"""
+    _capture_then_grow(torch, ft, 40)
+
+
+# each path owns a workspace of the handle that the larger call grows: the 3xTF32 lo parts, the split-K tiles, the wave
+# counters (8 units: many waves), the trace (66 units captured, 132 eager), the pre-pass checksum operand and the baseline's
+# vectors (cuBLAS loads its kernels on a first, eager call)
+@pytest.mark.parametrize("args", [dict(kid=40, precision=1), dict(kid=40, knobs={"splitk": 3}),
+                                  dict(kid=40, knobs={"wave_sync": 1, "grid": 8}), dict(kid=31, kid_big=16, knobs={"trace": 1}),
+                                  dict(kid=40, knobs={"enc_front": 0}), dict(kid=10, warm_up=True, baseline_host_sync=False)],
+                         ids=["lo", "sk", "wave_cnt", "trace", "chk", "aux"])
+def test_workspace_growth_after_capture(torch, ft, args):
+    _capture_then_grow(torch, ft, **args)
 
 
 # ------------------------------------------------------------------ several calls in one graph, make_graphed_callables
