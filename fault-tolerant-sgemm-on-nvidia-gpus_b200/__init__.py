@@ -610,9 +610,9 @@ class FtSgemm:
                 d["kind"] = r[7] >> 24
                 items.append(d)
             if items:
-                items[0]["enc_end"] = buf[(u * 64 + 63) * 8]  # helper warps finished their share of the in-kernel encode
-                items[0]["enc_start"] = buf[(u * 64 + 63) * 8 + 1]
-                items[0]["enc_worker0"] = (buf[(u * 64 + 63) * 8 + 2], buf[(u * 64 + 63) * 8 + 3], buf[(u * 64 + 63) * 8 + 5])
+                # the unit's front phase: (start after griddepcontrol.wait, last warp added to front_done) per CTA
+                f = buf[(u * 64 + 63) * 8:(u * 64 + 63) * 8 + 8]
+                items[0]["front"] = [(f[2 * r], f[2 * r + 1]) for r in range(4) if f[2 * r]]
             out.append(items)
         return out
 

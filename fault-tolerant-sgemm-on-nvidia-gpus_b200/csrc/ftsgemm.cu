@@ -825,7 +825,7 @@ int bind_plan(ftsgemm_handle_t h, const Variant &v, KernelParams &p, const PlanI
     if (fresh) h->trace_units = units;
     FT_CUDA(h, cudaMemsetAsync(h->d_trace.ptr, 0, bytes, stream));
     p.trace = bind<unsigned long long>(h, h->d_trace);
-    p.trace_cap = cap;
+    p.trace_cap = cap - 1;  // (the last row of a unit: its front phase)
   }
   return FTSGEMM_OK;
 }
@@ -1264,7 +1264,7 @@ int ftsgemm_create(ftsgemm_handle_t *out) {
     delete h;
     return FTSGEMM_ERR_CUBLAS;
   }
-  const LaunchSeq seq0 = {1ull, 0u, 0};  // epoch 1: above the 0 of fresh flag regions
+  const LaunchSeq seq0 = {1ull, 0u, 0, 0};  // epoch 1: above the 0 of fresh flag regions
   if (cudaMalloc(&h->d_stats, sizeof(DeviceStats)) != cudaSuccess ||
       cudaMemset(h->d_stats, 0, sizeof(DeviceStats)) != cudaSuccess ||
       cudaMalloc(&h->d_verify, 4 * sizeof(double)) != cudaSuccess ||

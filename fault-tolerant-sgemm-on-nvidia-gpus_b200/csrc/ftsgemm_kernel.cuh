@@ -77,11 +77,13 @@ struct DeviceStats {
 //               for it.  It is 64-bit and only grows, so a stale flag never equals a live epoch (2^64 launches do not wrap).
 //   exit_count  CTAs of the running launch that have finished
 //   front_done  warps of the running launch that have finished their front-phase share
-// The last CTA to finish resets exit_count and front_done and advances epoch (ftsgemm_tc_kernel's exit).
+//   front_next  front-phase items claimed so far by the warps of the running launch (front_phase)
+// The last CTA to finish resets exit_count, front_done and front_next and advances epoch (ftsgemm_tc_kernel's exit).
 struct LaunchSeq {
   unsigned long long epoch;
   unsigned int exit_count;
   int front_done;
+  int front_next;
 };
 using SeqFlag = unsigned long long;  // a checksum or cut-tile flag: the epoch of the launch that last raised it
 
@@ -168,9 +170,10 @@ struct KernelParams {
   int peer_world, peer_rank;
   double peer_seq;
   // debug timeline (ftsgemm_debug_trace): per unit and item 8 x u64 = %globaltimer ns at {producer start, producer end,
-  // MMA start, MMA issue end, epilogue start (accumulator complete), after check/fold, epilogue end}, tile | kind << 24
+  // MMA start, MMA issue end, epilogue start (accumulator complete), after check/fold, epilogue end}, tile | kind << 24;
+  // then one row of front-phase times per unit (trace_front)
   unsigned long long *trace;
-  int trace_cap;        // items recorded per unit
+  int trace_cap;        // items recorded per unit (rows per unit: trace_cap + 1)
   // Strided batch (ftsgemm_run_batched; read by the BATCH instantiations only): `batch` independent products, entry i on
   // A + i*stride_a, B + i*stride_b, C + i*stride_c (caller's buffers, element strides).  The workspace the kernel owns holds
   // one dense block per entry: the K-major copies (rows * ldk), the checksum operand (n_chk_cols * enc_ld), the expected
@@ -181,7 +184,14 @@ struct KernelParams {
 
 __device__ __forceinline__ unsigned long long globaltimer_ns() { return ptx::globaltimer(); }
 __device__ __forceinline__ void trace_put(const KernelParams &p, int unit, int item, int slot, unsigned long long v) {
-  if (p.trace != nullptr && item < p.trace_cap) p.trace[(static_cast<size_t>(unit) * p.trace_cap + item) * 8 + slot] = v;
+  if (p.trace != nullptr && item < p.trace_cap) p.trace[(static_cast<size_t>(unit) * (p.trace_cap + 1) + item) * 8 + slot] = v;
+}
+// the front phase of CTA rank r of a unit, in the row after the unit's items: slot 2r = start (after griddepcontrol.wait),
+// slot 2r + 1 = the last of its warps to add itself to front_done (latest = atomic max over the warps)
+__device__ __forceinline__ void trace_front(const KernelParams &p, int unit, int slot, unsigned long long v, bool latest = false) {
+  unsigned long long *dst = p.trace + (static_cast<size_t>(unit) * (p.trace_cap + 1) + p.trace_cap) * 8 + slot;
+  if (latest) atomicMax(dst, v);
+  else *dst = v;
 }
 
 #ifndef FTSGEMM_MAX_STAGES
@@ -205,7 +215,7 @@ struct TileCfg {
   static constexpr int kRingBytes = kStages * kStageBytes > kAccBytes ? kStages * kStageBytes : (kAccBytes + 1023) / 1024 * 1024;
   static constexpr int kSmemBytes = kRingBytes + 1024 + kBarBytes;
   static_assert(kRingBytes <= kMaxSmem, "shared memory");
-  static_assert(kRingBytes >= kThreads / 32 * 32 * 33 * 4, "front-phase transpose scratch");
+  static_assert(kRingBytes >= kThreads / 32 * 64 * kBK * 4, "front-phase transpose scratch (kTrScratch per warp)");
 };
 
 __device__ __forceinline__ float u2f(uint32_t u) { return __uint_as_float(u); }
@@ -1035,11 +1045,14 @@ __device__ __forceinline__ float4 ld_b16(const float4 *p) {
   return v;
 }
 
+// k-rows of one encode_b_warp item
+template <int BN, int KRQ>
+__host__ __device__ constexpr int enc_k_rows() { return BN >= 256 ? KRQ : 2 * KRQ; }
 template <int BN, int KRQ, bool STREAM = false>
 __device__ __forceinline__ void encode_b_warp(const float *__restrict__ B, int N, int K, int ldb, float *__restrict__ chk,
                                               int chk_ld, int rounding, int tiles_n, int gw, int nw, int lane) {
   constexpr int J = BN >= 128 ? BN / 128 : 0;   // float4 loads per lane and k-row
-  constexpr int KR = (J == 2) ? KRQ : 2 * KRQ;  // k-rows per item: 2 * KRQ float4 (J = 2, 1) in flight per lane
+  constexpr int KR = enc_k_rows<BN, KRQ>();     // k-rows per item: 2 * KRQ float4 (J = 2, 1) in flight per lane
   constexpr int NV = 2 * KR;
   if (J > 0 && N == tiles_n * BN && ldb == N) {
     // Linear path (every column block full, rows contiguous): B is one flat array of (k, t) segments of BN floats, k-major;
@@ -1223,73 +1236,179 @@ __device__ __forceinline__ void encode_bk_warp(const float *__restrict__ B, int 
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// Front phase: one warp transposes 32 x 32 blocks of a column-major rows x K operand (element (r, k) at src[r + k*ld])
-// into the K-major copy dst[r * ldk + k], through a 32 x 33 shared-memory tile (conflict-free both ways); blocks
-// rows-fastest so that warps running side by side read neighbouring segments of the same k rows.
+// Front phase transposer: an MN-major rows x K operand (element (r, k) at src[r + k*ld]) into its K-major copy
+// dst[r * ldk + k], 64 rows x 32 k (8 KiB) at a time, staged through the warp's share of the ring (free until the producers
+// start):
+//   tr_stage  512 cp.async of 16 bytes (16 per lane, all in flight at once, no registers held): lane l copies the 4-row
+//             chunk c = l & 15 of k-row 2i + (l >> 4); one instruction reads 256 contiguous bytes of two k-rows
+//   tr_block  lane = (k quad kq = l & 7, row quad rq = (l >> 3) + 4j): four 16-byte shared loads give a 4 x 4 block ...
+//   tr_store  ... written as four 16-byte global stores along k: one instruction writes four 128-byte K-major rows
+// Shared layout: k-row kk at kk * 256 bytes, its 16 chunks XOR-swizzled by tr_swz(kk) so that both the cp.async writes (8
+// lanes: one k-row, 8 chunks) and the transposing reads (8 lanes: kk = 4kq + u, one chunk) hit 8 distinct 16-byte bank
+// groups.  rows % 4 == 0, ld % 4 == 0 and 16-byte aligned bases (check_tc_args) make every chunk whole or absent, so
+// ragged M / N / K need no scalar path: a chunk past K is zero-filled and lands in the copy's padding [K, ldk).
 // ------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void transpose_block(const float *__restrict__ src, int rows, int K, int ld, float *__restrict__ dst,
-                                                int ldk, int r0, int k0, int lane, float *tile) {
-  const int r = r0 + lane;
-#pragma unroll 8
-  for (int j = 0; j < 32; ++j) {
-    const int k = k0 + j;
-    tile[j * 33 + lane] = (r < rows && k < K) ? __ldg(src + static_cast<size_t>(k) * ld + r) : 0.0f;
+constexpr int kTrRows = 64;                     // rows of one staged block (x kBK k)
+constexpr int kTrScratch = kTrRows * kBK * 4;   // bytes of warp scratch
+__device__ __forceinline__ uint32_t tr_swz(int kk) { return static_cast<uint32_t>(((kk >> 2) ^ ((kk & 3) << 1)) & 7); }
+
+__device__ __forceinline__ void tr_stage(const float *__restrict__ src, int rows, int K, int ld, int r0, int k0, int lane,
+                                         uint32_t scratch) {
+  const int c = lane & 15;
+  const bool chunk_ok = r0 + 4 * c < rows;
+#pragma unroll
+  for (int i = 0; i < kBK / 2; ++i) {
+    const int kk = 2 * i + (lane >> 4);
+    const bool ok = chunk_ok && k0 + kk < K;
+    const float *g = ok ? src + static_cast<size_t>(k0 + kk) * ld + r0 + 4 * c : src;
+    ptx::cp_async_16(scratch + kk * 256 + ((c ^ tr_swz(kk)) << 4), g, ok ? 16u : 0u);
   }
-  __syncwarp();
-  const int k = k0 + lane;
-#pragma unroll 8
-  for (int i = 0; i < 32; ++i)
-    if (r0 + i < rows && k < K) dst[static_cast<size_t>(r0 + i) * ldk + k] = tile[lane * 33 + i];
+  ptx::cp_async_wait_all();
   __syncwarp();
 }
-__device__ __forceinline__ void transpose_warp(const float *__restrict__ src, int rows, int K, int ld, float *__restrict__ dst,
-                                               int ldk, int gw, int nw, int lane, float *tile) {
-  const int rb = (rows + 31) / 32, kb = (K + 31) / 32;
-  const long long total = static_cast<long long>(rb) * kb;
-  for (long long t = gw; t < total; t += nw)
-    transpose_block(src, rows, K, ld, dst, ldk, static_cast<int>(t % rb) * 32, static_cast<int>(t / rb) * 32, lane, tile);
+// x[u] = rows 4rq .. 4rq + 3 of k-row 4kq + u
+__device__ __forceinline__ void tr_block(uint32_t scratch, int lane, int j, float4 (&x)[4]) {
+  const int kq = lane & 7, rq = (lane >> 3) + 4 * j;
+#pragma unroll
+  for (int u = 0; u < 4; ++u) x[u] = ptx::ld_shared_f4(scratch + (4 * kq + u) * 256 + ((rq ^ tr_swz(4 * kq + u)) << 4));
+}
+__device__ __forceinline__ void tr_store(float *__restrict__ dst, int rows, int K, int ldk, int r0, int k0, int lane, int j,
+                                         const float4 (&x)[4]) {
+  const int k = k0 + 4 * (lane & 7), r = r0 + 4 * ((lane >> 3) + 4 * j);
+  if (r < rows && k < K) {  // (k + 3 may reach past K: still inside the row stride ldk)
+    float4 *d = reinterpret_cast<float4 *>(dst + static_cast<size_t>(r) * ldk + k);
+    const size_t s = static_cast<size_t>(ldk) / 4;
+    d[0] = make_float4(x[0].x, x[1].x, x[2].x, x[3].x);
+    d[s] = make_float4(x[0].y, x[1].y, x[2].y, x[3].y);
+    d[2 * s] = make_float4(x[0].z, x[1].z, x[2].z, x[3].z);
+    d[3 * s] = make_float4(x[0].w, x[1].w, x[2].w, x[3].w);
+  }
+}
+__device__ __forceinline__ void transpose_item(const float *__restrict__ src, int rows, int K, int ld, float *__restrict__ dst,
+                                               int ldk, int r0, int k0, int lane, uint32_t scratch) {
+  tr_stage(src, rows, K, ld, r0, k0, lane, scratch);
+#pragma unroll
+  for (int j = 0; j < kTrRows / 16; ++j) {
+    float4 x[4];
+    tr_block(scratch, lane, j, x);
+    tr_store(dst, rows, K, ldk, r0, k0, lane, j, x);
+  }
+  __syncwarp();  // every lane's scratch reads are done before the next item's copies overwrite it
 }
 
-// The front phase when at least one operand is K-major: transpose only the MN-major one, encode B in its own layout.  Out of
-// line, so that the GEMM kernel's register allocation sees the reference layout's front phase only (inlined, this branch
-// raised the spills of the 256-wide fault-tolerant instantiations; out of line, the plain instantiations stopped spilling).
-// (front_phase_batched with batch = 1 does the same work, but calling it here moved the spills of the fault-tolerant
-// 128 x 128 kernel from 664 / 448 to 668 / 452 bytes of stores / loads)
-template <int BN, bool FT>
-__device__ __noinline__ void front_phase_kmajor(const float *A, const float *B, int M, int N, int K, int lda, int ldb,
-                                                int a_kmajor, int b_kmajor, float *At, float *Bt, int ldk, int enc_front,
-                                                float *enc_out, int enc_ld, int tiles_n, int gw, int nw, int lane, float *tile) {
-  if (!a_kmajor) transpose_warp(A, M, K, lda, At, ldk, gw, nw, lane, tile);
-  if (!b_kmajor) transpose_warp(B, N, K, ldb, Bt, ldk, gw, nw, lane, tile);
-  if (FT && enc_front) {
-    if (b_kmajor) encode_bk_warp<BN>(B, N, K, ldb, enc_out, enc_ld, 0, tiles_n, gw, nw, lane);
-    else encode_b_warp<BN, 8>(B, N, K, ldb, enc_out, enc_ld, 0, tiles_n, gw, nw, lane);
+// One item of an MN-major B that is transposed and encoded in the same pass: the BN rows of N-tile t x 32 k, staged in
+// BN / 64 blocks; B is read once instead of twice.  The checksum operand is bit for bit encode_b_warp's, because the sums
+// are grouped as there (only where encode_b_warp uses that grouping: encode_fused): encode_b_warp's lane L sums, per k, the
+// row quads L and L + 32 (J = BN / 128 of them, in that order) in FP32 from 0, and the 32 lanes are added in FP64 in
+// butterfly order (lane bit 4 first, then 3, 2, 1, 0).  Here the quad Q = 16 * block + rq lands in "lane" L = Q % 32 at
+// position jj = Q / 32: L bit 4 = block & 1 and bits 3..2 = j are kept in registers (ae, aw: per k of the lane's k quad),
+// bits 1..0 = lane bits 4..3 are two shuffles.  Lane group rg = lane / 8 then stores row rg of the tile's four checksum rows
+// (e hi, e lo, w hi, w lo) for the lane's four k.
+template <int BN>
+__device__ __noinline__ void transpose_encode_item(const float *__restrict__ src, int N, int K, int ld, float *__restrict__ dst,
+                                                      int ldk, float *__restrict__ enc, int enc_ld, int t, int k0, int lane,
+                                                      uint32_t scratch) {
+  static_assert(BN == 128 || BN == 256, "full-block grouping of encode_b_warp");
+  float ae[2][4][4], aw[2][4][4];  // [L bit 4][j][u]
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+#pragma unroll
+      for (int u = 0; u < 4; ++u) ae[h][j][u] = aw[h][j][u] = 0.0f;
+#pragma unroll 1
+  for (int jj = 0; jj < BN / 128; ++jj)  // (the position of a quad in its "lane": the FP32 sums run in this order)
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int blk = 2 * jj + h;
+    const int r0 = t * BN + blk * kTrRows;
+    tr_stage(src, N, K, ld, r0, k0, lane, scratch);
+#pragma unroll
+    for (int j = 0; j < kTrRows / 16; ++j) {
+      float4 x[4];
+      tr_block(scratch, lane, j, x);
+      tr_store(dst, N, K, ldk, r0, k0, lane, j, x);
+      const float wj = static_cast<float>(4 * (16 * blk + (lane >> 3) + 4 * j) + 1);
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const float b0 = tf32_bits(x[u].x, 0), b1 = tf32_bits(x[u].y, 0), b2 = tf32_bits(x[u].z, 0), b3 = tf32_bits(x[u].w, 0);
+        ae[h][j][u] += (b0 + b1) + (b2 + b3);
+        aw[h][j][u] += (b0 * wj + b1 * (wj + 1.0f)) + (b2 * (wj + 2.0f) + b3 * (wj + 3.0f));
+      }
+    }
+    __syncwarp();
   }
+  float o[4];
+  const int rg = lane >> 3;
+#pragma unroll
+  for (int u = 0; u < 4; ++u) {
+    double e[4], w[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {  // L bit 4
+      e[j] = static_cast<double>(ae[0][j][u]) + static_cast<double>(ae[1][j][u]);
+      w[j] = static_cast<double>(aw[0][j][u]) + static_cast<double>(aw[1][j][u]);
+    }
+    double es = (e[0] + e[2]) + (e[1] + e[3]), ws = (w[0] + w[2]) + (w[1] + w[3]);  // L bits 3, 2
+    es += __shfl_xor_sync(0xffffffffu, es, 16);  // L bit 1
+    ws += __shfl_xor_sync(0xffffffffu, ws, 16);
+    es += __shfl_xor_sync(0xffffffffu, es, 8);   // L bit 0
+    ws += __shfl_xor_sync(0xffffffffu, ws, 8);
+    float h, l;
+    split2_tf32(rg < 2 ? es : ws, h, l);
+    o[u] = (rg & 1) ? l : h;
+  }
+  const int k = k0 + 4 * (lane & 7);
+  if (k < K) *reinterpret_cast<float4 *>(enc + static_cast<size_t>(t * kChkPerTile + rg) * enc_ld + k) = make_float4(o[0], o[1], o[2], o[3]);
+}
+// Whether encode_b_warp<BN, 8> sums every (N-tile, k) of this B in its full-block grouping, so that transpose_encode_item
+// reproduces it: 128- or 256-wide tiles, no partial N-tile, and no k-item that straddles K (its strided path only).
+template <int BN>
+__device__ __forceinline__ bool encode_fused(int N, int K, int ldb) {
+  return (BN == 128 || BN == 256) && N % BN == 0 && (ldb == N || K % enc_k_rows<BN, 8>() == 0);
 }
 
-// The front phase of a strided batch: the transposes grid-stride over (entry, 32 x 32 block) -- entry i of an MN-major
-// operand at src + i*stride into its dense K-major copy dst + i*rows*ldk -- and the encode runs entry by entry, entry i's
-// checksum operand at enc_out + i*n_chk_cols*enc_ld.  Out of line, like front_phase_kmajor.
-__device__ __forceinline__ void transpose_warp_batched(const float *__restrict__ src, int rows, int K, int ld, long long stride, int batch,
-                                                       float *__restrict__ dst, int ldk, int gw, int nw, int lane, float *tile) {
-  const int rb = (rows + 31) / 32, kb = (K + 31) / 32;
-  const long long per = static_cast<long long>(rb) * kb, total = per * batch;
-  for (long long t = gw; t < total; t += nw) {
-    const long long e = t / per, te = t - e * per;
-    transpose_block(src + e * stride, rows, K, ld, dst + e * static_cast<long long>(rows) * ldk, ldk, static_cast<int>(te % rb) * 32,
-                    static_cast<int>(te / rb) * 32, lane, tile);
-  }
-}
+// The front phase of every layout and batch size, out of line: the GEMM kernel's register allocation is sensitive to what
+// is inlined beside its main loop (DESIGN.md section 2).  The items of both MN-major operands form one list -- B's first,
+// then A's; per operand, entry, k block, row block (fastest, so that warps running side by side read neighbouring segments
+// of the same k-rows) -- and every warp claims the next item from the launch's counter (*claim, LaunchSeq::front_next)
+// until the list is done, so that warps that run slower (placement, HBM contention) take fewer items and the grid-wide
+// release does not wait on a tail.  An item is 64 rows x 32 k, or with the fused encode a whole N-tile of B x 32 k.  Entry
+// e of an operand is read at src + e*stride and written to its dense copy dst + e*rows*ldk, its checksum operand at
+// enc_out + e*n_chk_cols*enc_ld.  Where the encode cannot be fused it runs afterwards, entry by entry.
 // (scalars by value: a reference to the parameter block would force a local copy of all of it)
 template <int BN, bool FT>
-__device__ __noinline__ void front_phase_batched(const float *A, const float *B, int M, int N, int K, int lda, int ldb, int a_kmajor,
-                                                 int b_kmajor, long long stride_a, long long stride_b, int batch, float *At, float *Bt,
-                                                 int ldk, int enc_front, float *enc_out, int enc_ld, int n_chk_cols, int tiles_n, int gw,
-                                                 int nw, int lane, float *tile) {
-  if (!a_kmajor) transpose_warp_batched(A, M, K, lda, stride_a, batch, At, ldk, gw, nw, lane, tile);
-  if (!b_kmajor) transpose_warp_batched(B, N, K, ldb, stride_b, batch, Bt, ldk, gw, nw, lane, tile);
-  if (FT && enc_front) {
-    const long long enc_stride = static_cast<long long>(n_chk_cols) * enc_ld;
+__device__ __noinline__ void front_phase(const float *A, const float *B, int M, int N, int K, int lda, int ldb, int a_kmajor,
+                                         int b_kmajor, long long stride_a, long long stride_b, int batch, float *At, float *Bt,
+                                         int ldk, int enc_front, float *enc_out, int enc_ld, int n_chk_cols, int tiles_n, int gw,
+                                         int nw, int lane, uint32_t scratch, int *claim) {
+  const bool fuse = FT && enc_front && !b_kmajor && encode_fused<BN>(N, K, ldb);
+  const int kb = (K + kBK - 1) / kBK;
+  const int rb_a = (M + kTrRows - 1) / kTrRows, rb_b = fuse ? tiles_n : (N + kTrRows - 1) / kTrRows;
+  const long long per_a = a_kmajor ? 0 : static_cast<long long>(rb_a) * kb, per_b = b_kmajor ? 0 : static_cast<long long>(rb_b) * kb;
+  const long long items_b = per_b * batch, total = items_b + per_a * batch;
+  const long long enc_stride = static_cast<long long>(n_chk_cols) * enc_ld;
+  // Item gw first, then nw + the claimed count: a warp claims its next item as it starts on the current one, so the
+  // claim's latency hides behind the item, and no warp waits for a claim (or all warps for one counter) at the start.
+  // Every count is claimed once; the warp that draws nw + count >= total is done.
+  int next = 0;
+  for (long long t = gw; t < total; t = nw + static_cast<long long>(__shfl_sync(0xffffffffu, next, 0))) {
+    if (lane == 0) next = atomicAdd(claim, 1);
+    const bool is_b = t < items_b;
+    const long long te = is_b ? t : t - items_b, per = is_b ? per_b : per_a;
+    const long long e = te / per, ti = te - e * per;
+    const int rb = is_b ? rb_b : rb_a;
+    const int kblk = static_cast<int>(ti / rb), rblk = static_cast<int>(ti - static_cast<long long>(kblk) * rb);
+    if (is_b && fuse) {
+      if constexpr (FT && (BN == 128 || BN == 256))
+        transpose_encode_item<BN>(B + e * stride_b, N, K, ldb, Bt + e * static_cast<long long>(N) * ldk, ldk, enc_out + e * enc_stride,
+                                  enc_ld, rblk, kblk * kBK, lane, scratch);
+    } else {
+      const int rows = is_b ? N : M;
+      transpose_item((is_b ? B : A) + e * (is_b ? stride_b : stride_a), rows, K, is_b ? ldb : lda,
+                     (is_b ? Bt : At) + e * static_cast<long long>(rows) * ldk, ldk, rblk * kTrRows, kblk * kBK, lane, scratch);
+    }
+  }
+  if (FT && enc_front && !fuse) {
     for (int e = 0; e < batch; ++e) {
       const float *Be = B + e * stride_b;
       float *out = enc_out + e * enc_stride;
@@ -1368,27 +1487,20 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if constexpr (CG == 2) ptx::cluster_sync();
   else __syncthreads();
   if (p.pdl_wait) ptx::pdl_wait();  // everything before this line touched no global memory
+  if (p.trace != nullptr && threadIdx.x == 0) trace_front(p, unit, 2 * cta_rank, globaltimer_ns());
 
   {
     // front phase: transposes of the MN-major operands (+ the encode of B); the ring is free scratch until the producer starts
     const int gw = static_cast<int>(blockIdx.x) * (kThreads / 32) + warp, nw = static_cast<int>(gridDim.x) * (kThreads / 32);
-    float *tile = smem_f + warp * 32 * 33;
-    if constexpr (BATCH) {
-      front_phase_batched<BN, FT>(p.A, p.B, p.M, p.N, p.K, p.lda, p.ldb, p.a_kmajor, p.b_kmajor, p.stride_a, p.stride_b, p.batch, p.At,
-                                  p.Bt, p.ldk, p.enc_front, p.enc_out, p.enc_ld, p.n_chk_cols, p.tiles_n, gw, nw, lane, tile);
-    } else if ((p.a_kmajor | p.b_kmajor) == 0) {  // the reference layout
-      transpose_warp(p.A, p.M, p.K, p.lda, p.At, p.ldk, gw, nw, lane, tile);
-      transpose_warp(p.B, p.N, p.K, p.ldb, p.Bt, p.ldk, gw, nw, lane, tile);
-      if (FT && p.enc_front) encode_b_warp<BN, 8>(p.B, p.N, p.K, p.ldb, p.enc_out, p.enc_ld, 0, p.tiles_n, gw, nw, lane);
-    } else {
-      front_phase_kmajor<BN, FT>(p.A, p.B, p.M, p.N, p.K, p.lda, p.ldb, p.a_kmajor, p.b_kmajor, p.At, p.Bt, p.ldk, p.enc_front,
-                                 p.enc_out, p.enc_ld, p.tiles_n, gw, nw, lane, tile);
-    }
+    front_phase<BN, FT>(p.A, p.B, p.M, p.N, p.K, p.lda, p.ldb, p.a_kmajor, p.b_kmajor, BATCH ? p.stride_a : 0, BATCH ? p.stride_b : 0, BATCH ? p.batch : 1, p.At, p.Bt,
+                        p.ldk, p.enc_front, p.enc_out, p.enc_ld, p.n_chk_cols, p.tiles_n, gw, nw, lane, smem_base + warp * kTrScratch,
+                        &p.seq->front_next);
     ptx::fence_proxy_async();  // this warp's shared-memory scratch accesses before the TMA writes into the ring
     __syncwarp();              // the warp's stores are ordered before lane 0's release (cumulativity)
     if (lane == 0) {
       ptx::fence_acq_rel_gpu();
       atomicAdd(&p.seq->front_done, 1);
+      if (p.trace != nullptr) trace_front(p, unit, 2 * cta_rank + 1, globaltimer_ns(), true);
     }
   }
   if (warp == 0) {
@@ -1725,6 +1837,7 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
       p.seq->front_done = 0;
+      p.seq->front_next = 0;
       p.seq->exit_count = 0u;
       const SeqFlag next = live_epoch(p) + 1ull;
       asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(&p.seq->epoch), "l"(next) : "memory");

@@ -199,6 +199,19 @@ __device__ __forceinline__ float ld_shared_f1(uint32_t addr) {
   asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
   return v;
 }
+// (volatile + memory clobber: ordered after the cp.async wait that filled the scratch it reads)
+__device__ __forceinline__ float4 ld_shared_f4(uint32_t addr) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
+  return v;
+}
+
+// ----------------------------------------------------------------------------- cp.async (global -> shared, no registers)
+// 16 bytes; src_bytes < 16 zero-fills the rest (0: nothing is read, the address is not dereferenced)
+__device__ __forceinline__ void cp_async_16(uint32_t dst, const void *src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------- accumulator tile in shared memory
 // After its main loop a tile's FP32 accumulator (registers of the two consumer warpgroups) is written to shared memory as
