@@ -37,6 +37,11 @@ LAYOUT_MN_MAJOR, LAYOUT_K_MAJOR = 0, 1
 # bias of run_bias (include/ftsgemm.h): ROW adds bias[m] to row m of C (length M), COL adds bias[n] to column n (length N)
 BIAS_NONE, BIAS_ROW, BIAS_COL = 0, 1, 2
 
+# activation of run_act (include/ftsgemm.h): C = act(z) with z the run_bias value; RELU is torch.relu, GELU torch's exact
+# (erf) gelu.  ACTIVATIONS maps the names matmul and linear take.
+ACT_NONE, ACT_RELU, ACT_GELU = 0, 1, 2
+ACTIVATIONS = {None: ACT_NONE, "relu": ACT_RELU, "gelu": ACT_GELU}
+
 
 class FtsgemmError(RuntimeError):
     def __init__(self, code: int, msg: str):
@@ -92,7 +97,7 @@ EXPORTED_SYMBOLS = [
     "ftsgemm_default_opts", "ftsgemm_kernel_table", "ftsgemm_kernel_lookup", "ftsgemm_run", "ftsgemm_run_ex", "ftsgemm_run_bias", "ftsgemm_get_stats",
     "ftsgemm_run_host", "ftsgemm_baseline", "ftsgemm_verify", "ftsgemm_debug_set", "ftsgemm_debug_schedule",
     "ftsgemm_verify_bad_count", "ftsgemm_debug_trace", "ftsgemm_stats_device", "ftsgemm_select_kernel", "ftsgemm_launch_count", "ftsgemm_peer_export", "ftsgemm_peer_connect",
-    "ftsgemm_peer_verdict", "ftsgemm_run_batched", "ftsgemm_debug_schedule_batched",
+    "ftsgemm_peer_verdict", "ftsgemm_run_batched", "ftsgemm_debug_schedule_batched", "ftsgemm_run_act",
 ]
 
 _lib = None
@@ -127,6 +132,8 @@ def lib():
         L.ftsgemm_run.argtypes = [vp, ip, ip, ip, ip, vp, vp, vp, fp, fp, C.POINTER(Opts)]
         L.ftsgemm_run_ex.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, vp, ip, ip, vp, ip, fp, fp, C.POINTER(Opts)]
         L.ftsgemm_run_bias.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, vp, ip, ip, vp, ip, fp, fp, vp, ip, C.POINTER(Opts)]
+        L.ftsgemm_run_act.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, vp, ip, ip, vp, ip, fp, fp, vp, ip, ip, vp,
+                                      C.POINTER(Opts)]
         ll = C.c_longlong
         L.ftsgemm_run_batched.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, ll, vp, ip, ip, ll, vp, ip, ll, ip, fp, fp, vp, ip,
                                           C.POINTER(Opts)]
@@ -422,6 +429,17 @@ class FtSgemm:
                                                  _ptr(dC), ldc, alpha, beta, _ptr(bias) if bias is not None else None, bias_mode,
                                                  C.byref(opts) if opts is not None else None))
 
+    def run_act(self, kernel_id: int, M: int, N: int, K: int, dA, layout_a: int, lda: int, dB, layout_b: int, ldb: int, dC,
+                ldc: int, alpha: float = 1.0, beta: float = 0.0, bias=None, bias_mode: int = BIAS_NONE,
+                activation: int = ACT_NONE, dZ=None, opts: Opts | None = None) -> None:
+        """C = act(z) with z = (alpha * A * B^T + beta * C) + bias, bit for bit what run_bias stores; z also into dZ (C's
+        geometry: M x N column-major, ldc) when given.  ACT_RELU / ACT_GELU are applied in the store pass; ABFT verifies z,
+        not the activation's own arithmetic (include/ftsgemm.h: ftsgemm_run_act)."""
+        self._run_checked(lib().ftsgemm_run_act(self._h, kernel_id, M, N, K, _ptr(dA), layout_a, lda, _ptr(dB), layout_b, ldb,
+                                                _ptr(dC), ldc, alpha, beta, _ptr(bias) if bias is not None else None, bias_mode,
+                                                activation, _ptr(dZ) if dZ is not None else None,
+                                                C.byref(opts) if opts is not None else None))
+
     def run_batched(self, kernel_id: int, M: int, N: int, K: int, dA, layout_a: int, lda: int, stride_a: int, dB, layout_b: int,
                     ldb: int, stride_b: int, dC, ldc: int, stride_c: int, batch: int, alpha: float = 1.0, beta: float = 0.0,
                     bias=None, bias_mode: int = BIAS_NONE, opts: Opts | None = None) -> None:
@@ -487,8 +505,8 @@ class FtSgemm:
             out.copy_(dst)
         return out
 
-    def matmul(self, a, b, out=None, *, bias=None, kernel_id: int = ID_ABFT_AUTO, alpha: float = 1.0, beta: float = 0.0,
-               opts: Opts | None = None):
+    def matmul(self, a, b, out=None, *, bias=None, activation=None, preact=None, kernel_id: int = ID_ABFT_AUTO,
+               alpha: float = 1.0, beta: float = 0.0, opts: Opts | None = None):
         """out = alpha * (a @ b) + beta * out + bias for 2-D float32 CUDA tensors a: (M, K), b: (K, N) and an optional 1-D
         float32 bias of length N (one value per column of out, added in the fused store pass); returns out.
 
@@ -503,7 +521,11 @@ class FtSgemm:
         N (after the mapping) that is not a multiple of 4 raises FtsgemmError(-2) for the tensor-core ids, as run does.
         Runs on the current torch stream unless opts.stream says otherwise.  No autograd: linear() is the differentiable
         F.linear.  This is bmm on a batch of one entry (a run_batched call with batch = 1, which is run_bias).  Capturable in a
-        CUDA graph (see the class docstring)."""
+        CUDA graph (see the class docstring).
+
+        activation = "relu" | "gelu" stores act(z) with z the value above, in the same store pass (one run_act call), and z
+        into preact when given.  preact must have out's shape and strides, and out and preact must both be writable in place
+        (else ValueError: there is no copy path for them); a, b and the bias are copied as above when needed."""
         import torch
         for name, t in (("a", a), ("b", b)):
             if t.dim() != 2 or t.dtype != torch.float32 or not t.is_cuda:
@@ -520,11 +542,33 @@ class FtSgemm:
             raise ValueError(f"bias must be a float32 ({N},) tensor on {a.device}")
         if K != K2:
             raise ValueError(f"inner dimensions differ: {tuple(a.shape)} @ {tuple(b.shape)}")
-        self.bmm(a.unsqueeze(0), b.unsqueeze(0), out.unsqueeze(0), bias=bias, kernel_id=kernel_id, alpha=alpha, beta=beta,
-                 opts=opts)
+        if activation is None and preact is None:
+            self.bmm(a.unsqueeze(0), b.unsqueeze(0), out.unsqueeze(0), bias=bias, kernel_id=kernel_id, alpha=alpha, beta=beta,
+                     opts=opts)
+            return out
+        if activation not in ("relu", "gelu"):
+            raise ValueError(f"activation must be None, 'relu' or 'gelu' (preact needs one), not {activation!r}")
+        if preact is not None and (preact.shape != out.shape or preact.stride() != out.stride() or
+                                   preact.dtype != torch.float32 or preact.device != a.device):
+            raise ValueError("preact must be a float32 tensor with out's shape and strides on out's device")
+        plan = matmul_plan((M, K), a.stride(), (K, N), b.stride(), out.stride(), a.data_ptr(), b.data_ptr(), out.data_ptr(),
+                           bias.stride(0) if bias is not None else None, bias.data_ptr() if bias is not None else 0)
+        if plan["copy_out"]:
+            raise ValueError("out (and so preact) must be writable in place with an activation: unit stride, 16-byte aligned")
+        if plan["copy_bias"]:
+            bias = torch.empty(N, device=a.device, dtype=torch.float32).copy_(bias)
+        if plan["copy_a"]:
+            a = torch.empty(M, _pad4(K), device=a.device, dtype=torch.float32)[:, :K].copy_(a)
+        if plan["copy_b"]:
+            b = torch.empty(N, _pad4(K), device=a.device, dtype=torch.float32)[:, :K].copy_(b.t()).t()
+        if opts is None:
+            opts = make_opts(stream=torch.cuda.current_stream(a.device).cuda_stream)
+        kA, kB = (b, a) if plan["swap"] else (a, b)
+        self.run_act(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], kB, plan["layout_b"],
+                     plan["ldb"], out, plan["ldc"], alpha, beta, bias, plan["bias_mode"], ACTIVATIONS[activation], preact, opts)
         return out
 
-    def linear(self, x, weight, bias=None, *, kernel_id: int = ID_ABFT_AUTO, opts: Opts | None = None):
+    def linear(self, x, weight, bias=None, *, activation=None, kernel_id: int = ID_ABFT_AUTO, opts: Opts | None = None):
         """F.linear(x, weight, bias) = x @ weight.T + bias under ABFT protection, differentiable: x (..., K), weight (N, K),
         bias (N,) or None, all float32 CUDA tensors; returns (..., N).
 
@@ -534,7 +578,12 @@ class FtSgemm:
         grad_y.sum(0) in torch.  Faults injected through opts land in the forward product only; faults detected in any of
         the three products are counted in stats().  The forward runs on the current torch stream unless opts.stream names
         one; the backward runs on the stream autograd runs it on.  Forward and backward can be captured in a CUDA graph, also
-        through torch.cuda.make_graphed_callables (see the class docstring)."""
+        through torch.cuda.make_graphed_callables (see the class docstring).
+
+        activation = "relu" | "gelu" gives F.relu / F.gelu(F.linear(...)) from the same single matmul, the activation fused
+        into its store pass.  The pre-activation value is written only where the backward needs it: for GELU, when grad mode
+        is on and an input requires grad (ReLU's backward reads y > 0).  Backward: grad_z = threshold_backward(grad_y, y, 0)
+        or gelu_backward(grad_y, z) in torch, then the three gradients as above from grad_z."""
         import torch
         if x.dtype != torch.float32 or not x.is_cuda or x.dim() < 1:
             raise TypeError("x must be a float32 CUDA tensor with at least one dimension")
@@ -546,7 +595,13 @@ class FtSgemm:
         fwd = Opts.from_buffer_copy(opts) if opts is not None else make_opts()
         if not fwd.stream:
             fwd.stream = torch.cuda.current_stream(x.device).cuda_stream
-        y = _linear_fn().apply(x2, weight, bias, self, kernel_id, fwd)
+        if activation is None:
+            y = _linear_fn().apply(x2, weight, bias, self, kernel_id, fwd)
+        else:
+            if activation not in ("relu", "gelu"):
+                raise ValueError(f"activation must be None, 'relu' or 'gelu', not {activation!r}")
+            grad = torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x, weight, bias))
+            y = _linear_act_fn().apply(x2, weight, bias, self, kernel_id, fwd, activation, grad)
         return y.view(lp["out_shape"])
 
     def run_host(self, kernel_id: int, M: int, N: int, K: int, hA, hB, hC, alpha: float = 1.0, beta: float = 0.0,
@@ -658,6 +713,51 @@ def _linear_fn():
 
         _LINEAR_FN = LinearFn
     return _LINEAR_FN
+
+
+_LINEAR_ACT_FN = None
+
+
+def _linear_act_fn():
+    """The torch.autograd.Function behind FtSgemm.linear(activation=...): one run_act forward, the activation's backward in
+    torch, then the products of _linear_fn's backward."""
+    global _LINEAR_ACT_FN
+    if _LINEAR_ACT_FN is None:
+        import torch
+
+        class LinearActFn(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, x2, weight, bias, dev, kernel_id, opts, activation, grad):
+                # (grad: grad mode was on and an input requires grad -- forward itself runs with grad mode off)
+                z = None
+                if grad and activation == "gelu":
+                    z = torch.empty(x2.shape[0], weight.shape[0], device=x2.device, dtype=torch.float32)
+                y = dev.matmul(x2, weight.t(), bias=bias, activation=activation, preact=z, kernel_id=kernel_id, opts=opts)
+                ctx.save_for_backward(x2, weight, y if activation == "relu" else z)
+                ctx.dev, ctx.kernel_id, ctx.opts, ctx.activation = dev, kernel_id, opts, activation
+                return y
+
+            @staticmethod
+            def backward(ctx, gy):
+                x2, weight, saved = ctx.saved_tensors
+                if ctx.activation == "relu":
+                    gz = torch.ops.aten.threshold_backward(gy, saved, 0)
+                else:
+                    gz = torch.ops.aten.gelu_backward(gy, saved)
+                bwd = Opts.from_buffer_copy(ctx.opts)
+                bwd.inject_mode, bwd.n_faults = 0, 0
+                bwd.stream = torch.cuda.current_stream(gy.device).cuda_stream
+                gx = gw = gb = None
+                if ctx.needs_input_grad[0]:
+                    gx = ctx.dev.matmul(gz, weight, kernel_id=ctx.kernel_id, opts=bwd)
+                if ctx.needs_input_grad[1]:
+                    gw = ctx.dev.matmul(gz.t(), x2, kernel_id=ctx.kernel_id, opts=bwd)
+                if ctx.needs_input_grad[2]:
+                    gb = gz.sum(0)
+                return gx, gw, gb, None, None, None, None, None
+
+        _LINEAR_ACT_FN = LinearActFn
+    return _LINEAR_ACT_FN
 
 
 def run_cli(args, timeout=None) -> subprocess.CompletedProcess:

@@ -29,6 +29,7 @@ namespace {
 
 using namespace ftsgemm;
 static_assert(kBiasNone == FTSGEMM_BIAS_NONE && kBiasRow == FTSGEMM_BIAS_ROW && kBiasCol == FTSGEMM_BIAS_COL, "bias modes");
+static_assert(kActNone == FTSGEMM_ACT_NONE && kActRelu == FTSGEMM_ACT_RELU && kActGelu == FTSGEMM_ACT_GELU, "activations");
 
 // ------------------------------------------------------------------------------------------- variant table
 struct Variant {
@@ -308,12 +309,12 @@ int query_max_units(ftsgemm_handle_t h, int *out) {
   return FTSGEMM_OK;
 }
 
-template <int BN, bool FT, int CG, bool PROT, bool SEED, bool BIAS, bool BATCH>
+template <int BN, bool FT, int CG, bool PROT, bool SEED, bool BIAS, bool BATCH, bool ACT = false>
 int launch_tc(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
               const KernelParams &p, int units, cudaStream_t stream) {
   // p.pdl_wait: the launch may overlap the tail of its predecessor in the stream (KernelParams::pdl_wait)
   using Cfg = TileCfg<BN, FT, CG>;
-  auto kern = ftsgemm_tc_kernel<BN, FT, CG, PROT, SEED, BIAS, BATCH>;
+  auto kern = ftsgemm_tc_kernel<BN, FT, CG, PROT, SEED, BIAS, BATCH, ACT>;
   int resident = 0;
   const int qrc = query_max_units<BN, FT, CG, PROT>(h, &resident);
   if (qrc) return qrc;
@@ -367,9 +368,18 @@ int with_flag(bool b, F &&f) {
 
 // The kernel instantiation of a launch: SEED for a plan with cut tiles, BIAS for a bias (KernelParams::bias,
 // ftsgemm_tc_kernel), BATCH for a batch of more than one entry, PROT (fault-tolerant kernels only) for opts.protect_epilogue.
+// An activation (a single product; the bias mode is then a run-time field) selects the ACT kernels instead of BIAS / BATCH.
 template <int BN, int CG>
 int launch_variant(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
                    const KernelParams &p, int units, cudaStream_t stream, bool ft, bool prot) {
+  if (p.act != kActNone) {
+    if (p.batch > 1) return FTSGEMM_ERR_UNSUPPORTED;
+    return with_flag(p.sk_tiles > 0, [&](auto seed) {
+      if (!ft) return launch_tc<BN, false, CG, false, seed, false, false, true>(h, tmA, tmB, tmC, p, units, stream);
+      if (prot) return launch_tc<BN, true, CG, true, seed, false, false, true>(h, tmA, tmB, tmC, p, units, stream);
+      return launch_tc<BN, true, CG, false, seed, false, false, true>(h, tmA, tmB, tmC, p, units, stream);
+    });
+  }
   return with_flag(p.sk_tiles > 0, [&](auto seed) {
     return with_flag(p.bias_mode != kBiasNone, [&](auto bias) {
       return with_flag(p.batch > 1, [&](auto batch) {
@@ -551,6 +561,12 @@ struct BatchArg {
   long long sa, sb, sc;
 };
 const BatchArg kSingle = {1, 0, 0, 0};
+// The activation of ftsgemm_run_act: its kind and the caller's Z (null: not written).  kNoAct everywhere else.
+struct ActArg {
+  int kind;
+  float *z;
+};
+const ActArg kNoAct = {kActNone, nullptr};
 
 // Shapes and operands the wgmma kernels can run (also checked before the 3xTF32 split kernels read the operands with
 // 16-byte loads).
@@ -570,7 +586,7 @@ int check_tc_args(const Variant &v, int M, int N, int K, const Operand &A, const
 // The kernel parameters that follow from the call's arguments and options (the tile grid and work plan come later).
 KernelParams make_params(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B,
                          float *dC, int ldc, float alpha, float beta, const float *bias, int bias_mode,
-                         const ftsgemm_opts &o, const BatchArg &batch_arg) {
+                         const ftsgemm_opts &o, const BatchArg &batch_arg, const ActArg &act) {
   const bool ft = v.info.fault_tolerant != 0;
   // (one entry runs the kernels without BATCH, on 2-D tensor maps; its strides are ignored)
   const BatchArg bt = batch_arg.count > 1 ? batch_arg : kSingle;
@@ -580,6 +596,7 @@ KernelParams make_params(ftsgemm_handle_t h, const Variant &v, int M, int N, int
   p.C = dC; p.ldc = ldc;
   p.alpha = alpha; p.beta = beta;
   p.bias = bias; p.bias_mode = bias_mode;
+  p.act = act.kind; p.z = act.z;
   p.batch = bt.count;
   p.stride_a = bt.sa;
   p.stride_b = bt.sb;
@@ -834,10 +851,10 @@ int bind_plan(ftsgemm_handle_t h, const Variant &v, KernelParams &p, const PlanI
 // work plan, per-plan workspaces, launch.
 int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC, int ldc,
            float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o, cudaStream_t stream,
-           const BatchArg &bt = kSingle) {
+           const BatchArg &bt = kSingle, const ActArg &act = kNoAct) {
   int rc = check_tc_args(v, M, N, K, A, B, dC, bt.count);
   if (rc) return rc;
-  KernelParams p = make_params(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, bt);
+  KernelParams p = make_params(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, bt, act);
   CUtensorMap tmA, tmB, tmC;
   PlanInput pin;
   if ((rc = bind_operands(h, v, p, &tmA, &tmB)) || (rc = plan_on_device(h, v, p, &pin))) return rc;
@@ -1026,7 +1043,7 @@ int run_baseline(ftsgemm_handle_t h, int M, int N, int K, const float *dA, const
 // complete fault-tolerant GEMM with its own checksum vectors, so ABFT covers the whole 3-pass product.
 int run_3xtf32(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC,
                int ldc, float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o,
-               cudaStream_t stream, const BatchArg &bt) {
+               cudaStream_t stream, const BatchArg &bt, const ActArg &act) {
   // (before the split kernels read the operands with 16-byte loads)
   int rc = check_tc_args(v, M, N, K, A, B, dC, bt.count);
   if (rc) return rc;
@@ -1070,25 +1087,26 @@ int run_3xtf32(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const 
   o3.precision = 0;
   ftsgemm_opts o_quiet = o3;  // injected faults belong to the main product only
   o_quiet.inject_mode = 0;
-  // (the bias goes to the last pass only: added once, after the final alpha*acc + C)
+  // (the bias and the activation go to the last pass only: applied once, after the final alpha*acc + C)
   const BatchArg lo = {bt.count, static_cast<long long>(a_floats), static_cast<long long>(b_floats), bt.sc};
   rc = run_tc(h, v, M, N, K, Alo, Bs, dC, ldc, alpha, beta, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo);
   if (!rc) rc = run_tc(h, v, M, N, K, As, Blo, dC, ldc, alpha, 1.0f, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo);
-  if (!rc) rc = run_tc(h, v, M, N, K, A, B, dC, ldc, alpha, 1.0f, bias, bias_mode, o3, stream, bt);
+  if (!rc) rc = run_tc(h, v, M, N, K, A, B, dC, ldc, alpha, 1.0f, bias, bias_mode, o3, stream, bt, act);
   return rc;
 }
 
 int run_resolved(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC,
                  int ldc, float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o,
-                 cudaStream_t stream, const BatchArg &bt);
+                 cudaStream_t stream, const BatchArg &bt, const ActArg &act = kNoAct);
 
 // Intra-K checking (ftsgemm_opts::check_segments): S consecutive K-segments, each a complete fault-tolerant GEMM.  A
 // segment of an operand is a pointer offset: k0 * ld for an MN-major operand (k is the slow index), k0 for a K-major one;
 // segment boundaries are multiples of the stage depth (32 k-rows), so the offsets keep 16-byte alignment.  Injected
-// faults (tests) go to the first segment only, the bias to the last one (added once, after the final alpha*acc + C).
+// faults (tests) go to the first segment only, the bias and the activation to the last one (applied once, after the final
+// alpha*acc + C).
 int run_segments(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC,
                  int ldc, float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o,
-                 cudaStream_t stream, const BatchArg &bt) {
+                 cudaStream_t stream, const BatchArg &bt, const ActArg &act) {
   const int num_kb = (K + kBK - 1) / kBK;
   const int S = std::min(o.check_segments, num_kb);
   ftsgemm_opts os = o;
@@ -1104,7 +1122,7 @@ int run_segments(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, cons
     const Operand Bs = {B.p + (B.kmajor ? static_cast<size_t>(k0) : static_cast<size_t>(k0) * B.ld), B.kmajor, B.ld};
     const bool last = sg == S - 1;
     rc = run_resolved(h, v, M, N, k1 - k0, As, Bs, dC, ldc, alpha, sg == 0 ? beta : 1.0f, last ? bias : nullptr,
-                      last ? bias_mode : FTSGEMM_BIAS_NONE, os, stream, bt);
+                      last ? bias_mode : FTSGEMM_BIAS_NONE, os, stream, bt, last ? act : kNoAct);
   }
   return rc;
 }
@@ -1113,14 +1131,14 @@ int run_segments(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, cons
 // loaded and h->capturing set.
 int run_resolved(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC,
                  int ldc, float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o,
-                 cudaStream_t stream, const BatchArg &bt) {
+                 cudaStream_t stream, const BatchArg &bt, const ActArg &act) {
   const bool tc = v.info.engine == 1;
   if (tc && o.check_segments > 1 && v.info.fault_tolerant)
-    return run_segments(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt);
-  if (tc && o.precision == 1) return run_3xtf32(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt);
+    return run_segments(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt, act);
+  if (tc && o.precision == 1) return run_3xtf32(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt, act);
   switch (v.info.engine) {
     case 0: return run_cublas(h, v.info.id == 7, M, N, K, A, B, dC, ldc, alpha, beta, stream, bt);
-    case 1: return run_tc(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt);
+    case 1: return run_tc(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt, act);
     case 2:
       // the non-fused baseline keeps the reference's call sequence, on the reference layout only
       if (A.kmajor || B.kmajor || A.ld != M || B.ld != N || ldc != M) return FTSGEMM_ERR_UNSUPPORTED;
@@ -1343,10 +1361,11 @@ int ftsgemm_run_bias(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, con
                              bias_mode, opts);
 }
 
-int ftsgemm_run_batched(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
-                        long long stride_a, const float *dB, int layout_b, int ldb, long long stride_b, float *dC, int ldc,
-                        long long stride_c, int batch, float alpha, float beta, const float *bias, int bias_mode,
-                        const ftsgemm_opts *opts) {
+// ftsgemm_run_batched and ftsgemm_run_act: validation, options, capture state, variant; then run_resolved.
+static int run_call(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
+                    long long stride_a, const float *dB, int layout_b, int ldb, long long stride_b, float *dC, int ldc,
+                    long long stride_c, int batch, float alpha, float beta, const float *bias, int bias_mode, const ActArg &act,
+                    const ftsgemm_opts *opts) {
   if (!h) return FTSGEMM_ERR_NO_DEVICE;
   if (!dA || !dB || !dC || M <= 0 || N <= 0 || K <= 0 || batch < 1) return FTSGEMM_ERR_INVALID_ARG;
   const Variant *v = find_variant(kernel_id);
@@ -1360,6 +1379,7 @@ int ftsgemm_run_batched(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, 
   if (bias_mode == FTSGEMM_BIAS_NONE) bias = nullptr;
   else if (!bias || (reinterpret_cast<uintptr_t>(bias) & 3)) return FTSGEMM_ERR_INVALID_ARG;
   if (bias && v->info.engine != 1) return FTSGEMM_ERR_UNSUPPORTED;  // the bias is fused into the wgmma kernels' store pass only
+  if (act.kind != kActNone && v->info.engine != 1) return FTSGEMM_ERR_UNSUPPORTED;  // so is the activation
   // A batch of one entry is the single product (strides ignored).  Otherwise the wgmma kernels need 16-byte entry strides
   // (TMA global strides, the 16-byte aligned C of the store passes), C entries that do not overlap, and no broadcast entry.
   const BatchArg bt = batch > 1 ? BatchArg{batch, stride_a, stride_b, stride_c} : kSingle;
@@ -1386,7 +1406,25 @@ int ftsgemm_run_batched(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, 
     v = find_variant(select_variant(M, N, v->info.fault_tolerant != 0, bt.count));
     if (!v) return FTSGEMM_ERR_UNSUPPORTED;
   }
-  return run_resolved(h, *v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt);
+  return run_resolved(h, *v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt, act);
+}
+
+int ftsgemm_run_batched(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
+                        long long stride_a, const float *dB, int layout_b, int ldb, long long stride_b, float *dC, int ldc,
+                        long long stride_c, int batch, float alpha, float beta, const float *bias, int bias_mode,
+                        const ftsgemm_opts *opts) {
+  return run_call(h, kernel_id, M, N, K, dA, layout_a, lda, stride_a, dB, layout_b, ldb, stride_b, dC, ldc, stride_c, batch, alpha,
+                  beta, bias, bias_mode, kNoAct, opts);
+}
+
+int ftsgemm_run_act(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
+                    const float *dB, int layout_b, int ldb, float *dC, int ldc, float alpha, float beta, const float *bias,
+                    int bias_mode, int activation, float *dZ, const ftsgemm_opts *opts) {
+  if (!h) return FTSGEMM_ERR_NO_DEVICE;
+  if (activation < FTSGEMM_ACT_NONE || activation > FTSGEMM_ACT_GELU) return FTSGEMM_ERR_INVALID_ARG;
+  if (dZ && (activation == FTSGEMM_ACT_NONE || dZ == dC || (reinterpret_cast<uintptr_t>(dZ) & 3))) return FTSGEMM_ERR_INVALID_ARG;
+  return run_call(h, kernel_id, M, N, K, dA, layout_a, lda, 0, dB, layout_b, ldb, 0, dC, ldc, 0, 1, alpha, beta, bias, bias_mode,
+                  ActArg{activation, dZ}, opts);
 }
 
 int ftsgemm_get_stats(ftsgemm_handle_t h, ftsgemm_stats *out) {

@@ -180,6 +180,11 @@ struct KernelParams {
   // checksums (M * n_chk_cols * chk_slices) and tiles_m * CG * 4 slabs of checksum flags.
   int batch;
   long long stride_a, stride_b, stride_c;
+  // Activation (ftsgemm_run_act; read by the ACT instantiations only, which take bias_mode at run time, NONE included):
+  // the final value z = (alpha*acc + beta*C_old) (+ b) of a data tile is stored as C = act(z), and z itself into z (C's
+  // geometry, ld = ldc) unless it is null.  (Appended: the fields above keep their offsets in the parameter block.)
+  int act;
+  float *z;
 };
 
 __device__ __forceinline__ unsigned long long globaltimer_ns() { return ptx::globaltimer(); }
@@ -380,9 +385,53 @@ __device__ __forceinline__ BiasRef make_bias(const float *p, int mode, int m, bo
   return b;
 }
 
-template <int BN, bool BIAS = false>
+// ACT: the activation of the final value, written as torch's CUDA kernels write it (relu = clamp_min(z, 0), which keeps
+// NaN; gelu with approximate='none', the exact erf form).  The bias of an ACT kernel is a run-time mode: NONE skips the add
+// (-0 + 0 would be +0), so z is bit for bit what the BIAS / plain kernel stores.  z is written to zrow[off] when zrow is
+// set (Z + m: the pre-activation value the GELU backward needs).
+constexpr int kActNone = 0, kActRelu = 1, kActGelu = 2;
+struct ActRef {
+  int kind;
+  float *zrow;  // Z + m, or null
+};
+__device__ __forceinline__ float act_apply(int kind, float z) {
+  if (kind == kActRelu) return isnan(z) ? z : fmaxf(z, 0.0f);
+  return z * 0.5f * (1.0f + erff(z * 0.707106781186547524f));  // (float)M_SQRT1_2
+}
+// z = x (+ b), stored to Z when requested; returns act(z)  (one element: the ragged-N and recompute paths)
+__device__ __forceinline__ float act_value(float x, const BiasRef &bias, int n, const ActRef &act, size_t off) {
+  if (bias.mode != kBiasNone) x = __fadd_rn(x, bias.at(n));
+  if (act.zrow != nullptr) act.zrow[off] = x;
+  return act_apply(act.kind, x);
+}
+// the same for the 32 columns [nb, nb + 32) of one chunk, the warp-uniform branches taken once per chunk, not per element
+__device__ __forceinline__ void act_chunk(uint32_t (&v)[32], const BiasRef &bias, int nb, const ActRef &act, int ldc) {
+  if (bias.mode != kBiasNone) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) v[i] = f2u(__fadd_rn(u2f(v[i]), bias.at(nb + i)));
+  }
+  if (act.zrow != nullptr) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) act.zrow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
+  }
+  if (act.kind == kActRelu) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) v[i] = f2u(act_apply(kActRelu, u2f(v[i])));
+  } else {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) v[i] = f2u(act_apply(kActGelu, u2f(v[i])));
+  }
+}
+template <bool ACT>
+__device__ __forceinline__ ActRef act_of(const KernelParams &p, int m) {
+  if constexpr (ACT) return ActRef{p.act, p.z != nullptr ? p.z + m : nullptr};
+  else return ActRef{kActNone, nullptr};
+}
+
+template <int BN, bool BIAS = false, bool ACT = false>
 __device__ __forceinline__ void store_tile(uint32_t taddr, float *crow, bool row_ok, int n0, int n_limit, int ldc,
-                                           float alpha, float beta, int c_begin = 0, int c_end = BN / 32, BiasRef bias = {}) {
+                                           float alpha, float beta, int c_begin = 0, int c_end = BN / 32, BiasRef bias = {},
+                                           ActRef act = {}) {
   const bool full_n = (n0 + BN <= n_limit);
   if (full_n && beta != 0.0f) {
     // Software pipeline: the old values of chunk c + 1 are fetched while chunk c is stored (a chunk's 32 loads would
@@ -404,6 +453,7 @@ __device__ __forceinline__ void store_tile(uint32_t taddr, float *crow, bool row
           v[i] = f2u(alpha * u2f(v[i]) + beta * old[i]);
           if constexpr (BIAS) v[i] = f2u(__fadd_rn(u2f(v[i]), bias.at(nb + i)));
         }
+        if constexpr (ACT) act_chunk(v, bias, nb, act, ldc);
         if (c + 1 < c_end) {
 #pragma unroll
           for (int i = 0; i < 32; ++i) old[i] = crow[static_cast<size_t>(nb + 32 + i) * ldc];
@@ -421,11 +471,19 @@ __device__ __forceinline__ void store_tile(uint32_t taddr, float *crow, bool row
     const int nb = n0 + c * 32;
     if (!row_ok) continue;
     if (full_n) {
+      if constexpr (ACT) {
 #pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        float x = alpha * u2f(v[i]);
-        if constexpr (BIAS) x = __fadd_rn(x, bias.at(nb + i));
-        crow[static_cast<size_t>(nb + i) * ldc] = x;
+        for (int i = 0; i < 32; ++i) v[i] = f2u(alpha * u2f(v[i]));
+        act_chunk(v, bias, nb, act, ldc);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) crow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
+      } else {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          float x = alpha * u2f(v[i]);
+          if constexpr (BIAS) x = __fadd_rn(x, bias.at(nb + i));
+          crow[static_cast<size_t>(nb + i) * ldc] = x;
+        }
       }
     } else {
 #pragma unroll
@@ -435,6 +493,7 @@ __device__ __forceinline__ void store_tile(uint32_t taddr, float *crow, bool row
           const float o = (beta == 0.0f) ? 0.0f : beta * (*dst);
           float x = alpha * u2f(v[i]) + o;
           if constexpr (BIAS) x = __fadd_rn(x, bias.at(nb + i));
+          if constexpr (ACT) x = act_value(x, bias, nb + i, act, static_cast<size_t>(nb + i) * ldc);
           *dst = x;
         }
       }
@@ -723,10 +782,13 @@ struct StoreVerdict {
   float resid;
   bool bad;
 };
-template <int BN, bool BIAS>
+// ACT: the pass verifies z -- the values it sums are the pre-activation values, with the run-time bias in sum(b) as above
+// -- and then stores act(z) to C and z to Z.  The activation's own arithmetic is elementwise and nonlinear: no linear
+// checksum covers it, so an upset inside it or after it is not detected.
+template <int BN, bool BIAS, bool ACT = false>
 __device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, float *crow, bool row_ok, int n0, int ldc, float alpha,
                                                           float beta, int c_begin, int c_end, float chk_s1, bool chk_s1_valid,
-                                                          int bad_col, uint32_t bad_mask, const BiasRef &bias) {
+                                                          int bad_col, uint32_t bad_mask, const BiasRef &bias, ActRef act = {}) {
   float s1 = 0.0f, s2 = 0.0f, sabs = 0.0f, so0 = 0.0f, so1 = 0.0f, sold0 = 0.0f, sold1 = 0.0f, aold0 = 0.0f, aold1 = 0.0f;
   float sb = 0.0f, ab = 0.0f;  // sum(b), sum|b| of the segment
   const bool rmw = beta != 0.0f;
@@ -770,6 +832,17 @@ __device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, flo
           ab += fabsf(b);
         }
       }
+      if constexpr (ACT) {
+        if (bias.mode != kBiasNone) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) {
+            const float b = bias.at(nb + i);
+            v[i] = f2u(__fadd_rn(u2f(v[i]), b));
+            sb += b;
+            ab += fabsf(b);
+          }
+        }
+      }
       if (bad_col >= c * 32 && bad_col < c * 32 + 32) {
 #pragma unroll
         for (int i = 0; i < 32; ++i)
@@ -780,13 +853,26 @@ __device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, flo
         so0 += u2f(v[i]);
         so1 += u2f(v[i + 1]);
       }
+      if constexpr (ACT) {
+        if (act.zrow != nullptr) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) act.zrow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
+        }
+        if (act.kind == kActRelu) {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) v[i] = f2u(act_apply(kActRelu, u2f(v[i])));
+        } else {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) v[i] = f2u(act_apply(kActGelu, u2f(v[i])));
+        }
+      }
 #pragma unroll
       for (int i = 0; i < 32; ++i) crow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
     }
   }
   float ref = alpha * s1 + beta * (sold0 + sold1);
   float tol = 1.6e-5f * (fabsf(alpha) * sabs + fabsf(beta) * (aold0 + aold1)) + 1e-30f;
-  if constexpr (BIAS) {
+  if constexpr (BIAS || ACT) {  // (ACT without a bias: sb = ab = 0)
     ref += sb;
     tol = 1.6e-5f * (fabsf(alpha) * sabs + fabsf(beta) * (aold0 + aold1) + ab) + 1e-30f;
   }
@@ -806,10 +892,11 @@ __device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, flo
 // kmajor: bit 0 = A is K-major, bit 1 = B is K-major.
 // ------------------------------------------------------------------------------------------------------------
 // (scalars by value: a reference to the __grid_constant__ parameter block would force a local copy of all of it)
-template <int BN, bool BIAS>
+// ACT: the bias mode is read at run time and the row is stored as act(z), with z into Z (when not null).
+template <int BN, bool BIAS, bool ACT = false>
 __device__ __forceinline__ void recompute_row_body(const float *A, const float *B, float *C, int lda, int ldb, int kmajor, int ldc,
                                                    int N, int K, float alpha, float beta, int m, int n0, int lane, const float *bias,
-                                                   int bias_mode) {
+                                                   int bias_mode, int act_kind = kActNone, float *Z = nullptr) {
   constexpr int J = BN / 32;
   float acc[J];
 #pragma unroll
@@ -837,6 +924,11 @@ __device__ __forceinline__ void recompute_row_body(const float *A, const float *
       const float o = (beta == 0.0f) ? 0.0f : beta * (*dst);
       float x = alpha * acc[j] + o;
       if constexpr (BIAS) x = __fadd_rn(x, __ldg(bias + (bias_mode == kBiasRow ? m : n)));
+      if constexpr (ACT) {
+        if (bias_mode != kBiasNone) x = __fadd_rn(x, __ldg(bias + (bias_mode == kBiasRow ? m : n)));
+        if (Z != nullptr) Z[m + static_cast<size_t>(n) * ldc] = x;
+        x = act_apply(act_kind, x);
+      }
       *dst = x;
     }
   }
@@ -854,9 +946,16 @@ __device__ __noinline__ void recompute_row_bias(const float *A, const float *B, 
                                                 int bias_mode) {
   recompute_row_body<BN, true>(A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, m, n0, lane, bias, bias_mode);
 }
-template <int BN, bool BIAS, typename... Args>
-__device__ __forceinline__ void recompute(const float *bias, int bias_mode, Args... args) {
-  if constexpr (BIAS) recompute_row_bias<BN>(args..., bias, bias_mode);
+template <int BN>
+__device__ __noinline__ void recompute_row_act(const float *A, const float *B, float *C, int lda, int ldb, int kmajor, int ldc,
+                                               int N, int K, float alpha, float beta, int m, int n0, int lane, const float *bias,
+                                               int bias_mode, int act_kind, float *Z) {
+  recompute_row_body<BN, false, true>(A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, m, n0, lane, bias, bias_mode, act_kind, Z);
+}
+template <int BN, bool BIAS, bool ACT = false, typename... Args>
+__device__ __forceinline__ void recompute(const float *bias, int bias_mode, int act_kind, float *Z, Args... args) {
+  if constexpr (ACT) recompute_row_act<BN>(args..., bias, bias_mode, act_kind, Z);
+  else if constexpr (BIAS) recompute_row_bias<BN>(args..., bias, bias_mode);
   else recompute_row<BN>(args...);
 }
 
@@ -864,14 +963,16 @@ __device__ __forceinline__ void recompute(const float *bias, int bias_mode, Args
 // common epilogue registers (inlined it pushed the kernel into spills), and a reference to the __grid_constant__ parameter
 // block would force a local copy of all of it.  Row segments that fail are counted and, with beta == 0, recomputed from A
 // and B (with beta != 0 the old values of C are already overwritten: reported as uncorrectable).
-template <int BN, bool BIAS>
+template <int BN, bool BIAS, bool ACT = false>
 __device__ __forceinline__ void protected_store_body(uint32_t taddr, const float *A, const float *B, float *C, int lda, int ldb,
                                                      int kmajor, int ldc, int N, int K, float alpha, float beta, DeviceStats *stats,
                                                      bool can_recompute, int m, int row0, bool row_ok, int n0, int c_begin, int c_end,
                                                      float chk_s1, bool chk_s1_valid, int bad_col, uint32_t bad_mask, int lane,
-                                                     const float *bias, int bias_mode, int row_ofs) {
-  const StoreVerdict sv = store_tile_protected<BN, BIAS>(taddr, C + m, row_ok, n0, ldc, alpha, beta, c_begin, c_end, chk_s1, chk_s1_valid,
-                                                         bad_col, bad_mask, make_bias(bias, bias_mode, m, BIAS && row_ok));
+                                                     const float *bias, int bias_mode, int row_ofs, int act_kind = kActNone,
+                                                     float *Z = nullptr) {
+  const StoreVerdict sv = store_tile_protected<BN, BIAS, ACT>(
+      taddr, C + m, row_ok, n0, ldc, alpha, beta, c_begin, c_end, chk_s1, chk_s1_valid, bad_col, bad_mask,
+      make_bias(bias, bias_mode, m, (BIAS || ACT) && row_ok), ActRef{act_kind, (ACT && Z != nullptr) ? Z + m : nullptr});
   unsigned mask = __ballot_sync(0xffffffffu, sv.bad);
   if (mask == 0u) return;
   const bool can_fix = beta == 0.0f && can_recompute;
@@ -894,10 +995,11 @@ __device__ __forceinline__ void protected_store_body(uint32_t taddr, const float
     const int r = __ffs(mask) - 1;
     mask &= mask - 1u;
     if (c_end - c_begin == BN / 32) {
-      recompute<BN, BIAS>(bias, bias_mode, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r, n0, lane);
+      recompute<BN, BIAS, ACT>(bias, bias_mode, act_kind, Z, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r, n0, lane);
     } else {
       if constexpr (BN >= 64)
-        recompute<BN / 2, BIAS>(bias, bias_mode, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r, n0 + c_begin * 32, lane);
+        recompute<BN / 2, BIAS, ACT>(bias, bias_mode, act_kind, Z, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r,
+                                     n0 + c_begin * 32, lane);
     }
   }
 }
@@ -918,6 +1020,11 @@ template <int BN>
 __device__ __noinline__ void protected_store_pass_bias(FT_PROT_PARAMS, const float *bias, int bias_mode) {
   protected_store_body<BN, true>(FT_PROT_ARGS, bias, bias_mode, 0);
 }
+// (the ACT kernels: the bias mode at run time, the activation and Z; a third entry, so the two above keep their lists)
+template <int BN>
+__device__ __noinline__ void protected_store_pass_act(FT_PROT_PARAMS, const float *bias, int bias_mode, int act_kind, float *Z) {
+  protected_store_body<BN, false, true>(FT_PROT_ARGS, bias, bias_mode, 0, act_kind, Z);
+}
 // strided batch: A, B, C are the entry's, row_ofs = entry * M (events carry stacked rows)
 template <int BN, bool BIAS>
 __device__ __noinline__ void protected_store_pass_batched(FT_PROT_PARAMS, const float *bias, int bias_mode, int row_ofs) {
@@ -925,9 +1032,10 @@ __device__ __noinline__ void protected_store_pass_batched(FT_PROT_PARAMS, const 
 }
 #undef FT_PROT_PARAMS
 #undef FT_PROT_ARGS
-template <int BN, bool BIAS, bool BATCH, typename... Args>
-__device__ __forceinline__ void protected_store(const float *bias, int bias_mode, int row_ofs, Args... args) {
-  if constexpr (BATCH) protected_store_pass_batched<BN, BIAS>(args..., bias, bias_mode, row_ofs);
+template <int BN, bool BIAS, bool BATCH, bool ACT, typename... Args>
+__device__ __forceinline__ void protected_store(const float *bias, int bias_mode, int row_ofs, int act_kind, float *Z, Args... args) {
+  if constexpr (ACT) protected_store_pass_act<BN>(args..., bias, bias_mode, act_kind, Z);
+  else if constexpr (BATCH) protected_store_pass_batched<BN, BIAS>(args..., bias, bias_mode, row_ofs);
   else if constexpr (BIAS) protected_store_pass_bias<BN>(args..., bias, bias_mode);
   else protected_store_pass<BN>(args...);
 }
@@ -1439,10 +1547,14 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t a_desc, 
 // BATCH: the instantiation for strided batches (ftsgemm_run_batched with batch > 1): 3-D tensor maps with the entry as the
 // outer coordinate, and every per-tile address offset by the item's entry.  Without it the entry is the constant 0 and
 // the code is that of the kernel before batching existed.
-template <int BN, bool FT, int CG, bool PROT = false, bool SEED = false, bool BIAS = false, bool BATCH = false>
+// ACT: the instantiation for calls with an activation (ftsgemm_run_act; single products only, never with BIAS or BATCH).
+// The final epilogue of a data tile stores act(z) and, when p.z is set, z; the bias mode, the activation and Z are run-time
+// fields.  Like BIAS, its own binary, so that the other kernels are compiled exactly as without the feature.
+template <int BN, bool FT, int CG, bool PROT = false, bool SEED = false, bool BIAS = false, bool BATCH = false, bool ACT = false>
 __global__ void __launch_bounds__(kThreads, 1)
 ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmChk, const KernelParams p) {
+  static_assert(!(ACT && (BIAS || BATCH)), "the ACT kernels are single products with a run-time bias");
   using Cfg = TileCfg<BN, FT, CG>;
   constexpr int kStages = Cfg::kStages;
   constexpr int kAccRegs = BN / 2;  // per thread of a consumer warpgroup: 64 x BN FP32
@@ -1710,12 +1822,12 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N) {
             uint32_t bad_bits = 0u;
             const int bad_col = stored_value_fault<BN, BATCH>(p, q, lane, m0_cta, n0, kMid, BN / 32, bad_bits, row_ofs);
-            protected_store<BN, BIAS, BATCH>(p.bias, p.bias_mode, row_ofs, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
+            protected_store<BN, BIAS, BATCH, ACT>(p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? p.z : nullptr, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
                                       p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32,
                                       m < p.M && !skip, n0, kMid, BN / 32, s1, stale == 0u, bad_col, bad_bits, lane);
           } else {
-            store_tile<BN, BIAS>(taddr, (BATCH ? Cb : p.C) + m, m < p.M && !skip, n0, p.N, p.ldc, p.alpha, p.beta, kMid, BN / 32,
-                                 make_bias(p.bias, p.bias_mode, m, BIAS && m < p.M && !skip));
+            store_tile<BN, BIAS, ACT>(taddr, (BATCH ? Cb : p.C) + m, m < p.M && !skip, n0, p.N, p.ldc, p.alpha, p.beta, kMid, BN / 32,
+                                      make_bias(p.bias, p.bias_mode, m, (BIAS || ACT) && m < p.M && !skip), act_of<ACT>(p, m));
           }
           ptx::named_bar_sync(4 + q, 64);  // both halves are out of the accumulator
         }
@@ -1773,19 +1885,19 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N) {
           uint32_t bad_bits = 0u;
           const int bad_col = stored_value_fault<BN, BATCH>(p, q, lane, m0_cta, n0, 0, c_mid, bad_bits, row_ofs);
-          protected_store<BN, BIAS, BATCH>(p.bias, p.bias_mode, row_ofs, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
+          protected_store<BN, BIAS, BATCH, ACT>(p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? p.z : nullptr, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
                                     p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32,
                                     m < p.M && !redo, n0, 0, c_mid, own_s1, ((stale_mask >> lane) & 1u) == 0u, bad_col, bad_bits, lane);
         } else {
-          store_tile<BN, BIAS>(taddr, (BATCH ? Cb : p.C) + m, m < p.M && !redo, n0, p.N, p.ldc, p.alpha, p.beta, 0, c_mid,
-                               make_bias(p.bias, p.bias_mode, m, BIAS && m < p.M && !redo));
+          store_tile<BN, BIAS, ACT>(taddr, (BATCH ? Cb : p.C) + m, m < p.M && !redo, n0, p.N, p.ldc, p.alpha, p.beta, 0, c_mid,
+                                    make_bias(p.bias, p.bias_mode, m, (BIAS || ACT) && m < p.M && !redo), act_of<ACT>(p, m));
         }
         if (FT && redo_mask != 0u) {  // rare, warp-uniform: recompute the flagged rows from global memory
           unsigned rm = redo_mask;
           while (rm != 0u) {
             const int r = __ffs(rm) - 1;
             rm &= rm - 1u;
-            recompute<BN, BIAS>(p.bias, p.bias_mode, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K,
+            recompute<BN, BIAS, ACT>(p.bias, p.bias_mode, ACT ? p.act : 0, ACT ? p.z : nullptr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K,
                                 p.alpha, p.beta, m0_cta + q * 32 + r, n0, lane);
           }
         }

@@ -181,7 +181,7 @@ int ftsgemm_create(ftsgemm_handle_t *out);   /* binds to the current CUDA device
                                                  stream at a time (use one handle per concurrently used stream). */
 /* CUDA graphs.  The compute calls may be captured into a CUDA graph (stream capture in any mode, e.g. torch.cuda.graph) and
  * replayed; a replay computes what the same call computes eagerly on the buffers' contents at replay time, bit for bit.
- *  - Captured as they are: ftsgemm_run / _run_ex / _run_bias / _run_batched on the tensor-core ids (with every option:
+ *  - Captured as they are: ftsgemm_run / _run_ex / _run_bias / _run_batched / _run_act on the tensor-core ids (with every option:
  *    3xTF32, check_segments, protect_epilogue, injected faults) and the cuBLAS ids 0 / 7, the encode pre-pass,
  *    and ftsgemm_stats_device.  A first call of a new shape may be
  *    captured: its workspaces and work plan are allocated and uploaded outside the capture.  reuse_b_checksums has no
@@ -287,6 +287,37 @@ int ftsgemm_run_batched(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, 
                         long long stride_a, const float *B, int layout_b, int ldb, long long stride_b, float *C, int ldc,
                         long long stride_c, int batch, float alpha, float beta, const float *bias, int bias_mode,
                         const ftsgemm_opts *opts);
+
+/* ---- activation fused into the store pass  (new work: the reference's epilogue has no activation) --------------------------
+ * The product of ftsgemm_run_bias followed by an elementwise activation, applied where the kernel stores a tile's final value:
+ *   z(m,n) = (alpha * acc(m,n) + beta * C_old(m,n)) + b      bit for bit what ftsgemm_run_bias stores for the same call
+ *   C(m,n) = act(z(m,n))
+ * and, when dZ is not NULL, Z(m,n) = z(m,n): the pre-activation value (what a GELU backward needs), with C's geometry --
+ * M x N, column-major, leading dimension ldc.  Without a bias the add is skipped, not performed with 0.  The activations
+ * are written as torch's CUDA kernels write them:
+ *   FTSGEMM_ACT_RELU   isnan(z) ? z : fmaxf(z, 0)                       (torch.relu, i.e. clamp_min)
+ *   FTSGEMM_ACT_GELU   z * 0.5f * (1 + erff(z * (float)M_SQRT1_2))       (torch's gelu, approximate='none')
+ * GELU depends on the device's erff, so it matches torch's to within a few ulp rather than bit for bit.
+ * FTSGEMM_ACT_NONE with dZ = NULL is ftsgemm_run_bias: the same kernels and the same result.
+ * Single products only: there is no batched form.  Every option applies: with opts.precision = 1 the activation and Z go to
+ * the last of the three passes, with opts.check_segments = S to the last segment, like the bias.
+ * ABFT coverage.  The accumulator check runs before alpha, beta, the bias and the activation and is unchanged: a corrected
+ * element is repaired in the accumulator, so C = act(corrected z).  The protected store pass (opts.protect_epilogue) verifies
+ * z -- the values it sums are the pre-activation ones, with today's tolerance -- and then applies the activation; an upset of
+ * the value about to be stored (fault mode 3) is an upset of z, and with beta == 0 the recomputed row restores C and Z.
+ * NOT covered: the activation's own arithmetic.  It is elementwise and nonlinear, so no linear checksum covers it: an upset
+ * inside erff / fmaxf or after the activation is not detected.
+ * Errors: an activation outside 0..2, dZ with FTSGEMM_ACT_NONE, dZ == dC, or dZ not 4-byte aligned: FTSGEMM_ERR_INVALID_ARG;
+ * an activation with the cuBLAS ids 0 / 7 or the baseline ids 10 / 30: FTSGEMM_ERR_UNSUPPORTED (no unfused fallback).
+ * Every other argument as for ftsgemm_run_bias. */
+enum {
+  FTSGEMM_ACT_NONE = 0,
+  FTSGEMM_ACT_RELU = 1,
+  FTSGEMM_ACT_GELU = 2
+};
+int ftsgemm_run_act(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
+                    const float *dB, int layout_b, int ldb, float *dC, int ldc, float alpha, float beta,
+                    const float *bias, int bias_mode, int activation, float *dZ, const ftsgemm_opts *opts);
 
 /* Counters of all FT launches since the previous call (synchronises the handle's last stream, then resets). */
 int ftsgemm_get_stats(ftsgemm_handle_t h, ftsgemm_stats *out);
