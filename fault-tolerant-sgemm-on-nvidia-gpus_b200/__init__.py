@@ -192,7 +192,9 @@ def make_opts(stream=None, selftest=None, faults=None, tau_abs=0.0, tau_rel=0.0,
               protect_epilogue=False) -> Opts:
     """selftest: None | (value, tile_row, tile_col)  -> the reference's always-on injector (ft_sgemm_huge.cuh:324-327)
     faults: list of dicts {row, col, add=float} or {row, col, xor=int}; with xor, where="epilogue_tmem" | "epilogue_value"
-    places the upset after the accumulator check (ftsgemm_fault.mode 2 / 3)"""
+    places the upset after the accumulator check (ftsgemm_fault.mode 2 / 3)
+    protect_epilogue: False / 0 = unprotected store pass; True / 1 = checked store pass; 2 = every chunk verified before it
+    is written and repaired whatever beta is (include/ftsgemm.h: ftsgemm_opts.protect_epilogue)"""
     o = default_opts()
     o.stream = stream
     if selftest is not None:

@@ -12,6 +12,9 @@ ROOT = HERE.parent
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-ccbin", "/usr/bin/g++"]
+# ptxas compiles the library's ~230 kernels on up to 8 threads: the same machine code as a serial run (SASS identical),
+# in about half the build time; the cap bounds its memory (~1 GB per thread)
+PTXAS_THREADS = ["-Xptxas", f"--split-compile={max(1, min(8, os.cpu_count() or 1))}"]
 
 LIB = HERE / "libftsgemm.so"
 CLI = HERE / "ft_sgemm"
@@ -28,7 +31,7 @@ def build(force: bool = False, verbose: bool = False) -> None:
     lib_src = [CSRC / "ftsgemm.cu"]
     lib_dep = lib_src + sorted(CSRC.glob("*.cuh")) + sorted(CSRC.glob("*.h")) + [ROOT / "include" / "ftsgemm.h"]
     if force or _stale(LIB, lib_dep):
-        cmd = [NVCC, *ARCH, *COMMON, "-shared", "-Xptxas", "-v", *map(str, lib_src), "-o", str(LIB), "-lcublas"]
+        cmd = [NVCC, *ARCH, *COMMON, *PTXAS_THREADS, "-shared", "-Xptxas", "-v", *map(str, lib_src), "-o", str(LIB), "-lcublas"]
         out = subprocess.run(cmd, capture_output=True, text=True)
         (HERE / "build_ptxas.log").write_text(out.stderr)
         if verbose or out.returncode != 0:

@@ -129,7 +129,9 @@ int main(int argc, char **argv) {
   // optional modes of the wgmma engines (not in the reference's argv: environment only)
   if (getenv("FTSGEMM_PRECISION") && !strcmp(getenv("FTSGEMM_PRECISION"), "x3")) opts.precision = 1;  // 3xTF32, FP32-grade
   opts.check_segments = env_int("FTSGEMM_CHECK_SEGMENTS", 0);  // S > 1: intra-K checking, S verified K-segments
-  opts.protect_epilogue = env_int("FTSGEMM_PROTECT_EPILOGUE", 0) ? 1 : 0;  // checked store pass (stats.epilogue_faults)
+  // checked store pass (stats.epilogue_faults): 2 = verify every chunk before it is written, any other non-zero value = 1
+  const int protect = env_int("FTSGEMM_PROTECT_EPILOGUE", 0);
+  opts.protect_epilogue = protect == 2 ? 2 : (protect ? 1 : 0);
 
   if (cpu_verify) {
     Chost.resize(count);

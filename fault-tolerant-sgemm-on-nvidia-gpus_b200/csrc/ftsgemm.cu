@@ -605,6 +605,7 @@ KernelParams make_params(ftsgemm_handle_t h, const Variant &v, int M, int N, int
   p.tau_rel = o.tau_rel > 0 ? o.tau_rel : 1e-5f;  // DESIGN.md section 5
   p.detect_only = o.detect_only;
   p.recompute = o.no_recompute ? 0 : 1;
+  p.protect = o.protect_epilogue;  // (the PROT kernels are selected for any non-zero level)
   p.A = A.p;
   p.B = B.p;
   p.lda = A.ld;
@@ -1336,7 +1337,7 @@ static int load_opts(const ftsgemm_opts *opts, ftsgemm_opts *o) {
   if (opts->struct_size < FTSGEMM_OPTS_V1_SIZE) return FTSGEMM_ERR_INVALID_ARG;
   memcpy(o, opts, opts->struct_size < sizeof(*o) ? opts->struct_size : sizeof(*o));
   o->struct_size = sizeof(*o);
-  if (o->check_segments < 0 || o->check_segments > 4096 || o->precision < 0 || o->precision > 1 || o->inject_mode < 0 || o->inject_mode > 2 || o->protect_epilogue < 0 || o->protect_epilogue > 1 || o->selftest_row < 0 || o->selftest_col < 0 || o->n_faults < 0 ||
+  if (o->check_segments < 0 || o->check_segments > 4096 || o->precision < 0 || o->precision > 1 || o->inject_mode < 0 || o->inject_mode > 2 || o->protect_epilogue < 0 || o->protect_epilogue > 2 || o->selftest_row < 0 || o->selftest_col < 0 || o->n_faults < 0 ||
       o->n_faults > FTSGEMM_MAX_FAULTS)
     return FTSGEMM_ERR_INVALID_ARG;
   return FTSGEMM_OK;

@@ -185,6 +185,9 @@ struct KernelParams {
   // geometry, ld = ldc) unless it is null.  (Appended: the fields above keep their offsets in the parameter block.)
   int act;
   float *z;
+  // opts.protect_epilogue of the call (read by the PROT instantiations only): 1 sums a row segment as it stores it and
+  // judges it at the end; 2 verifies every 32-column chunk before it is written (protected_store_pass_v2)
+  int protect;
 };
 
 __device__ __forceinline__ unsigned long long globaltimer_ns() { return ptx::globaltimer(); }
@@ -1073,6 +1076,212 @@ __device__ __forceinline__ int stored_value_fault(const KernelParams &p, int q, 
 }
 
 // ------------------------------------------------------------------------------------------------------------
+// Repairing protected store pass (opts.protect_epilogue = 2): nothing is written before it is verified, so a failed chunk
+// is recomputed from A, B and the old C it has not overwritten, whatever beta is.  A warp's row segment is the chunks
+// [c_begin, c_end) of one row (lane = row):
+//   pass 1  re-reads every chunk and forms its sum sc_c with the association of abft_chunk_sums; their running sum must
+//           equal, bit for bit, the sum the accumulator check verified (chk_s1), or the accumulator was upset after the
+//           check and every chunk of the segment is recomputed
+//   pass 2  per chunk: re-read it and require its sum to be sc_c bit for bit (an upset between the passes); form the outputs
+//           z = alpha * acc + beta * old (+ b); require sum(z) to lie within the chunk's tolerance of alpha * sc_c +
+//           beta * sum(old) (+ sum(b)) -- the formula of store_tile_protected over 32 columns instead of the segment; only
+//           then store z (to Z) and act(z) (to C, ACT) or z (to C).  A failing chunk is not written.
+// Chunks wholly past N are skipped; the one that straddles N loads, stores and adds a bias only below N (old = b = 0
+// beyond, where the accumulator holds the zero-filled columns, so the sums still agree).  The outputs are formed as
+// store_tile forms them, so a fault-free pass stores its bits.  A row that fails counts once, in epilogue_faults and in
+// recomputed (status 6), however many chunks fail; with no_recompute / detect_only its chunks are stored as computed and
+// it counts as uncorrectable (status 7).  Out of line and shared by every tile width: its code is independent of BN.
+// ------------------------------------------------------------------------------------------------------------
+constexpr int kMaxChunks = 8;  // chunks of one row segment: BN / 32 at BN = 256
+// the mode-3 upsets of one lane: up to two (tile column, xor mask) pairs, column -1 = none
+struct StoreUpsets {
+  int col0, col1;
+  uint32_t mask0, mask1;
+};
+template <int BN, bool BATCH = false>
+__device__ __forceinline__ StoreUpsets stored_value_upsets(const KernelParams &p, int q, int lane, int m0_cta, int n0, int c_begin,
+                                                           int c_end, int row_ofs = 0) {
+  StoreUpsets u{-1, -1, 0u, 0u};
+  if (p.inject_mode == 2)
+    for (int f = 0; f < p.n_faults; ++f) {
+      const int tr = p.faults[f].row - (m0_cta + row_ofs), tc = p.faults[f].col - n0;
+      if (p.faults[f].mode == 3 && tr >= 0 && tr < kBM && (tr >> 5) == q && lane == (tr & 31) && tc >= c_begin * 32 && tc < c_end * 32 &&
+          fault_in_entry<BATCH>(p, m0_cta, tr)) {
+        if (u.col0 < 0) {
+          u.col0 = tc;
+          u.mask0 = p.faults[f].xor_mask;
+        } else {
+          u.col1 = tc;
+          u.mask1 = p.faults[f].xor_mask;
+        }
+      }
+    }
+  return u;
+}
+// sum_i v[i] of one chunk as abft_chunk_sums forms it (two chains), and sum_i |v[i]|
+__device__ __forceinline__ float chunk_sum(const uint32_t (&v)[32], float &sabs) {
+  float a0 = 0.0f, a1 = 0.0f, b0 = 0.0f, b1 = 0.0f;
+#pragma unroll
+  for (int i = 0; i < 32; i += 2) {
+    a0 += u2f(v[i]);
+    a1 += u2f(v[i + 1]);
+    b0 += fabsf(u2f(v[i]));
+    b1 += fabsf(u2f(v[i + 1]));
+  }
+  sabs = b0 + b1;
+  return a0 + a1;
+}
+template <bool BIAS, bool ACT>
+__device__ __noinline__ void protected_store_pass_v2(uint32_t taddr, const float *A, const float *B, float *C, int lda, int ldb,
+                                                     int kmajor, int ldc, int N, int K, float alpha, float beta, DeviceStats *stats,
+                                                     bool can_recompute, int m, int row0, bool row_ok, int n0, bool ragged_n,
+                                                     int c_begin, int c_end, float chk_s1, bool chk_s1_valid, StoreUpsets up,
+                                                     int lane,
+                                                     const float *bias, int bias_mode, int row_ofs, int act_kind, float *Z) {
+  // ---- pass 1: the chunk sums, and their running sum against the check's ----
+  float sc[kMaxChunks];
+  float s1 = 0.0f;
+#pragma unroll
+  for (int k = 0; k < kMaxChunks; ++k) {
+    sc[k] = 0.0f;
+    if (c_begin + k < c_end) {  // (warp-uniform)
+      uint32_t v[32];
+      __syncwarp();
+      ptx::acc_ld_x32(taddr + (c_begin + k) * 32, v);
+      float sabs;
+      sc[k] = chunk_sum(v, sabs);
+      s1 += sc[k];
+    }
+  }
+  const bool reread_differs = row_ok && chk_s1_valid && f2u(s1) != f2u(chk_s1);
+  float ev_resid = reread_differs ? chk_s1 - s1 : 0.0f;
+  // ---- pass 2: verify each chunk, then store it ----
+  const bool has_bias = BIAS || (ACT && bias_mode != kBiasNone);
+  const BiasRef b = make_bias(bias, bias_mode, m, has_bias && row_ok);
+  float *crow = C + m;
+  float *zrow = (ACT && Z != nullptr) ? Z + m : nullptr;
+  const bool rmw = beta != 0.0f;
+  const int c_stop = min(c_end, (N - n0 + 31) / 32);  // chunks wholly past N are skipped
+  uint32_t bad_chunks = reread_differs ? (1u << (c_end - c_begin)) - 1u : 0u;
+  float old[32];
+  auto load_old = [&](int nb) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) old[i] = (nb + i < N) ? crow[static_cast<size_t>(nb + i) * ldc] : 0.0f;
+  };
+  if (row_ok && rmw && c_begin < c_stop) load_old(n0 + c_begin * 32);
+#pragma unroll 1
+  for (int c = c_begin; c < c_stop; ++c) {
+    uint32_t v[32];
+    __syncwarp();
+    ptx::acc_ld_x32(taddr + c * 32, v);
+    float sabs;
+    const float sc_c = chunk_sum(v, sabs);
+    float want = 0.0f;
+#pragma unroll
+    for (int k = 0; k < kMaxChunks; ++k)
+      if (k == c - c_begin) want = sc[k];
+    const int nb = n0 + c * 32;
+    const bool full = nb + 32 <= N;
+    if (!row_ok) continue;
+    float so0 = 0.0f, so1 = 0.0f, sold0 = 0.0f, sold1 = 0.0f, aold0 = 0.0f, aold1 = 0.0f, sb = 0.0f, ab = 0.0f;
+    if (rmw) {
+#pragma unroll
+      for (int i = 0; i < 32; i += 2) {
+        sold0 += old[i];
+        sold1 += old[i + 1];
+        aold0 += fabsf(old[i]);
+        aold1 += fabsf(old[i + 1]);
+      }
+#pragma unroll
+      for (int i = 0; i < 32; ++i) v[i] = f2u(alpha * u2f(v[i]) + beta * old[i]);
+      if (c + 1 < c_stop) load_old(nb + 32);
+    } else if (!ragged_n) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) v[i] = f2u(alpha * u2f(v[i]));
+    } else {
+      // (in a tile ragged in N, store_tile's element loop adds the zero old term: -0 becomes +0)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) v[i] = f2u(alpha * u2f(v[i]) + 0.0f);
+    }
+    if (has_bias) {
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const float bi = (nb + i < N) ? b.at(nb + i) : 0.0f;
+        v[i] = f2u(__fadd_rn(u2f(v[i]), bi));
+        sb += bi;
+        ab += fabsf(bi);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      if (c * 32 + i == up.col0) v[i] ^= up.mask0;
+      if (c * 32 + i == up.col1) v[i] ^= up.mask1;
+    }
+#pragma unroll
+    for (int i = 0; i < 32; i += 2) {
+      so0 += u2f(v[i]);
+      so1 += u2f(v[i + 1]);
+    }
+    const float ref = alpha * sc_c + beta * (sold0 + sold1) + sb;
+    const float tol = 1.6e-5f * (fabsf(alpha) * sabs + fabsf(beta) * (aold0 + aold1) + ab) + 1e-30f;
+    const float resid = (so0 + so1) - ref;
+    // (a non-finite reference -- Inf / NaN already in the old C -- cannot be verified and is not an upset)
+    const bool bad = f2u(sc_c) != f2u(want) || (isfinite(ref) && !(fabsf(resid) <= tol));
+    if (bad && bad_chunks == 0u) ev_resid = resid;
+    if (bad) bad_chunks |= 1u << (c - c_begin);
+    if (((bad_chunks >> (c - c_begin)) & 1u) && can_recompute) continue;  // not written: recomputed below
+    if (ACT) {
+      if (zrow != nullptr) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i)
+          if (full || nb + i < N) zrow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
+      }
+      if (act_kind == kActRelu) {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) v[i] = f2u(act_apply(kActRelu, u2f(v[i])));
+      } else {
+#pragma unroll
+        for (int i = 0; i < 32; ++i) v[i] = f2u(act_apply(kActGelu, u2f(v[i])));
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 32; ++i)
+      if (full || nb + i < N) crow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
+  }
+  // chunks of a segment that failed pass 1 but lie wholly past N hold nothing to repair
+  if (c_stop < c_end) bad_chunks &= (c_stop > c_begin) ? (1u << (c_stop - c_begin)) - 1u : 0u;
+  const bool seg_bad = bad_chunks != 0u;
+  unsigned mask = __ballot_sync(0xffffffffu, seg_bad);
+  if (mask == 0u) return;
+  if (seg_bad && stats) {
+    atomicAdd(&stats->epilogue_faults, 1ull);
+    atomicAdd(can_recompute ? &stats->recomputed : &stats->uncorrectable, 1ull);
+    const int slot = atomicAdd(&stats->n_events, 1);
+    if (slot < kMaxEvents) {
+      DeviceEvent ev;
+      ev.row = m + row_ofs;
+      ev.col = -1;
+      ev.residual = ev_resid;
+      ev.corrected_value = 0.0f;
+      ev.status = can_recompute ? 6 : 7;
+      stats->events[slot] = ev;
+    }
+  }
+  if (!can_recompute) return;
+  while (mask != 0u) {  // rare, warp-uniform: the failed chunks of each row, 32 columns at a time
+    const int r = __ffs(mask) - 1;
+    mask &= mask - 1u;
+    uint32_t chunks = __shfl_sync(0xffffffffu, bad_chunks, r);
+    while (chunks != 0u) {
+      const int k = __ffs(chunks) - 1;
+      chunks &= chunks - 1u;
+      recompute<32, BIAS, ACT>(bias, bias_mode, act_kind, Z, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r,
+                               n0 + (c_begin + k) * 32, lane);
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------
 // Cut tiles (plan.h).  Epilogue warps (lane = row) of a non-final piece park the raw accumulator slab; the consumer
 // warps of the unit that owns the next piece load it into their registers before that piece's first wgmma.
 // ------------------------------------------------------------------------------------------------------------
@@ -1819,7 +2028,13 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             skip = (ptx::ld_acquire_shared_u32(xchg_base(q)) >> lane) & 1u;  // rows the epilogue warp recomputes
             if constexpr (PROT) stale = (ptx::ld_acquire_shared_u32(xchg_base(q) + 4) >> lane) & 1u;  // rows it repaired
           }
-          if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N) {
+          if (PROT && FT && !(p.dbg_flags & 1) && p.protect == 2) {
+            protected_store_pass_v2<BIAS, ACT>(taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1),
+                                               p.ldc, p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m,
+                                               m0_cta + q * 32, m < p.M && !skip, n0, n0 + BN > p.N, kMid, BN / 32, s1, stale == 0u,
+                                               stored_value_upsets<BN, BATCH>(p, q, lane, m0_cta, n0, kMid, BN / 32, row_ofs), lane,
+                                               (BIAS || ACT) ? p.bias : nullptr, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? p.z : nullptr);
+          } else if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N) {
             uint32_t bad_bits = 0u;
             const int bad_col = stored_value_fault<BN, BATCH>(p, q, lane, m0_cta, n0, kMid, BN / 32, bad_bits, row_ofs);
             protected_store<BN, BIAS, BATCH, ACT>(p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? p.z : nullptr, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
@@ -1882,7 +2097,14 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           if (p.inject_mode == 2) inject_after_check<BN, BATCH>(p, taddr, q, lane, m0_cta, n0, row_ofs);
         }
         if (assist_on && FT && !(p.dbg_flags & 1)) ptx::named_bar_sync(4 + q, 64);  // corrections are in place
-        if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N) {
+        if (PROT && FT && !(p.dbg_flags & 1) && p.protect == 2) {
+          protected_store_pass_v2<BIAS, ACT>(taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1),
+                                             p.ldc, p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m,
+                                             m0_cta + q * 32, m < p.M && !redo, n0, n0 + BN > p.N, 0, c_mid, own_s1,
+                                             ((stale_mask >> lane) & 1u) == 0u,
+                                             stored_value_upsets<BN, BATCH>(p, q, lane, m0_cta, n0, 0, c_mid, row_ofs), lane,
+                                             (BIAS || ACT) ? p.bias : nullptr, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? p.z : nullptr);
+        } else if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N) {
           uint32_t bad_bits = 0u;
           const int bad_col = stored_value_fault<BN, BATCH>(p, q, lane, m0_cta, n0, 0, c_mid, bad_bits, row_ofs);
           protected_store<BN, BIAS, BATCH, ACT>(p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? p.z : nullptr, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,

@@ -137,9 +137,18 @@ typedef struct ftsgemm_opts {
                             the sums the check verified) and sums what it stores (must equal alpha * that + beta * sum of the
                             old values within rounding).  A row segment that fails is counted in stats.epilogue_faults
                             and, when beta == 0, recomputed from A and B; with beta != 0 the old values are gone: it is
-                            counted in stats.uncorrectable.  Tiles that are ragged in N are not covered; Inf / NaN already in the old C are
-                            not verifiable and not flagged.  A separate kernel instantiation (the opt-in path costs the
-                            default one no registers); bench.py reports its rate as modes.protect_epilogue_gflops. */
+                            counted in stats.uncorrectable.  Tiles that are ragged in N are not covered.
+                            2: verify before write.  Every 32-column chunk of C (and of Z, ftsgemm_run_act) is stored only
+                            after its values pass the same check, with the tolerance taken over the chunk; a chunk that
+                            fails is not written but recomputed from A, B and the still-intact old C (with the bias and
+                            the activation), WHATEVER beta is -- so also in the beta = 1 passes of 3xTF32 and check_segments.
+                            Tiles ragged in N are covered.  A failed row segment counts once in stats.epilogue_faults and
+                            stats.recomputed (event status 6); only no_recompute / detect_only leave it as computed
+                            (stats.uncorrectable, status 7).  Costs a second read of the accumulator.
+                            Both levels: Inf / NaN already in the old C, and rows whose expected checksum is not finite, are
+                            not verifiable and not flagged; the activation's own arithmetic is not covered.  A separate
+                            kernel instantiation (the opt-in path costs the default one no registers); bench.py reports
+                            level 1's rate as modes.protect_epilogue_gflops.  Values above 2 are FTSGEMM_ERR_INVALID_ARG. */
 } ftsgemm_opts;
 /* sizeof(ftsgemm_opts) of ABI version 1: the smallest struct_size the library accepts (a zero-initialised struct is
  * rejected with FTSGEMM_ERR_INVALID_ARG instead of silently meaning "all defaults on the default stream"). */
@@ -151,7 +160,8 @@ typedef struct ftsgemm_event {
   float residual;        /* expected - actual row checksum */
   float corrected_value; /* accumulator value after correction */
   int status;            /* 1 corrected, 2 detected only (detect_only), 3 uncorrectable, 4 checksum-column fault,
-                            5 row recomputed, 6 epilogue fault (row segment recomputed), 7 epilogue fault left in C (beta != 0) */
+                            5 row recomputed, 6 epilogue fault (row segment, or its failed chunks, recomputed), 7 epilogue
+                            fault left in C (protect_epilogue = 1 with beta != 0; no_recompute / detect_only) */
 } ftsgemm_event;
 
 typedef struct ftsgemm_stats {
