@@ -98,6 +98,7 @@ EXPORTED_SYMBOLS = [
     "ftsgemm_run_host", "ftsgemm_baseline", "ftsgemm_verify", "ftsgemm_debug_set", "ftsgemm_debug_schedule",
     "ftsgemm_verify_bad_count", "ftsgemm_debug_trace", "ftsgemm_stats_device", "ftsgemm_select_kernel", "ftsgemm_launch_count", "ftsgemm_peer_export", "ftsgemm_peer_connect",
     "ftsgemm_peer_verdict", "ftsgemm_run_batched", "ftsgemm_debug_schedule_batched", "ftsgemm_run_act",
+    "ftsgemm_run_batched_act",
 ]
 
 _lib = None
@@ -137,6 +138,8 @@ def lib():
         ll = C.c_longlong
         L.ftsgemm_run_batched.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, ll, vp, ip, ip, ll, vp, ip, ll, ip, fp, fp, vp, ip,
                                           C.POINTER(Opts)]
+        L.ftsgemm_run_batched_act.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, ll, vp, ip, ip, ll, vp, ip, ll, ip, fp, fp, vp, ip,
+                                              ll, ip, vp, C.POINTER(Opts)]
         L.ftsgemm_get_stats.argtypes = [vp, C.POINTER(Stats)]
         L.ftsgemm_run_host.argtypes = [vp, ip, ip, ip, ip, vp, vp, vp, fp, fp, C.POINTER(Opts)]
         L.ftsgemm_stats_device.argtypes = [vp, vp, vp]
@@ -311,13 +314,18 @@ def matmul_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0
 
 
 def bmm_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0, b_ptr: int = 0, out_ptr: int = 0,
-             bias_stride=None, bias_ptr: int = 0) -> dict:
+             bias_stride=None, bias_ptr: int = 0, bias_entry_stride=None) -> dict:
     """run_batched arguments for out = a @ b with a: (Bt, M, K), b: (Bt, K, N), out: (Bt, M, N), from shapes, element strides
     and addresses.  Each matrix is mapped as in matmul_plan (layouts, lds, swap, bias_mode); stride_a / stride_b / stride_c
     are the batch strides of the kernel's A, B and C (b's and a's when swapped).  With more than one entry a tensor is also
     marked for copying when its batch stride is not a positive multiple of 4 floats (an expanded operand has stride 0), and
     out when its entries would overlap; the arguments returned then describe the dense copies bmm makes (a row-major and b
-    column-major with rows padded to a multiple of 4, out contiguous row-major)."""
+    column-major with rows padded to a multiple of 4, out contiguous row-major).
+
+    bias_entry_stride is the entry stride of a (Bt, N) bias, one bias per entry (None: a (N,) bias shared by all entries).
+    stride_bias is the entry stride run_batched_act takes: 0 for a shared bias, an expanded one (entry stride 0) or a single
+    entry.  copy_bias also marks a per-entry bias with a negative entry stride; the copy bmm makes of a per-entry bias is
+    (Bt, N) contiguous (stride_bias = N), of a shared one (N,)."""
     Bt, M, K = a_shape
     Bt2, K2, N = b_shape
     if Bt != Bt2:
@@ -344,6 +352,10 @@ def bmm_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0, b
     mp["batch"] = Bt
     mp["stride_a"], mp["stride_b"] = (sb, sa) if mp["swap"] else (sa, sb)
     mp["stride_c"] = so
+    mp["stride_bias"] = 0
+    if bias_entry_stride is not None and Bt > 1 and bias_entry_stride != 0:
+        mp["copy_bias"] = mp["copy_bias"] or bias_entry_stride < 0
+        mp["stride_bias"] = N if mp["copy_bias"] else bias_entry_stride
     return mp
 
 
@@ -380,8 +392,8 @@ def _ptr(x) -> int:
 class FtSgemm:
     """One handle = one device context (cuBLAS handle, checksum workspace, fault counters).
 
-    CUDA graphs: matmul, bmm and linear (forward and backward) can be captured with torch.cuda.graph (its default global
-    capture mode) or torch.cuda.make_graphed_callables, first calls of a shape included.  A replay reads the tensors the
+    CUDA graphs: matmul, bmm and linear (bmm and linear forward and backward) can be captured with torch.cuda.graph (its
+    default global capture mode) or torch.cuda.make_graphed_callables, first calls of a shape included.  A replay reads the tensors the
     capture used -- copy new inputs into those same static tensors -- and writes C bit for bit as the eager call would; eager
     calls and replays may interleave on one handle in stream order.  stats() synchronises only the stream of the handle's
     last call, so synchronise the replay stream first; inside a capture it raises FtsgemmError(-2), as run_host, verify and
@@ -453,18 +465,46 @@ class FtSgemm:
                                                     _ptr(bias) if bias is not None else None, bias_mode,
                                                     C.byref(opts) if opts is not None else None))
 
-    def bmm(self, a, b, out=None, *, bias=None, kernel_id: int = ID_ABFT_AUTO, alpha: float = 1.0, beta: float = 0.0,
-            opts: Opts | None = None):
-        """out = alpha * (a @ b) + beta * out + bias for 3-D float32 CUDA tensors a: (Bt, M, K), b: (Bt, K, N), out: (Bt, M, N)
-        and an optional bias (N,) shared by all entries -- torch.baddbmm plus a bias -- as ONE run_batched call; returns out.
+    def run_batched_act(self, kernel_id: int, M: int, N: int, K: int, dA, layout_a: int, lda: int, stride_a: int, dB,
+                        layout_b: int, ldb: int, stride_b: int, dC, ldc: int, stride_c: int, batch: int, alpha: float = 1.0,
+                        beta: float = 0.0, bias=None, bias_mode: int = BIAS_NONE, stride_bias: int = 0,
+                        activation: int = ACT_NONE, dZ=None, opts: Opts | None = None) -> None:
+        """`batch` run_act products in one launch: entry i is run_act on dA + i*stride_a, dB + i*stride_b, dC + i*stride_c
+        with the bias bias + i*stride_bias (0: shared by all entries) and z into dZ + i*stride_c when dZ is given
+        (include/ftsgemm.h: ftsgemm_run_batched_act).  Fault and event rows are stacked rows i*M + m."""
+        self._run_checked(lib().ftsgemm_run_batched_act(self._h, kernel_id, M, N, K, _ptr(dA), layout_a, lda, stride_a, _ptr(dB),
+                                                        layout_b, ldb, stride_b, _ptr(dC), ldc, stride_c, batch, alpha, beta,
+                                                        _ptr(bias) if bias is not None else None, bias_mode, stride_bias,
+                                                        activation, _ptr(dZ) if dZ is not None else None,
+                                                        C.byref(opts) if opts is not None else None))
+
+    def bmm(self, a, b, out=None, *, bias=None, activation=None, preact=None, kernel_id: int = ID_ABFT_AUTO,
+            alpha: float = 1.0, beta: float = 0.0, opts: Opts | None = None):
+        """out = act(alpha * (a @ b) + beta * out + bias) for 3-D float32 CUDA tensors a: (Bt, M, K), b: (Bt, K, N), out:
+        (Bt, M, N), an optional bias (N,) shared by all entries or (Bt, N) one per entry, and an optional activation --
+        torch.baddbmm plus a bias and an activation -- as ONE run_batched (run_batched_act) call; returns out.
 
         Every matrix may be row- or column-major with any leading stride that keeps 16-byte rows, and is read in place when
         its batch stride is a multiple of 4 floats: contiguous bmm operands and q @ k.transpose(-1, -2) copy nothing.  An
         expanded operand (batch stride 0), a batch stride that is not a multiple of 4, or a matrix matmul could not read in
         place is copied once (bmm_plan); an out that cannot be written in place is computed in a contiguous buffer and copied
         back.  Fault and event coordinates (opts, stats()) are stacked kernel rows entry * kernel_M + row, transposed against
-        out when the call is swapped (a row-major out: the kernel's rows are out's columns).  No autograd.  Capturable in a
-        CUDA graph (see the class docstring); copies it makes are then graph-pool tensors, refreshed on every replay."""
+        out when the call is swapped (a row-major out: the kernel's rows are out's columns).  Capturable in a CUDA graph (see
+        the class docstring); copies it makes are then graph-pool tensors, refreshed on every replay.
+
+        activation = "relu" | "gelu" stores act(z) with z the value above, in the same store pass, and z into preact when
+        given (preact must have out's shape and strides; out and preact must be writable in place, else ValueError), as
+        matmul does.  A per-entry bias (bmm_plan: stride_bias) or an activation runs run_batched_act; anything else the
+        run_batched call.
+
+        Autograd: with out=None, grad mode on and any of a, b, bias requiring grad, bmm is differentiable.  The forward is
+        the same single call; z is written for GELU only (ReLU's backward reads out > 0).  Backward: grad_z =
+        threshold_backward / gelu_backward in torch (grad_out itself without an activation), grad_a = alpha * grad_z @ b^T and
+        grad_b = alpha * a^T @ grad_z through bmm with the same kernel id and opts (injected faults stripped, on the stream
+        autograd runs the backward on), grad_bias = grad_z summed over the entries' rows (per-entry bias) or over entries
+        and rows (shared bias).  An expanded operand is copied as above and autograd sums its gradient.  With out= given
+        nothing is recorded (as torch.bmm(out=...)).  Forward and backward can be captured in a CUDA graph, also through
+        torch.cuda.make_graphed_callables."""
         import torch
         for name, t in (("a", a), ("b", b)):
             if t.dim() != 3 or t.dtype != torch.float32 or not t.is_cuda:
@@ -473,21 +513,41 @@ class FtSgemm:
         N = b.shape[2]
         if b.shape[0] != Bt or b.shape[1] != K or b.device != a.device:
             raise ValueError(f"b must be a ({Bt}, {K}, N) tensor on {a.device}")
+        if activation not in ACTIVATIONS:
+            raise ValueError(f"activation must be None, 'relu' or 'gelu', not {activation!r}")
+        if preact is not None and activation is None:
+            raise ValueError("preact needs an activation")
+        if out is None and torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (a, b, bias)):
+            if beta != 0.0:
+                raise ValueError("beta != 0 needs an out tensor")
+            fwd = Opts.from_buffer_copy(opts) if opts is not None else make_opts()
+            if not fwd.stream:
+                fwd.stream = torch.cuda.current_stream(a.device).cuda_stream
+            return _bmm_fn().apply(a, b, bias, preact, self, kernel_id, alpha, fwd, activation)
         if out is None:
             if beta != 0.0:
                 raise ValueError("beta != 0 needs an out tensor")
             out = torch.empty(Bt, M, N, device=a.device, dtype=torch.float32)
         if out.shape != (Bt, M, N) or out.dtype != torch.float32 or out.device != a.device:
             raise ValueError(f"out must be a float32 ({Bt}, {M}, {N}) tensor on {a.device}")
-        if bias is not None and (bias.shape != (N,) or bias.dtype != torch.float32 or bias.device != a.device):
-            raise ValueError(f"bias must be a float32 ({N},) tensor on {a.device}")
+        if bias is not None and (bias.shape not in ((N,), (Bt, N)) or bias.dtype != torch.float32 or bias.device != a.device):
+            raise ValueError(f"bias must be a float32 ({N},) or ({Bt}, {N}) tensor on {a.device}")
+        if preact is not None and (preact.shape != out.shape or preact.stride() != out.stride() or
+                                   preact.dtype != torch.float32 or preact.device != a.device):
+            raise ValueError("preact must be a float32 tensor with out's shape and strides on out's device")
         if Bt == 0:  # an empty batch (torch.bmm accepts it): nothing to compute
             return out
-        bias_stride = bias.stride(0) if bias is not None else None
+        per_entry = bias is not None and bias.dim() == 2
+        bias_stride = bias.stride(-1) if bias is not None else None
         plan = bmm_plan(tuple(a.shape), a.stride(), tuple(b.shape), b.stride(), out.stride(), a.data_ptr(), b.data_ptr(),
-                        out.data_ptr(), bias_stride, bias.data_ptr() if bias is not None else 0)
+                        out.data_ptr(), bias_stride, bias.data_ptr() if bias is not None else 0,
+                        bias.stride(0) if per_entry else None)
+        fused = activation is not None or plan["stride_bias"] != 0
+        if activation is not None and plan["copy_out"]:
+            raise ValueError("out (and so preact) must be writable in place with an activation: 16-byte rows and entries")
         if plan["copy_bias"]:
-            bias = torch.empty(N, device=a.device, dtype=torch.float32).copy_(bias)
+            bias = (torch.empty(Bt, N, device=a.device, dtype=torch.float32).copy_(bias) if plan["stride_bias"] != 0 else
+                    torch.empty(N, device=a.device, dtype=torch.float32).copy_(bias[0] if per_entry else bias))
         if plan["copy_a"]:
             a = torch.empty(Bt, M, _pad4(K), device=a.device, dtype=torch.float32)[:, :, :K].copy_(a)
         if plan["copy_b"]:
@@ -500,9 +560,14 @@ class FtSgemm:
         if opts is None:
             opts = make_opts(stream=torch.cuda.current_stream(a.device).cuda_stream)
         kA, kB = (b, a) if plan["swap"] else (a, b)
-        self.run_batched(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], plan["stride_a"], kB,
-                         plan["layout_b"], plan["ldb"], plan["stride_b"], dst, plan["ldc"], plan["stride_c"], Bt, alpha, beta,
-                         bias, plan["bias_mode"], opts)
+        if fused:
+            self.run_batched_act(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], plan["stride_a"],
+                                 kB, plan["layout_b"], plan["ldb"], plan["stride_b"], dst, plan["ldc"], plan["stride_c"], Bt, alpha,
+                                 beta, bias, plan["bias_mode"], plan["stride_bias"], ACTIVATIONS[activation], preact, opts)
+        else:
+            self.run_batched(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], plan["stride_a"], kB,
+                             plan["layout_b"], plan["ldb"], plan["stride_b"], dst, plan["ldc"], plan["stride_c"], Bt, alpha, beta,
+                             bias, plan["bias_mode"], opts)
         if dst is not out:
             out.copy_(dst)
         return out
@@ -760,6 +825,53 @@ def _linear_act_fn():
 
         _LINEAR_ACT_FN = LinearActFn
     return _LINEAR_ACT_FN
+
+
+_BMM_FN = None
+
+
+def _bmm_fn():
+    """The torch.autograd.Function behind a differentiable FtSgemm.bmm: one run_batched / run_batched_act forward, the
+    activation's backward in torch, then the two gradient products through bmm."""
+    global _BMM_FN
+    if _BMM_FN is None:
+        import torch
+
+        class BmmFn(torch.autograd.Function):
+            @staticmethod
+            def forward(ctx, a, b, bias, preact, dev, kernel_id, alpha, opts, activation):
+                z = preact
+                if z is None and activation == "gelu":
+                    z = torch.empty(a.shape[0], a.shape[1], b.shape[2], device=a.device, dtype=torch.float32)
+                y = dev.bmm(a, b, bias=bias, activation=activation, preact=z, kernel_id=kernel_id, alpha=alpha, opts=opts)
+                ctx.save_for_backward(a, b, y if activation == "relu" else z)
+                ctx.dev, ctx.kernel_id, ctx.alpha, ctx.opts, ctx.activation = dev, kernel_id, alpha, opts, activation
+                ctx.per_entry_bias = bias is not None and bias.dim() == 2
+                return y
+
+            @staticmethod
+            def backward(ctx, gy):
+                a, b, saved = ctx.saved_tensors
+                if ctx.activation == "relu":
+                    gz = torch.ops.aten.threshold_backward(gy, saved, 0)
+                elif ctx.activation == "gelu":
+                    gz = torch.ops.aten.gelu_backward(gy, saved)
+                else:
+                    gz = gy
+                bwd = Opts.from_buffer_copy(ctx.opts)
+                bwd.inject_mode, bwd.n_faults = 0, 0
+                bwd.stream = torch.cuda.current_stream(gy.device).cuda_stream
+                ga = gb = gbias = None
+                if ctx.needs_input_grad[0]:
+                    ga = ctx.dev.bmm(gz, b.transpose(1, 2), kernel_id=ctx.kernel_id, alpha=ctx.alpha, opts=bwd)
+                if ctx.needs_input_grad[1]:
+                    gb = ctx.dev.bmm(a.transpose(1, 2), gz, kernel_id=ctx.kernel_id, alpha=ctx.alpha, opts=bwd)
+                if ctx.needs_input_grad[2]:
+                    gbias = gz.sum(1) if ctx.per_entry_bias else gz.sum((0, 1))
+                return ga, gb, gbias, None, None, None, None, None, None
+
+        _BMM_FN = BmmFn
+    return _BMM_FN
 
 
 def run_cli(args, timeout=None) -> subprocess.CompletedProcess:

@@ -368,16 +368,18 @@ int with_flag(bool b, F &&f) {
 
 // The kernel instantiation of a launch: SEED for a plan with cut tiles, BIAS for a bias (KernelParams::bias,
 // ftsgemm_tc_kernel), BATCH for a batch of more than one entry, PROT (fault-tolerant kernels only) for opts.protect_epilogue.
-// An activation (a single product; the bias mode is then a run-time field) selects the ACT kernels instead of BIAS / BATCH.
+// An activation (the bias mode is then a run-time field) selects the ACT kernels instead of BIAS: with BATCH for a batch of
+// more than one entry.
 template <int BN, int CG>
 int launch_variant(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
                    const KernelParams &p, int units, cudaStream_t stream, bool ft, bool prot) {
   if (p.act != kActNone) {
-    if (p.batch > 1) return FTSGEMM_ERR_UNSUPPORTED;
     return with_flag(p.sk_tiles > 0, [&](auto seed) {
-      if (!ft) return launch_tc<BN, false, CG, false, seed, false, false, true>(h, tmA, tmB, tmC, p, units, stream);
-      if (prot) return launch_tc<BN, true, CG, true, seed, false, false, true>(h, tmA, tmB, tmC, p, units, stream);
-      return launch_tc<BN, true, CG, false, seed, false, false, true>(h, tmA, tmB, tmC, p, units, stream);
+      return with_flag(p.batch > 1, [&](auto batch) {
+        if (!ft) return launch_tc<BN, false, CG, false, seed, false, batch, true>(h, tmA, tmB, tmC, p, units, stream);
+        if (prot) return launch_tc<BN, true, CG, true, seed, false, batch, true>(h, tmA, tmB, tmC, p, units, stream);
+        return launch_tc<BN, true, CG, false, seed, false, batch, true>(h, tmA, tmB, tmC, p, units, stream);
+      });
     });
   }
   return with_flag(p.sk_tiles > 0, [&](auto seed) {
@@ -555,12 +557,14 @@ struct Operand {
   int ld;
 };
 
-// The entries of a strided batch (ftsgemm_run_batched): their number and the element strides of A, B and C between them.
+// The entries of a strided batch (ftsgemm_run_batched_act): their number, the element strides of A, B and C between them,
+// and that of the bias (0: one bias shared by all entries).
 struct BatchArg {
   int count;
   long long sa, sb, sc;
+  long long sbias;
 };
-const BatchArg kSingle = {1, 0, 0, 0};
+const BatchArg kSingle = {1, 0, 0, 0, 0};
 // The activation of ftsgemm_run_act: its kind and the caller's Z (null: not written).  kNoAct everywhere else.
 struct ActArg {
   int kind;
@@ -601,6 +605,7 @@ KernelParams make_params(ftsgemm_handle_t h, const Variant &v, int M, int N, int
   p.stride_a = bt.sa;
   p.stride_b = bt.sb;
   p.stride_c = bt.sc;
+  p.stride_bias = bias ? bt.sbias : 0;
   p.tau_abs = o.tau_abs > 0 ? o.tau_abs : 1e-3f;
   p.tau_rel = o.tau_rel > 0 ? o.tau_rel : 1e-5f;  // DESIGN.md section 5
   p.detect_only = o.detect_only;
@@ -1089,7 +1094,7 @@ int run_3xtf32(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const 
   ftsgemm_opts o_quiet = o3;  // injected faults belong to the main product only
   o_quiet.inject_mode = 0;
   // (the bias and the activation go to the last pass only: applied once, after the final alpha*acc + C)
-  const BatchArg lo = {bt.count, static_cast<long long>(a_floats), static_cast<long long>(b_floats), bt.sc};
+  const BatchArg lo = {bt.count, static_cast<long long>(a_floats), static_cast<long long>(b_floats), bt.sc, 0};
   rc = run_tc(h, v, M, N, K, Alo, Bs, dC, ldc, alpha, beta, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo);
   if (!rc) rc = run_tc(h, v, M, N, K, As, Blo, dC, ldc, alpha, 1.0f, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo);
   if (!rc) rc = run_tc(h, v, M, N, K, A, B, dC, ldc, alpha, 1.0f, bias, bias_mode, o3, stream, bt, act);
@@ -1362,11 +1367,12 @@ int ftsgemm_run_bias(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, con
                              bias_mode, opts);
 }
 
-// ftsgemm_run_batched and ftsgemm_run_act: validation, options, capture state, variant; then run_resolved.
+// ftsgemm_run_batched_act (and through it every run entry point): validation, options, capture state, variant; then
+// run_resolved.
 static int run_call(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
                     long long stride_a, const float *dB, int layout_b, int ldb, long long stride_b, float *dC, int ldc,
-                    long long stride_c, int batch, float alpha, float beta, const float *bias, int bias_mode, const ActArg &act,
-                    const ftsgemm_opts *opts) {
+                    long long stride_c, int batch, float alpha, float beta, const float *bias, int bias_mode,
+                    long long stride_bias, const ActArg &act, const ftsgemm_opts *opts) {
   if (!h) return FTSGEMM_ERR_NO_DEVICE;
   if (!dA || !dB || !dC || M <= 0 || N <= 0 || K <= 0 || batch < 1) return FTSGEMM_ERR_INVALID_ARG;
   const Variant *v = find_variant(kernel_id);
@@ -1383,7 +1389,9 @@ static int run_call(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, cons
   if (act.kind != kActNone && v->info.engine != 1) return FTSGEMM_ERR_UNSUPPORTED;  // so is the activation
   // A batch of one entry is the single product (strides ignored).  Otherwise the wgmma kernels need 16-byte entry strides
   // (TMA global strides, the 16-byte aligned C of the store passes), C entries that do not overlap, and no broadcast entry.
-  const BatchArg bt = batch > 1 ? BatchArg{batch, stride_a, stride_b, stride_c} : kSingle;
+  // (the entry stride of the bias is read only for a bias and more than one entry)
+  if (bias && batch > 1 && stride_bias < 0) return FTSGEMM_ERR_INVALID_ARG;
+  const BatchArg bt = batch > 1 ? BatchArg{batch, stride_a, stride_b, stride_c, bias ? stride_bias : 0} : kSingle;
   if (batch > 1 && v->info.engine == 2) return FTSGEMM_ERR_UNSUPPORTED;  // the baseline has no batched form
   if (batch > 1 && v->info.engine == 1) {
     if (stride_a <= 0 || stride_b <= 0 || stride_c <= 0 || (stride_a % 4) || (stride_b % 4) || (stride_c % 4))
@@ -1414,18 +1422,26 @@ int ftsgemm_run_batched(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, 
                         long long stride_a, const float *dB, int layout_b, int ldb, long long stride_b, float *dC, int ldc,
                         long long stride_c, int batch, float alpha, float beta, const float *bias, int bias_mode,
                         const ftsgemm_opts *opts) {
-  return run_call(h, kernel_id, M, N, K, dA, layout_a, lda, stride_a, dB, layout_b, ldb, stride_b, dC, ldc, stride_c, batch, alpha,
-                  beta, bias, bias_mode, kNoAct, opts);
+  return ftsgemm_run_batched_act(h, kernel_id, M, N, K, dA, layout_a, lda, stride_a, dB, layout_b, ldb, stride_b, dC, ldc,
+                                 stride_c, batch, alpha, beta, bias, bias_mode, 0, FTSGEMM_ACT_NONE, nullptr, opts);
 }
 
 int ftsgemm_run_act(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
                     const float *dB, int layout_b, int ldb, float *dC, int ldc, float alpha, float beta, const float *bias,
                     int bias_mode, int activation, float *dZ, const ftsgemm_opts *opts) {
+  return ftsgemm_run_batched_act(h, kernel_id, M, N, K, dA, layout_a, lda, 0, dB, layout_b, ldb, 0, dC, ldc, 0, 1, alpha, beta,
+                                 bias, bias_mode, 0, activation, dZ, opts);
+}
+
+int ftsgemm_run_batched_act(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
+                            long long stride_a, const float *dB, int layout_b, int ldb, long long stride_b, float *dC, int ldc,
+                            long long stride_c, int batch, float alpha, float beta, const float *bias, int bias_mode,
+                            long long stride_bias, int activation, float *dZ, const ftsgemm_opts *opts) {
   if (!h) return FTSGEMM_ERR_NO_DEVICE;
   if (activation < FTSGEMM_ACT_NONE || activation > FTSGEMM_ACT_GELU) return FTSGEMM_ERR_INVALID_ARG;
   if (dZ && (activation == FTSGEMM_ACT_NONE || dZ == dC || (reinterpret_cast<uintptr_t>(dZ) & 3))) return FTSGEMM_ERR_INVALID_ARG;
-  return run_call(h, kernel_id, M, N, K, dA, layout_a, lda, 0, dB, layout_b, ldb, 0, dC, ldc, 0, 1, alpha, beta, bias, bias_mode,
-                  ActArg{activation, dZ}, opts);
+  return run_call(h, kernel_id, M, N, K, dA, layout_a, lda, stride_a, dB, layout_b, ldb, stride_b, dC, ldc, stride_c, batch, alpha,
+                  beta, bias, bias_mode, stride_bias, ActArg{activation, dZ}, opts);
 }
 
 int ftsgemm_get_stats(ftsgemm_handle_t h, ftsgemm_stats *out) {

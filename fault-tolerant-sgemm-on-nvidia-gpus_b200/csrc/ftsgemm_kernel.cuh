@@ -188,6 +188,9 @@ struct KernelParams {
   // opts.protect_epilogue of the call (read by the PROT instantiations only): 1 sums a row segment as it stores it and
   // judges it at the end; 2 verifies every 32-column chunk before it is written (protected_store_pass_v2)
   int protect;
+  // Per-entry bias of a strided batch (ftsgemm_run_batched_act; read by the BATCH instantiations only): entry i adds
+  // bias + i*stride_bias.  0 for a bias shared by all entries and for every single product.
+  long long stride_bias;
 };
 
 __device__ __forceinline__ unsigned long long globaltimer_ns() { return ptx::globaltimer(); }
@@ -428,6 +431,12 @@ __device__ __forceinline__ void act_chunk(uint32_t (&v)[32], const BiasRef &bias
 template <bool ACT>
 __device__ __forceinline__ ActRef act_of(const KernelParams &p, int m) {
   if constexpr (ACT) return ActRef{p.act, p.z != nullptr ? p.z + m : nullptr};
+  else return ActRef{kActNone, nullptr};
+}
+// (strided batch: Z is the entry's, null when not written)
+template <bool ACT>
+__device__ __forceinline__ ActRef act_of_entry(const KernelParams &p, float *Z, int m) {
+  if constexpr (ACT) return ActRef{p.act, Z != nullptr ? Z + m : nullptr};
   else return ActRef{kActNone, nullptr};
 }
 
@@ -949,15 +958,17 @@ __device__ __noinline__ void recompute_row_bias(const float *A, const float *B, 
                                                 int bias_mode) {
   recompute_row_body<BN, true>(A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, m, n0, lane, bias, bias_mode);
 }
-template <int BN>
+// ENTRY: a separate copy for the ACT x BATCH kernels.  ptxas allocates a callee's registers around all its callers, so a
+// callee shared with them moved the stack frames of the single-product ACT kernels.
+template <int BN, bool ENTRY = false>
 __device__ __noinline__ void recompute_row_act(const float *A, const float *B, float *C, int lda, int ldb, int kmajor, int ldc,
                                                int N, int K, float alpha, float beta, int m, int n0, int lane, const float *bias,
                                                int bias_mode, int act_kind, float *Z) {
   recompute_row_body<BN, false, true>(A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, m, n0, lane, bias, bias_mode, act_kind, Z);
 }
-template <int BN, bool BIAS, bool ACT = false, typename... Args>
+template <int BN, bool BIAS, bool ACT = false, bool ENTRY = false, typename... Args>
 __device__ __forceinline__ void recompute(const float *bias, int bias_mode, int act_kind, float *Z, Args... args) {
-  if constexpr (ACT) recompute_row_act<BN>(args..., bias, bias_mode, act_kind, Z);
+  if constexpr (ACT) recompute_row_act<BN, ENTRY>(args..., bias, bias_mode, act_kind, Z);
   else if constexpr (BIAS) recompute_row_bias<BN>(args..., bias, bias_mode);
   else recompute_row<BN>(args...);
 }
@@ -966,7 +977,7 @@ __device__ __forceinline__ void recompute(const float *bias, int bias_mode, int 
 // common epilogue registers (inlined it pushed the kernel into spills), and a reference to the __grid_constant__ parameter
 // block would force a local copy of all of it.  Row segments that fail are counted and, with beta == 0, recomputed from A
 // and B (with beta != 0 the old values of C are already overwritten: reported as uncorrectable).
-template <int BN, bool BIAS, bool ACT = false>
+template <int BN, bool BIAS, bool ACT = false, bool ENTRY = false>
 __device__ __forceinline__ void protected_store_body(uint32_t taddr, const float *A, const float *B, float *C, int lda, int ldb,
                                                      int kmajor, int ldc, int N, int K, float alpha, float beta, DeviceStats *stats,
                                                      bool can_recompute, int m, int row0, bool row_ok, int n0, int c_begin, int c_end,
@@ -998,10 +1009,11 @@ __device__ __forceinline__ void protected_store_body(uint32_t taddr, const float
     const int r = __ffs(mask) - 1;
     mask &= mask - 1u;
     if (c_end - c_begin == BN / 32) {
-      recompute<BN, BIAS, ACT>(bias, bias_mode, act_kind, Z, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r, n0, lane);
+      recompute<BN, BIAS, ACT, ENTRY>(bias, bias_mode, act_kind, Z, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r, n0,
+                                      lane);
     } else {
       if constexpr (BN >= 64)
-        recompute<BN / 2, BIAS, ACT>(bias, bias_mode, act_kind, Z, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r,
+        recompute<BN / 2, BIAS, ACT, ENTRY>(bias, bias_mode, act_kind, Z, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r,
                                      n0 + c_begin * 32, lane);
     }
   }
@@ -1033,11 +1045,18 @@ template <int BN, bool BIAS>
 __device__ __noinline__ void protected_store_pass_batched(FT_PROT_PARAMS, const float *bias, int bias_mode, int row_ofs) {
   protected_store_body<BN, BIAS>(FT_PROT_ARGS, bias, bias_mode, row_ofs);
 }
+// (the ACT x BATCH kernels: A, B, C, the bias and Z are the entry's; a fourth entry, so the three above keep their lists)
+template <int BN>
+__device__ __noinline__ void protected_store_pass_act_batched(FT_PROT_PARAMS, const float *bias, int bias_mode, int row_ofs,
+                                                             int act_kind, float *Z) {
+  protected_store_body<BN, false, true, true>(FT_PROT_ARGS, bias, bias_mode, row_ofs, act_kind, Z);
+}
 #undef FT_PROT_PARAMS
 #undef FT_PROT_ARGS
 template <int BN, bool BIAS, bool BATCH, bool ACT, typename... Args>
 __device__ __forceinline__ void protected_store(const float *bias, int bias_mode, int row_ofs, int act_kind, float *Z, Args... args) {
-  if constexpr (ACT) protected_store_pass_act<BN>(args..., bias, bias_mode, act_kind, Z);
+  if constexpr (ACT && BATCH) protected_store_pass_act_batched<BN>(args..., bias, bias_mode, row_ofs, act_kind, Z);
+  else if constexpr (ACT) protected_store_pass_act<BN>(args..., bias, bias_mode, act_kind, Z);
   else if constexpr (BATCH) protected_store_pass_batched<BN, BIAS>(args..., bias, bias_mode, row_ofs);
   else if constexpr (BIAS) protected_store_pass_bias<BN>(args..., bias, bias_mode);
   else protected_store_pass<BN>(args...);
@@ -1131,7 +1150,8 @@ __device__ __forceinline__ float chunk_sum(const uint32_t (&v)[32], float &sabs)
   sabs = b0 + b1;
   return a0 + a1;
 }
-template <bool BIAS, bool ACT>
+// (ENTRY: the ACT x BATCH kernels' own copy, see recompute_row_act)
+template <bool BIAS, bool ACT, bool ENTRY = false>
 __device__ __noinline__ void protected_store_pass_v2(uint32_t taddr, const float *A, const float *B, float *C, int lda, int ldb,
                                                      int kmajor, int ldc, int N, int K, float alpha, float beta, DeviceStats *stats,
                                                      bool can_recompute, int m, int row0, bool row_ok, int n0, bool ragged_n,
@@ -1275,7 +1295,7 @@ __device__ __noinline__ void protected_store_pass_v2(uint32_t taddr, const float
     while (chunks != 0u) {
       const int k = __ffs(chunks) - 1;
       chunks &= chunks - 1u;
-      recompute<32, BIAS, ACT>(bias, bias_mode, act_kind, Z, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r,
+      recompute<32, BIAS, ACT, ENTRY>(bias, bias_mode, act_kind, Z, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r,
                                n0 + (c_begin + k) * 32, lane);
     }
   }
@@ -1756,14 +1776,15 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t a_desc, 
 // BATCH: the instantiation for strided batches (ftsgemm_run_batched with batch > 1): 3-D tensor maps with the entry as the
 // outer coordinate, and every per-tile address offset by the item's entry.  Without it the entry is the constant 0 and
 // the code is that of the kernel before batching existed.
-// ACT: the instantiation for calls with an activation (ftsgemm_run_act; single products only, never with BIAS or BATCH).
+// ACT: the instantiation for calls with an activation (ftsgemm_run_act, ftsgemm_run_batched_act; never with BIAS).
 // The final epilogue of a data tile stores act(z) and, when p.z is set, z; the bias mode, the activation and Z are run-time
-// fields.  Like BIAS, its own binary, so that the other kernels are compiled exactly as without the feature.
+// fields.  Like BIAS, its own binary, so that the other kernels are compiled exactly as without the feature.  With BATCH,
+// the entry's Z is p.z + entry * stride_c (C's geometry) and its bias p.bias + entry * stride_bias.
 template <int BN, bool FT, int CG, bool PROT = false, bool SEED = false, bool BIAS = false, bool BATCH = false, bool ACT = false>
 __global__ void __launch_bounds__(kThreads, 1)
 ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmChk, const KernelParams p) {
-  static_assert(!(ACT && (BIAS || BATCH)), "the ACT kernels are single products with a run-time bias");
+  static_assert(!(ACT && BIAS), "the ACT kernels take the bias mode at run time");
   using Cfg = TileCfg<BN, FT, CG>;
   constexpr int kStages = Cfg::kStages;
   constexpr int kAccRegs = BN / 2;  // per thread of a consumer warpgroup: 64 x BN FP32
@@ -1938,6 +1959,8 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const float *const Ab = BATCH ? p.A + bt * p.stride_a : nullptr;
       const float *const Bb = BATCH ? p.B + bt * p.stride_b : nullptr;
       float *const Cb = BATCH ? p.C + bt * p.stride_c : nullptr;
+      const float *const biasb = BATCH ? p.bias + ((BIAS || ACT) ? bt * p.stride_bias : 0) : nullptr;  // (the entry's bias)
+      float *const Zb = (BATCH && ACT && p.z != nullptr) ? p.z + bt * p.stride_c : nullptr;          // (Z: C's geometry)
       const int row_ofs = bt * p.M;                           // stacked rows: fault list and events
       const int slab_ofs = bt * (p.tiles_m * CG * (kBM / 32));  // the entry's checksum flags
       const size_t chk_ofs = static_cast<size_t>(bt) * p.M * p.n_chk_cols * (p.chk_slices > 1 ? p.chk_slices : 1);
@@ -2029,20 +2052,21 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             if constexpr (PROT) stale = (ptx::ld_acquire_shared_u32(xchg_base(q) + 4) >> lane) & 1u;  // rows it repaired
           }
           if (PROT && FT && !(p.dbg_flags & 1) && p.protect == 2) {
-            protected_store_pass_v2<BIAS, ACT>(taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1),
+            protected_store_pass_v2<BIAS, ACT, ACT && BATCH>(taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1),
                                                p.ldc, p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m,
                                                m0_cta + q * 32, m < p.M && !skip, n0, n0 + BN > p.N, kMid, BN / 32, s1, stale == 0u,
                                                stored_value_upsets<BN, BATCH>(p, q, lane, m0_cta, n0, kMid, BN / 32, row_ofs), lane,
-                                               (BIAS || ACT) ? p.bias : nullptr, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? p.z : nullptr);
+                                               (BIAS || ACT) ? (BATCH ? biasb : p.bias) : nullptr, p.bias_mode, row_ofs, ACT ? p.act : 0,
+                                               ACT ? (BATCH ? Zb : p.z) : nullptr);
           } else if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N) {
             uint32_t bad_bits = 0u;
             const int bad_col = stored_value_fault<BN, BATCH>(p, q, lane, m0_cta, n0, kMid, BN / 32, bad_bits, row_ofs);
-            protected_store<BN, BIAS, BATCH, ACT>(p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? p.z : nullptr, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
+            protected_store<BN, BIAS, BATCH, ACT>(BATCH ? biasb : p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? (BATCH ? Zb : p.z) : nullptr, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
                                       p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32,
                                       m < p.M && !skip, n0, kMid, BN / 32, s1, stale == 0u, bad_col, bad_bits, lane);
           } else {
             store_tile<BN, BIAS, ACT>(taddr, (BATCH ? Cb : p.C) + m, m < p.M && !skip, n0, p.N, p.ldc, p.alpha, p.beta, kMid, BN / 32,
-                                      make_bias(p.bias, p.bias_mode, m, (BIAS || ACT) && m < p.M && !skip), act_of<ACT>(p, m));
+                                      make_bias(BATCH ? biasb : p.bias, p.bias_mode, m, (BIAS || ACT) && m < p.M && !skip), BATCH ? act_of_entry<ACT>(p, Zb, m) : act_of<ACT>(p, m));
           }
           ptx::named_bar_sync(4 + q, 64);  // both halves are out of the accumulator
         }
@@ -2098,28 +2122,29 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
         if (assist_on && FT && !(p.dbg_flags & 1)) ptx::named_bar_sync(4 + q, 64);  // corrections are in place
         if (PROT && FT && !(p.dbg_flags & 1) && p.protect == 2) {
-          protected_store_pass_v2<BIAS, ACT>(taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1),
+          protected_store_pass_v2<BIAS, ACT, ACT && BATCH>(taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1),
                                              p.ldc, p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m,
                                              m0_cta + q * 32, m < p.M && !redo, n0, n0 + BN > p.N, 0, c_mid, own_s1,
                                              ((stale_mask >> lane) & 1u) == 0u,
                                              stored_value_upsets<BN, BATCH>(p, q, lane, m0_cta, n0, 0, c_mid, row_ofs), lane,
-                                             (BIAS || ACT) ? p.bias : nullptr, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? p.z : nullptr);
+                                             (BIAS || ACT) ? (BATCH ? biasb : p.bias) : nullptr, p.bias_mode, row_ofs, ACT ? p.act : 0,
+                                             ACT ? (BATCH ? Zb : p.z) : nullptr);
         } else if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N) {
           uint32_t bad_bits = 0u;
           const int bad_col = stored_value_fault<BN, BATCH>(p, q, lane, m0_cta, n0, 0, c_mid, bad_bits, row_ofs);
-          protected_store<BN, BIAS, BATCH, ACT>(p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? p.z : nullptr, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
+          protected_store<BN, BIAS, BATCH, ACT>(BATCH ? biasb : p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? (BATCH ? Zb : p.z) : nullptr, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
                                     p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32,
                                     m < p.M && !redo, n0, 0, c_mid, own_s1, ((stale_mask >> lane) & 1u) == 0u, bad_col, bad_bits, lane);
         } else {
           store_tile<BN, BIAS, ACT>(taddr, (BATCH ? Cb : p.C) + m, m < p.M && !redo, n0, p.N, p.ldc, p.alpha, p.beta, 0, c_mid,
-                                    make_bias(p.bias, p.bias_mode, m, (BIAS || ACT) && m < p.M && !redo), act_of<ACT>(p, m));
+                                    make_bias(BATCH ? biasb : p.bias, p.bias_mode, m, (BIAS || ACT) && m < p.M && !redo), BATCH ? act_of_entry<ACT>(p, Zb, m) : act_of<ACT>(p, m));
         }
         if (FT && redo_mask != 0u) {  // rare, warp-uniform: recompute the flagged rows from global memory
           unsigned rm = redo_mask;
           while (rm != 0u) {
             const int r = __ffs(rm) - 1;
             rm &= rm - 1u;
-            recompute<BN, BIAS, ACT>(p.bias, p.bias_mode, ACT ? p.act : 0, ACT ? p.z : nullptr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K,
+            recompute<BN, BIAS, ACT, ACT && BATCH>(BATCH ? biasb : p.bias, p.bias_mode, ACT ? p.act : 0, ACT ? (BATCH ? Zb : p.z) : nullptr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K,
                                 p.alpha, p.beta, m0_cta + q * 32 + r, n0, lane);
           }
         }

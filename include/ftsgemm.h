@@ -283,8 +283,8 @@ int ftsgemm_run_bias(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, con
 /* ---- strided batch  (new work: the reference computes one product per launch; the contract is cuBLAS's
  *      cublasSgemmStridedBatched, with this library's layouts, ABFT options and fused bias) ---------------------------------
  * batch independent products: entry i in [0, batch) is exactly the ftsgemm_run_bias product on A + i*stride_a, B + i*stride_b
- * and C + i*stride_c (strides in floats).  The bias, if any, is one vector shared by all entries.  ftsgemm_run_bias is this
- * call with batch = 1, where the strides are ignored.
+ * and C + i*stride_c (strides in floats).  The bias, if any, is one vector shared by all entries (ftsgemm_run_batched_act
+ * below takes one bias per entry).  ftsgemm_run_bias is this call with batch = 1, where the strides are ignored.
  * The wgmma ids run the whole batch in ONE launch of the persistent kernel (plus the encode pre-pass below ~8 MB of B for
  * all entries together): the tiles of all entries form one work plan.  Every option applies per entry (3xTF32, check_segments,
  * protect_epilogue, reuse_b_checksums -- keyed on stride_b and batch as well --, no_recompute, detect_only, injection: the
@@ -309,8 +309,9 @@ int ftsgemm_run_batched(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, 
  *   FTSGEMM_ACT_GELU   z * 0.5f * (1 + erff(z * (float)M_SQRT1_2))       (torch's gelu, approximate='none')
  * GELU depends on the device's erff, so it matches torch's to within a few ulp rather than bit for bit.
  * FTSGEMM_ACT_NONE with dZ = NULL is ftsgemm_run_bias: the same kernels and the same result.
- * Single products only: there is no batched form.  Every option applies: with opts.precision = 1 the activation and Z go to
- * the last of the three passes, with opts.check_segments = S to the last segment, like the bias.
+ * ftsgemm_run_batched_act below is the batched form (this call is it with batch = 1).  Every option applies: with
+ * opts.precision = 1 the activation and Z go to the last of the three passes, with opts.check_segments = S to the last
+ * segment, like the bias.
  * ABFT coverage.  The accumulator check runs before alpha, beta, the bias and the activation and is unchanged: a corrected
  * element is repaired in the accumulator, so C = act(corrected z).  The protected store pass (opts.protect_epilogue) verifies
  * z -- the values it sums are the pre-activation ones, with today's tolerance -- and then applies the activation; an upset of
@@ -328,6 +329,23 @@ enum {
 int ftsgemm_run_act(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
                     const float *dB, int layout_b, int ldb, float *dC, int ldc, float alpha, float beta,
                     const float *bias, int bias_mode, int activation, float *dZ, const ftsgemm_opts *opts);
+
+/* ---- strided batch with a per-entry bias and an activation --------------------------------------------------------------
+ * Entry i in [0, batch) is exactly ftsgemm_run_act on A + i*stride_a, B + i*stride_b and C + i*stride_c, with the bias
+ * bias + i*stride_bias and Z at dZ + i*stride_c (Z has C's geometry per entry): the same device code, so the same bits, GELU
+ * included.  stride_bias = 0 is one bias shared by all entries (ftsgemm_run_batched); a (batch, len) bias of an expert
+ * layer has stride_bias = len.  stride_bias is ignored with FTSGEMM_BIAS_NONE or batch = 1.
+ * ftsgemm_run_batched is this call with stride_bias = 0, FTSGEMM_ACT_NONE and dZ = NULL; ftsgemm_run_act is it with
+ * batch = 1.  The wgmma ids run the whole batch in one launch, as ftsgemm_run_batched does, and every option applies per
+ * entry, as there: 3xTF32 and check_segments apply the bias and the activation once (last pass / segment), both
+ * protect_epilogue levels verify z of every entry, and fault and event rows are stacked rows i*M + m.
+ * Errors: those of ftsgemm_run_batched and ftsgemm_run_act; a negative stride_bias (with a bias and batch > 1):
+ * FTSGEMM_ERR_INVALID_ARG; an activation or a bias (shared or per entry) with the cuBLAS ids 0 / 7 or the baseline ids
+ * 10 / 30: FTSGEMM_ERR_UNSUPPORTED. */
+int ftsgemm_run_batched_act(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *A, int layout_a, int lda,
+                            long long stride_a, const float *B, int layout_b, int ldb, long long stride_b, float *C, int ldc,
+                            long long stride_c, int batch, float alpha, float beta, const float *bias, int bias_mode,
+                            long long stride_bias, int activation, float *dZ, const ftsgemm_opts *opts);
 
 /* Counters of all FT launches since the previous call (synchronises the handle's last stream, then resets). */
 int ftsgemm_get_stats(ftsgemm_handle_t h, ftsgemm_stats *out);
