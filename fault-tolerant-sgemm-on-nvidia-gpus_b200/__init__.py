@@ -98,7 +98,7 @@ EXPORTED_SYMBOLS = [
     "ftsgemm_run_host", "ftsgemm_baseline", "ftsgemm_verify", "ftsgemm_debug_set", "ftsgemm_debug_schedule",
     "ftsgemm_verify_bad_count", "ftsgemm_debug_trace", "ftsgemm_stats_device", "ftsgemm_select_kernel", "ftsgemm_launch_count", "ftsgemm_peer_export", "ftsgemm_peer_connect",
     "ftsgemm_peer_verdict", "ftsgemm_run_batched", "ftsgemm_debug_schedule_batched", "ftsgemm_run_act",
-    "ftsgemm_run_batched_act",
+    "ftsgemm_run_batched_act", "ftsgemm_run_out", "ftsgemm_run_batched_out",
 ]
 
 _lib = None
@@ -140,6 +140,10 @@ def lib():
                                           C.POINTER(Opts)]
         L.ftsgemm_run_batched_act.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, ll, vp, ip, ip, ll, vp, ip, ll, ip, fp, fp, vp, ip,
                                               ll, ip, vp, C.POINTER(Opts)]
+        L.ftsgemm_run_out.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, vp, ip, ip, vp, ip, vp, fp, fp, vp, ip, ip, vp,
+                                      C.POINTER(Opts)]
+        L.ftsgemm_run_batched_out.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, ll, vp, ip, ip, ll, vp, ip, ll, vp, ip, fp, fp,
+                                              vp, ip, ll, ip, vp, C.POINTER(Opts)]
         L.ftsgemm_get_stats.argtypes = [vp, C.POINTER(Stats)]
         L.ftsgemm_run_host.argtypes = [vp, ip, ip, ip, ip, vp, vp, vp, fp, fp, C.POINTER(Opts)]
         L.ftsgemm_stats_device.argtypes = [vp, vp, vp]
@@ -478,7 +482,31 @@ class FtSgemm:
                                                         activation, _ptr(dZ) if dZ is not None else None,
                                                         C.byref(opts) if opts is not None else None))
 
-    def bmm(self, a, b, out=None, *, bias=None, activation=None, preact=None, kernel_id: int = ID_ABFT_AUTO,
+    def run_out(self, kernel_id: int, M: int, N: int, K: int, dA, layout_a: int, lda: int, dB, layout_b: int, ldb: int, dC,
+                ldc: int, dD, alpha: float = 1.0, beta: float = 0.0, bias=None, bias_mode: int = BIAS_NONE,
+                activation: int = ACT_NONE, dZ=None, opts: Opts | None = None) -> None:
+        """run_act with the result written to dD (C's geometry: ldc) and C read-only: bit for bit run_act on a copy of C in
+        dD.  dC may be None with beta = 0 (C is not read); dD == dC is run_act itself (include/ftsgemm.h:
+        ftsgemm_run_out)."""
+        self._run_checked(lib().ftsgemm_run_out(self._h, kernel_id, M, N, K, _ptr(dA), layout_a, lda, _ptr(dB), layout_b, ldb,
+                                                _ptr(dC) if dC is not None else None, ldc, _ptr(dD), alpha, beta,
+                                                _ptr(bias) if bias is not None else None, bias_mode, activation,
+                                                _ptr(dZ) if dZ is not None else None, C.byref(opts) if opts is not None else None))
+
+    def run_batched_out(self, kernel_id: int, M: int, N: int, K: int, dA, layout_a: int, lda: int, stride_a: int, dB,
+                        layout_b: int, ldb: int, stride_b: int, dC, ldc: int, stride_c: int, dD, batch: int, alpha: float = 1.0,
+                        beta: float = 0.0, bias=None, bias_mode: int = BIAS_NONE, stride_bias: int = 0,
+                        activation: int = ACT_NONE, dZ=None, opts: Opts | None = None) -> None:
+        """run_batched_act with the results written to dD (C's geometry: ldc, entry i at dD + i*stride_c) and C read-only:
+        bit for bit run_batched_act on a copy of C in dD (include/ftsgemm.h: ftsgemm_run_batched_out)."""
+        self._run_checked(lib().ftsgemm_run_batched_out(self._h, kernel_id, M, N, K, _ptr(dA), layout_a, lda, stride_a, _ptr(dB),
+                                                        layout_b, ldb, stride_b, _ptr(dC) if dC is not None else None, ldc,
+                                                        stride_c, _ptr(dD), batch, alpha, beta,
+                                                        _ptr(bias) if bias is not None else None, bias_mode, stride_bias,
+                                                        activation, _ptr(dZ) if dZ is not None else None,
+                                                        C.byref(opts) if opts is not None else None))
+
+    def bmm(self, a, b, out=None, *, c=None, bias=None, activation=None, preact=None, kernel_id: int = ID_ABFT_AUTO,
             alpha: float = 1.0, beta: float = 0.0, opts: Opts | None = None):
         """out = act(alpha * (a @ b) + beta * out + bias) for 3-D float32 CUDA tensors a: (Bt, M, K), b: (Bt, K, N), out:
         (Bt, M, N), an optional bias (N,) shared by all entries or (Bt, N) one per entry, and an optional activation --
@@ -504,7 +532,13 @@ class FtSgemm:
         autograd runs the backward on), grad_bias = grad_z summed over the entries' rows (per-entry bias) or over entries
         and rows (shared bias).  An expanded operand is copied as above and autograd sums its gradient.  With out= given
         nothing is recorded (as torch.bmm(out=...)).  Forward and backward can be captured in a CUDA graph, also through
-        torch.cuda.make_graphed_callables."""
+        torch.cuda.make_graphed_callables.
+
+        c: a (Bt, M, N) tensor read in place of out's old values and never written -- out = act(alpha * (a @ b) + beta * c
+        + bias), bit for bit what the call gives with out holding a copy of c (one run_batched_out call).  beta must not be
+        0 (c would not be read: ValueError).  With out=None, out is allocated with c's strides (c dense) and the call is
+        differentiable in c as well: grad_c = beta * grad_z.  The kernels read c with out's geometry: a c with other strides
+        (or a base that is not 16-byte aligned) is copied once into that geometry first."""
         import torch
         for name, t in (("a", a), ("b", b)):
             if t.dim() != 3 or t.dtype != torch.float32 or not t.is_cuda:
@@ -517,17 +551,25 @@ class FtSgemm:
             raise ValueError(f"activation must be None, 'relu' or 'gelu', not {activation!r}")
         if preact is not None and activation is None:
             raise ValueError("preact needs an activation")
-        if out is None and torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (a, b, bias)):
-            if beta != 0.0:
-                raise ValueError("beta != 0 needs an out tensor")
+        if c is not None:
+            if beta == 0.0:
+                raise ValueError("c is not read with beta = 0")
+            if c.shape != (Bt, M, N) or c.dtype != torch.float32 or c.device != a.device:
+                raise ValueError(f"c must be a float32 ({Bt}, {M}, {N}) tensor on {a.device}")
+        if out is None and torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (a, b, bias, c)):
+            if beta != 0.0 and c is None:
+                raise ValueError("beta != 0 needs an out tensor or c")
             fwd = Opts.from_buffer_copy(opts) if opts is not None else make_opts()
             if not fwd.stream:
                 fwd.stream = torch.cuda.current_stream(a.device).cuda_stream
-            return _bmm_fn().apply(a, b, bias, preact, self, kernel_id, alpha, fwd, activation)
+            return _bmm_fn().apply(a, b, bias, preact, c, self, kernel_id, alpha, beta, fwd, activation)
         if out is None:
-            if beta != 0.0:
-                raise ValueError("beta != 0 needs an out tensor")
-            out = torch.empty(Bt, M, N, device=a.device, dtype=torch.float32)
+            if c is not None:
+                out = torch.empty_like(c, memory_format=torch.preserve_format)
+            elif beta != 0.0:
+                raise ValueError("beta != 0 needs an out tensor or c")
+            else:
+                out = torch.empty(Bt, M, N, device=a.device, dtype=torch.float32)
         if out.shape != (Bt, M, N) or out.dtype != torch.float32 or out.device != a.device:
             raise ValueError(f"out must be a float32 ({Bt}, {M}, {N}) tensor on {a.device}")
         if bias is not None and (bias.shape not in ((N,), (Bt, N)) or bias.dtype != torch.float32 or bias.device != a.device):
@@ -554,13 +596,20 @@ class FtSgemm:
             b = torch.empty(Bt, N, _pad4(K), device=a.device, dtype=torch.float32)[:, :, :K].copy_(b.transpose(1, 2)).transpose(1, 2)
         dst = out
         if plan["copy_out"]:
-            dst = (out.contiguous() if beta != 0.0 else torch.empty(Bt, M, N, device=a.device, dtype=torch.float32))
+            dst = (out.contiguous() if beta != 0.0 and c is None else
+                   torch.empty(Bt, M, N, device=a.device, dtype=torch.float32))
             if dst is out:
                 dst = out.clone()
+        if c is not None and (c.stride() != dst.stride() or c.data_ptr() % 16 != 0):
+            c = torch.empty_strided(dst.shape, dst.stride(), device=a.device, dtype=torch.float32).copy_(c)
         if opts is None:
             opts = make_opts(stream=torch.cuda.current_stream(a.device).cuda_stream)
         kA, kB = (b, a) if plan["swap"] else (a, b)
-        if fused:
+        if c is not None:
+            self.run_batched_out(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], plan["stride_a"],
+                                 kB, plan["layout_b"], plan["ldb"], plan["stride_b"], c, plan["ldc"], plan["stride_c"], dst, Bt,
+                                 alpha, beta, bias, plan["bias_mode"], plan["stride_bias"], ACTIVATIONS[activation], preact, opts)
+        elif fused:
             self.run_batched_act(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], plan["stride_a"],
                                  kB, plan["layout_b"], plan["ldb"], plan["stride_b"], dst, plan["ldc"], plan["stride_c"], Bt, alpha,
                                  beta, bias, plan["bias_mode"], plan["stride_bias"], ACTIVATIONS[activation], preact, opts)
@@ -572,7 +621,7 @@ class FtSgemm:
             out.copy_(dst)
         return out
 
-    def matmul(self, a, b, out=None, *, bias=None, activation=None, preact=None, kernel_id: int = ID_ABFT_AUTO,
+    def matmul(self, a, b, out=None, *, c=None, bias=None, activation=None, preact=None, kernel_id: int = ID_ABFT_AUTO,
                alpha: float = 1.0, beta: float = 0.0, opts: Opts | None = None):
         """out = alpha * (a @ b) + beta * out + bias for 2-D float32 CUDA tensors a: (M, K), b: (K, N) and an optional 1-D
         float32 bias of length N (one value per column of out, added in the fused store pass); returns out.
@@ -592,17 +641,31 @@ class FtSgemm:
 
         activation = "relu" | "gelu" stores act(z) with z the value above, in the same store pass (one run_act call), and z
         into preact when given.  preact must have out's shape and strides, and out and preact must both be writable in place
-        (else ValueError: there is no copy path for them); a, b and the bias are copied as above when needed."""
+        (else ValueError: there is no copy path for them); a, b and the bias are copied as above when needed.
+
+        c: an (M, N) tensor read in place of out's old values and never written -- out = act(alpha * (a @ b) + beta * c +
+        bias), bit for bit what the call gives with out holding a copy of c (one run_out / run_batched_out call).  beta must
+        not be 0 (c would not be read: ValueError).  With out=None, out is allocated with c's strides (c dense).  The kernels
+        read c with out's geometry: a c with other strides (or a base that is not 16-byte aligned) is copied once into that
+        geometry first."""
         import torch
         for name, t in (("a", a), ("b", b)):
             if t.dim() != 2 or t.dtype != torch.float32 or not t.is_cuda:
                 raise TypeError(f"{name} must be a 2-D float32 CUDA tensor")
         M, K = a.shape
         K2, N = b.shape
+        if c is not None:
+            if beta == 0.0:
+                raise ValueError("c is not read with beta = 0")
+            if c.shape != (M, N) or c.dtype != torch.float32 or c.device != a.device:
+                raise ValueError(f"c must be a float32 ({M}, {N}) tensor on {a.device}")
         if out is None:
-            if beta != 0.0:
-                raise ValueError("beta != 0 needs an out tensor")
-            out = torch.empty(M, N, device=a.device, dtype=torch.float32)
+            if c is not None:
+                out = torch.empty_like(c, memory_format=torch.preserve_format)
+            elif beta != 0.0:
+                raise ValueError("beta != 0 needs an out tensor or c")
+            else:
+                out = torch.empty(M, N, device=a.device, dtype=torch.float32)
         if out.shape != (M, N) or out.dtype != torch.float32 or out.device != a.device or b.device != a.device:
             raise ValueError(f"out must be a float32 ({M}, {N}) tensor on {a.device}")
         if bias is not None and (bias.shape != (N,) or bias.dtype != torch.float32 or bias.device != a.device):
@@ -610,8 +673,8 @@ class FtSgemm:
         if K != K2:
             raise ValueError(f"inner dimensions differ: {tuple(a.shape)} @ {tuple(b.shape)}")
         if activation is None and preact is None:
-            self.bmm(a.unsqueeze(0), b.unsqueeze(0), out.unsqueeze(0), bias=bias, kernel_id=kernel_id, alpha=alpha, beta=beta,
-                     opts=opts)
+            self.bmm(a.unsqueeze(0), b.unsqueeze(0), out.unsqueeze(0), c=c.unsqueeze(0) if c is not None else None, bias=bias,
+                     kernel_id=kernel_id, alpha=alpha, beta=beta, opts=opts)
             return out
         if activation not in ("relu", "gelu"):
             raise ValueError(f"activation must be None, 'relu' or 'gelu' (preact needs one), not {activation!r}")
@@ -631,11 +694,19 @@ class FtSgemm:
         if opts is None:
             opts = make_opts(stream=torch.cuda.current_stream(a.device).cuda_stream)
         kA, kB = (b, a) if plan["swap"] else (a, b)
+        if c is not None:
+            if c.stride() != out.stride() or c.data_ptr() % 16 != 0:
+                c = torch.empty_strided(out.shape, out.stride(), device=a.device, dtype=torch.float32).copy_(c)
+            self.run_out(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], kB, plan["layout_b"],
+                         plan["ldb"], c, plan["ldc"], out, alpha, beta, bias, plan["bias_mode"], ACTIVATIONS[activation], preact,
+                         opts)
+            return out
         self.run_act(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], kB, plan["layout_b"],
                      plan["ldb"], out, plan["ldc"], alpha, beta, bias, plan["bias_mode"], ACTIVATIONS[activation], preact, opts)
         return out
 
-    def linear(self, x, weight, bias=None, *, activation=None, kernel_id: int = ID_ABFT_AUTO, opts: Opts | None = None):
+    def linear(self, x, weight, bias=None, *, activation=None, residual=None, kernel_id: int = ID_ABFT_AUTO,
+               opts: Opts | None = None):
         """F.linear(x, weight, bias) = x @ weight.T + bias under ABFT protection, differentiable: x (..., K), weight (N, K),
         bias (N,) or None, all float32 CUDA tensors; returns (..., N).
 
@@ -650,7 +721,13 @@ class FtSgemm:
         activation = "relu" | "gelu" gives F.relu / F.gelu(F.linear(...)) from the same single matmul, the activation fused
         into its store pass.  The pre-activation value is written only where the backward needs it: for GELU, when grad mode
         is on and an input requires grad (ReLU's backward reads y > 0).  Backward: grad_z = threshold_backward(grad_y, y, 0)
-        or gelu_backward(grad_y, z) in torch, then the three gradients as above from grad_z."""
+        or gelu_backward(grad_y, z) in torch, then the three gradients as above from grad_z.
+
+        residual = r, a tensor of the output's shape (..., N): y = (x @ weight.T + r) + bias -- the residual connection of a
+        transformer block -- from the same single matmul (beta = 1, r read in place of the old output and never written),
+        under the same ABFT protection.  The bias is added after the residual, the kernel's order, so y can differ from
+        F.linear(x, weight, bias) + r in the last bits.  y has r's strides when r is dense.  Backward: grad_r = grad_y, the
+        other gradients as above.  A residual with an activation raises ValueError."""
         import torch
         if x.dtype != torch.float32 or not x.is_cuda or x.dim() < 1:
             raise TypeError("x must be a float32 CUDA tensor with at least one dimension")
@@ -659,11 +736,18 @@ class FtSgemm:
         lp = linear_plan(tuple(x.shape), x.stride(), tuple(weight.shape))
         x2 = (x.as_strided((lp["M"], lp["K"]), lp["view"], x.storage_offset()) if lp["view"] is not None
               else x.reshape(lp["M"], lp["K"]).contiguous())
+        r2 = None
+        if residual is not None:
+            if activation is not None:
+                raise ValueError("a residual cannot be combined with an activation")
+            if tuple(residual.shape) != lp["out_shape"] or residual.dtype != torch.float32 or residual.device != x.device:
+                raise ValueError(f"residual must be a float32 {lp['out_shape']} tensor on {x.device}")
+            r2 = residual.reshape(lp["M"], lp["N"])
         fwd = Opts.from_buffer_copy(opts) if opts is not None else make_opts()
         if not fwd.stream:
             fwd.stream = torch.cuda.current_stream(x.device).cuda_stream
         if activation is None:
-            y = _linear_fn().apply(x2, weight, bias, self, kernel_id, fwd)
+            y = _linear_fn().apply(x2, weight, bias, r2, self, kernel_id, fwd)
         else:
             if activation not in ("relu", "gelu"):
                 raise ValueError(f"activation must be None, 'relu' or 'gelu', not {activation!r}")
@@ -758,10 +842,12 @@ def _linear_fn():
 
         class LinearFn(torch.autograd.Function):
             @staticmethod
-            def forward(ctx, x2, weight, bias, dev, kernel_id, opts):
+            def forward(ctx, x2, weight, bias, residual, dev, kernel_id, opts):
                 ctx.save_for_backward(x2, weight)
                 ctx.dev, ctx.kernel_id, ctx.opts = dev, kernel_id, opts
-                return dev.matmul(x2, weight.t(), bias=bias, kernel_id=kernel_id, opts=opts)
+                if residual is None:
+                    return dev.matmul(x2, weight.t(), bias=bias, kernel_id=kernel_id, opts=opts)
+                return dev.matmul(x2, weight.t(), c=residual, bias=bias, kernel_id=kernel_id, beta=1.0, opts=opts)
 
             @staticmethod
             def backward(ctx, gy):
@@ -776,7 +862,7 @@ def _linear_fn():
                     gw = ctx.dev.matmul(gy.t(), x2, kernel_id=ctx.kernel_id, opts=bwd)
                 if ctx.needs_input_grad[2]:
                     gb = gy.sum(0)
-                return gx, gw, gb, None, None, None
+                return gx, gw, gb, gy if ctx.needs_input_grad[3] else None, None, None, None
 
         _LINEAR_FN = LinearFn
     return _LINEAR_FN
@@ -839,13 +925,14 @@ def _bmm_fn():
 
         class BmmFn(torch.autograd.Function):
             @staticmethod
-            def forward(ctx, a, b, bias, preact, dev, kernel_id, alpha, opts, activation):
+            def forward(ctx, a, b, bias, preact, c, dev, kernel_id, alpha, beta, opts, activation):
                 z = preact
                 if z is None and activation == "gelu":
                     z = torch.empty(a.shape[0], a.shape[1], b.shape[2], device=a.device, dtype=torch.float32)
-                y = dev.bmm(a, b, bias=bias, activation=activation, preact=z, kernel_id=kernel_id, alpha=alpha, opts=opts)
+                y = dev.bmm(a, b, c=c, bias=bias, activation=activation, preact=z, kernel_id=kernel_id, alpha=alpha,
+                            beta=beta if c is not None else 0.0, opts=opts)
                 ctx.save_for_backward(a, b, y if activation == "relu" else z)
-                ctx.dev, ctx.kernel_id, ctx.alpha, ctx.opts, ctx.activation = dev, kernel_id, alpha, opts, activation
+                ctx.dev, ctx.kernel_id, ctx.alpha, ctx.beta, ctx.opts, ctx.activation = dev, kernel_id, alpha, beta, opts, activation
                 ctx.per_entry_bias = bias is not None and bias.dim() == 2
                 return y
 
@@ -861,14 +948,16 @@ def _bmm_fn():
                 bwd = Opts.from_buffer_copy(ctx.opts)
                 bwd.inject_mode, bwd.n_faults = 0, 0
                 bwd.stream = torch.cuda.current_stream(gy.device).cuda_stream
-                ga = gb = gbias = None
+                ga = gb = gbias = gc = None
                 if ctx.needs_input_grad[0]:
                     ga = ctx.dev.bmm(gz, b.transpose(1, 2), kernel_id=ctx.kernel_id, alpha=ctx.alpha, opts=bwd)
                 if ctx.needs_input_grad[1]:
                     gb = ctx.dev.bmm(a.transpose(1, 2), gz, kernel_id=ctx.kernel_id, alpha=ctx.alpha, opts=bwd)
                 if ctx.needs_input_grad[2]:
                     gbias = gz.sum(1) if ctx.per_entry_bias else gz.sum((0, 1))
-                return ga, gb, gbias, None, None, None, None, None, None
+                if ctx.needs_input_grad[4]:
+                    gc = ctx.beta * gz
+                return ga, gb, gbias, None, gc, None, None, None, None, None, None
 
         _BMM_FN = BmmFn
     return _BMM_FN

@@ -4,6 +4,7 @@ from __future__ import annotations
 import os
 import subprocess
 import sys
+import tempfile
 from pathlib import Path
 
 HERE = Path(__file__).resolve().parent
@@ -28,15 +29,28 @@ def _stale(target: Path, sources) -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> None:
-    lib_src = [CSRC / "ftsgemm.cu"]
+    # two translation units compiled at the same time (their device compilation is single-threaded up to ptxas): the library
+    # and the OUT kernels of ftsgemm_run_batched_out (ftsgemm_out.cu); then one link
+    lib_src = [CSRC / "ftsgemm.cu", CSRC / "ftsgemm_out.cu"]
     lib_dep = lib_src + sorted(CSRC.glob("*.cuh")) + sorted(CSRC.glob("*.h")) + [ROOT / "include" / "ftsgemm.h"]
     if force or _stale(LIB, lib_dep):
-        cmd = [NVCC, *ARCH, *COMMON, *PTXAS_THREADS, "-shared", "-Xptxas", "-v", *map(str, lib_src), "-o", str(LIB), "-lcublas"]
-        out = subprocess.run(cmd, capture_output=True, text=True)
-        (HERE / "build_ptxas.log").write_text(out.stderr)
-        if verbose or out.returncode != 0:
-            print(out.stdout, out.stderr, file=sys.stderr)
-        if out.returncode != 0:
+        with tempfile.TemporaryDirectory() as tmp:
+            objs = [Path(tmp) / (src.stem + ".o") for src in lib_src]
+            procs = [subprocess.Popen([NVCC, *ARCH, *COMMON, *PTXAS_THREADS, "-c", "-Xptxas", "-v", str(src), "-o", str(obj)],
+                                      stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True)
+                     for src, obj in zip(lib_src, objs)]
+            outs = [p.communicate() for p in procs]
+            err = "".join(e for _, e in outs)
+            rc = max(p.returncode for p in procs)
+            if rc == 0:
+                link = subprocess.run([NVCC, *ARCH, "-ccbin", "/usr/bin/g++", "-shared", *map(str, objs), "-o", str(LIB),
+                                       "-lcublas"], capture_output=True, text=True)
+                err += link.stderr
+                rc = link.returncode
+        (HERE / "build_ptxas.log").write_text(err)
+        if verbose or rc != 0:
+            print("".join(o for o, _ in outs), err, file=sys.stderr)
+        if rc != 0:
             raise RuntimeError("nvcc failed building libftsgemm.so")
     cli_src = CSRC / "ft_sgemm_main.cu"
     if cli_src.exists() and (force or _stale(CLI, [cli_src, LIB])):

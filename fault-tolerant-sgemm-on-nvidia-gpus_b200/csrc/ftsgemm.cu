@@ -141,6 +141,7 @@ struct ftsgemm_handle_s {
   cublasHandle_t cublas = nullptr;
   EncodeTiledFn encode_tiled = nullptr;
   DeviceStats *d_stats = nullptr;
+  bool out_launched = false;    // an OUT kernel (ftsgemm_out.cu: its own abort flag) has run through the handle
   DevBuf d_chk;                 // encoded checksum vectors [K][tiles_n*8]  (extra "rows" of B)
   DevBuf d_chk_out;             // slab flags, then the expected checksums M x (tiles_n*8), column-major
   size_t chk_flag_bytes = kChkFlagBytes;  // bytes of d_chk_out in front of the expected checksums: the slab flags
@@ -237,9 +238,11 @@ struct DeviceGuard {
 
 // The kernels' watchdog (ptx.cuh) raises a device-wide flag instead of trapping; reported once, then cleared.
 int check_abort_flag(ftsgemm_handle_t h) {
-  int flag = 0;
+  int flag = 0, out_flag = 0;
   FT_CUDA(h, cudaMemcpyFromSymbol(&flag, ptx::g_abort_flag, sizeof(int)));
-  if (flag == 0) return FTSGEMM_OK;
+  // (the OUT kernels' translation unit has its own copy, read once one of them has run through this handle)
+  if (h->out_launched) FT_CUDA(h, tc_out_abort_flag(&out_flag));
+  if (flag == 0) return out_flag == 0 ? FTSGEMM_OK : FTSGEMM_ERR_TIMEOUT;
   flag = 0;
   FT_CUDA(h, cudaMemcpyToSymbol(ptx::g_abort_flag, &flag, sizeof(int)));
   return FTSGEMM_ERR_TIMEOUT;
@@ -309,12 +312,19 @@ int query_max_units(ftsgemm_handle_t h, int *out) {
   return FTSGEMM_OK;
 }
 
-template <int BN, bool FT, int CG, bool PROT, bool SEED, bool BIAS, bool BATCH, bool ACT = false>
+template <int BN, bool FT, int CG, bool PROT, bool SEED, bool BIAS, bool BATCH, bool ACT = false, bool OUT = false>
 int launch_tc(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
               const KernelParams &p, int units, cudaStream_t stream) {
   // p.pdl_wait: the launch may overlap the tail of its predecessor in the stream (KernelParams::pdl_wait)
   using Cfg = TileCfg<BN, FT, CG>;
-  auto kern = ftsgemm_tc_kernel<BN, FT, CG, PROT, SEED, BIAS, BATCH, ACT>;
+  TcKernel kern;
+  if constexpr (OUT) {  // (compiled in ftsgemm_out.cu)
+    kern = tc_out_kernel(BN, CG, FT, PROT, SEED, BATCH);
+    if (!kern) return FTSGEMM_ERR_UNSUPPORTED;
+    h->out_launched = true;
+  } else {
+    kern = ftsgemm_tc_kernel<BN, FT, CG, PROT, SEED, BIAS, BATCH, ACT>;
+  }
   int resident = 0;
   const int qrc = query_max_units<BN, FT, CG, PROT>(h, &resident);
   if (qrc) return qrc;
@@ -369,16 +379,18 @@ int with_flag(bool b, F &&f) {
 // The kernel instantiation of a launch: SEED for a plan with cut tiles, BIAS for a bias (KernelParams::bias,
 // ftsgemm_tc_kernel), BATCH for a batch of more than one entry, PROT (fault-tolerant kernels only) for opts.protect_epilogue.
 // An activation (the bias mode is then a run-time field) selects the ACT kernels instead of BIAS: with BATCH for a batch of
-// more than one entry.
+// more than one entry.  A separate output D (p.d, with or without an activation) selects the OUT form of the ACT kernels.
 template <int BN, int CG>
 int launch_variant(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
                    const KernelParams &p, int units, cudaStream_t stream, bool ft, bool prot) {
-  if (p.act != kActNone) {
+  if (p.act != kActNone || p.d != nullptr) {
     return with_flag(p.sk_tiles > 0, [&](auto seed) {
       return with_flag(p.batch > 1, [&](auto batch) {
-        if (!ft) return launch_tc<BN, false, CG, false, seed, false, batch, true>(h, tmA, tmB, tmC, p, units, stream);
-        if (prot) return launch_tc<BN, true, CG, true, seed, false, batch, true>(h, tmA, tmB, tmC, p, units, stream);
-        return launch_tc<BN, true, CG, false, seed, false, batch, true>(h, tmA, tmB, tmC, p, units, stream);
+        return with_flag(p.d != nullptr, [&](auto out) {
+          if (!ft) return launch_tc<BN, false, CG, false, seed, false, batch, true, out>(h, tmA, tmB, tmC, p, units, stream);
+          if (prot) return launch_tc<BN, true, CG, true, seed, false, batch, true, out>(h, tmA, tmB, tmC, p, units, stream);
+          return launch_tc<BN, true, CG, false, seed, false, batch, true, out>(h, tmA, tmB, tmC, p, units, stream);
+        });
       });
     });
   }
@@ -590,7 +602,7 @@ int check_tc_args(const Variant &v, int M, int N, int K, const Operand &A, const
 // The kernel parameters that follow from the call's arguments and options (the tile grid and work plan come later).
 KernelParams make_params(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B,
                          float *dC, int ldc, float alpha, float beta, const float *bias, int bias_mode,
-                         const ftsgemm_opts &o, const BatchArg &batch_arg, const ActArg &act) {
+                         const ftsgemm_opts &o, const BatchArg &batch_arg, const ActArg &act, float *dD) {
   const bool ft = v.info.fault_tolerant != 0;
   // (one entry runs the kernels without BATCH, on 2-D tensor maps; its strides are ignored)
   const BatchArg bt = batch_arg.count > 1 ? batch_arg : kSingle;
@@ -601,6 +613,7 @@ KernelParams make_params(ftsgemm_handle_t h, const Variant &v, int M, int N, int
   p.alpha = alpha; p.beta = beta;
   p.bias = bias; p.bias_mode = bias_mode;
   p.act = act.kind; p.z = act.z;
+  p.d = dD;
   p.batch = bt.count;
   p.stride_a = bt.sa;
   p.stride_b = bt.sb;
@@ -854,13 +867,13 @@ int bind_plan(ftsgemm_handle_t h, const Variant &v, KernelParams &p, const PlanI
 }
 
 // One product on the wgmma kernels, in stages: argument checks, kernel parameters, operands, launch plan, checksums, cached
-// work plan, per-plan workspaces, launch.
+// work plan, per-plan workspaces, launch.  dD: a separate output (C read-only), null in place.
 int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC, int ldc,
            float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o, cudaStream_t stream,
-           const BatchArg &bt = kSingle, const ActArg &act = kNoAct) {
+           const BatchArg &bt = kSingle, const ActArg &act = kNoAct, float *dD = nullptr) {
   int rc = check_tc_args(v, M, N, K, A, B, dC, bt.count);
   if (rc) return rc;
-  KernelParams p = make_params(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, bt, act);
+  KernelParams p = make_params(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, bt, act, dD);
   CUtensorMap tmA, tmB, tmC;
   PlanInput pin;
   if ((rc = bind_operands(h, v, p, &tmA, &tmB)) || (rc = plan_on_device(h, v, p, &pin))) return rc;
@@ -1046,10 +1059,11 @@ int run_baseline(ftsgemm_handle_t h, int M, int N, int K, const float *dA, const
 // x = hi + lo (hi = the 11 significant bits the tensor core reads, lo = x - hi exactly),
 //   A B^T ~= A_lo B_hi^T + A_hi B_lo^T + A_hi B_hi^T       (A_lo B_lo^T ~ 2^-22 relative is dropped)
 // as three launches of the same kernel, smallest terms first, each accumulating into C -- every one of them a
-// complete fault-tolerant GEMM with its own checksum vectors, so ABFT covers the whole 3-pass product.
+// complete fault-tolerant GEMM with its own checksum vectors, so ABFT covers the whole 3-pass product.  With a separate
+// output D only the first pass reads C; the other two accumulate into D in place.
 int run_3xtf32(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC,
                int ldc, float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o,
-               cudaStream_t stream, const BatchArg &bt, const ActArg &act) {
+               cudaStream_t stream, const BatchArg &bt, const ActArg &act, float *dD) {
   // (before the split kernels read the operands with 16-byte loads)
   int rc = check_tc_args(v, M, N, K, A, B, dC, bt.count);
   if (rc) return rc;
@@ -1095,30 +1109,32 @@ int run_3xtf32(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const 
   o_quiet.inject_mode = 0;
   // (the bias and the activation go to the last pass only: applied once, after the final alpha*acc + C)
   const BatchArg lo = {bt.count, static_cast<long long>(a_floats), static_cast<long long>(b_floats), bt.sc, 0};
-  rc = run_tc(h, v, M, N, K, Alo, Bs, dC, ldc, alpha, beta, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo);
-  if (!rc) rc = run_tc(h, v, M, N, K, As, Blo, dC, ldc, alpha, 1.0f, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo);
-  if (!rc) rc = run_tc(h, v, M, N, K, A, B, dC, ldc, alpha, 1.0f, bias, bias_mode, o3, stream, bt, act);
+  float *const out = dD ? dD : dC;
+  rc = run_tc(h, v, M, N, K, Alo, Bs, dC, ldc, alpha, beta, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo, kNoAct, dD);
+  if (!rc) rc = run_tc(h, v, M, N, K, As, Blo, out, ldc, alpha, 1.0f, nullptr, FTSGEMM_BIAS_NONE, o_quiet, stream, lo);
+  if (!rc) rc = run_tc(h, v, M, N, K, A, B, out, ldc, alpha, 1.0f, bias, bias_mode, o3, stream, bt, act);
   return rc;
 }
 
 int run_resolved(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC,
                  int ldc, float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o,
-                 cudaStream_t stream, const BatchArg &bt, const ActArg &act = kNoAct);
+                 cudaStream_t stream, const BatchArg &bt, const ActArg &act = kNoAct, float *dD = nullptr);
 
 // Intra-K checking (ftsgemm_opts::check_segments): S consecutive K-segments, each a complete fault-tolerant GEMM.  A
 // segment of an operand is a pointer offset: k0 * ld for an MN-major operand (k is the slow index), k0 for a K-major one;
 // segment boundaries are multiples of the stage depth (32 k-rows), so the offsets keep 16-byte alignment.  Injected
 // faults (tests) go to the first segment only, the bias and the activation to the last one (applied once, after the final
-// alpha*acc + C).
+// alpha*acc + C).  With a separate output D only the first segment reads C; the others accumulate into D in place.
 int run_segments(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC,
                  int ldc, float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o,
-                 cudaStream_t stream, const BatchArg &bt, const ActArg &act) {
+                 cudaStream_t stream, const BatchArg &bt, const ActArg &act, float *dD) {
   const int num_kb = (K + kBK - 1) / kBK;
   const int S = std::min(o.check_segments, num_kb);
   ftsgemm_opts os = o;
   os.check_segments = 1;
   os.reuse_b_checksums = 0;
   int rc = FTSGEMM_OK;
+  float *const out = dD ? dD : dC;
   for (int sg = 0; sg < S && !rc; ++sg) {
     const int k0 = static_cast<int>(static_cast<long long>(num_kb) * sg / S) * kBK;
     const int k1 = std::min(K, static_cast<int>(static_cast<long long>(num_kb) * (sg + 1) / S) * kBK);
@@ -1127,24 +1143,25 @@ int run_segments(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, cons
     const Operand As = {A.p + (A.kmajor ? static_cast<size_t>(k0) : static_cast<size_t>(k0) * A.ld), A.kmajor, A.ld};
     const Operand Bs = {B.p + (B.kmajor ? static_cast<size_t>(k0) : static_cast<size_t>(k0) * B.ld), B.kmajor, B.ld};
     const bool last = sg == S - 1;
-    rc = run_resolved(h, v, M, N, k1 - k0, As, Bs, dC, ldc, alpha, sg == 0 ? beta : 1.0f, last ? bias : nullptr,
-                      last ? bias_mode : FTSGEMM_BIAS_NONE, os, stream, bt, last ? act : kNoAct);
+    rc = run_resolved(h, v, M, N, k1 - k0, As, Bs, sg == 0 ? dC : out, ldc, alpha, sg == 0 ? beta : 1.0f, last ? bias : nullptr,
+                      last ? bias_mode : FTSGEMM_BIAS_NONE, os, stream, bt, last ? act : kNoAct, sg == 0 ? dD : nullptr);
   }
   return rc;
 }
 
 // One call of ftsgemm_run_batched after validation: its variant resolved (ids 20 / 40 chosen per shape), its options
-// loaded and h->capturing set.
+// loaded and h->capturing set.  dD (a separate output, wgmma ids only) is null in place.
 int run_resolved(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC,
                  int ldc, float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o,
-                 cudaStream_t stream, const BatchArg &bt, const ActArg &act) {
+                 cudaStream_t stream, const BatchArg &bt, const ActArg &act, float *dD) {
   const bool tc = v.info.engine == 1;
   if (tc && o.check_segments > 1 && v.info.fault_tolerant)
-    return run_segments(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt, act);
-  if (tc && o.precision == 1) return run_3xtf32(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt, act);
+    return run_segments(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt, act, dD);
+  if (tc && o.precision == 1)
+    return run_3xtf32(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt, act, dD);
   switch (v.info.engine) {
     case 0: return run_cublas(h, v.info.id == 7, M, N, K, A, B, dC, ldc, alpha, beta, stream, bt);
-    case 1: return run_tc(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt, act);
+    case 1: return run_tc(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt, act, dD);
     case 2:
       // the non-fused baseline keeps the reference's call sequence, on the reference layout only
       if (A.kmajor || B.kmajor || A.ld != M || B.ld != N || ldc != M) return FTSGEMM_ERR_UNSUPPORTED;
@@ -1367,14 +1384,22 @@ int ftsgemm_run_bias(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, con
                              bias_mode, opts);
 }
 
-// ftsgemm_run_batched_act (and through it every run entry point): validation, options, capture state, variant; then
-// run_resolved.
+// [p, p + n floats) and [q, q + n floats) share an address
+static bool overlaps(const float *p, const float *q, long long n) {
+  const uintptr_t a = reinterpret_cast<uintptr_t>(p), b = reinterpret_cast<uintptr_t>(q), bytes = static_cast<uintptr_t>(n) * 4u;
+  return a < b + bytes && b < a + bytes;
+}
+
+// ftsgemm_run_batched_out (and through it every run entry point): validation, options, capture state, variant; then
+// run_resolved.  dD == dC is the in-place call.
 static int run_call(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
-                    long long stride_a, const float *dB, int layout_b, int ldb, long long stride_b, float *dC, int ldc,
-                    long long stride_c, int batch, float alpha, float beta, const float *bias, int bias_mode,
+                    long long stride_a, const float *dB, int layout_b, int ldb, long long stride_b, const float *dC, int ldc,
+                    long long stride_c, float *dD, int batch, float alpha, float beta, const float *bias, int bias_mode,
                     long long stride_bias, const ActArg &act, const ftsgemm_opts *opts) {
   if (!h) return FTSGEMM_ERR_NO_DEVICE;
-  if (!dA || !dB || !dC || M <= 0 || N <= 0 || K <= 0 || batch < 1) return FTSGEMM_ERR_INVALID_ARG;
+  const bool sep = dD != dC;  // a separate output: C is read-only, and not read at all with beta == 0 (may be null)
+  if (!dA || !dB || !dD || (!dC && !(sep && beta == 0.0f)) || M <= 0 || N <= 0 || K <= 0 || batch < 1)
+    return FTSGEMM_ERR_INVALID_ARG;
   const Variant *v = find_variant(kernel_id);
   if (!v) return FTSGEMM_ERR_INVALID_ARG;
   if ((layout_a != FTSGEMM_LAYOUT_MN_MAJOR && layout_a != FTSGEMM_LAYOUT_K_MAJOR) ||
@@ -1398,6 +1423,19 @@ static int run_call(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, cons
       return FTSGEMM_ERR_INVALID_ARG;
     if (stride_c < static_cast<long long>(ldc) * N) return FTSGEMM_ERR_INVALID_ARG;
   }
+  // C (the old values), D (the results) and Z: with D != C the kernels read C while they write D and Z
+  float *dOld = dD, *dSep = nullptr;
+  if (sep) {
+    if (v->info.engine != 1) return FTSGEMM_ERR_UNSUPPORTED;  // only the wgmma kernels store to a separate output
+    if (reinterpret_cast<uintptr_t>(dD) & 15) return FTSGEMM_ERR_INVALID_ARG;
+    const long long span = (batch > 1 ? (batch - 1) * stride_c : 0) + static_cast<long long>(N - 1) * ldc + M;
+    if (dC && overlaps(dC, dD, span)) return FTSGEMM_ERR_INVALID_ARG;
+    if (act.z && (overlaps(act.z, dD, span) || (dC && overlaps(act.z, dC, span)))) return FTSGEMM_ERR_INVALID_ARG;
+    if (beta != 0.0f) {  // (beta == 0: the in-place call on D)
+      dOld = const_cast<float *>(dC);  // (read only: the kernels store to dSep)
+      dSep = dD;
+    }
+  }
   ftsgemm_opts o;
   const int orc = load_opts(opts, &o);
   if (orc) return orc;
@@ -1415,7 +1453,7 @@ static int run_call(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, cons
     v = find_variant(select_variant(M, N, v->info.fault_tolerant != 0, bt.count));
     if (!v) return FTSGEMM_ERR_UNSUPPORTED;
   }
-  return run_resolved(h, *v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt, act);
+  return run_resolved(h, *v, M, N, K, A, B, dOld, ldc, alpha, beta, bias, bias_mode, o, stream, bt, act, dSep);
 }
 
 int ftsgemm_run_batched(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
@@ -1437,11 +1475,27 @@ int ftsgemm_run_batched_act(ftsgemm_handle_t h, int kernel_id, int M, int N, int
                             long long stride_a, const float *dB, int layout_b, int ldb, long long stride_b, float *dC, int ldc,
                             long long stride_c, int batch, float alpha, float beta, const float *bias, int bias_mode,
                             long long stride_bias, int activation, float *dZ, const ftsgemm_opts *opts) {
+  return ftsgemm_run_batched_out(h, kernel_id, M, N, K, dA, layout_a, lda, stride_a, dB, layout_b, ldb, stride_b, dC, ldc, stride_c,
+                                 dC, batch, alpha, beta, bias, bias_mode, stride_bias, activation, dZ, opts);
+}
+
+int ftsgemm_run_out(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
+                    const float *dB, int layout_b, int ldb, const float *dC, int ldc, float *dD, float alpha, float beta,
+                    const float *bias, int bias_mode, int activation, float *dZ, const ftsgemm_opts *opts) {
+  return ftsgemm_run_batched_out(h, kernel_id, M, N, K, dA, layout_a, lda, 0, dB, layout_b, ldb, 0, dC, ldc, 0, dD, 1, alpha, beta,
+                                 bias, bias_mode, 0, activation, dZ, opts);
+}
+
+int ftsgemm_run_batched_out(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
+                            long long stride_a, const float *dB, int layout_b, int ldb, long long stride_b, const float *dC,
+                            int ldc, long long stride_c, float *dD, int batch, float alpha, float beta, const float *bias,
+                            int bias_mode, long long stride_bias, int activation, float *dZ, const ftsgemm_opts *opts) {
   if (!h) return FTSGEMM_ERR_NO_DEVICE;
   if (activation < FTSGEMM_ACT_NONE || activation > FTSGEMM_ACT_GELU) return FTSGEMM_ERR_INVALID_ARG;
-  if (dZ && (activation == FTSGEMM_ACT_NONE || dZ == dC || (reinterpret_cast<uintptr_t>(dZ) & 3))) return FTSGEMM_ERR_INVALID_ARG;
-  return run_call(h, kernel_id, M, N, K, dA, layout_a, lda, stride_a, dB, layout_b, ldb, stride_b, dC, ldc, stride_c, batch, alpha,
-                  beta, bias, bias_mode, stride_bias, ActArg{activation, dZ}, opts);
+  if (dZ && (activation == FTSGEMM_ACT_NONE || dZ == dC || dZ == dD || (reinterpret_cast<uintptr_t>(dZ) & 3)))
+    return FTSGEMM_ERR_INVALID_ARG;
+  return run_call(h, kernel_id, M, N, K, dA, layout_a, lda, stride_a, dB, layout_b, ldb, stride_b, dC, ldc, stride_c, dD, batch,
+                  alpha, beta, bias, bias_mode, stride_bias, ActArg{activation, dZ}, opts);
 }
 
 int ftsgemm_get_stats(ftsgemm_handle_t h, ftsgemm_stats *out) {

@@ -191,6 +191,10 @@ struct KernelParams {
   // Per-entry bias of a strided batch (ftsgemm_run_batched_act; read by the BATCH instantiations only): entry i adds
   // bias + i*stride_bias.  0 for a bias shared by all entries and for every single product.
   long long stride_bias;
+  // Separate output D (ftsgemm_run_out, ftsgemm_run_batched_out; read by the OUT instantiations only): every final value
+  // reads its old value from C and is stored to D (C's geometry: ldc, entry i at d + i*stride_c); C is not written.  Null:
+  // in place.
+  float *d;
 };
 
 __device__ __forceinline__ unsigned long long globaltimer_ns() { return ptx::globaltimer(); }
@@ -395,22 +399,29 @@ __device__ __forceinline__ BiasRef make_bias(const float *p, int mode, int m, bo
 // NaN; gelu with approximate='none', the exact erf form).  The bias of an ACT kernel is a run-time mode: NONE skips the add
 // (-0 + 0 would be +0), so z is bit for bit what the BIAS / plain kernel stores.  z is written to zrow[off] when zrow is
 // set (Z + m: the pre-activation value the GELU backward needs).
+// OUT (the ACT code with a separate output D): the value is stored to drow (D + m), its old value read from C + m, and
+// NONE is the identity -- a call with D and no activation runs these kernels too.
 constexpr int kActNone = 0, kActRelu = 1, kActGelu = 2;
 struct ActRef {
   int kind;
   float *zrow;  // Z + m, or null
+  float *drow;  // D + m (OUT only)
 };
+template <bool OUT = false>
 __device__ __forceinline__ float act_apply(int kind, float z) {
+  if (OUT && kind == kActNone) return z;
   if (kind == kActRelu) return isnan(z) ? z : fmaxf(z, 0.0f);
   return z * 0.5f * (1.0f + erff(z * 0.707106781186547524f));  // (float)M_SQRT1_2
 }
 // z = x (+ b), stored to Z when requested; returns act(z)  (one element: the ragged-N and recompute paths)
+template <bool OUT = false>
 __device__ __forceinline__ float act_value(float x, const BiasRef &bias, int n, const ActRef &act, size_t off) {
   if (bias.mode != kBiasNone) x = __fadd_rn(x, bias.at(n));
   if (act.zrow != nullptr) act.zrow[off] = x;
-  return act_apply(act.kind, x);
+  return act_apply<OUT>(act.kind, x);
 }
 // the same for the 32 columns [nb, nb + 32) of one chunk, the warp-uniform branches taken once per chunk, not per element
+template <bool OUT = false>
 __device__ __forceinline__ void act_chunk(uint32_t (&v)[32], const BiasRef &bias, int nb, const ActRef &act, int ldc) {
   if (bias.mode != kBiasNone) {
 #pragma unroll
@@ -423,27 +434,34 @@ __device__ __forceinline__ void act_chunk(uint32_t (&v)[32], const BiasRef &bias
   if (act.kind == kActRelu) {
 #pragma unroll
     for (int i = 0; i < 32; ++i) v[i] = f2u(act_apply(kActRelu, u2f(v[i])));
-  } else {
+  } else if (!OUT || act.kind == kActGelu) {
 #pragma unroll
     for (int i = 0; i < 32; ++i) v[i] = f2u(act_apply(kActGelu, u2f(v[i])));
   }
 }
 template <bool ACT>
 __device__ __forceinline__ ActRef act_of(const KernelParams &p, int m) {
-  if constexpr (ACT) return ActRef{p.act, p.z != nullptr ? p.z + m : nullptr};
-  else return ActRef{kActNone, nullptr};
+  if constexpr (ACT) return ActRef{p.act, p.z != nullptr ? p.z + m : nullptr, nullptr};
+  else return ActRef{kActNone, nullptr, nullptr};
 }
 // (strided batch: Z is the entry's, null when not written)
 template <bool ACT>
 __device__ __forceinline__ ActRef act_of_entry(const KernelParams &p, float *Z, int m) {
-  if constexpr (ACT) return ActRef{p.act, Z != nullptr ? Z + m : nullptr};
-  else return ActRef{kActNone, nullptr};
+  if constexpr (ACT) return ActRef{p.act, Z != nullptr ? Z + m : nullptr, nullptr};
+  else return ActRef{kActNone, nullptr, nullptr};
+}
+// (OUT: the output row D + m as well)
+template <bool OUT>
+__device__ __forceinline__ ActRef with_out(ActRef a, float *D, int m) {
+  if constexpr (OUT) a.drow = D + m;
+  return a;
 }
 
-template <int BN, bool BIAS = false, bool ACT = false>
+template <int BN, bool BIAS = false, bool ACT = false, bool OUT = false>
 __device__ __forceinline__ void store_tile(uint32_t taddr, float *crow, bool row_ok, int n0, int n_limit, int ldc,
                                            float alpha, float beta, int c_begin = 0, int c_end = BN / 32, BiasRef bias = {},
                                            ActRef act = {}) {
+  float *const drow = OUT ? act.drow : crow;  // (OUT: the old values come from C, the results go to D)
   const bool full_n = (n0 + BN <= n_limit);
   if (full_n && beta != 0.0f) {
     // Software pipeline: the old values of chunk c + 1 are fetched while chunk c is stored (a chunk's 32 loads would
@@ -465,13 +483,13 @@ __device__ __forceinline__ void store_tile(uint32_t taddr, float *crow, bool row
           v[i] = f2u(alpha * u2f(v[i]) + beta * old[i]);
           if constexpr (BIAS) v[i] = f2u(__fadd_rn(u2f(v[i]), bias.at(nb + i)));
         }
-        if constexpr (ACT) act_chunk(v, bias, nb, act, ldc);
+        if constexpr (ACT) act_chunk<OUT>(v, bias, nb, act, ldc);
         if (c + 1 < c_end) {
 #pragma unroll
           for (int i = 0; i < 32; ++i) old[i] = crow[static_cast<size_t>(nb + 32 + i) * ldc];
         }
 #pragma unroll
-        for (int i = 0; i < 32; ++i) crow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
+        for (int i = 0; i < 32; ++i) drow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
       }
     }
     return;
@@ -486,9 +504,9 @@ __device__ __forceinline__ void store_tile(uint32_t taddr, float *crow, bool row
       if constexpr (ACT) {
 #pragma unroll
         for (int i = 0; i < 32; ++i) v[i] = f2u(alpha * u2f(v[i]));
-        act_chunk(v, bias, nb, act, ldc);
+        act_chunk<OUT>(v, bias, nb, act, ldc);
 #pragma unroll
-        for (int i = 0; i < 32; ++i) crow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
+        for (int i = 0; i < 32; ++i) drow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
       } else {
 #pragma unroll
         for (int i = 0; i < 32; ++i) {
@@ -505,7 +523,8 @@ __device__ __forceinline__ void store_tile(uint32_t taddr, float *crow, bool row
           const float o = (beta == 0.0f) ? 0.0f : beta * (*dst);
           float x = alpha * u2f(v[i]) + o;
           if constexpr (BIAS) x = __fadd_rn(x, bias.at(nb + i));
-          if constexpr (ACT) x = act_value(x, bias, nb + i, act, static_cast<size_t>(nb + i) * ldc);
+          if constexpr (ACT) x = act_value<OUT>(x, bias, nb + i, act, static_cast<size_t>(nb + i) * ldc);
+          if constexpr (OUT) dst = drow + static_cast<size_t>(nb + i) * ldc;
           *dst = x;
         }
       }
@@ -797,7 +816,7 @@ struct StoreVerdict {
 // ACT: the pass verifies z -- the values it sums are the pre-activation values, with the run-time bias in sum(b) as above
 // -- and then stores act(z) to C and z to Z.  The activation's own arithmetic is elementwise and nonlinear: no linear
 // checksum covers it, so an upset inside it or after it is not detected.
-template <int BN, bool BIAS, bool ACT = false>
+template <int BN, bool BIAS, bool ACT = false, bool OUT = false>
 __device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, float *crow, bool row_ok, int n0, int ldc, float alpha,
                                                           float beta, int c_begin, int c_end, float chk_s1, bool chk_s1_valid,
                                                           int bad_col, uint32_t bad_mask, const BiasRef &bias, ActRef act = {}) {
@@ -873,13 +892,14 @@ __device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, flo
         if (act.kind == kActRelu) {
 #pragma unroll
           for (int i = 0; i < 32; ++i) v[i] = f2u(act_apply(kActRelu, u2f(v[i])));
-        } else {
+        } else if (!OUT || act.kind == kActGelu) {
 #pragma unroll
           for (int i = 0; i < 32; ++i) v[i] = f2u(act_apply(kActGelu, u2f(v[i])));
         }
       }
+      float *const drow = OUT ? act.drow : crow;
 #pragma unroll
-      for (int i = 0; i < 32; ++i) crow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
+      for (int i = 0; i < 32; ++i) drow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
     }
   }
   float ref = alpha * s1 + beta * (sold0 + sold1);
@@ -904,11 +924,11 @@ __device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, flo
 // kmajor: bit 0 = A is K-major, bit 1 = B is K-major.
 // ------------------------------------------------------------------------------------------------------------
 // (scalars by value: a reference to the __grid_constant__ parameter block would force a local copy of all of it)
-// ACT: the bias mode is read at run time and the row is stored as act(z), with z into Z (when not null).
-template <int BN, bool BIAS, bool ACT = false>
+// ACT: the bias mode is read at run time and the row is stored as act(z), with z into Z (when not null); OUT: to D.
+template <int BN, bool BIAS, bool ACT = false, bool OUT = false>
 __device__ __forceinline__ void recompute_row_body(const float *A, const float *B, float *C, int lda, int ldb, int kmajor, int ldc,
                                                    int N, int K, float alpha, float beta, int m, int n0, int lane, const float *bias,
-                                                   int bias_mode, int act_kind = kActNone, float *Z = nullptr) {
+                                                   int bias_mode, int act_kind = kActNone, float *Z = nullptr, float *D = nullptr) {
   constexpr int J = BN / 32;
   float acc[J];
 #pragma unroll
@@ -939,7 +959,8 @@ __device__ __forceinline__ void recompute_row_body(const float *A, const float *
       if constexpr (ACT) {
         if (bias_mode != kBiasNone) x = __fadd_rn(x, __ldg(bias + (bias_mode == kBiasRow ? m : n)));
         if (Z != nullptr) Z[m + static_cast<size_t>(n) * ldc] = x;
-        x = act_apply(act_kind, x);
+        x = act_apply<OUT>(act_kind, x);
+        if constexpr (OUT) dst = D + m + static_cast<size_t>(n) * ldc;
       }
       *dst = x;
     }
@@ -966,9 +987,19 @@ __device__ __noinline__ void recompute_row_act(const float *A, const float *B, f
                                                int bias_mode, int act_kind, float *Z) {
   recompute_row_body<BN, false, true>(A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, m, n0, lane, bias, bias_mode, act_kind, Z);
 }
-template <int BN, bool BIAS, bool ACT = false, bool ENTRY = false, typename... Args>
-__device__ __forceinline__ void recompute(const float *bias, int bias_mode, int act_kind, float *Z, Args... args) {
-  if constexpr (ACT) recompute_row_act<BN, ENTRY>(args..., bias, bias_mode, act_kind, Z);
+// (the OUT kernels: the row is stored to D; their own entry, so the ACT one keeps its list)
+template <int BN, bool ENTRY = false>
+__device__ __noinline__ void recompute_row_out(const float *A, const float *B, float *C, int lda, int ldb, int kmajor, int ldc,
+                                               int N, int K, float alpha, float beta, int m, int n0, int lane, const float *bias,
+                                               int bias_mode, int act_kind, float *Z, float *D) {
+  recompute_row_body<BN, false, true, true>(A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, m, n0, lane, bias, bias_mode, act_kind,
+                                            Z, D);
+}
+// (D: OUT only, the output the row is stored to)
+template <int BN, bool BIAS, bool ACT = false, bool ENTRY = false, bool OUT = false, typename... Args>
+__device__ __forceinline__ void recompute(const float *bias, int bias_mode, int act_kind, float *Z, float *D, Args... args) {
+  if constexpr (OUT) recompute_row_out<BN, ENTRY>(args..., bias, bias_mode, act_kind, Z, D);
+  else if constexpr (ACT) recompute_row_act<BN, ENTRY>(args..., bias, bias_mode, act_kind, Z);
   else if constexpr (BIAS) recompute_row_bias<BN>(args..., bias, bias_mode);
   else recompute_row<BN>(args...);
 }
@@ -976,20 +1007,22 @@ __device__ __forceinline__ void recompute(const float *bias, int bias_mode, int 
 // The whole protected store pass of one warp, out of line and with scalars by value: an opt-in path must not cost the
 // common epilogue registers (inlined it pushed the kernel into spills), and a reference to the __grid_constant__ parameter
 // block would force a local copy of all of it.  Row segments that fail are counted and, with beta == 0, recomputed from A
-// and B (with beta != 0 the old values of C are already overwritten: reported as uncorrectable).
-template <int BN, bool BIAS, bool ACT = false, bool ENTRY = false>
+// and B (with beta != 0 the old values of C are already overwritten: reported as uncorrectable -- unless the results go
+// to a separate output D (OUT), which leaves C intact: then the segment is recomputed into D whatever beta is).
+template <int BN, bool BIAS, bool ACT = false, bool ENTRY = false, bool OUT = false>
 __device__ __forceinline__ void protected_store_body(uint32_t taddr, const float *A, const float *B, float *C, int lda, int ldb,
                                                      int kmajor, int ldc, int N, int K, float alpha, float beta, DeviceStats *stats,
                                                      bool can_recompute, int m, int row0, bool row_ok, int n0, int c_begin, int c_end,
                                                      float chk_s1, bool chk_s1_valid, int bad_col, uint32_t bad_mask, int lane,
                                                      const float *bias, int bias_mode, int row_ofs, int act_kind = kActNone,
-                                                     float *Z = nullptr) {
-  const StoreVerdict sv = store_tile_protected<BN, BIAS, ACT>(
+                                                     float *Z = nullptr, float *D = nullptr) {
+  const StoreVerdict sv = store_tile_protected<BN, BIAS, ACT, OUT>(
       taddr, C + m, row_ok, n0, ldc, alpha, beta, c_begin, c_end, chk_s1, chk_s1_valid, bad_col, bad_mask,
-      make_bias(bias, bias_mode, m, (BIAS || ACT) && row_ok), ActRef{act_kind, (ACT && Z != nullptr) ? Z + m : nullptr});
+      make_bias(bias, bias_mode, m, (BIAS || ACT) && row_ok),
+      ActRef{act_kind, (ACT && Z != nullptr) ? Z + m : nullptr, OUT ? D + m : nullptr});
   unsigned mask = __ballot_sync(0xffffffffu, sv.bad);
   if (mask == 0u) return;
-  const bool can_fix = beta == 0.0f && can_recompute;
+  const bool can_fix = (beta == 0.0f || (OUT && D != C)) && can_recompute;
   if (sv.bad && stats) {
     atomicAdd(&stats->epilogue_faults, 1ull);
     atomicAdd(can_fix ? &stats->recomputed : &stats->uncorrectable, 1ull);
@@ -1009,12 +1042,12 @@ __device__ __forceinline__ void protected_store_body(uint32_t taddr, const float
     const int r = __ffs(mask) - 1;
     mask &= mask - 1u;
     if (c_end - c_begin == BN / 32) {
-      recompute<BN, BIAS, ACT, ENTRY>(bias, bias_mode, act_kind, Z, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r, n0,
-                                      lane);
+      recompute<BN, BIAS, ACT, ENTRY, OUT>(bias, bias_mode, act_kind, Z, D, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r,
+                                           n0, lane);
     } else {
       if constexpr (BN >= 64)
-        recompute<BN / 2, BIAS, ACT, ENTRY>(bias, bias_mode, act_kind, Z, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r,
-                                     n0 + c_begin * 32, lane);
+        recompute<BN / 2, BIAS, ACT, ENTRY, OUT>(bias, bias_mode, act_kind, Z, D, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta,
+                                                 row0 + r, n0 + c_begin * 32, lane);
     }
   }
 }
@@ -1051,11 +1084,20 @@ __device__ __noinline__ void protected_store_pass_act_batched(FT_PROT_PARAMS, co
                                                              int act_kind, float *Z) {
   protected_store_body<BN, false, true, true>(FT_PROT_ARGS, bias, bias_mode, row_ofs, act_kind, Z);
 }
+// (the OUT kernels, single (ENTRY = false) and batched: the ACT pass storing to D; their own entries, so the ACT ones keep
+// their lists)
+template <int BN, bool ENTRY>
+__device__ __noinline__ void protected_store_pass_out(FT_PROT_PARAMS, const float *bias, int bias_mode, int row_ofs, int act_kind,
+                                                      float *Z, float *D) {
+  protected_store_body<BN, false, true, ENTRY, true>(FT_PROT_ARGS, bias, bias_mode, row_ofs, act_kind, Z, D);
+}
 #undef FT_PROT_PARAMS
 #undef FT_PROT_ARGS
-template <int BN, bool BIAS, bool BATCH, bool ACT, typename... Args>
-__device__ __forceinline__ void protected_store(const float *bias, int bias_mode, int row_ofs, int act_kind, float *Z, Args... args) {
-  if constexpr (ACT && BATCH) protected_store_pass_act_batched<BN>(args..., bias, bias_mode, row_ofs, act_kind, Z);
+template <int BN, bool BIAS, bool BATCH, bool ACT, bool OUT, typename... Args>
+__device__ __forceinline__ void protected_store(const float *bias, int bias_mode, int row_ofs, int act_kind, float *Z, float *D,
+                                                Args... args) {
+  if constexpr (OUT) protected_store_pass_out<BN, BATCH>(args..., bias, bias_mode, row_ofs, act_kind, Z, D);
+  else if constexpr (ACT && BATCH) protected_store_pass_act_batched<BN>(args..., bias, bias_mode, row_ofs, act_kind, Z);
   else if constexpr (ACT) protected_store_pass_act<BN>(args..., bias, bias_mode, act_kind, Z);
   else if constexpr (BATCH) protected_store_pass_batched<BN, BIAS>(args..., bias, bias_mode, row_ofs);
   else if constexpr (BIAS) protected_store_pass_bias<BN>(args..., bias, bias_mode);
@@ -1150,14 +1192,17 @@ __device__ __forceinline__ float chunk_sum(const uint32_t (&v)[32], float &sabs)
   sabs = b0 + b1;
   return a0 + a1;
 }
-// (ENTRY: the ACT x BATCH kernels' own copy, see recompute_row_act)
-template <bool BIAS, bool ACT, bool ENTRY = false>
-__device__ __noinline__ void protected_store_pass_v2(uint32_t taddr, const float *A, const float *B, float *C, int lda, int ldb,
-                                                     int kmajor, int ldc, int N, int K, float alpha, float beta, DeviceStats *stats,
-                                                     bool can_recompute, int m, int row0, bool row_ok, int n0, bool ragged_n,
-                                                     int c_begin, int c_end, float chk_s1, bool chk_s1_valid, StoreUpsets up,
-                                                     int lane,
-                                                     const float *bias, int bias_mode, int row_ofs, int act_kind, float *Z) {
+// The old values are read from C + m and the outputs stored to D + m (D = C but in the OUT kernels' entry).
+#define FT_PROT_V2_PARAMS                                                                                                       \
+  uint32_t taddr, const float *A, const float *B, float *C, int lda, int ldb, int kmajor, int ldc, int N, int K, float alpha,  \
+      float beta, DeviceStats *stats, bool can_recompute, int m, int row0, bool row_ok, int n0, bool ragged_n, int c_begin,    \
+      int c_end, float chk_s1, bool chk_s1_valid, StoreUpsets up, int lane, const float *bias, int bias_mode, int row_ofs,     \
+      int act_kind, float *Z
+#define FT_PROT_V2_ARGS                                                                                                          \
+  taddr, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, stats, can_recompute, m, row0, row_ok, n0, ragged_n, c_begin, c_end, \
+      chk_s1, chk_s1_valid, up, lane, bias, bias_mode, row_ofs, act_kind, Z
+template <bool BIAS, bool ACT, bool ENTRY, bool OUT>
+__device__ __forceinline__ void protected_store_v2_body(FT_PROT_V2_PARAMS, float *D) {
   // ---- pass 1: the chunk sums, and their running sum against the check's ----
   float sc[kMaxChunks];
   float s1 = 0.0f;
@@ -1179,6 +1224,7 @@ __device__ __noinline__ void protected_store_pass_v2(uint32_t taddr, const float
   const bool has_bias = BIAS || (ACT && bias_mode != kBiasNone);
   const BiasRef b = make_bias(bias, bias_mode, m, has_bias && row_ok);
   float *crow = C + m;
+  float *drow = D + m;
   float *zrow = (ACT && Z != nullptr) ? Z + m : nullptr;
   const bool rmw = beta != 0.0f;
   const int c_stop = min(c_end, (N - n0 + 31) / 32);  // chunks wholly past N are skipped
@@ -1259,14 +1305,14 @@ __device__ __noinline__ void protected_store_pass_v2(uint32_t taddr, const float
       if (act_kind == kActRelu) {
 #pragma unroll
         for (int i = 0; i < 32; ++i) v[i] = f2u(act_apply(kActRelu, u2f(v[i])));
-      } else {
+      } else if (!OUT || act_kind == kActGelu) {
 #pragma unroll
         for (int i = 0; i < 32; ++i) v[i] = f2u(act_apply(kActGelu, u2f(v[i])));
       }
     }
 #pragma unroll
     for (int i = 0; i < 32; ++i)
-      if (full || nb + i < N) crow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
+      if (full || nb + i < N) drow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
   }
   // chunks of a segment that failed pass 1 but lie wholly past N hold nothing to repair
   if (c_stop < c_end) bad_chunks &= (c_stop > c_begin) ? (1u << (c_stop - c_begin)) - 1u : 0u;
@@ -1295,10 +1341,27 @@ __device__ __noinline__ void protected_store_pass_v2(uint32_t taddr, const float
     while (chunks != 0u) {
       const int k = __ffs(chunks) - 1;
       chunks &= chunks - 1u;
-      recompute<32, BIAS, ACT, ENTRY>(bias, bias_mode, act_kind, Z, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, row0 + r,
-                               n0 + (c_begin + k) * 32, lane);
+      recompute<32, BIAS, ACT, ENTRY, OUT>(bias, bias_mode, act_kind, Z, D, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta,
+                                           row0 + r, n0 + (c_begin + k) * 32, lane);
     }
   }
+}
+// (ENTRY: the ACT x BATCH kernels' own copy, see recompute_row_act)
+template <bool BIAS, bool ACT, bool ENTRY = false>
+__device__ __noinline__ void protected_store_pass_v2(FT_PROT_V2_PARAMS) {
+  protected_store_v2_body<BIAS, ACT, ENTRY, false>(FT_PROT_V2_ARGS, C);
+}
+// (the OUT kernels, which also take the output D: their own entry, so the one above keeps its list)
+template <bool ENTRY>
+__device__ __noinline__ void protected_store_pass_v2_out(FT_PROT_V2_PARAMS, float *D) {
+  protected_store_v2_body<false, true, ENTRY, true>(FT_PROT_V2_ARGS, D);
+}
+#undef FT_PROT_V2_PARAMS
+#undef FT_PROT_V2_ARGS
+template <bool BIAS, bool ACT, bool ENTRY, bool OUT, typename... Args>
+__device__ __forceinline__ void protected_store_v2(float *D, Args... args) {
+  if constexpr (OUT) protected_store_pass_v2_out<ENTRY>(args..., D);
+  else protected_store_pass_v2<BIAS, ACT, ENTRY>(args...);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1780,11 +1843,16 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t a_desc, 
 // The final epilogue of a data tile stores act(z) and, when p.z is set, z; the bias mode, the activation and Z are run-time
 // fields.  Like BIAS, its own binary, so that the other kernels are compiled exactly as without the feature.  With BATCH,
 // the entry's Z is p.z + entry * stride_c (C's geometry) and its bias p.bias + entry * stride_bias.
-template <int BN, bool FT, int CG, bool PROT = false, bool SEED = false, bool BIAS = false, bool BATCH = false, bool ACT = false>
+// OUT: the ACT instantiation for calls with a separate output D (ftsgemm_run_batched_out): every final value reads its old
+// value from C and is stored to p.d (C's geometry; with BATCH p.d + entry * stride_c), ACT_NONE included.  Its own binary,
+// so that the ACT kernels are compiled exactly as without the feature.
+template <int BN, bool FT, int CG, bool PROT = false, bool SEED = false, bool BIAS = false, bool BATCH = false, bool ACT = false,
+          bool OUT = false>
 __global__ void __launch_bounds__(kThreads, 1)
 ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmChk, const KernelParams p) {
   static_assert(!(ACT && BIAS), "the ACT kernels take the bias mode at run time");
+  static_assert(!OUT || ACT, "the OUT kernels are ACT kernels");
   using Cfg = TileCfg<BN, FT, CG>;
   constexpr int kStages = Cfg::kStages;
   constexpr int kAccRegs = BN / 2;  // per thread of a consumer warpgroup: 64 x BN FP32
@@ -1961,6 +2029,7 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       float *const Cb = BATCH ? p.C + bt * p.stride_c : nullptr;
       const float *const biasb = BATCH ? p.bias + ((BIAS || ACT) ? bt * p.stride_bias : 0) : nullptr;  // (the entry's bias)
       float *const Zb = (BATCH && ACT && p.z != nullptr) ? p.z + bt * p.stride_c : nullptr;          // (Z: C's geometry)
+      float *const Db = OUT ? p.d + (BATCH ? bt * p.stride_c : 0) : nullptr;  // (OUT: the entry's D, C's geometry)
       const int row_ofs = bt * p.M;                           // stacked rows: fault list and events
       const int slab_ofs = bt * (p.tiles_m * CG * (kBM / 32));  // the entry's checksum flags
       const size_t chk_ofs = static_cast<size_t>(bt) * p.M * p.n_chk_cols * (p.chk_slices > 1 ? p.chk_slices : 1);
@@ -2052,7 +2121,7 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             if constexpr (PROT) stale = (ptx::ld_acquire_shared_u32(xchg_base(q) + 4) >> lane) & 1u;  // rows it repaired
           }
           if (PROT && FT && !(p.dbg_flags & 1) && p.protect == 2) {
-            protected_store_pass_v2<BIAS, ACT, ACT && BATCH>(taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1),
+            protected_store_v2<BIAS, ACT, ACT && BATCH, OUT>(Db, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1),
                                                p.ldc, p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m,
                                                m0_cta + q * 32, m < p.M && !skip, n0, n0 + BN > p.N, kMid, BN / 32, s1, stale == 0u,
                                                stored_value_upsets<BN, BATCH>(p, q, lane, m0_cta, n0, kMid, BN / 32, row_ofs), lane,
@@ -2061,12 +2130,13 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           } else if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N) {
             uint32_t bad_bits = 0u;
             const int bad_col = stored_value_fault<BN, BATCH>(p, q, lane, m0_cta, n0, kMid, BN / 32, bad_bits, row_ofs);
-            protected_store<BN, BIAS, BATCH, ACT>(BATCH ? biasb : p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? (BATCH ? Zb : p.z) : nullptr, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
+            protected_store<BN, BIAS, BATCH, ACT, OUT>(BATCH ? biasb : p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? (BATCH ? Zb : p.z) : nullptr, Db, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
                                       p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32,
                                       m < p.M && !skip, n0, kMid, BN / 32, s1, stale == 0u, bad_col, bad_bits, lane);
           } else {
-            store_tile<BN, BIAS, ACT>(taddr, (BATCH ? Cb : p.C) + m, m < p.M && !skip, n0, p.N, p.ldc, p.alpha, p.beta, kMid, BN / 32,
-                                      make_bias(BATCH ? biasb : p.bias, p.bias_mode, m, (BIAS || ACT) && m < p.M && !skip), BATCH ? act_of_entry<ACT>(p, Zb, m) : act_of<ACT>(p, m));
+            store_tile<BN, BIAS, ACT, OUT>(taddr, (BATCH ? Cb : p.C) + m, m < p.M && !skip, n0, p.N, p.ldc, p.alpha, p.beta, kMid, BN / 32,
+                                      make_bias(BATCH ? biasb : p.bias, p.bias_mode, m, (BIAS || ACT) && m < p.M && !skip),
+                                      with_out<OUT>(BATCH ? act_of_entry<ACT>(p, Zb, m) : act_of<ACT>(p, m), Db, m));
           }
           ptx::named_bar_sync(4 + q, 64);  // both halves are out of the accumulator
         }
@@ -2122,7 +2192,7 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
         if (assist_on && FT && !(p.dbg_flags & 1)) ptx::named_bar_sync(4 + q, 64);  // corrections are in place
         if (PROT && FT && !(p.dbg_flags & 1) && p.protect == 2) {
-          protected_store_pass_v2<BIAS, ACT, ACT && BATCH>(taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1),
+          protected_store_v2<BIAS, ACT, ACT && BATCH, OUT>(Db, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1),
                                              p.ldc, p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m,
                                              m0_cta + q * 32, m < p.M && !redo, n0, n0 + BN > p.N, 0, c_mid, own_s1,
                                              ((stale_mask >> lane) & 1u) == 0u,
@@ -2132,19 +2202,20 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         } else if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N) {
           uint32_t bad_bits = 0u;
           const int bad_col = stored_value_fault<BN, BATCH>(p, q, lane, m0_cta, n0, 0, c_mid, bad_bits, row_ofs);
-          protected_store<BN, BIAS, BATCH, ACT>(BATCH ? biasb : p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? (BATCH ? Zb : p.z) : nullptr, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
+          protected_store<BN, BIAS, BATCH, ACT, OUT>(BATCH ? biasb : p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? (BATCH ? Zb : p.z) : nullptr, Db, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
                                     p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32,
                                     m < p.M && !redo, n0, 0, c_mid, own_s1, ((stale_mask >> lane) & 1u) == 0u, bad_col, bad_bits, lane);
         } else {
-          store_tile<BN, BIAS, ACT>(taddr, (BATCH ? Cb : p.C) + m, m < p.M && !redo, n0, p.N, p.ldc, p.alpha, p.beta, 0, c_mid,
-                                    make_bias(BATCH ? biasb : p.bias, p.bias_mode, m, (BIAS || ACT) && m < p.M && !redo), BATCH ? act_of_entry<ACT>(p, Zb, m) : act_of<ACT>(p, m));
+          store_tile<BN, BIAS, ACT, OUT>(taddr, (BATCH ? Cb : p.C) + m, m < p.M && !redo, n0, p.N, p.ldc, p.alpha, p.beta, 0, c_mid,
+                                    make_bias(BATCH ? biasb : p.bias, p.bias_mode, m, (BIAS || ACT) && m < p.M && !redo),
+                                    with_out<OUT>(BATCH ? act_of_entry<ACT>(p, Zb, m) : act_of<ACT>(p, m), Db, m));
         }
         if (FT && redo_mask != 0u) {  // rare, warp-uniform: recompute the flagged rows from global memory
           unsigned rm = redo_mask;
           while (rm != 0u) {
             const int r = __ffs(rm) - 1;
             rm &= rm - 1u;
-            recompute<BN, BIAS, ACT, ACT && BATCH>(BATCH ? biasb : p.bias, p.bias_mode, ACT ? p.act : 0, ACT ? (BATCH ? Zb : p.z) : nullptr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K,
+            recompute<BN, BIAS, ACT, ACT && BATCH, OUT>(BATCH ? biasb : p.bias, p.bias_mode, ACT ? p.act : 0, ACT ? (BATCH ? Zb : p.z) : nullptr, Db, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K,
                                 p.alpha, p.beta, m0_cta + q * 32 + r, n0, lane);
           }
         }
@@ -2232,5 +2303,12 @@ encode_kernel(const float *__restrict__ B, int N, int K, int ldb, long long stri
       encode_b_warp<BN, KRQ, STREAM>(B + e * stride_b, N, K, ldb, chk + e * chk_stride, chk_ld, rounding, tiles_n, gw, nw, lane);
   }
 }
+
+// The OUT instantiations of ftsgemm_tc_kernel are compiled in their own translation unit (ftsgemm_out.cu): tc_out_kernel
+// returns the one of a tile (BN, CG) and flags (FT, PROT, SEED, BATCH), or null.  That unit's kernels have their own copy
+// of ptx::g_abort_flag; tc_out_abort_flag reads it into *flag and clears it.
+using TcKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, KernelParams);
+TcKernel tc_out_kernel(int bn, int cg, bool ft, bool prot, bool seed, bool batch);
+cudaError_t tc_out_abort_flag(int *flag);
 
 }  // namespace ftsgemm

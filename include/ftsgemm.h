@@ -347,6 +347,35 @@ int ftsgemm_run_batched_act(ftsgemm_handle_t h, int kernel_id, int M, int N, int
                             long long stride_c, int batch, float alpha, float beta, const float *bias, int bias_mode,
                             long long stride_bias, int activation, float *dZ, const ftsgemm_opts *opts);
 
+/* ---- separate output D  (the contract of cublasLt: D = alpha * A * B + beta * C with C read-only) ----------------------------
+ * ftsgemm_run_batched_act with the results written to D instead of C.  The call is defined as: copy C into D, then run
+ * ftsgemm_run_batched_act on D with every other argument unchanged.  D holds that result bit for bit, and C is not written
+ * (its bytes after the call are its bytes before):
+ *   z = (alpha * acc + beta * C_old) + b      D = act(z)      Z = z (when dZ is not NULL)
+ * D has C's geometry: leading dimension ldc, entry i at D + i*stride_c.  D == C (the same pointer) is the in-place call,
+ * ftsgemm_run_batched_act itself.  With beta == 0, C is not read and may be NULL: the call is the in-place call on D.
+ * With D != C:
+ *  - the wgmma ids run the OUT form of the ACT kernels (FTSGEMM_ACT_NONE included), which read every old value from C and
+ *    store to D.  With opts.precision = 1 only the first pass reads C and writes D, the other two accumulate into D in
+ *    place; with opts.check_segments = S only the first segment does, the others accumulate into D in place.
+ *  - protect_epilogue = 1 repairs a failed row segment whatever beta is: the old C is intact, so the segment is recomputed
+ *    into D from A, B and C (stats.recomputed, event status 6).  Status 7 remains for no_recompute / detect_only, and for the
+ *    passes and segments that run in place on D.
+ *  - it makes a CUDA graph replay idempotent: a captured call with beta != 0 reads C and writes D, so every replay writes
+ *    the same D (an in-place capture accumulates into C on every replay).
+ * Errors: those of ftsgemm_run_batched_act (dZ == D included); D NULL or not 16-byte aligned, D's footprint overlapping C's
+ * unless D == C exactly, or (D != C) Z's footprint overlapping C's or D's: FTSGEMM_ERR_INVALID_ARG.  D != C with the cuBLAS
+ * ids 0 / 7 or the baseline ids 10 / 30: FTSGEMM_ERR_UNSUPPORTED (no unfused fallback).  A footprint is the elements
+ * [0, (batch - 1) * stride_c + (N - 1) * ldc + M) from the base. */
+int ftsgemm_run_batched_out(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *A, int layout_a, int lda,
+                            long long stride_a, const float *B, int layout_b, int ldb, long long stride_b, const float *C,
+                            int ldc, long long stride_c, float *D, int batch, float alpha, float beta, const float *bias,
+                            int bias_mode, long long stride_bias, int activation, float *dZ, const ftsgemm_opts *opts);
+/* ftsgemm_run_batched_out with batch = 1 (the strides are ignored). */
+int ftsgemm_run_out(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
+                    const float *dB, int layout_b, int ldb, const float *dC, int ldc, float *dD, float alpha, float beta,
+                    const float *bias, int bias_mode, int activation, float *dZ, const ftsgemm_opts *opts);
+
 /* Counters of all FT launches since the previous call (synchronises the handle's last stream, then resets). */
 int ftsgemm_get_stats(ftsgemm_handle_t h, ftsgemm_stats *out);
 
