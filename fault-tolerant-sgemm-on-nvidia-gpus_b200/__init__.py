@@ -98,8 +98,11 @@ EXPORTED_SYMBOLS = [
     "ftsgemm_run_host", "ftsgemm_baseline", "ftsgemm_verify", "ftsgemm_debug_set", "ftsgemm_debug_schedule",
     "ftsgemm_verify_bad_count", "ftsgemm_debug_trace", "ftsgemm_stats_device", "ftsgemm_select_kernel", "ftsgemm_launch_count", "ftsgemm_peer_export", "ftsgemm_peer_connect",
     "ftsgemm_peer_verdict", "ftsgemm_run_batched", "ftsgemm_debug_schedule_batched", "ftsgemm_run_act",
-    "ftsgemm_run_batched_act", "ftsgemm_run_out", "ftsgemm_run_batched_out",
+    "ftsgemm_run_batched_act", "ftsgemm_run_out", "ftsgemm_run_batched_out", "ftsgemm_run_typed", "ftsgemm_run_batched_typed",
 ]
+
+# operand element types of run_typed / run_batched_typed (include/ftsgemm.h: FTSGEMM_TYPE_*)
+TYPE_F32, TYPE_BF16 = 0, 1
 
 _lib = None
 
@@ -144,6 +147,10 @@ def lib():
                                       C.POINTER(Opts)]
         L.ftsgemm_run_batched_out.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, ll, vp, ip, ip, ll, vp, ip, ll, vp, ip, fp, fp,
                                               vp, ip, ll, ip, vp, C.POINTER(Opts)]
+        L.ftsgemm_run_typed.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, vp, ip, ip, ip, vp, ip, vp, fp, fp, vp, ip, ip, vp,
+                                        C.POINTER(Opts)]
+        L.ftsgemm_run_batched_typed.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, ll, vp, ip, ip, ll, ip, vp, ip, ll, vp, ip, fp,
+                                                fp, vp, ip, ll, ip, vp, C.POINTER(Opts)]
         L.ftsgemm_get_stats.argtypes = [vp, C.POINTER(Stats)]
         L.ftsgemm_run_host.argtypes = [vp, ip, ip, ip, ip, vp, vp, vp, fp, fp, C.POINTER(Opts)]
         L.ftsgemm_stats_device.argtypes = [vp, vp, vp]
@@ -262,26 +269,33 @@ def _pad4(n: int) -> int:
     return (n + 3) // 4 * 4
 
 
-def _view(shape, stride, ptr: int, ld4: bool):
+def _pad8(n: int) -> int:
+    """_pad4 for BF16 operands: 16-byte rows are 8 elements."""
+    return (n + 7) // 8 * 8
+
+
+def _view(shape, stride, ptr: int, ld4: bool, elems16: int = 4):
     """("row", ld) or ("col", ld) of a 2-D matrix the library can read in place, None if it cannot: it needs a unit
-    stride, a leading stride of at least the row length, a 16-byte aligned base and -- for A and B (ld4) -- 16-byte rows."""
+    stride, a leading stride of at least the row length, a 16-byte aligned base and -- for A and B (ld4) -- 16-byte rows
+    (ld a multiple of elems16: 4 FP32 or 8 BF16 elements)."""
     R, Cn = shape
     s0, s1 = stride
+    pad = _pad8 if elems16 == 8 else _pad4
     if ptr % 16:
         return None
     if s1 == 1 or Cn == 1:  # row-major (a one-column matrix is both)
-        ld = s0 if R > 1 else _pad4(Cn)
-        if ld >= Cn and (not ld4 or ld % 4 == 0):
+        ld = s0 if R > 1 else pad(Cn)
+        if ld >= Cn and (not ld4 or ld % elems16 == 0):
             return ("row", ld)
     if s0 == 1 or R == 1:  # column-major
-        ld = s1 if Cn > 1 else _pad4(R)
-        if ld >= R and (not ld4 or ld % 4 == 0):
+        ld = s1 if Cn > 1 else pad(R)
+        if ld >= R and (not ld4 or ld % elems16 == 0):
             return ("col", ld)
     return None
 
 
 def matmul_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0, b_ptr: int = 0, out_ptr: int = 0,
-                bias_stride=None, bias_ptr: int = 0) -> dict:
+                bias_stride=None, bias_ptr: int = 0, bf16: bool = False) -> dict:
     """run_ex arguments for out = a @ b with a: (M, K), b: (K, N), out: (M, N), from shapes, element strides and addresses.
 
     Column-major out: C = out, kernel A = a, kernel B = b^T.  Row-major out: C = out^T = b^T a^T (swap = True), so the
@@ -291,17 +305,19 @@ def matmul_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0
     column-major with the row length padded to a multiple of 4 (both K-major for the kernel), out as a contiguous
     row-major matrix.  bias_stride (the element stride of a length-N bias, None without a bias) gives bias_mode: a bias
     over out's columns is one per kernel column (BIAS_COL), or per kernel row (BIAS_ROW) when swapped; copy_bias marks a
-    bias without unit stride or with a base that is not 4-byte aligned."""
+    bias without unit stride or with a base that is not 4-byte aligned.  bf16: a and b are BF16 (run_typed), whose 16-byte
+    rows are 8 elements: leading strides and the copies' padded rows are multiples of 8."""
     M, K = a_shape
     K2, N = b_shape
     if K != K2:
         raise ValueError(f"inner dimensions differ: {tuple(a_shape)} @ {tuple(b_shape)}")
-    va = _view(a_shape, a_stride, a_ptr, True)
-    vb = _view(b_shape, b_stride, b_ptr, True)
+    e16, pad = (8, _pad8) if bf16 else (4, _pad4)
+    va = _view(a_shape, a_stride, a_ptr, True, e16)
+    vb = _view(b_shape, b_stride, b_ptr, True, e16)
     vo = _view((M, N), out_stride, out_ptr, False)
     copies = {"copy_a": va is None, "copy_b": vb is None, "copy_out": vo is None}
-    va = va or ("row", _pad4(K))
-    vb = vb or ("col", _pad4(K))
+    va = va or ("row", pad(K))
+    vb = vb or ("col", pad(K))
     vo = vo or ("row", N)
     a_kmajor, b_kmajor = va[0] == "row", vb[0] == "col"  # a(m, k) along k / b(k, n) along k
     lay = {True: LAYOUT_K_MAJOR, False: LAYOUT_MN_MAJOR}
@@ -318,7 +334,7 @@ def matmul_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0
 
 
 def bmm_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0, b_ptr: int = 0, out_ptr: int = 0,
-             bias_stride=None, bias_ptr: int = 0, bias_entry_stride=None) -> dict:
+             bias_stride=None, bias_ptr: int = 0, bias_entry_stride=None, bf16: bool = False) -> dict:
     """run_batched arguments for out = a @ b with a: (Bt, M, K), b: (Bt, K, N), out: (Bt, M, N), from shapes, element strides
     and addresses.  Each matrix is mapped as in matmul_plan (layouts, lds, swap, bias_mode); stride_a / stride_b / stride_c
     are the batch strides of the kernel's A, B and C (b's and a's when swapped).  With more than one entry a tensor is also
@@ -329,28 +345,30 @@ def bmm_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0, b
     bias_entry_stride is the entry stride of a (Bt, N) bias, one bias per entry (None: a (N,) bias shared by all entries).
     stride_bias is the entry stride run_batched_act takes: 0 for a shared bias, an expanded one (entry stride 0) or a single
     entry.  copy_bias also marks a per-entry bias with a negative entry stride; the copy bmm makes of a per-entry bias is
-    (Bt, N) contiguous (stride_bias = N), of a shared one (N,)."""
+    (Bt, N) contiguous (stride_bias = N), of a shared one (N,).  bf16: a and b are BF16 (run_batched_typed): their rows,
+    batch strides and copies' padded rows are multiples of 8 elements (16 bytes) instead of 4."""
     Bt, M, K = a_shape
     Bt2, K2, N = b_shape
     if Bt != Bt2:
         raise ValueError(f"batch sizes differ: {tuple(a_shape)} @ {tuple(b_shape)}")
     mp = matmul_plan((M, K), tuple(a_stride[1:]), (K2, N), tuple(b_stride[1:]), tuple(out_stride[1:]), a_ptr, b_ptr, out_ptr,
-                     bias_stride, bias_ptr)
+                     bias_stride, bias_ptr, bf16)
     sa, sb, so = a_stride[0], b_stride[0], out_stride[0]
+    e16, pad = (8, _pad8) if bf16 else (4, _pad4)
     if Bt > 1:
-        def bad(st):
-            return st <= 0 or st % 4 != 0
-        mp["copy_a"] = mp["copy_a"] or bad(sa)
-        mp["copy_b"] = mp["copy_b"] or bad(sb)
+        def bad(st, e=4):
+            return st <= 0 or st % e != 0
+        mp["copy_a"] = mp["copy_a"] or bad(sa, e16)
+        mp["copy_b"] = mp["copy_b"] or bad(sb, e16)
         mp["copy_out"] = mp["copy_out"] or bad(so) or so < mp["ldc"] * mp["N"]
     if mp["copy_a"] or mp["copy_b"] or mp["copy_out"]:
-        # the copies: a (Bt, M, pad4(K)) row-major, b as (Bt, N, pad4(K)) transposed, out (Bt, M, N) contiguous
-        a_st = (M * _pad4(K), _pad4(K), 1) if mp["copy_a"] else tuple(a_stride)
-        b_st = (N * _pad4(K), 1, _pad4(K)) if mp["copy_b"] else tuple(b_stride)
+        # the copies: a (Bt, M, pad4(K)) row-major, b as (Bt, N, pad4(K)) transposed, out (Bt, M, N) contiguous (pad8: BF16)
+        a_st = (M * pad(K), pad(K), 1) if mp["copy_a"] else tuple(a_stride)
+        b_st = (N * pad(K), 1, pad(K)) if mp["copy_b"] else tuple(b_stride)
         o_st = (M * N, N, 1) if mp["copy_out"] else tuple(out_stride)
         copies = {k: mp[k] for k in ("copy_a", "copy_b", "copy_out", "copy_bias")}
         mp = matmul_plan((M, K), a_st[1:], (K, N), b_st[1:], o_st[1:], 0 if copies["copy_a"] else a_ptr,
-                         0 if copies["copy_b"] else b_ptr, 0 if copies["copy_out"] else out_ptr, bias_stride, bias_ptr)
+                         0 if copies["copy_b"] else b_ptr, 0 if copies["copy_out"] else out_ptr, bias_stride, bias_ptr, bf16)
         mp.update(copies)
         sa, sb, so = a_st[0], b_st[0], o_st[0]
     mp["batch"] = Bt
@@ -506,6 +524,29 @@ class FtSgemm:
                                                         activation, _ptr(dZ) if dZ is not None else None,
                                                         C.byref(opts) if opts is not None else None))
 
+    def run_batched_typed(self, kernel_id: int, M: int, N: int, K: int, dA, layout_a: int, lda: int, stride_a: int, dB,
+                          layout_b: int, ldb: int, stride_b: int, ab_type: int, dC, ldc: int, stride_c: int, dD, batch: int,
+                          alpha: float = 1.0, beta: float = 0.0, bias=None, bias_mode: int = BIAS_NONE, stride_bias: int = 0,
+                          activation: int = ACT_NONE, dZ=None, opts: Opts | None = None) -> None:
+        """run_batched_out with A and B of element type ab_type (TYPE_F32: run_batched_out itself; TYPE_BF16: BF16 A and B,
+        leading dimensions and entry strides in elements, FP32 accumulate, C / D / Z / bias FP32; include/ftsgemm.h:
+        ftsgemm_run_batched_typed)."""
+        self._run_checked(lib().ftsgemm_run_batched_typed(self._h, kernel_id, M, N, K, _ptr(dA), layout_a, lda, stride_a,
+                                                          _ptr(dB), layout_b, ldb, stride_b, ab_type,
+                                                          _ptr(dC) if dC is not None else None, ldc, stride_c, _ptr(dD), batch,
+                                                          alpha, beta, _ptr(bias) if bias is not None else None, bias_mode,
+                                                          stride_bias, activation, _ptr(dZ) if dZ is not None else None,
+                                                          C.byref(opts) if opts is not None else None))
+
+    def run_typed(self, kernel_id: int, M: int, N: int, K: int, dA, layout_a: int, lda: int, dB, layout_b: int, ldb: int,
+                  ab_type: int, dC, ldc: int, dD, alpha: float = 1.0, beta: float = 0.0, bias=None, bias_mode: int = BIAS_NONE,
+                  activation: int = ACT_NONE, dZ=None, opts: Opts | None = None) -> None:
+        """run_batched_typed with batch = 1 (include/ftsgemm.h: ftsgemm_run_typed)."""
+        self._run_checked(lib().ftsgemm_run_typed(self._h, kernel_id, M, N, K, _ptr(dA), layout_a, lda, _ptr(dB), layout_b, ldb,
+                                                  ab_type, _ptr(dC) if dC is not None else None, ldc, _ptr(dD), alpha, beta,
+                                                  _ptr(bias) if bias is not None else None, bias_mode, activation,
+                                                  _ptr(dZ) if dZ is not None else None, C.byref(opts) if opts is not None else None))
+
     def bmm(self, a, b, out=None, *, c=None, bias=None, activation=None, preact=None, kernel_id: int = ID_ABFT_AUTO,
             alpha: float = 1.0, beta: float = 0.0, opts: Opts | None = None):
         """out = act(alpha * (a @ b) + beta * out + bias) for 3-D float32 CUDA tensors a: (Bt, M, K), b: (Bt, K, N), out:
@@ -538,11 +579,20 @@ class FtSgemm:
         + bias), bit for bit what the call gives with out holding a copy of c (one run_batched_out call).  beta must not be
         0 (c would not be read: ValueError).  With out=None, out is allocated with c's strides (c dense) and the call is
         differentiable in c as well: grad_c = beta * grad_z.  The kernels read c with out's geometry: a c with other strides
-        (or a base that is not 16-byte aligned) is copied once into that geometry first."""
+        (or a base that is not 16-byte aligned) is copied once into that geometry first.
+
+        a and b may also both be bfloat16 (mixed with float32: TypeError): one run_batched_typed call on the BF16 kernels,
+        FP32 accumulate, with out, c and preact float32 as above and a bfloat16 bias upcast (exactly) into a float32
+        temporary; copies pad rows to 8 elements (bmm_plan with bf16).  Autograd as above, with grad_z rounded to bfloat16
+        once for the two gradient products (the rounding of torch autocast's BF16 backward), which run on the BF16 kernels;
+        grad_a, grad_b and grad_bias come back in the dtypes of a, b and the bias."""
         import torch
         for name, t in (("a", a), ("b", b)):
-            if t.dim() != 3 or t.dtype != torch.float32 or not t.is_cuda:
-                raise TypeError(f"{name} must be a 3-D float32 CUDA tensor")
+            if t.dim() != 3 or t.dtype not in (torch.float32, torch.bfloat16) or not t.is_cuda:
+                raise TypeError(f"{name} must be a 3-D float32 or bfloat16 CUDA tensor")
+        if a.dtype != b.dtype:
+            raise TypeError(f"a and b must both be float32 or both bfloat16, not {a.dtype} and {b.dtype}")
+        bf16 = a.dtype == torch.bfloat16
         Bt, M, K = a.shape
         N = b.shape[2]
         if b.shape[0] != Bt or b.shape[1] != K or b.device != a.device:
@@ -557,6 +607,7 @@ class FtSgemm:
             if c.shape != (Bt, M, N) or c.dtype != torch.float32 or c.device != a.device:
                 raise ValueError(f"c must be a float32 ({Bt}, {M}, {N}) tensor on {a.device}")
         if out is None and torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (a, b, bias, c)):
+            # (a bfloat16 bias is upcast inside the forward, which runs without grad: autograd sees the caller's tensor)
             if beta != 0.0 and c is None:
                 raise ValueError("beta != 0 needs an out tensor or c")
             fwd = Opts.from_buffer_copy(opts) if opts is not None else make_opts()
@@ -572,6 +623,8 @@ class FtSgemm:
                 out = torch.empty(Bt, M, N, device=a.device, dtype=torch.float32)
         if out.shape != (Bt, M, N) or out.dtype != torch.float32 or out.device != a.device:
             raise ValueError(f"out must be a float32 ({Bt}, {M}, {N}) tensor on {a.device}")
+        if bf16 and bias is not None and bias.dtype == torch.bfloat16:
+            bias = bias.float()
         if bias is not None and (bias.shape not in ((N,), (Bt, N)) or bias.dtype != torch.float32 or bias.device != a.device):
             raise ValueError(f"bias must be a float32 ({N},) or ({Bt}, {N}) tensor on {a.device}")
         if preact is not None and (preact.shape != out.shape or preact.stride() != out.stride() or
@@ -583,17 +636,18 @@ class FtSgemm:
         bias_stride = bias.stride(-1) if bias is not None else None
         plan = bmm_plan(tuple(a.shape), a.stride(), tuple(b.shape), b.stride(), out.stride(), a.data_ptr(), b.data_ptr(),
                         out.data_ptr(), bias_stride, bias.data_ptr() if bias is not None else 0,
-                        bias.stride(0) if per_entry else None)
+                        bias.stride(0) if per_entry else None, bf16)
         fused = activation is not None or plan["stride_bias"] != 0
         if activation is not None and plan["copy_out"]:
             raise ValueError("out (and so preact) must be writable in place with an activation: 16-byte rows and entries")
         if plan["copy_bias"]:
             bias = (torch.empty(Bt, N, device=a.device, dtype=torch.float32).copy_(bias) if plan["stride_bias"] != 0 else
                     torch.empty(N, device=a.device, dtype=torch.float32).copy_(bias[0] if per_entry else bias))
+        pad = _pad8 if bf16 else _pad4
         if plan["copy_a"]:
-            a = torch.empty(Bt, M, _pad4(K), device=a.device, dtype=torch.float32)[:, :, :K].copy_(a)
+            a = torch.empty(Bt, M, pad(K), device=a.device, dtype=a.dtype)[:, :, :K].copy_(a)
         if plan["copy_b"]:
-            b = torch.empty(Bt, N, _pad4(K), device=a.device, dtype=torch.float32)[:, :, :K].copy_(b.transpose(1, 2)).transpose(1, 2)
+            b = torch.empty(Bt, N, pad(K), device=a.device, dtype=b.dtype)[:, :, :K].copy_(b.transpose(1, 2)).transpose(1, 2)
         dst = out
         if plan["copy_out"]:
             dst = (out.contiguous() if beta != 0.0 and c is None else
@@ -605,7 +659,12 @@ class FtSgemm:
         if opts is None:
             opts = make_opts(stream=torch.cuda.current_stream(a.device).cuda_stream)
         kA, kB = (b, a) if plan["swap"] else (a, b)
-        if c is not None:
+        if bf16:
+            self.run_batched_typed(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], plan["stride_a"],
+                                   kB, plan["layout_b"], plan["ldb"], plan["stride_b"], TYPE_BF16, c if c is not None else dst,
+                                   plan["ldc"], plan["stride_c"], dst, Bt, alpha, beta, bias, plan["bias_mode"],
+                                   plan["stride_bias"], ACTIVATIONS[activation], preact, opts)
+        elif c is not None:
             self.run_batched_out(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], plan["stride_a"],
                                  kB, plan["layout_b"], plan["ldb"], plan["stride_b"], c, plan["ldc"], plan["stride_c"], dst, Bt,
                                  alpha, beta, bias, plan["bias_mode"], plan["stride_bias"], ACTIVATIONS[activation], preact, opts)
@@ -647,11 +706,20 @@ class FtSgemm:
         bias), bit for bit what the call gives with out holding a copy of c (one run_out / run_batched_out call).  beta must
         not be 0 (c would not be read: ValueError).  With out=None, out is allocated with c's strides (c dense).  The kernels
         read c with out's geometry: a c with other strides (or a base that is not 16-byte aligned) is copied once into that
-        geometry first."""
+        geometry first.
+
+        a and b may also both be bfloat16 (float32 and bfloat16 mixed raise TypeError): bmm on a batch of one entry, one
+        run_batched_typed call on the BF16 kernels, FP32 accumulate, with out, c and preact float32 as above; a bfloat16 bias
+        is upcast (exactly) into a float32 temporary.  Their copies pad rows to 8 elements (matmul_plan with bf16)."""
         import torch
         for name, t in (("a", a), ("b", b)):
-            if t.dim() != 2 or t.dtype != torch.float32 or not t.is_cuda:
-                raise TypeError(f"{name} must be a 2-D float32 CUDA tensor")
+            if t.dim() != 2 or t.dtype not in (torch.float32, torch.bfloat16) or not t.is_cuda:
+                raise TypeError(f"{name} must be a 2-D float32 or bfloat16 CUDA tensor")
+        if a.dtype != b.dtype:
+            raise TypeError(f"a and b must both be float32 or both bfloat16, not {a.dtype} and {b.dtype}")
+        bf16 = a.dtype == torch.bfloat16
+        if bf16 and bias is not None and bias.dtype == torch.bfloat16:
+            bias = bias.float()
         M, K = a.shape
         K2, N = b.shape
         if c is not None:
@@ -672,6 +740,11 @@ class FtSgemm:
             raise ValueError(f"bias must be a float32 ({N},) tensor on {a.device}")
         if K != K2:
             raise ValueError(f"inner dimensions differ: {tuple(a.shape)} @ {tuple(b.shape)}")
+        if bf16:  # (one run_batched_typed call: bmm on a batch of one entry)
+            self.bmm(a.unsqueeze(0), b.unsqueeze(0), out.unsqueeze(0), c=c.unsqueeze(0) if c is not None else None, bias=bias,
+                     activation=activation, preact=preact.unsqueeze(0) if preact is not None else None, kernel_id=kernel_id,
+                     alpha=alpha, beta=beta, opts=opts)
+            return out
         if activation is None and preact is None:
             self.bmm(a.unsqueeze(0), b.unsqueeze(0), out.unsqueeze(0), c=c.unsqueeze(0) if c is not None else None, bias=bias,
                      kernel_id=kernel_id, alpha=alpha, beta=beta, opts=opts)
@@ -727,12 +800,19 @@ class FtSgemm:
         transformer block -- from the same single matmul (beta = 1, r read in place of the old output and never written),
         under the same ABFT protection.  The bias is added after the residual, the kernel's order, so y can differ from
         F.linear(x, weight, bias) + r in the last bits.  y has r's strides when r is dense.  Backward: grad_r = grad_y, the
-        other gradients as above.  A residual with an activation raises ValueError."""
+        other gradients as above.  A residual with an activation raises ValueError.
+
+        x and weight may also both be bfloat16 (mixed with float32: TypeError): the product runs on the BF16 kernels (FP32
+        accumulate) and y is float32, as are the residual and the pre-activation value; a bfloat16 bias is upcast exactly.
+        The backward rounds grad_z to bfloat16 once (the rounding of torch autocast's BF16 backward) and runs grad_x and
+        grad_weight on the BF16 kernels; the gradients come back in the dtypes of x, weight and the bias."""
         import torch
-        if x.dtype != torch.float32 or not x.is_cuda or x.dim() < 1:
-            raise TypeError("x must be a float32 CUDA tensor with at least one dimension")
+        if x.dtype not in (torch.float32, torch.bfloat16) or not x.is_cuda or x.dim() < 1:
+            raise TypeError("x must be a float32 or bfloat16 CUDA tensor with at least one dimension")
         if weight.dim() != 2:
             raise TypeError("weight must be 2-D (out_features, in_features)")
+        if weight.dtype != x.dtype:
+            raise TypeError(f"x and weight must both be float32 or both bfloat16, not {x.dtype} and {weight.dtype}")
         lp = linear_plan(tuple(x.shape), x.stride(), tuple(weight.shape))
         x2 = (x.as_strided((lp["M"], lp["K"]), lp["view"], x.storage_offset()) if lp["view"] is not None
               else x.reshape(lp["M"], lp["K"]).contiguous())
@@ -845,6 +925,7 @@ def _linear_fn():
             def forward(ctx, x2, weight, bias, residual, dev, kernel_id, opts):
                 ctx.save_for_backward(x2, weight)
                 ctx.dev, ctx.kernel_id, ctx.opts = dev, kernel_id, opts
+                ctx.bias_dtype = bias.dtype if bias is not None else None
                 if residual is None:
                     return dev.matmul(x2, weight.t(), bias=bias, kernel_id=kernel_id, opts=opts)
                 return dev.matmul(x2, weight.t(), c=residual, bias=bias, kernel_id=kernel_id, beta=1.0, opts=opts)
@@ -855,17 +936,27 @@ def _linear_fn():
                 bwd = Opts.from_buffer_copy(ctx.opts)
                 bwd.inject_mode, bwd.n_faults = 0, 0
                 bwd.stream = torch.cuda.current_stream(gy.device).cuda_stream
-                gx = gw = gb = None
-                if ctx.needs_input_grad[0]:
-                    gx = ctx.dev.matmul(gy, weight, kernel_id=ctx.kernel_id, opts=bwd)
-                if ctx.needs_input_grad[1]:
-                    gw = ctx.dev.matmul(gy.t(), x2, kernel_id=ctx.kernel_id, opts=bwd)
-                if ctx.needs_input_grad[2]:
-                    gb = gy.sum(0)
+                gx, gw, gb = _linear_grads(ctx, gy, x2, weight, bwd)
                 return gx, gw, gb, gy if ctx.needs_input_grad[3] else None, None, None, None
 
         _LINEAR_FN = LinearFn
     return _LINEAR_FN
+
+
+def _linear_grads(ctx, gz, x2, weight, bwd):
+    """grad_x = grad_z @ weight, grad_weight = grad_z^T @ x through matmul, grad_bias = grad_z summed over the rows (the
+    needed ones, None otherwise).  BF16 x and weight: grad_z is rounded to bfloat16 once and the products run on the BF16
+    kernels; every gradient is returned in its input's dtype."""
+    import torch
+    gx = gw = gb = None
+    g = gz.to(torch.bfloat16) if x2.dtype == torch.bfloat16 else gz
+    if ctx.needs_input_grad[0]:
+        gx = ctx.dev.matmul(g, weight, kernel_id=ctx.kernel_id, opts=bwd).to(x2.dtype)
+    if ctx.needs_input_grad[1]:
+        gw = ctx.dev.matmul(g.t(), x2, kernel_id=ctx.kernel_id, opts=bwd).to(weight.dtype)
+    if ctx.needs_input_grad[2]:
+        gb = g.float().sum(0).to(ctx.bias_dtype)
+    return gx, gw, gb
 
 
 _LINEAR_ACT_FN = None
@@ -888,6 +979,7 @@ def _linear_act_fn():
                 y = dev.matmul(x2, weight.t(), bias=bias, activation=activation, preact=z, kernel_id=kernel_id, opts=opts)
                 ctx.save_for_backward(x2, weight, y if activation == "relu" else z)
                 ctx.dev, ctx.kernel_id, ctx.opts, ctx.activation = dev, kernel_id, opts, activation
+                ctx.bias_dtype = bias.dtype if bias is not None else None
                 return y
 
             @staticmethod
@@ -900,13 +992,7 @@ def _linear_act_fn():
                 bwd = Opts.from_buffer_copy(ctx.opts)
                 bwd.inject_mode, bwd.n_faults = 0, 0
                 bwd.stream = torch.cuda.current_stream(gy.device).cuda_stream
-                gx = gw = gb = None
-                if ctx.needs_input_grad[0]:
-                    gx = ctx.dev.matmul(gz, weight, kernel_id=ctx.kernel_id, opts=bwd)
-                if ctx.needs_input_grad[1]:
-                    gw = ctx.dev.matmul(gz.t(), x2, kernel_id=ctx.kernel_id, opts=bwd)
-                if ctx.needs_input_grad[2]:
-                    gb = gz.sum(0)
+                gx, gw, gb = _linear_grads(ctx, gz, x2, weight, bwd)
                 return gx, gw, gb, None, None, None, None, None
 
         _LINEAR_ACT_FN = LinearActFn
@@ -934,6 +1020,7 @@ def _bmm_fn():
                 ctx.save_for_backward(a, b, y if activation == "relu" else z)
                 ctx.dev, ctx.kernel_id, ctx.alpha, ctx.beta, ctx.opts, ctx.activation = dev, kernel_id, alpha, beta, opts, activation
                 ctx.per_entry_bias = bias is not None and bias.dim() == 2
+                ctx.bias_dtype = bias.dtype if bias is not None else None
                 return y
 
             @staticmethod
@@ -949,12 +1036,15 @@ def _bmm_fn():
                 bwd.inject_mode, bwd.n_faults = 0, 0
                 bwd.stream = torch.cuda.current_stream(gy.device).cuda_stream
                 ga = gb = gbias = gc = None
+                # (BF16 operands: grad_z rounded to bfloat16 once for the products, gradients in the inputs' dtypes)
+                g = gz.to(torch.bfloat16) if a.dtype == torch.bfloat16 else gz
                 if ctx.needs_input_grad[0]:
-                    ga = ctx.dev.bmm(gz, b.transpose(1, 2), kernel_id=ctx.kernel_id, alpha=ctx.alpha, opts=bwd)
+                    ga = ctx.dev.bmm(g, b.transpose(1, 2), kernel_id=ctx.kernel_id, alpha=ctx.alpha, opts=bwd).to(a.dtype)
                 if ctx.needs_input_grad[1]:
-                    gb = ctx.dev.bmm(a.transpose(1, 2), gz, kernel_id=ctx.kernel_id, alpha=ctx.alpha, opts=bwd)
+                    gb = ctx.dev.bmm(a.transpose(1, 2), g, kernel_id=ctx.kernel_id, alpha=ctx.alpha, opts=bwd).to(b.dtype)
                 if ctx.needs_input_grad[2]:
-                    gbias = gz.sum(1) if ctx.per_entry_bias else gz.sum((0, 1))
+                    gf = g.float() if a.dtype == torch.bfloat16 else gz
+                    gbias = (gf.sum(1) if ctx.per_entry_bias else gf.sum((0, 1))).to(ctx.bias_dtype)
                 if ctx.needs_input_grad[4]:
                     gc = ctx.beta * gz
                 return ga, gb, gbias, None, gc, None, None, None, None, None, None

@@ -29,9 +29,10 @@ def _stale(target: Path, sources) -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> None:
-    # two translation units compiled at the same time (their device compilation is single-threaded up to ptxas): the library
-    # and the OUT kernels of ftsgemm_run_batched_out (ftsgemm_out.cu); then one link
-    lib_src = [CSRC / "ftsgemm.cu", CSRC / "ftsgemm_out.cu"]
+    # three translation units compiled at the same time (their device compilation is single-threaded up to ptxas): the
+    # library, the OUT kernels of ftsgemm_run_batched_out (ftsgemm_out.cu) and the BF16 kernels of ftsgemm_run_batched_typed
+    # (ftsgemm_bf16.cu); then one link
+    lib_src = [CSRC / "ftsgemm.cu", CSRC / "ftsgemm_out.cu", CSRC / "ftsgemm_bf16.cu"]
     lib_dep = lib_src + sorted(CSRC.glob("*.cuh")) + sorted(CSRC.glob("*.h")) + [ROOT / "include" / "ftsgemm.h"]
     if force or _stale(LIB, lib_dep):
         with tempfile.TemporaryDirectory() as tmp:

@@ -118,9 +118,10 @@ struct ChkKey {
   int ldb = 0;
   int batch = 1;
   long long stride_b = 0;
+  bool bf16 = false;  // the element type of B: the same bytes read as another type are another B
   bool operator==(const ChkKey &o) const {
     return b == o.b && n == o.n && k == o.k && bn == o.bn && b_kmajor == o.b_kmajor && ldb == o.ldb && batch == o.batch &&
-           stride_b == o.stride_b;
+           stride_b == o.stride_b && bf16 == o.bf16;
   }
 };
 
@@ -142,6 +143,7 @@ struct ftsgemm_handle_s {
   EncodeTiledFn encode_tiled = nullptr;
   DeviceStats *d_stats = nullptr;
   bool out_launched = false;    // an OUT kernel (ftsgemm_out.cu: its own abort flag) has run through the handle
+  bool bf16_launched = false;   // a BF16 kernel (ftsgemm_bf16.cu: its own abort flag) has run through the handle
   DevBuf d_chk;                 // encoded checksum vectors [K][tiles_n*8]  (extra "rows" of B)
   DevBuf d_chk_out;             // slab flags, then the expected checksums M x (tiles_n*8), column-major
   size_t chk_flag_bytes = kChkFlagBytes;  // bytes of d_chk_out in front of the expected checksums: the slab flags
@@ -170,7 +172,7 @@ struct ftsgemm_handle_s {
     bool uploaded = false;
     std::array<DevBuf *, 3> bufs() { return {&d_items, &d_off, &d_wave_target}; }
   };
-  std::map<std::array<long long, 7>, CachedPlan> plans;  // key: kernel id, M, N, K, units, forced slices, batch
+  std::map<std::array<long long, 8>, CachedPlan> plans;  // key: kernel id, M, N, K, units, forced slices, batch, BF16
   DevBuf d_wave_cnt;            // wave re-synchronisation counters (cleared per launch)
   DevBuf d_sk;                  // split-K flags + partial tiles
   DevBuf d_trace;               // debug timeline (ftsgemm_debug_trace), allocated on first use
@@ -238,11 +240,12 @@ struct DeviceGuard {
 
 // The kernels' watchdog (ptx.cuh) raises a device-wide flag instead of trapping; reported once, then cleared.
 int check_abort_flag(ftsgemm_handle_t h) {
-  int flag = 0, out_flag = 0;
+  int flag = 0, out_flag = 0, bf16_flag = 0;
   FT_CUDA(h, cudaMemcpyFromSymbol(&flag, ptx::g_abort_flag, sizeof(int)));
-  // (the OUT kernels' translation unit has its own copy, read once one of them has run through this handle)
+  // (the OUT and BF16 kernels' translation units have their own copies, read once one of them has run through this handle)
   if (h->out_launched) FT_CUDA(h, tc_out_abort_flag(&out_flag));
-  if (flag == 0) return out_flag == 0 ? FTSGEMM_OK : FTSGEMM_ERR_TIMEOUT;
+  if (h->bf16_launched) FT_CUDA(h, tc_bf16_abort_flag(&bf16_flag));
+  if (flag == 0) return (out_flag == 0 && bf16_flag == 0) ? FTSGEMM_OK : FTSGEMM_ERR_TIMEOUT;
   flag = 0;
   FT_CUDA(h, cudaMemcpyToSymbol(ptx::g_abort_flag, &flag, sizeof(int)));
   return FTSGEMM_ERR_TIMEOUT;
@@ -269,6 +272,27 @@ int make_tmap_kmajor(ftsgemm_handle_t h, CUtensorMap *tm, const float *base, uin
   return FTSGEMM_OK;
 }
 
+// A BF16 operand (rows x K elements of 2 bytes, row stride ld, entry stride entry_stride elements), always as a 3-D map with
+// the entry as the outer dimension (the BF16 kernels are BATCH kernels; a single product is a batch of one).  K-major: box
+// 64 k (128 bytes) x box_rows rows, the layout of ptx::make_smem_desc_k128; MN-major: box 64 rows (128 bytes) x 64 k, the
+// layout of ptx::make_smem_desc_mn128.  Elements beyond the operand are zero-filled.
+int make_tmap_bf16(ftsgemm_handle_t h, CUtensorMap *tm, const void *base, bool kmajor, uint64_t rows, uint64_t K, uint64_t ld,
+                   uint64_t entry_stride, uint64_t batch, uint32_t box_rows) {
+  const uint64_t es = batch > 1 ? entry_stride : ld * (kmajor ? rows : K);  // (one entry: any valid stride)
+  const cuuint64_t dims[3] = {kmajor ? K : rows, kmajor ? rows : K, batch};
+  const cuuint64_t strides[2] = {ld * 2, es * 2};
+  const cuuint32_t box[3] = {64, kmajor ? box_rows : 64u, 1};
+  const cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = h->encode_tiled(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void *>(base), dims, strides, box, estr,
+                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    h->last_cuda_error = static_cast<int>(r);
+    return FTSGEMM_ERR_CUDA;
+  }
+  return FTSGEMM_OK;
+}
+
 // Largest grid (in work units of CG CTAs) of this instantiation whose CTAs can all be resident at once: one CTA per SM the
 // device reports (multiProcessorCount, which an MPS active-thread percentage reduces), at most as many two-CTA clusters as
 // the device can hold at once (CG = 2), or none when a CTA does not fit.
@@ -276,16 +300,16 @@ int make_tmap_kmajor(ftsgemm_handle_t h, CUtensorMap *tm, const float *base, uin
 // deadlock-free for such a grid, so the planner never gets more units than this.  If SMs are nevertheless held by other
 // work so that the grid cannot become resident, the waits' watchdog (ptx.cuh) ends the launch with FTSGEMM_ERR_TIMEOUT
 // instead of hanging.  Cached per handle (= per device).
+// (kern: the instantiation to measure, cached under `key`; by default the FP32 kernel <BN, FT, CG, PROT>)
 template <int BN, bool FT, int CG, bool PROT = false>
-int query_max_units(ftsgemm_handle_t h, int *out) {
+int query_max_units(ftsgemm_handle_t h, int *out, TcKernel kern = ftsgemm_tc_kernel<BN, FT, CG, PROT>,
+                    int key = BN * 16 + (PROT ? 8 : 0) + (FT ? 4 : 0) + CG) {
   using Cfg = TileCfg<BN, FT, CG>;
-  const int key = BN * 16 + (PROT ? 8 : 0) + (FT ? 4 : 0) + CG;
   auto it = h->max_units.find(key);
   if (it != h->max_units.end()) {
     *out = it->second;
     return FTSGEMM_OK;
   }
-  auto kern = ftsgemm_tc_kernel<BN, FT, CG, PROT>;
   FT_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
   int per_sm = 0;
   FT_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, Cfg::kSmemBytes));
@@ -312,11 +336,24 @@ int query_max_units(ftsgemm_handle_t h, int *out) {
   return FTSGEMM_OK;
 }
 
+template <int BN, int CG>
+int launch_kernel(ftsgemm_handle_t h, TcKernel kern, int resident, const CUtensorMap &tmA, const CUtensorMap &tmB,
+                  const CUtensorMap &tmC, const KernelParams &p, int units, cudaStream_t stream);
+
+// query_max_units of the BF16 kernel of a tile, flags and layouts (ftsgemm_bf16.cu), cached under its own key
+template <int BN, int CG>
+int query_bf16_units(ftsgemm_handle_t h, bool ft, bool seed, bool a_kmajor, bool b_kmajor, int *out) {
+  const TcKernel kern = tc_bf16_kernel(BN, ft, seed, a_kmajor, b_kmajor);
+  if (!kern || CG != 2) return FTSGEMM_ERR_UNSUPPORTED;
+  const int key = (1 << 20) | (BN << 8) | ((ft ? 1 : 0) << 4) | ((seed ? 1 : 0) << 3) | ((a_kmajor ? 1 : 0) << 2) |
+                  ((b_kmajor ? 1 : 0) << 1) | (CG - 1);
+  return query_max_units<BN, true, CG>(h, out, kern, key);
+}
+
 template <int BN, bool FT, int CG, bool PROT, bool SEED, bool BIAS, bool BATCH, bool ACT = false, bool OUT = false>
 int launch_tc(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
               const KernelParams &p, int units, cudaStream_t stream) {
   // p.pdl_wait: the launch may overlap the tail of its predecessor in the stream (KernelParams::pdl_wait)
-  using Cfg = TileCfg<BN, FT, CG>;
   TcKernel kern;
   if constexpr (OUT) {  // (compiled in ftsgemm_out.cu)
     kern = tc_out_kernel(BN, CG, FT, PROT, SEED, BATCH);
@@ -328,6 +365,14 @@ int launch_tc(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB
   int resident = 0;
   const int qrc = query_max_units<BN, FT, CG, PROT>(h, &resident);
   if (qrc) return qrc;
+  return launch_kernel<BN, CG>(h, kern, resident, tmA, tmB, tmC, p, units, stream);
+}
+
+// The launch of one instantiation of ftsgemm_tc_kernel (resident: query_max_units of the tile)
+template <int BN, int CG>
+int launch_kernel(ftsgemm_handle_t h, TcKernel kern, int resident, const CUtensorMap &tmA, const CUtensorMap &tmB,
+                  const CUtensorMap &tmC, const KernelParams &p, int units, cudaStream_t stream) {
+  using Cfg = TileCfg<BN, true, CG>;  // (the shared memory of a tile does not depend on the flags)
   if (units > resident) return FTSGEMM_ERR_UNSUPPORTED;  // the plan was built for more units than can be co-resident
   FT_CUDA(h, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
   cudaLaunchConfig_t cfg = {};
@@ -380,9 +425,19 @@ int with_flag(bool b, F &&f) {
 // ftsgemm_tc_kernel), BATCH for a batch of more than one entry, PROT (fault-tolerant kernels only) for opts.protect_epilogue.
 // An activation (the bias mode is then a run-time field) selects the ACT kernels instead of BIAS: with BATCH for a batch of
 // more than one entry.  A separate output D (p.d, with or without an activation) selects the OUT form of the ACT kernels.
+// bf16: the BF16 kernels (ftsgemm_bf16.cu), which take the bias, the activation, D and the protection level at run time.
 template <int BN, int CG>
 int launch_variant(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
-                   const KernelParams &p, int units, cudaStream_t stream, bool ft, bool prot) {
+                   const KernelParams &p, int units, cudaStream_t stream, bool ft, bool prot, bool bf16 = false) {
+  if (bf16) {
+    const TcKernel kern = tc_bf16_kernel(BN, ft, p.sk_tiles > 0, p.a_kmajor != 0, p.b_kmajor != 0);
+    if (!kern || CG != 2) return FTSGEMM_ERR_UNSUPPORTED;
+    int resident = 0;
+    const int qrc = query_bf16_units<BN, CG>(h, ft, p.sk_tiles > 0, p.a_kmajor != 0, p.b_kmajor != 0, &resident);
+    if (qrc) return qrc;
+    h->bf16_launched = true;
+    return launch_kernel<BN, CG>(h, kern, resident, tmA, tmB, tmC, p, units, stream);
+  }
   if (p.act != kActNone || p.d != nullptr) {
     return with_flag(p.sk_tiles > 0, [&](auto seed) {
       return with_flag(p.batch > 1, [&](auto batch) {
@@ -411,7 +466,9 @@ int launch_variant(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap
 // owner a fixed latency after the piece's last k-block.  (Constants carried over from the previous target, not re-tuned
 // for H100.)
 // l2_bytes: the device's L2 size (cudaDevAttrL2CacheSize)
-PlanInput make_plan_input(int max_units, int CG, int BN, int K, const KernelParams &p, long long l2_bytes) {
+// kbk: k extent of a k-block (a shared-memory stage: 32 FP32 or 64 BF16 values); elem: bytes per operand element
+PlanInput make_plan_input(int max_units, int CG, int BN, int K, const KernelParams &p, long long l2_bytes, int kbk = kBK,
+                          int elem = 4) {
   PlanInput in;
   long long units = dbg("grid", 0);
   in.units = (units > 0 && units <= max_units) ? static_cast<int>(units) : max_units;
@@ -419,14 +476,14 @@ PlanInput make_plan_input(int max_units, int CG, int BN, int K, const KernelPara
   // a strided batch is one tile space: its checksum tile-columns stack the row blocks of all entries (decode_tile_batched)
   in.n_chk_tiles = p.tiles_c * p.tiles_m * p.batch * in.chk_slices;
   in.n_data_tiles = p.tiles_m * p.tiles_n * p.batch;
-  in.num_kb = (K + kBK - 1) / kBK;
+  in.num_kb = (K + kbk - 1) / kbk;
   in.tiles_m = p.tiles_m * p.batch;
   // operands larger than ~3/4 of the L2 (A and B panels cannot stay resident while the units stream them): keep the units
   // in k-lockstep (plan.h).  In a batch one entry's footprint counts: units running at the same time work on neighbouring
   // entries.
   const long long lock = dbg("lockstep", -2);
   in.lockstep = lock >= 0 ? static_cast<int>(lock)
-                          : (4.0 * K * (static_cast<double>(p.M) + p.N) > 0.75 * static_cast<double>(l2_bytes) ? 1 : 0);
+                          : (static_cast<double>(elem) * K * (static_cast<double>(p.M) + p.N) > 0.75 * static_cast<double>(l2_bytes) ? 1 : 0);
   // a checksum item's main loop costs a fixed fraction of a data tile's: larger where data tiles run out of L2, smaller
   // where they are HBM-bound
   const double chk_floor = static_cast<double>(dbg("chk_cost_permille", in.lockstep ? 580 : 680)) * 1e-3;
@@ -450,9 +507,9 @@ PlanInput make_plan_input(int max_units, int CG, int BN, int K, const KernelPara
 // K-slices of the checksum items (KernelParams::chk_slices): only where units would otherwise idle -- all data tiles and
 // all slices run concurrently in one wave -- and a slice keeps at least 8 k-blocks: in such small problems the checksum
 // item's K loop (after the encode) + its epilogue are the critical path.
-int choose_chk_slices(const KernelParams &p, int units, int K) {
+int choose_chk_slices(const KernelParams &p, int units, int K, int kbk = kBK) {
   const long long forced = dbg("chk_slices", -2);
-  const int num_kb = (K + kBK - 1) / kBK;
+  const int num_kb = (K + kbk - 1) / kbk;
   if (p.tiles_c != 1) return 1;
   int s = 1;
   if (forced >= 1) s = static_cast<int>(forced);
@@ -466,7 +523,7 @@ int choose_chk_slices(const KernelParams &p, int units, int K) {
   return s < 1 ? 1 : s;
 }
 
-void plan_tiles(int M, int N, int BN, int CG, bool ft, KernelParams *p) {
+void plan_tiles(int M, int N, int BN, int CG, bool ft, KernelParams *p, bool bf16 = false) {
   p->tiles_m = (M + kBM * CG - 1) / (kBM * CG);
   p->tiles_n = (N + BN - 1) / BN;
   long long g = dbg("group_n", 0);
@@ -475,7 +532,7 @@ void plan_tiles(int M, int N, int BN, int CG, bool ft, KernelParams *p) {
   p->n_chk_cols = 0;
   p->tiles_c = 0;
   if (ft) {
-    p->n_chk_cols = p->tiles_n * kChkPerTile;
+    p->n_chk_cols = p->tiles_n * (bf16 ? kChkPerTileBf16 : kChkPerTile);
     const int cw = chk_cols_per_tile(BN);
     p->tiles_c = (p->n_chk_cols + cw - 1) / cw;
     if (dbg("ft_dbg", 0) & 2) p->tiles_c = 0;  // experiment: no checksum tile-columns (expected checksums are garbage)
@@ -485,11 +542,13 @@ void plan_tiles(int M, int N, int BN, int CG, bool ft, KernelParams *p) {
 // The launch plan of the product in p (M, N, K, batch) for max_units co-resident work units: sets p's tile grid and
 // checksum slices and returns the planner input.  A launch passes the device's co-residency limit, ftsgemm_debug_schedule
 // num_sms / CG -- the schedule it reports is the one a launch on such a device runs.
-PlanInput plan_launch(const Variant &v, int max_units, long long l2_bytes, KernelParams *p) {
+// (bf16: BF16 operands, k-blocks of 64 k and three-term checksums)
+PlanInput plan_launch(const Variant &v, int max_units, long long l2_bytes, KernelParams *p, bool bf16 = false) {
   const bool ft = v.info.fault_tolerant != 0;
-  plan_tiles(p->M, p->N, v.bn, v.cg, ft, p);
-  if (ft) p->chk_slices = choose_chk_slices(*p, max_units, p->K);
-  return make_plan_input(max_units, v.cg, v.bn, p->K, *p, l2_bytes);
+  const int kbk = bf16 ? 2 * kBK : kBK;
+  plan_tiles(p->M, p->N, v.bn, v.cg, ft, p, bf16);
+  if (ft) p->chk_slices = choose_chk_slices(*p, max_units, p->K, kbk);
+  return make_plan_input(max_units, v.cg, v.bn, p->K, *p, l2_bytes, kbk, bf16 ? 2 : 4);
 }
 
 // ------------------------------------------------------------------------------------------- CUDA graph capture
@@ -563,11 +622,19 @@ T *bind(ftsgemm_handle_t h, DevBuf &b) {
 }
 
 // One operand of ftsgemm_run_ex: MN-major (the reference's: element (r, k) at p[r + k*ld]) or K-major (p[k + r*ld]).
+// bf16: the elements are BF16 (ftsgemm_run_batched_typed), p is then their address; ld and the entry strides count elements.
 struct Operand {
   const float *p;
   bool kmajor;
   int ld;
+  bool bf16 = false;
 };
+// the operand advanced by `elems` elements of its type
+Operand offset(const Operand &x, size_t elems) {
+  Operand o = x;
+  o.p = reinterpret_cast<const float *>(reinterpret_cast<const char *>(x.p) + elems * (x.bf16 ? 2 : 4));
+  return o;
+}
 
 // The entries of a strided batch (ftsgemm_run_batched_act): their number, the element strides of A, B and C between them,
 // and that of the bias (0: one bias shared by all entries).
@@ -589,8 +656,10 @@ const ActArg kNoAct = {kActNone, nullptr};
 int check_tc_args(const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, const float *dC, int batch) {
   if ((M % 4) || (N % 4)) return FTSGEMM_ERR_UNSUPPORTED;  // TMA global strides must be multiples of 16 bytes
   if ((A.ld % 4) || (B.ld % 4)) return FTSGEMM_ERR_INVALID_ARG;  // (the same for the rows of an operand)
+  if (A.bf16 && ((A.ld % 8) || (B.ld % 8))) return FTSGEMM_ERR_INVALID_ARG;  // (16-byte rows of BF16)
+  const int kbk = A.bf16 ? 2 * kBK : kBK;
   // work-plan items carry k-block indices in 16 bits and tile indices in 31; the trace / wave tables are sized per unit
-  if ((K + kBK - 1) / kBK > 65535) return FTSGEMM_ERR_UNSUPPORTED;
+  if ((K + kbk - 1) / kbk > 65535) return FTSGEMM_ERR_UNSUPPORTED;
   if ((static_cast<long long>(M + kBM * v.cg - 1) / (kBM * v.cg)) * ((N + v.bn - 1) / v.bn) * batch > (1ll << 28))
     return FTSGEMM_ERR_UNSUPPORTED;
   if (static_cast<long long>(M) * batch > 0x7fffffffll) return FTSGEMM_ERR_UNSUPPORTED;  // stacked rows are ints
@@ -657,7 +726,12 @@ KernelParams make_params(ftsgemm_handle_t h, const Variant &v, int M, int N, int
 // The tensor maps read K-major operands: a K-major operand in place, an MN-major one through its K-major copy (written by
 // the kernel's front phase, row stride ldk: TMA needs 16-byte row strides).  The main loop is the same either way.
 // (a batch: 3-D maps with the entry as the outer dimension; the copies hold one dense rows x ldk block per entry)
-int bind_operands(ftsgemm_handle_t h, const Variant &v, KernelParams &p, CUtensorMap *tmA, CUtensorMap *tmB) {
+// (BF16 operands: always read in place, no copies)
+int bind_operands(ftsgemm_handle_t h, const Variant &v, KernelParams &p, CUtensorMap *tmA, CUtensorMap *tmB, bool bf16 = false) {
+  if (bf16) {
+    const int rc = make_tmap_bf16(h, tmA, p.A, p.a_kmajor != 0, p.M, p.K, p.lda, p.stride_a, p.batch, kBM);
+    return rc ? rc : make_tmap_bf16(h, tmB, p.B, p.b_kmajor != 0, p.N, p.K, p.ldb, p.stride_b, p.batch, v.bn / v.cg);
+  }
   const long long a_copy = static_cast<long long>(p.M) * p.ldk, b_copy = static_cast<long long>(p.N) * p.ldk;
   int rc;
   if (p.a_kmajor) {
@@ -675,14 +749,16 @@ int bind_operands(ftsgemm_handle_t h, const Variant &v, KernelParams &p, CUtenso
 }
 
 // The launch plan for as many work units as the device holds at once.
-int plan_on_device(ftsgemm_handle_t h, const Variant &v, KernelParams &p, PlanInput *pin) {
+int plan_on_device(ftsgemm_handle_t h, const Variant &v, KernelParams &p, PlanInput *pin, bool bf16 = false) {
   int max_units = 0;
   const int rc = with_tile(v.bn, v.cg, [&](auto bn, auto cg) {
+    if (bf16)  // (the BF16 kernel the launch runs; its SEED twin has the same resources and is checked at the launch)
+      return query_bf16_units<bn, cg>(h, v.info.fault_tolerant != 0, false, p.a_kmajor != 0, p.b_kmajor != 0, &max_units);
     return v.info.fault_tolerant ? query_max_units<bn, true, cg>(h, &max_units) : query_max_units<bn, false, cg>(h, &max_units);
   });
   if (rc) return rc;
   if (max_units < 1) return FTSGEMM_ERR_UNSUPPORTED;  // not a single CTA (pair) of this kernel fits on the device partition
-  *pin = plan_launch(v, max_units, h->l2_bytes, &p);
+  *pin = plan_launch(v, max_units, h->l2_bytes, &p, bf16);
   return FTSGEMM_OK;
 }
 
@@ -727,11 +803,14 @@ int launch_encode(ftsgemm_handle_t h, const Variant &v, const KernelParams &p, f
 // The checksum operand (checksum vectors of B: 8 columns per N-tile, appended to B as extra tile-columns of the same GEMM;
 // K-major like B^T: n_chk_cols rows of K, row stride ldk), its encode, and the expected checksums with their slab flags.
 // (a batch: one checksum operand, one block of expected checksums and one run of slab flags per entry)
+// (BF16: a BF16 checksum operand in the layout of B -- K-major: row stride K rounded up to 8; MN-major: [k][checksum
+// column], row stride n_chk_cols rounded up to 8 -- encoded by the kernel's front phase or the pre-pass by the same rule)
 int bind_checksums(ftsgemm_handle_t h, const Variant &v, KernelParams &p, const ftsgemm_opts &o, cudaStream_t stream,
-                   CUtensorMap *tmC) {
+                   CUtensorMap *tmC, bool bf16 = false) {
   p.dbg_flags = static_cast<int>(dbg("ft_dbg", 0)) & 1;
-  const long long chk_entry = static_cast<long long>(p.n_chk_cols) * p.ldk;
-  const size_t chk_bytes = static_cast<size_t>(chk_entry) * p.batch * sizeof(float);
+  const int chk_ld = !bf16 ? p.ldk : p.b_kmajor ? (p.K + 7) / 8 * 8 : (p.n_chk_cols + 7) / 8 * 8;
+  const long long chk_entry = static_cast<long long>(bf16 && !p.b_kmajor ? p.K : p.n_chk_cols) * chk_ld;
+  const size_t chk_bytes = static_cast<size_t>(chk_entry) * p.batch * (bf16 ? 2 : sizeof(float));
   float *chk = nullptr;
   int rc;
   if (h->capturing) {
@@ -757,12 +836,27 @@ int bind_checksums(ftsgemm_handle_t h, const Variant &v, KernelParams &p, const 
   if ((rc = grow(h, h->d_chk_out, flag_bytes + out_floats * sizeof(float), flag_bytes))) return rc;
   p.chk_flags = bind<SeqFlag>(h, h->d_chk_out);
   p.chk_out = bind(h, h->d_chk_out) + flag_bytes / sizeof(float);
-  const ChkKey chk_key = {p.B, p.N, p.K, v.bn, p.b_kmajor != 0, p.ldb, p.batch, p.stride_b};
+  const ChkKey chk_key = {p.B, p.N, p.K, v.bn, p.b_kmajor != 0, p.ldb, p.batch, p.stride_b, bf16};
   const bool reuse = !h->capturing && o.reuse_b_checksums && h->chk_key == chk_key;
   // Default: the encode is part of the FRONT PHASE of the GEMM kernel (KernelParams::enc_front) -- one launch per fused
-  // GEMM, like the reference (sgemm.cu:191-192); only below ~8 MB of B the stand-alone pre-pass is used.
+  // GEMM, like the reference (sgemm.cu:191-192); only below ~8 MB of B (counted in bytes: 4 per FP32, 2 per BF16 element)
+  // the stand-alone pre-pass is used.
   const long long ef = dbg("enc_front", -2);
-  const bool enc_front = !reuse && (ef >= 0 ? ef != 0 : 4.0 * p.N * static_cast<double>(p.K) * p.batch >= static_cast<double>(dbg("enc_front_min_mb", 8)) * 1048576.0);
+  const bool enc_front = !reuse && (ef >= 0 ? ef != 0 : (bf16 ? 2.0 : 4.0) * p.N * static_cast<double>(p.K) * p.batch >= static_cast<double>(dbg("enc_front_min_mb", 8)) * 1048576.0);
+  if (bf16) {
+    if (enc_front) {  // (front_encode_bf16)
+      p.enc_front = 1;
+      p.enc_out = chk;
+      p.enc_ld = chk_ld;
+    } else if (!reuse) {
+      const int blocks = static_cast<int>(dbg("enc_blocks_per_sm", 4)) * h->num_sms;
+      FT_CUDA(h, launch_encode_bf16(v.bn, p.b_kmajor != 0, p.B, p.N, p.K, p.ldb, p.stride_b, p.batch, chk, chk_ld,
+                                    p.batch > 1 ? chk_entry : 0, p.tiles_n, blocks, stream));
+      ++h->launch_count;
+    }
+    if (!reuse && !h->capturing) h->chk_key = chk_key;
+    return make_tmap_bf16(h, tmC, chk, p.b_kmajor != 0, p.n_chk_cols, p.K, chk_ld, chk_entry, p.batch, v.bn / v.cg);
+  }
   if (enc_front) {
     p.enc_front = 1;
     p.enc_out = chk;
@@ -776,10 +870,11 @@ int bind_checksums(ftsgemm_handle_t h, const Variant &v, KernelParams &p, const 
 using CachedPlan = ftsgemm_handle_s::CachedPlan;
 
 // The work plan (plan.h), built and uploaded on first use and cached per shape on the handle.
-int cached_plan(ftsgemm_handle_t h, const Variant &v, const KernelParams &p, const PlanInput &pin, CachedPlan **out) {
-  const std::array<long long, 7> key = {v.info.id, p.M, p.N, p.K, pin.units,
+int cached_plan(ftsgemm_handle_t h, const Variant &v, const KernelParams &p, const PlanInput &pin, CachedPlan **out,
+                bool bf16 = false) {
+  const std::array<long long, 8> key = {v.info.id, p.M, p.N, p.K, pin.units,
                                         pin.force_slices * 16 + pin.max_slices + pin.lockstep * 8192 + pin.full_search * 16384 + pin.chk_slices * 65536,
-                                        p.batch};
+                                        p.batch, bf16 ? 1 : 0};
   CachedPlan &cp = h->plans[key];
   *out = &cp;
   if (cp.uploaded) return FTSGEMM_OK;
@@ -873,14 +968,16 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
            const BatchArg &bt = kSingle, const ActArg &act = kNoAct, float *dD = nullptr) {
   int rc = check_tc_args(v, M, N, K, A, B, dC, bt.count);
   if (rc) return rc;
-  KernelParams p = make_params(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, bt, act, dD);
+  const bool bf16 = A.bf16;
+  // (BF16: the kernels store through D, which is C for an in-place call)
+  KernelParams p = make_params(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, bt, act, bf16 && !dD ? dC : dD);
   CUtensorMap tmA, tmB, tmC;
   PlanInput pin;
-  if ((rc = bind_operands(h, v, p, &tmA, &tmB)) || (rc = plan_on_device(h, v, p, &pin))) return rc;
+  if ((rc = bind_operands(h, v, p, &tmA, &tmB, bf16)) || (rc = plan_on_device(h, v, p, &pin, bf16))) return rc;
   tmC = tmB;
-  if (v.info.fault_tolerant && (rc = bind_checksums(h, v, p, o, stream, &tmC))) return rc;
+  if (v.info.fault_tolerant && (rc = bind_checksums(h, v, p, o, stream, &tmC, bf16))) return rc;
   CachedPlan *cp = nullptr;
-  if ((rc = cached_plan(h, v, p, pin, &cp)) || (rc = bind_plan(h, v, p, pin, *cp, stream))) return rc;
+  if ((rc = cached_plan(h, v, p, pin, &cp, bf16)) || (rc = bind_plan(h, v, p, pin, *cp, stream))) return rc;
   // Programmatic dependent launch by default: the kernel's launch latency and prologue overlap the tail of whatever
   // precedes it in the stream; every thread executes griddepcontrol.wait before the first global access.
   p.pdl_wait = dbg("pdl_chain", 1) != 0 ? 1 : 0;
@@ -888,7 +985,7 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
   ++h->launch_count;
   return with_tile(v.bn, v.cg, [&](auto bn, auto cg) {
     return launch_variant<bn, cg>(h, tmA, tmB, tmC, p, cp->plan.units, stream, v.info.fault_tolerant != 0,
-                                  o.protect_epilogue != 0);
+                                  o.protect_epilogue != 0, bf16);
   });
 }
 
@@ -897,6 +994,13 @@ int run_cublas(ftsgemm_handle_t h, bool tf32, int M, int N, int K, const Operand
   FT_CUBLAS(h, cublasSetStream(h->cublas, stream));
   FT_CUBLAS(h, cublasSetPointerMode(h->cublas, CUBLAS_POINTER_MODE_HOST));
   FT_CUBLAS(h, cublasSetMathMode(h->cublas, tf32 ? CUBLAS_TF32_TENSOR_OP_MATH : CUBLAS_DEFAULT_MATH));
+  if (A.bf16) {  // BF16 A and B, FP32 C, FP32 compute (ids 0 and 7 alike); one entry: strides 0
+    FT_CUBLAS(h, cublasGemmStridedBatchedEx(h->cublas, A.kmajor ? CUBLAS_OP_T : CUBLAS_OP_N, B.kmajor ? CUBLAS_OP_N : CUBLAS_OP_T, M,
+                                            N, K, &alpha, A.p, CUDA_R_16BF, A.ld, bt.sa, B.p, CUDA_R_16BF, B.ld, bt.sb, &beta, dC,
+                                            CUDA_R_32F, ldc, bt.sc, bt.count, CUBLAS_COMPUTE_32F, CUBLAS_GEMM_DEFAULT));
+    h->last_stream = stream;
+    return FTSGEMM_OK;
+  }
   // C = A B^T on column-major buffers: the reference layout is NT, as the reference's verification call (sgemm.cu:108); a
   // K-major A is an M x K matrix stored transposed (OP_T), a K-major B is the K x N matrix B^T itself (OP_N)
   if (bt.count > 1)  // the same transpose flags, one strided-batched call
@@ -1128,7 +1232,8 @@ int run_resolved(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, cons
 int run_segments(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC,
                  int ldc, float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o,
                  cudaStream_t stream, const BatchArg &bt, const ActArg &act, float *dD) {
-  const int num_kb = (K + kBK - 1) / kBK;
+  const int kbk = A.bf16 ? 2 * kBK : kBK;  // (segment boundaries at multiples of the stage depth)
+  const int num_kb = (K + kbk - 1) / kbk;
   const int S = std::min(o.check_segments, num_kb);
   ftsgemm_opts os = o;
   os.check_segments = 1;
@@ -1136,12 +1241,12 @@ int run_segments(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, cons
   int rc = FTSGEMM_OK;
   float *const out = dD ? dD : dC;
   for (int sg = 0; sg < S && !rc; ++sg) {
-    const int k0 = static_cast<int>(static_cast<long long>(num_kb) * sg / S) * kBK;
-    const int k1 = std::min(K, static_cast<int>(static_cast<long long>(num_kb) * (sg + 1) / S) * kBK);
+    const int k0 = static_cast<int>(static_cast<long long>(num_kb) * sg / S) * kbk;
+    const int k1 = std::min(K, static_cast<int>(static_cast<long long>(num_kb) * (sg + 1) / S) * kbk);
     if (sg > 0) os.inject_mode = 0;
     // (a batch: the offsets apply to the base pointers, the entry strides are unchanged)
-    const Operand As = {A.p + (A.kmajor ? static_cast<size_t>(k0) : static_cast<size_t>(k0) * A.ld), A.kmajor, A.ld};
-    const Operand Bs = {B.p + (B.kmajor ? static_cast<size_t>(k0) : static_cast<size_t>(k0) * B.ld), B.kmajor, B.ld};
+    const Operand As = offset(A, A.kmajor ? static_cast<size_t>(k0) : static_cast<size_t>(k0) * A.ld);
+    const Operand Bs = offset(B, B.kmajor ? static_cast<size_t>(k0) : static_cast<size_t>(k0) * B.ld);
     const bool last = sg == S - 1;
     rc = run_resolved(h, v, M, N, k1 - k0, As, Bs, sg == 0 ? dC : out, ldc, alpha, sg == 0 ? beta : 1.0f, last ? bias : nullptr,
                       last ? bias_mode : FTSGEMM_BIAS_NONE, os, stream, bt, last ? act : kNoAct, sg == 0 ? dD : nullptr);
@@ -1392,10 +1497,11 @@ static bool overlaps(const float *p, const float *q, long long n) {
 
 // ftsgemm_run_batched_out (and through it every run entry point): validation, options, capture state, variant; then
 // run_resolved.  dD == dC is the in-place call.
+// (bf16: A and B are BF16, ftsgemm_run_batched_typed)
 static int run_call(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
                     long long stride_a, const float *dB, int layout_b, int ldb, long long stride_b, const float *dC, int ldc,
                     long long stride_c, float *dD, int batch, float alpha, float beta, const float *bias, int bias_mode,
-                    long long stride_bias, const ActArg &act, const ftsgemm_opts *opts) {
+                    long long stride_bias, const ActArg &act, const ftsgemm_opts *opts, bool bf16 = false) {
   if (!h) return FTSGEMM_ERR_NO_DEVICE;
   const bool sep = dD != dC;  // a separate output: C is read-only, and not read at all with beta == 0 (may be null)
   if (!dA || !dB || !dD || (!dC && !(sep && beta == 0.0f)) || M <= 0 || N <= 0 || K <= 0 || batch < 1)
@@ -1405,7 +1511,15 @@ static int run_call(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, cons
   if ((layout_a != FTSGEMM_LAYOUT_MN_MAJOR && layout_a != FTSGEMM_LAYOUT_K_MAJOR) ||
       (layout_b != FTSGEMM_LAYOUT_MN_MAJOR && layout_b != FTSGEMM_LAYOUT_K_MAJOR))
     return FTSGEMM_ERR_INVALID_ARG;
-  const Operand A = {dA, layout_a == FTSGEMM_LAYOUT_K_MAJOR, lda}, B = {dB, layout_b == FTSGEMM_LAYOUT_K_MAJOR, ldb};
+  const Operand A = {dA, layout_a == FTSGEMM_LAYOUT_K_MAJOR, lda, bf16}, B = {dB, layout_b == FTSGEMM_LAYOUT_K_MAJOR, ldb, bf16};
+  // BF16: cuBLAS and the two-CTA wgmma tiles (AUTO resolves to them); TMA needs 16-byte rows and entry strides
+  if (bf16) {
+    if (!(v->info.engine == 0 || (v->info.engine == 1 && (v->bn == 0 || (v->cg == 2 && v->bn >= 128)))))
+      return FTSGEMM_ERR_UNSUPPORTED;
+    if ((lda % 8) || (ldb % 8) || ((reinterpret_cast<uintptr_t>(dA) | reinterpret_cast<uintptr_t>(dB)) & 15))
+      return FTSGEMM_ERR_INVALID_ARG;
+    if (batch > 1 && ((stride_a % 8) || (stride_b % 8))) return FTSGEMM_ERR_INVALID_ARG;
+  }
   if (lda < (A.kmajor ? K : M) || ldb < (B.kmajor ? K : N) || ldc < M) return FTSGEMM_ERR_INVALID_ARG;
   if (bias_mode < FTSGEMM_BIAS_NONE || bias_mode > FTSGEMM_BIAS_COL) return FTSGEMM_ERR_INVALID_ARG;
   if (bias_mode == FTSGEMM_BIAS_NONE) bias = nullptr;
@@ -1439,6 +1553,7 @@ static int run_call(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, cons
   ftsgemm_opts o;
   const int orc = load_opts(opts, &o);
   if (orc) return orc;
+  if (bf16 && o.precision == 1) return FTSGEMM_ERR_INVALID_ARG;  // BF16 products are exact in FP32: nothing to split
   DeviceGuard guard(h);
   cudaStream_t stream = static_cast<cudaStream_t>(o.stream);
   {
@@ -1490,12 +1605,31 @@ int ftsgemm_run_batched_out(ftsgemm_handle_t h, int kernel_id, int M, int N, int
                             long long stride_a, const float *dB, int layout_b, int ldb, long long stride_b, const float *dC,
                             int ldc, long long stride_c, float *dD, int batch, float alpha, float beta, const float *bias,
                             int bias_mode, long long stride_bias, int activation, float *dZ, const ftsgemm_opts *opts) {
+  return ftsgemm_run_batched_typed(h, kernel_id, M, N, K, dA, layout_a, lda, stride_a, dB, layout_b, ldb, stride_b,
+                                   FTSGEMM_TYPE_F32, dC, ldc, stride_c, dD, batch, alpha, beta, bias, bias_mode, stride_bias,
+                                   activation, dZ, opts);
+}
+
+int ftsgemm_run_typed(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const void *dA, int layout_a, int lda,
+                      const void *dB, int layout_b, int ldb, int ab_type, const float *dC, int ldc, float *dD, float alpha,
+                      float beta, const float *bias, int bias_mode, int activation, float *dZ, const ftsgemm_opts *opts) {
+  return ftsgemm_run_batched_typed(h, kernel_id, M, N, K, dA, layout_a, lda, 0, dB, layout_b, ldb, 0, ab_type, dC, ldc, 0, dD, 1,
+                                   alpha, beta, bias, bias_mode, 0, activation, dZ, opts);
+}
+
+int ftsgemm_run_batched_typed(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const void *dA, int layout_a, int lda,
+                              long long stride_a, const void *dB, int layout_b, int ldb, long long stride_b, int ab_type,
+                              const float *dC, int ldc, long long stride_c, float *dD, int batch, float alpha, float beta,
+                              const float *bias, int bias_mode, long long stride_bias, int activation, float *dZ,
+                              const ftsgemm_opts *opts) {
   if (!h) return FTSGEMM_ERR_NO_DEVICE;
+  if (ab_type != FTSGEMM_TYPE_F32 && ab_type != FTSGEMM_TYPE_BF16) return FTSGEMM_ERR_INVALID_ARG;
   if (activation < FTSGEMM_ACT_NONE || activation > FTSGEMM_ACT_GELU) return FTSGEMM_ERR_INVALID_ARG;
   if (dZ && (activation == FTSGEMM_ACT_NONE || dZ == dC || dZ == dD || (reinterpret_cast<uintptr_t>(dZ) & 3)))
     return FTSGEMM_ERR_INVALID_ARG;
-  return run_call(h, kernel_id, M, N, K, dA, layout_a, lda, stride_a, dB, layout_b, ldb, stride_b, dC, ldc, stride_c, dD, batch,
-                  alpha, beta, bias, bias_mode, stride_bias, ActArg{activation, dZ}, opts);
+  return run_call(h, kernel_id, M, N, K, static_cast<const float *>(dA), layout_a, lda, stride_a, static_cast<const float *>(dB),
+                  layout_b, ldb, stride_b, dC, ldc, stride_c, dD, batch, alpha, beta, bias, bias_mode, stride_bias,
+                  ActArg{activation, dZ}, opts, ab_type == FTSGEMM_TYPE_BF16);
 }
 
 int ftsgemm_get_stats(ftsgemm_handle_t h, ftsgemm_stats *out) {

@@ -32,10 +32,16 @@
 //   correct   acc[m,j] = r1[m] - sum_{n != j} acc[m,n]   (recomputed, so Inf/NaN/huge upsets are repaired too;
 //             reference :422-485 adds the row residual)
 // One error per (row, tile) is correctable, i.e. up to 128 per CTA tile (the reference: one per tile per check).
+// BF16 operands (the AB instantiations, csrc/ftsgemm_bf16.cu): wgmma.m64nBNk16 BF16 with the transpose immediates reads
+// either layout in place (the front phase holds at most the encode of B), and the checksum operand holds three BF16 terms
+// per checksum (DESIGN.md 2, 3.1).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
+#include <cuda_bf16.h>
 #include <math_constants.h>
+
+#include <type_traits>
 
 #include "ptx.cuh"
 
@@ -583,14 +589,37 @@ __device__ __forceinline__ void abft_row_sums(uint32_t taddr, int c_begin, int c
 // flags and loads them unless `ready` is already set.
 struct ExpectedChk {
   float e0, e1, w0, w1;
+  float e2, w2;  // (BF16 operands: the third term of each checksum)
   bool ready;
 };
 // (chk_ofs: the entry's block of expected checksums in a strided batch)
 // A row past M has no expected checksum: NaN, so that it is never flagged.  Its accumulator is not always 0 -- A is
 // zero-filled there, and 0 * Inf from a non-finite B is NaN -- and nothing of it is stored.
+// BF16: the checksum operand holds three BF16 terms per checksum (kChkPerTileBf16 columns per N-tile: e hi, mid, lo, w hi,
+// mid, lo); the check adds the three planes in that order.
+constexpr int kChkPerTileBf16 = 6;
+template <bool BF16 = false>
 __device__ __forceinline__ void load_expected(const KernelParams &p, int m, int n_blk, ExpectedChk &x, size_t chk_ofs) {
   x.e0 = CUDART_NAN_F;
   x.e1 = x.w0 = x.w1 = 0.0f;
+  if constexpr (BF16) {
+    x.e2 = x.w2 = 0.0f;
+    if (m < p.M) {
+      const size_t pm = static_cast<size_t>(p.M);
+      const float *cp = p.chk_out + chk_ofs + static_cast<size_t>(n_blk) * kChkPerTileBf16 * pm + m;
+      float v[kChkPerTileBf16];
+#pragma unroll
+      for (int i = 0; i < kChkPerTileBf16; ++i) v[i] = __ldcg(cp + i * pm);
+      const size_t plane = pm * p.n_chk_cols;
+      for (int sl = 1; sl < p.chk_slices; ++sl) {  // K-slices of the checksum product, added in slice order (deterministic)
+        cp += plane;
+#pragma unroll
+        for (int i = 0; i < kChkPerTileBf16; ++i) v[i] += __ldcg(cp + i * pm);
+      }
+      x.e0 = v[0], x.e1 = v[1], x.e2 = v[2], x.w0 = v[3], x.w1 = v[4], x.w2 = v[5];
+    }
+    return;
+  }
   if (m < p.M) {
     const float *cp = p.chk_out + chk_ofs + static_cast<size_t>(n_blk) * kChkPerTile * p.M + m;
     x.e0 = __ldcg(cp);
@@ -619,7 +648,7 @@ __device__ __forceinline__ bool fault_in_entry(const KernelParams &p, int m0_cta
   else return true;
 }
 
-template <int BN, bool BATCH = false>
+template <int BN, bool BATCH = false, bool BF16 = false>
 __device__ __forceinline__ void abft_check(const KernelParams &p, uint32_t taddr, int q, int lane, int m, int m0_cta,
                                            int n0, int n_blk, int &fix_col, float &fix_val, bool &redo, ExpectedChk &xp,
                                            float &own_s1, int c_mid = BN / 32, uint32_t xchg = 0u, int pair_bar = 0,
@@ -675,9 +704,13 @@ __device__ __forceinline__ void abft_check(const KernelParams &p, uint32_t taddr
       }
     }
     __syncwarp();
-    load_expected(p, m, n_blk, xp, chk_ofs);
+    load_expected<BF16>(p, m, n_blk, xp, chk_ofs);
   }
-  const float r1 = xp.e0 + xp.e1, r2 = xp.w0 + xp.w1;
+  float r1 = xp.e0 + xp.e1, r2 = xp.w0 + xp.w1;
+  if constexpr (BF16) {
+    r1 += xp.e2;
+    r2 += xp.w2;
+  }
   const float d1 = r1 - s1, d2 = r2 - s2;
   // (the magnitude term is clamped so that an upset to +-Inf, which makes sabs Inf, cannot make the threshold Inf)
   const float thr = p.tau_abs + p.tau_rel * fminf(sabs, CUDART_MAX_NORMAL_F);
@@ -925,8 +958,11 @@ __device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, flo
 // ------------------------------------------------------------------------------------------------------------
 // (scalars by value: a reference to the __grid_constant__ parameter block would force a local copy of all of it)
 // ACT: the bias mode is read at run time and the row is stored as act(z), with z into Z (when not null); OUT: to D.
-template <int BN, bool BIAS, bool ACT = false, bool OUT = false>
-__device__ __forceinline__ void recompute_row_body(const float *A, const float *B, float *C, int lda, int ldb, int kmajor, int ldc,
+// An operand element as the tensor core reads it: FP32 truncated to TF32, BF16 exactly (ftsgemm_run_batched_typed).
+__device__ __forceinline__ float op_load(const float *p) { return u2f(f2u(__ldg(p)) & 0xFFFFE000u); }
+__device__ __forceinline__ float op_load(const __nv_bfloat16 *p) { return __bfloat162float(__ldg(p)); }
+template <int BN, bool BIAS, bool ACT = false, bool OUT = false, typename T = float>
+__device__ __forceinline__ void recompute_row_body(const T *A, const T *B, float *C, int lda, int ldb, int kmajor, int ldc,
                                                    int N, int K, float alpha, float beta, int m, int n0, int lane, const float *bias,
                                                    int bias_mode, int act_kind = kActNone, float *Z = nullptr, float *D = nullptr) {
   constexpr int J = BN / 32;
@@ -936,15 +972,15 @@ __device__ __forceinline__ void recompute_row_body(const float *A, const float *
   // element (r, k) of an operand at base + r * rs + k * ks
   const size_t a_ks = (kmajor & 1) ? 1 : static_cast<size_t>(lda);
   const size_t b_ns = (kmajor & 2) ? static_cast<size_t>(ldb) : 1, b_ks = (kmajor & 2) ? 1 : static_cast<size_t>(ldb);
-  const float *a = A + static_cast<size_t>(m) * ((kmajor & 1) ? static_cast<size_t>(lda) : 1);
-  const float *b = B + static_cast<size_t>(n0 + lane) * b_ns;
+  const T *a = A + static_cast<size_t>(m) * ((kmajor & 1) ? static_cast<size_t>(lda) : 1);
+  const T *b = B + static_cast<size_t>(n0 + lane) * b_ns;
 #pragma unroll 2
   for (int k = 0; k < K; ++k) {
-    const float av = u2f(f2u(__ldg(a + static_cast<size_t>(k) * a_ks)) & 0xFFFFE000u);
-    const float *bk = b + static_cast<size_t>(k) * b_ks;
+    const float av = op_load(a + static_cast<size_t>(k) * a_ks);
+    const T *bk = b + static_cast<size_t>(k) * b_ks;
 #pragma unroll
     for (int j = 0; j < J; ++j) {
-      const float bv = (n0 + lane + 32 * j < N) ? u2f(f2u(__ldg(bk + 32 * j * b_ns)) & 0xFFFFE000u) : 0.0f;
+      const float bv = (n0 + lane + 32 * j < N) ? op_load(bk + 32 * j * b_ns) : 0.0f;
       acc[j] = fmaf(av, bv, acc[j]);
     }
   }
@@ -988,11 +1024,12 @@ __device__ __noinline__ void recompute_row_act(const float *A, const float *B, f
   recompute_row_body<BN, false, true>(A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, m, n0, lane, bias, bias_mode, act_kind, Z);
 }
 // (the OUT kernels: the row is stored to D; their own entry, so the ACT one keeps its list)
-template <int BN, bool ENTRY = false>
-__device__ __noinline__ void recompute_row_out(const float *A, const float *B, float *C, int lda, int ldb, int kmajor, int ldc,
+// (T: the operand type, float or __nv_bfloat16)
+template <int BN, bool ENTRY = false, typename T = float>
+__device__ __noinline__ void recompute_row_out(const T *A, const T *B, float *C, int lda, int ldb, int kmajor, int ldc,
                                                int N, int K, float alpha, float beta, int m, int n0, int lane, const float *bias,
                                                int bias_mode, int act_kind, float *Z, float *D) {
-  recompute_row_body<BN, false, true, true>(A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, m, n0, lane, bias, bias_mode, act_kind,
+  recompute_row_body<BN, false, true, true, T>(A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, m, n0, lane, bias, bias_mode, act_kind,
                                             Z, D);
 }
 // (D: OUT only, the output the row is stored to)
@@ -1009,8 +1046,8 @@ __device__ __forceinline__ void recompute(const float *bias, int bias_mode, int 
 // block would force a local copy of all of it.  Row segments that fail are counted and, with beta == 0, recomputed from A
 // and B (with beta != 0 the old values of C are already overwritten: reported as uncorrectable -- unless the results go
 // to a separate output D (OUT), which leaves C intact: then the segment is recomputed into D whatever beta is).
-template <int BN, bool BIAS, bool ACT = false, bool ENTRY = false, bool OUT = false>
-__device__ __forceinline__ void protected_store_body(uint32_t taddr, const float *A, const float *B, float *C, int lda, int ldb,
+template <int BN, bool BIAS, bool ACT = false, bool ENTRY = false, bool OUT = false, typename T = float>
+__device__ __forceinline__ void protected_store_body(uint32_t taddr, const T *A, const T *B, float *C, int lda, int ldb,
                                                      int kmajor, int ldc, int N, int K, float alpha, float beta, DeviceStats *stats,
                                                      bool can_recompute, int m, int row0, bool row_ok, int n0, int c_begin, int c_end,
                                                      float chk_s1, bool chk_s1_valid, int bad_col, uint32_t bad_mask, int lane,
@@ -1051,8 +1088,9 @@ __device__ __forceinline__ void protected_store_body(uint32_t taddr, const float
     }
   }
 }
-#define FT_PROT_PARAMS                                                                                                        \
-  uint32_t taddr, const float *A, const float *B, float *C, int lda, int ldb, int kmajor, int ldc, int N, int K, float alpha, \
+#define FT_PROT_PARAMS FT_PROT_PARAMS_T(float)
+#define FT_PROT_PARAMS_T(T)                                                                                                   \
+  uint32_t taddr, const T *A, const T *B, float *C, int lda, int ldb, int kmajor, int ldc, int N, int K, float alpha, \
       float beta, DeviceStats *stats, bool can_recompute, int m, int row0, bool row_ok, int n0, int c_begin, int c_end,        \
       float chk_s1, bool chk_s1_valid, int bad_col, uint32_t bad_mask, int lane
 #define FT_PROT_ARGS                                                                                                            \
@@ -1086,12 +1124,13 @@ __device__ __noinline__ void protected_store_pass_act_batched(FT_PROT_PARAMS, co
 }
 // (the OUT kernels, single (ENTRY = false) and batched: the ACT pass storing to D; their own entries, so the ACT ones keep
 // their lists)
-template <int BN, bool ENTRY>
-__device__ __noinline__ void protected_store_pass_out(FT_PROT_PARAMS, const float *bias, int bias_mode, int row_ofs, int act_kind,
+template <int BN, bool ENTRY, typename T = float>
+__device__ __noinline__ void protected_store_pass_out(FT_PROT_PARAMS_T(T), const float *bias, int bias_mode, int row_ofs, int act_kind,
                                                       float *Z, float *D) {
-  protected_store_body<BN, false, true, ENTRY, true>(FT_PROT_ARGS, bias, bias_mode, row_ofs, act_kind, Z, D);
+  protected_store_body<BN, false, true, ENTRY, true, T>(FT_PROT_ARGS, bias, bias_mode, row_ofs, act_kind, Z, D);
 }
 #undef FT_PROT_PARAMS
+#undef FT_PROT_PARAMS_T
 #undef FT_PROT_ARGS
 template <int BN, bool BIAS, bool BATCH, bool ACT, bool OUT, typename... Args>
 __device__ __forceinline__ void protected_store(const float *bias, int bias_mode, int row_ofs, int act_kind, float *Z, float *D,
@@ -1193,16 +1232,17 @@ __device__ __forceinline__ float chunk_sum(const uint32_t (&v)[32], float &sabs)
   return a0 + a1;
 }
 // The old values are read from C + m and the outputs stored to D + m (D = C but in the OUT kernels' entry).
-#define FT_PROT_V2_PARAMS                                                                                                       \
-  uint32_t taddr, const float *A, const float *B, float *C, int lda, int ldb, int kmajor, int ldc, int N, int K, float alpha,  \
+#define FT_PROT_V2_PARAMS FT_PROT_V2_PARAMS_T(float)
+#define FT_PROT_V2_PARAMS_T(T)                                                                                                  \
+  uint32_t taddr, const T *A, const T *B, float *C, int lda, int ldb, int kmajor, int ldc, int N, int K, float alpha,  \
       float beta, DeviceStats *stats, bool can_recompute, int m, int row0, bool row_ok, int n0, bool ragged_n, int c_begin,    \
       int c_end, float chk_s1, bool chk_s1_valid, StoreUpsets up, int lane, const float *bias, int bias_mode, int row_ofs,     \
       int act_kind, float *Z
 #define FT_PROT_V2_ARGS                                                                                                          \
   taddr, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, stats, can_recompute, m, row0, row_ok, n0, ragged_n, c_begin, c_end, \
       chk_s1, chk_s1_valid, up, lane, bias, bias_mode, row_ofs, act_kind, Z
-template <bool BIAS, bool ACT, bool ENTRY, bool OUT>
-__device__ __forceinline__ void protected_store_v2_body(FT_PROT_V2_PARAMS, float *D) {
+template <bool BIAS, bool ACT, bool ENTRY, bool OUT, typename T = float>
+__device__ __forceinline__ void protected_store_v2_body(FT_PROT_V2_PARAMS_T(T), float *D) {
   // ---- pass 1: the chunk sums, and their running sum against the check's ----
   float sc[kMaxChunks];
   float s1 = 0.0f;
@@ -1352,11 +1392,12 @@ __device__ __noinline__ void protected_store_pass_v2(FT_PROT_V2_PARAMS) {
   protected_store_v2_body<BIAS, ACT, ENTRY, false>(FT_PROT_V2_ARGS, C);
 }
 // (the OUT kernels, which also take the output D: their own entry, so the one above keeps its list)
-template <bool ENTRY>
-__device__ __noinline__ void protected_store_pass_v2_out(FT_PROT_V2_PARAMS, float *D) {
-  protected_store_v2_body<false, true, ENTRY, true>(FT_PROT_V2_ARGS, D);
+template <bool ENTRY, typename T = float>
+__device__ __noinline__ void protected_store_pass_v2_out(FT_PROT_V2_PARAMS_T(T), float *D) {
+  protected_store_v2_body<false, true, ENTRY, true, T>(FT_PROT_V2_ARGS, D);
 }
 #undef FT_PROT_V2_PARAMS
+#undef FT_PROT_V2_PARAMS_T
 #undef FT_PROT_V2_ARGS
 template <bool BIAS, bool ACT, bool ENTRY, bool OUT, typename... Args>
 __device__ __forceinline__ void protected_store_v2(float *D, Args... args) {
@@ -1818,6 +1859,102 @@ __device__ __noinline__ void front_phase(const float *A, const float *B, int M, 
   }
 }
 
+// ENCODE of a BF16 B (ftsgemm_run_batched_typed): per N-tile t and k, the plain and weighted column-block sums of the exact
+// BF16 values,
+//   e = sum_{n in block t} B[n,k]      w = sum_{n in block t} (n - n0 + 1) B[n,k]
+// as FP32 partial sums over groups of at most 8 elements (exact for BF16 inputs whose magnitudes differ by less than 2^8),
+// FP64 totals, each stored as three BF16 terms (hi, mid, lo: the remainder of the FP64 total after the terms before, rounded
+// to nearest), checksum columns t*6 + {0, 1, 2} (e) and t*6 + {3, 4, 5} (w) of the checksum operand, which has the layout
+// of B (K-major: chk[column][chk_ld], MN-major: chk[k][chk_ld]).  Run by the stand-alone pre-pass (ftsgemm_bf16.cu) or by
+// every warp of the GEMM kernel's front phase (front_encode_bf16), the same sums either way.
+__device__ __forceinline__ void store_split3(__nv_bfloat16 *dst, size_t ld, double x) {
+  const __nv_bfloat16 h = __float2bfloat16_rn(static_cast<float>(x));
+  const double r1 = x - static_cast<double>(__bfloat162float(h));
+  const __nv_bfloat16 m = __float2bfloat16_rn(static_cast<float>(r1));
+  const double r2 = r1 - static_cast<double>(__bfloat162float(m));
+  dst[0] = h;
+  dst[ld] = m;
+  dst[2 * ld] = __float2bfloat16_rn(static_cast<float>(r2));
+}
+// MN-major B (element (n, k) at B[n + k*ldb]), one entry: warp gw of nw takes the (k, N-tile) items gw, gw + nw, ...; lane L
+// sums the elements L, L + 32, ... of the block's row k (coalesced) in FP32, and the 32 lanes are added in FP64 (butterfly).
+template <int BN>
+__device__ __forceinline__ void encode_bf16_mn_items(const __nv_bfloat16 *__restrict__ B, int N, int K, int ldb,
+                                                     __nv_bfloat16 *__restrict__ chk, int chk_ld, int tiles_n, long long gw,
+                                                     long long nw, int lane) {
+  const long long items = static_cast<long long>(K) * tiles_n;
+  for (long long it = gw; it < items; it += nw) {
+    const int k = static_cast<int>(it / tiles_n), t = static_cast<int>(it - static_cast<long long>(k) * tiles_n);
+    const int n0 = t * BN;
+    const __nv_bfloat16 *row = B + static_cast<size_t>(k) * ldb;
+    float se = 0.0f, sw = 0.0f;
+#pragma unroll
+    for (int i = 0; i < BN / 32; ++i) {
+      const int j = lane + 32 * i;
+      const float b = (n0 + j < N) ? __bfloat162float(row[n0 + j]) : 0.0f;
+      se += b;
+      sw = fmaf(b, static_cast<float>(j + 1), sw);
+    }
+    double de = se, dw = sw;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      de += __shfl_xor_sync(0xffffffffu, de, o);
+      dw += __shfl_xor_sync(0xffffffffu, dw, o);
+    }
+    if (lane == 0) {
+      __nv_bfloat16 *row_k = chk + static_cast<size_t>(k) * chk_ld + t * kChkPerTileBf16;
+      store_split3(row_k, 1, de);
+      store_split3(row_k + 3, 1, dw);
+    }
+  }
+}
+// K-major B (element (n, k) at B[k + n*ldb]), one entry: thread gt of nt takes the (k, N-tile) items gt, gt + nt, ..., k
+// fastest (a warp reads 64 contiguous bytes of each row); FP32 partial sums over groups of 8 rows, FP64 totals.
+template <int BN>
+__device__ __forceinline__ void encode_bf16_k_items(const __nv_bfloat16 *__restrict__ B, int N, int K, int ldb,
+                                                    __nv_bfloat16 *__restrict__ chk, int chk_ld, int tiles_n, long long gt,
+                                                    long long nt) {
+  const long long items = static_cast<long long>(K) * tiles_n;
+  for (long long it = gt; it < items; it += nt) {
+    const int t = static_cast<int>(it / K), k = static_cast<int>(it - static_cast<long long>(t) * K);
+    const int n0 = t * BN;
+    const int rows = min(BN, N - n0);
+    const __nv_bfloat16 *src = B + static_cast<size_t>(n0) * ldb + k;
+    double de = 0.0, dw = 0.0;
+    for (int g = 0; g < rows; g += 8) {
+      float se = 0.0f, sw = 0.0f;
+#pragma unroll
+      for (int r = 0; r < 8; ++r) {
+        if (g + r < rows) {
+          const float b = __bfloat162float(src[static_cast<size_t>(g + r) * ldb]);
+          se += b;
+          sw = fmaf(b, static_cast<float>(g + r + 1), sw);
+        }
+      }
+      de += se;
+      dw += sw;
+    }
+    const size_t ld = static_cast<size_t>(chk_ld);
+    store_split3(chk + static_cast<size_t>(t * kChkPerTileBf16) * ld + k, ld, de);
+    store_split3(chk + static_cast<size_t>(t * kChkPerTileBf16 + 3) * ld + k, ld, dw);
+  }
+}
+// The front phase of a BF16 launch with enc_front (B of 8 MB or more): the encode of every entry of B, entry e at
+// B + e*stride_b into chk + e*chk_stride, split over all warps of the grid.  Out of line and with scalars by value, as
+// front_phase.
+template <int BN>
+__device__ __noinline__ void front_encode_bf16(const __nv_bfloat16 *B, int N, int K, int ldb, long long stride_b, int batch,
+                                               __nv_bfloat16 *chk, int chk_ld, long long chk_stride, int tiles_n, int b_kmajor,
+                                               int gw, int nw, int lane) {
+  for (int e = 0; e < batch; ++e) {
+    if (b_kmajor)
+      encode_bf16_k_items<BN>(B + e * stride_b, N, K, ldb, chk + e * chk_stride, chk_ld, tiles_n,
+                              static_cast<long long>(gw) * 32 + lane, static_cast<long long>(nw) * 32);
+    else
+      encode_bf16_mn_items<BN>(B + e * stride_b, N, K, ldb, chk + e * chk_stride, chk_ld, tiles_n, gw, nw, lane);
+  }
+}
+
 template <int BN>
 __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
   if constexpr (BN == 32) ptx::wgmma_tf32_n32(d, a_desc, b_desc, scale_d);
@@ -1825,6 +1962,29 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t a_desc, 
   else if constexpr (BN == 128) ptx::wgmma_tf32_n128(d, a_desc, b_desc, scale_d);
   else ptx::wgmma_tf32_n256(d, a_desc, b_desc, scale_d);
 }
+
+// BF16 operands: A_MN / B_MN select the transpose immediates (the operand is MN-major in shared memory)
+template <int BN, bool A_MN, bool B_MN>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[BN / 2], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  static_assert(BN == 128 || BN == 256, "BF16 tiles");
+  if constexpr (BN == 128) ptx::wgmma_bf16_n128<A_MN, B_MN>(d, a_desc, b_desc, scale_d);
+  else ptx::wgmma_bf16_n256<A_MN, B_MN>(d, a_desc, b_desc, scale_d);
+}
+// The operand form of an instantiation (ftsgemm_tc_kernel's AB): 0 = FP32 operands; BF16 operands with the layout of A and
+// of B in shared memory as compile-time bits, so that the transpose immediates are constants (wgmmas chosen by a run-time
+// branch are serialised by ptxas)
+constexpr int kAbBf16 = 1, kAbAMn = 2, kAbBMn = 4;
+// Whether a PROT kernel runs the level-1 protected store pass: the BF16 kernels take the level at run time (0: the plain
+// store pass), the FP32 PROT kernels are only launched with a level.  (A helper: the same test written as
+// `!BF16 || p.protect != 0` in the kernel moved the spills of the FP32 PROT kernels.)
+template <bool BF16>
+__device__ __forceinline__ bool level1_on(const KernelParams &p) {
+  if constexpr (BF16) return p.protect != 0;
+  else return true;
+}
+// the caller's operand pointer as the kernel's operand type (the identity for FP32)
+template <typename T>
+__device__ __forceinline__ const T *op_ptr(const float *p) { return reinterpret_cast<const T *>(p); }
 
 // ------------------------------------------------------------------------------------------------------------
 // The kernel.
@@ -1846,13 +2006,22 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[BN / 2], uint64_t a_desc, 
 // OUT: the ACT instantiation for calls with a separate output D (ftsgemm_run_batched_out): every final value reads its old
 // value from C and is stored to p.d (C's geometry; with BATCH p.d + entry * stride_c), ACT_NONE included.  Its own binary,
 // so that the ACT kernels are compiled exactly as without the feature.
+// AB != 0: the instantiations for BF16 operands (ftsgemm_run_batched_typed; compiled in ftsgemm_bf16.cu): p.A / p.B point at
+// BF16 elements (leading dimensions and entry strides in elements), a stage holds 64 k, and an MN-major operand is read in
+// place with TMA boxes in the MN-major layout and the wgmma transpose immediates -- no front phase.  The checksum operand
+// is BF16 with three terms per checksum (kChkPerTileBf16), in the layout of B.  The layouts of A and B are template bits
+// (kAbAMn, kAbBMn).  Only the OUT x BATCH form of the two-CTA tiles exists: bias mode, activation, Z and D (D == C in place)
+// are run-time fields, and with PROT the protection level is read at run time too (0: the plain store pass).
 template <int BN, bool FT, int CG, bool PROT = false, bool SEED = false, bool BIAS = false, bool BATCH = false, bool ACT = false,
-          bool OUT = false>
+          bool OUT = false, int AB = 0>
 __global__ void __launch_bounds__(kThreads, 1)
 ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmChk, const KernelParams p) {
+  constexpr bool BF16 = AB != 0, A_MN = (AB & kAbAMn) != 0, B_MN = (AB & kAbBMn) != 0;
   static_assert(!(ACT && BIAS), "the ACT kernels take the bias mode at run time");
   static_assert(!OUT || ACT, "the OUT kernels are ACT kernels");
+  static_assert(!BF16 || (OUT && BATCH && CG == 2 && BN >= 128), "BF16: the OUT x BATCH form of the two-CTA tiles");
+  using OpT = std::conditional_t<BF16, __nv_bfloat16, float>;  // operand element type
   using Cfg = TileCfg<BN, FT, CG>;
   constexpr int kStages = Cfg::kStages;
   constexpr int kAccRegs = BN / 2;  // per thread of a consumer warpgroup: 64 x BN FP32
@@ -1902,9 +2071,17 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   {
     // front phase: transposes of the MN-major operands (+ the encode of B); the ring is free scratch until the producer starts
     const int gw = static_cast<int>(blockIdx.x) * (kThreads / 32) + warp, nw = static_cast<int>(gridDim.x) * (kThreads / 32);
-    front_phase<BN, FT>(p.A, p.B, p.M, p.N, p.K, p.lda, p.ldb, p.a_kmajor, p.b_kmajor, BATCH ? p.stride_a : 0, BATCH ? p.stride_b : 0, BATCH ? p.batch : 1, p.At, p.Bt,
-                        p.ldk, p.enc_front, p.enc_out, p.enc_ld, p.n_chk_cols, p.tiles_n, gw, nw, lane, smem_base + warp * kTrScratch,
-                        &p.seq->front_next);
+    if constexpr (BF16) {  // (no transposes: only the encode of B, for B of 8 MB or more)
+      if (FT && p.enc_front)
+        front_encode_bf16<BN>(reinterpret_cast<const __nv_bfloat16 *>(p.B), p.N, p.K, p.ldb, p.stride_b, p.batch,
+                              reinterpret_cast<__nv_bfloat16 *>(p.enc_out), p.enc_ld,
+                              static_cast<long long>(p.b_kmajor ? p.n_chk_cols : p.K) * p.enc_ld, p.tiles_n, p.b_kmajor, gw, nw,
+                              lane);
+    } else {
+      front_phase<BN, FT>(p.A, p.B, p.M, p.N, p.K, p.lda, p.ldb, p.a_kmajor, p.b_kmajor, BATCH ? p.stride_a : 0, BATCH ? p.stride_b : 0, BATCH ? p.batch : 1, p.At, p.Bt,
+                          p.ldk, p.enc_front, p.enc_out, p.enc_ld, p.n_chk_cols, p.tiles_n, gw, nw, lane, smem_base + warp * kTrScratch,
+                          &p.seq->front_next);
+    }
     ptx::fence_proxy_async();  // this warp's shared-memory scratch accesses before the TMA writes into the ring
     __syncwarp();              // the warp's stores are ordered before lane 0's release (cumulativity)
     if (lane == 0) {
@@ -1958,11 +2135,29 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           ptx::mbar_wait(empty_bar(stage), phase ^ 1u);
           const uint32_t sA = smem_base + stage * Cfg::kStageBytes;
           const uint32_t sB = sA + Cfg::kABytes;
-          const int k0 = kb * kBK;
+          const int k0 = kb * (BF16 ? 2 * kBK : kBK);
           if (ptx::elect_one()) {
             // (CG = 2: own A box + own B half + the peer's B half = kStageBytes as well)
             ptx::mbar_arrive_expect_tx(full_bar(stage), static_cast<uint32_t>(Cfg::kStageBytes));
-            if constexpr (BATCH) {  // (the entry is the outer coordinate of every map, the checksum operand's too)
+            if constexpr (BF16) {
+              // K-major: one box of 64 k x rows; MN-major: boxes of 64 rows x 64 k, 8 KiB apart (ptx::make_smem_desc_mn128).
+              // The checksum operand has the layout of B.
+              if constexpr (!A_MN) {
+                ptx::tma_load_3d(sA, &tmA, full_bar(stage), k0, m0, tc.batch);
+              } else {
+                ptx::tma_load_3d(sA, &tmA, full_bar(stage), m0, k0, tc.batch);
+                ptx::tma_load_3d(sA + 8192, &tmA, full_bar(stage), m0 + 64, k0, tc.batch);
+              }
+              const uint32_t dst = sB + cta_rank * (Cfg::kBBytes / 2);
+              const int n_half = nb0 + cta_rank * (BN / 2);
+              if constexpr (!B_MN) {
+                ptx::tma_load_3d_multicast(dst, tmb, full_bar(stage), k0, n_half, tc.batch, 0x3);
+              } else {
+#pragma unroll
+                for (int j = 0; j < BN / 128; ++j)
+                  ptx::tma_load_3d_multicast(dst + j * 8192, tmb, full_bar(stage), n_half + 64 * j, k0, tc.batch, 0x3);
+              }
+            } else if constexpr (BATCH) {  // (the entry is the outer coordinate of every map, the checksum operand's too)
               ptx::tma_load_3d(sA, &tmA, full_bar(stage), k0, m0, tc.batch);
               if constexpr (CG == 2)
                 ptx::tma_load_3d_multicast(sB + cta_rank * (Cfg::kBBytes / 2), tmb, full_bar(stage), k0, nb0 + cta_rank * (BN / 2), tc.batch, 0x3);
@@ -2024,8 +2219,8 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const int bt = BATCH ? tc.batch : 0;
       // (without BATCH the call sites read p.A / p.B / p.C themselves: pointers formed up front, even equal to them, moved the
       // register allocation of the biased fault-tolerant kernels)
-      const float *const Ab = BATCH ? p.A + bt * p.stride_a : nullptr;
-      const float *const Bb = BATCH ? p.B + bt * p.stride_b : nullptr;
+      const OpT *const Ab = BATCH ? reinterpret_cast<const OpT *>(p.A) + bt * p.stride_a : nullptr;
+      const OpT *const Bb = BATCH ? reinterpret_cast<const OpT *>(p.B) + bt * p.stride_b : nullptr;
       float *const Cb = BATCH ? p.C + bt * p.stride_c : nullptr;
       const float *const biasb = BATCH ? p.bias + ((BIAS || ACT) ? bt * p.stride_bias : 0) : nullptr;  // (the entry's bias)
       float *const Zb = (BATCH && ACT && p.z != nullptr) ? p.z + bt * p.stride_c : nullptr;          // (Z: C's geometry)
@@ -2070,9 +2265,18 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const uint32_t sA = smem_base + stage * Cfg::kStageBytes + cw * (64 * kBK * 4);
         const uint32_t sB = smem_base + stage * Cfg::kStageBytes + Cfg::kABytes;
         ptx::wgmma_fence();
+        if constexpr (BF16) {
 #pragma unroll
-        for (int j = 0; j < kBK / 8; ++j)
-          wgmma_tf32<BN>(acc, ptx::make_smem_desc_k128(sA + 32 * j), ptx::make_smem_desc_k128(sB + 32 * j), j == 0 ? scale_d : 1u);
+          for (int j = 0; j < 2 * kBK / 16; ++j) {
+            const uint64_t da = A_MN ? ptx::make_smem_desc_mn128(sA + 2048 * j) : ptx::make_smem_desc_k128(sA + 32 * j);
+            const uint64_t db = B_MN ? ptx::make_smem_desc_mn128(sB + 2048 * j) : ptx::make_smem_desc_k128(sB + 32 * j);
+            wgmma_bf16<BN, A_MN, B_MN>(acc, da, db, j == 0 ? scale_d : 1u);
+          }
+        } else {
+#pragma unroll
+          for (int j = 0; j < kBK / 8; ++j)
+            wgmma_tf32<BN>(acc, ptx::make_smem_desc_k128(sA + 32 * j), ptx::make_smem_desc_k128(sB + 32 * j), j == 0 ? scale_d : 1u);
+        }
         scale_d = 1u;
         ptx::wgmma_commit();
         // one k-block stays in flight; the one before it is complete and its stage goes back to the producer
@@ -2121,16 +2325,16 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             if constexpr (PROT) stale = (ptx::ld_acquire_shared_u32(xchg_base(q) + 4) >> lane) & 1u;  // rows it repaired
           }
           if (PROT && FT && !(p.dbg_flags & 1) && p.protect == 2) {
-            protected_store_v2<BIAS, ACT, ACT && BATCH, OUT>(Db, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1),
+            protected_store_v2<BIAS, ACT, ACT && BATCH, OUT>(Db, taddr, BATCH ? Ab : op_ptr<OpT>(p.A), BATCH ? Bb : op_ptr<OpT>(p.B), BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1),
                                                p.ldc, p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m,
                                                m0_cta + q * 32, m < p.M && !skip, n0, n0 + BN > p.N, kMid, BN / 32, s1, stale == 0u,
                                                stored_value_upsets<BN, BATCH>(p, q, lane, m0_cta, n0, kMid, BN / 32, row_ofs), lane,
                                                (BIAS || ACT) ? (BATCH ? biasb : p.bias) : nullptr, p.bias_mode, row_ofs, ACT ? p.act : 0,
                                                ACT ? (BATCH ? Zb : p.z) : nullptr);
-          } else if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N) {
+          } else if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N && level1_on<BF16>(p)) {
             uint32_t bad_bits = 0u;
             const int bad_col = stored_value_fault<BN, BATCH>(p, q, lane, m0_cta, n0, kMid, BN / 32, bad_bits, row_ofs);
-            protected_store<BN, BIAS, BATCH, ACT, OUT>(BATCH ? biasb : p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? (BATCH ? Zb : p.z) : nullptr, Db, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
+            protected_store<BN, BIAS, BATCH, ACT, OUT>(BATCH ? biasb : p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? (BATCH ? Zb : p.z) : nullptr, Db, taddr, BATCH ? Ab : op_ptr<OpT>(p.A), BATCH ? Bb : op_ptr<OpT>(p.B), BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
                                       p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32,
                                       m < p.M && !skip, n0, kMid, BN / 32, s1, stale == 0u, bad_col, bad_bits, lane);
           } else {
@@ -2163,7 +2367,7 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         ExpectedChk xp;
         xp.ready = false;
         if (FT && !(p.dbg_flags & 1))
-          abft_check<BN, BATCH>(p, taddr, q, lane, m, m0_cta, n0, tc.n_blk, fix_col, fix_val, redo, xp, own_s1, c_mid, xchg_base(q), 4 + q,
+          abft_check<BN, BATCH, BF16>(p, taddr, q, lane, m, m0_cta, n0, tc.n_blk, fix_col, fix_val, redo, xp, own_s1, c_mid, xchg_base(q), 4 + q,
                          row_ofs, slab_ofs, chk_ofs);
         // rows to recompute are skipped by both store passes (the helper reads the mask after the pair barrier below)
         const unsigned redo_mask = FT ? __ballot_sync(0xffffffffu, redo) : 0u;
@@ -2192,17 +2396,17 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
         if (assist_on && FT && !(p.dbg_flags & 1)) ptx::named_bar_sync(4 + q, 64);  // corrections are in place
         if (PROT && FT && !(p.dbg_flags & 1) && p.protect == 2) {
-          protected_store_v2<BIAS, ACT, ACT && BATCH, OUT>(Db, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1),
+          protected_store_v2<BIAS, ACT, ACT && BATCH, OUT>(Db, taddr, BATCH ? Ab : op_ptr<OpT>(p.A), BATCH ? Bb : op_ptr<OpT>(p.B), BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1),
                                              p.ldc, p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m,
                                              m0_cta + q * 32, m < p.M && !redo, n0, n0 + BN > p.N, 0, c_mid, own_s1,
                                              ((stale_mask >> lane) & 1u) == 0u,
                                              stored_value_upsets<BN, BATCH>(p, q, lane, m0_cta, n0, 0, c_mid, row_ofs), lane,
                                              (BIAS || ACT) ? (BATCH ? biasb : p.bias) : nullptr, p.bias_mode, row_ofs, ACT ? p.act : 0,
                                              ACT ? (BATCH ? Zb : p.z) : nullptr);
-        } else if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N) {
+        } else if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N && level1_on<BF16>(p)) {
           uint32_t bad_bits = 0u;
           const int bad_col = stored_value_fault<BN, BATCH>(p, q, lane, m0_cta, n0, 0, c_mid, bad_bits, row_ofs);
-          protected_store<BN, BIAS, BATCH, ACT, OUT>(BATCH ? biasb : p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? (BATCH ? Zb : p.z) : nullptr, Db, taddr, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
+          protected_store<BN, BIAS, BATCH, ACT, OUT>(BATCH ? biasb : p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? (BATCH ? Zb : p.z) : nullptr, Db, taddr, BATCH ? Ab : op_ptr<OpT>(p.A), BATCH ? Bb : op_ptr<OpT>(p.B), BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
                                     p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32,
                                     m < p.M && !redo, n0, 0, c_mid, own_s1, ((stale_mask >> lane) & 1u) == 0u, bad_col, bad_bits, lane);
         } else {
@@ -2215,7 +2419,7 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           while (rm != 0u) {
             const int r = __ffs(rm) - 1;
             rm &= rm - 1u;
-            recompute<BN, BIAS, ACT, ACT && BATCH, OUT>(BATCH ? biasb : p.bias, p.bias_mode, ACT ? p.act : 0, ACT ? (BATCH ? Zb : p.z) : nullptr, Db, BATCH ? Ab : p.A, BATCH ? Bb : p.B, BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K,
+            recompute<BN, BIAS, ACT, ACT && BATCH, OUT>(BATCH ? biasb : p.bias, p.bias_mode, ACT ? p.act : 0, ACT ? (BATCH ? Zb : p.z) : nullptr, Db, BATCH ? Ab : op_ptr<OpT>(p.A), BATCH ? Bb : op_ptr<OpT>(p.B), BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K,
                                 p.alpha, p.beta, m0_cta + q * 32 + r, n0, lane);
           }
         }
@@ -2310,5 +2514,12 @@ encode_kernel(const float *__restrict__ B, int N, int K, int ldb, long long stri
 using TcKernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, KernelParams);
 TcKernel tc_out_kernel(int bn, int cg, bool ft, bool prot, bool seed, bool batch);
 cudaError_t tc_out_abort_flag(int *flag);
+// The BF16 kernels (ftsgemm_bf16.cu): the two-CTA tile of width bn (128 or 256) for A and B in the given layouts, fault-
+// tolerant or not, or null; the encode pre-pass of a BF16 B (both layouts, `batch` entries stride_b elements apart) into its
+// BF16 checksum operand, in B's layout (K-major: [checksum column][chk_ld]; MN-major: [k][chk_ld]); the unit's abort flag.
+TcKernel tc_bf16_kernel(int bn, bool ft, bool seed, bool a_kmajor, bool b_kmajor);
+cudaError_t launch_encode_bf16(int bn, bool b_kmajor, const void *B, int N, int K, int ldb, long long stride_b, int batch,
+                               void *chk, int chk_ld, long long chk_stride, int tiles_n, int blocks, cudaStream_t stream);
+cudaError_t tc_bf16_abort_flag(int *flag);
 
 }  // namespace ftsgemm

@@ -191,7 +191,8 @@ int ftsgemm_create(ftsgemm_handle_t *out);   /* binds to the current CUDA device
                                                  stream at a time (use one handle per concurrently used stream). */
 /* CUDA graphs.  The compute calls may be captured into a CUDA graph (stream capture in any mode, e.g. torch.cuda.graph) and
  * replayed; a replay computes what the same call computes eagerly on the buffers' contents at replay time, bit for bit.
- *  - Captured as they are: ftsgemm_run / _run_ex / _run_bias / _run_batched / _run_act on the tensor-core ids (with every option:
+ *  - Captured as they are: ftsgemm_run / _run_ex / _run_bias / _run_batched / _run_act / _run_out / _run_batched_out /
+ *    _run_typed / _run_batched_typed on the tensor-core ids (with every option:
  *    3xTF32, check_segments, protect_epilogue, injected faults) and the cuBLAS ids 0 / 7, the encode pre-pass,
  *    and ftsgemm_stats_device.  A first call of a new shape may be
  *    captured: its workspaces and work plan are allocated and uploaded outside the capture.  reuse_b_checksums has no
@@ -212,7 +213,8 @@ const char *ftsgemm_error_string(int code);
 int ftsgemm_last_cuda_error(ftsgemm_handle_t h); /* cudaError_t / CUresult of the last failure, 0 if none */
 /* Number of kernels of THIS library (fused GEMM, encode pre-pass, hi/lo split, verdict snapshot; not cuBLAS') launched
  * through the handle since it was created: a fused ABFT GEMM is 1 launch (the encode is a front phase of the kernel),
- * 2 below ~8 MB of B (separate pre-pass) -- what bench.py reports as gpu_launches. */
+ * 2 below ~8 MB of B (separate pre-pass) -- what bench.py reports as gpu_launches.  With BF16 operands
+ * (ftsgemm_run_batched_typed) the same rule counts B's bytes (2 per element): 1 launch from 8 MB of B, 2 below. */
 unsigned long long ftsgemm_launch_count(ftsgemm_handle_t h);
 void ftsgemm_default_opts(ftsgemm_opts *o);
 
@@ -375,6 +377,39 @@ int ftsgemm_run_batched_out(ftsgemm_handle_t h, int kernel_id, int M, int N, int
 int ftsgemm_run_out(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
                     const float *dB, int layout_b, int ldb, const float *dC, int ldc, float *dD, float alpha, float beta,
                     const float *bias, int bias_mode, int activation, float *dZ, const ftsgemm_opts *opts);
+
+/* Operand element types of ftsgemm_run_batched_typed. */
+#define FTSGEMM_TYPE_F32 0
+#define FTSGEMM_TYPE_BF16 1
+
+/* ftsgemm_run_batched_out with A and B of element type ab_type (both the same): cublasGemmStridedBatchedEx with
+ * CUDA_R_16BF A / B, FP32 C / D and CUBLAS_COMPUTE_32F.  Accumulation, C, D, Z and the bias are FP32; so are the
+ * checksums and everything after the main loop.  FTSGEMM_TYPE_F32 is ftsgemm_run_batched_out, bit for bit (which is this
+ * call's wrapper).
+ * BF16 (FTSGEMM_TYPE_BF16):
+ *  - lda, ldb, stride_a and stride_b count BF16 elements; lda % 8 == 0, ldb % 8 == 0, stride_a % 8 == 0 and stride_b % 8 == 0
+ *    (batch > 1), and A and B 16-byte aligned, or FTSGEMM_ERR_INVALID_ARG.  M % 4 and N % 4 as for FP32; K is free.
+ *  - Kernel ids: the two-CTA tiles 256 x 256 (21 / 31) and 256 x 128 (3 / 13 / 22 / 32), AUTO (20 / 40), and cuBLAS (0 and 7
+ *    alike: BF16 A / B, FP32 C, compute 32F).  Every other id, the baseline ids 10 / 30 included: FTSGEMM_ERR_UNSUPPORTED.
+ *  - Both layouts of A and of B are read in place by TMA (the wgmma transpose bits): no transposes, no workspace copies.
+ *  - A stage holds 64 k; opts.check_segments splits K at multiples of 64.
+ *  - The checksum operand holds each checksum of B as three BF16 terms (hi, mid, lo: 24 significant bits).  It is encoded
+ *    by the FP32 rule counted in bytes of B (2 per element): in the kernel's front phase from 8 MB of B (all entries of a
+ *    batch), by a separate pre-pass below.  A fault-tolerant call is therefore 1 launch from 8 MB of B and 2 below
+ *    (ftsgemm_launch_count); 1 with a reused encode (opts.reuse_b_checksums, which never reuses the checksums of B read as
+ *    the other element type) and for the plain ids.
+ *  - Every other option applies as for FP32; opts.precision = 1 (3xTF32) is FTSGEMM_ERR_INVALID_ARG: the products of BF16
+ *    values are exact in FP32.
+ * ab_type outside 0..1: FTSGEMM_ERR_INVALID_ARG.  Capturable into a CUDA graph like the other compute calls. */
+int ftsgemm_run_batched_typed(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const void *A, int layout_a, int lda,
+                              long long stride_a, const void *B, int layout_b, int ldb, long long stride_b, int ab_type,
+                              const float *C, int ldc, long long stride_c, float *D, int batch, float alpha, float beta,
+                              const float *bias, int bias_mode, long long stride_bias, int activation, float *dZ,
+                              const ftsgemm_opts *opts);
+/* ftsgemm_run_batched_typed with batch = 1 (the strides are ignored). */
+int ftsgemm_run_typed(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const void *A, int layout_a, int lda,
+                      const void *B, int layout_b, int ldb, int ab_type, const float *C, int ldc, float *D, float alpha,
+                      float beta, const float *bias, int bias_mode, int activation, float *dZ, const ftsgemm_opts *opts);
 
 /* Counters of all FT launches since the previous call (synchronises the handle's last stream, then resets). */
 int ftsgemm_get_stats(ftsgemm_handle_t h, ftsgemm_stats *out);
