@@ -551,7 +551,7 @@ class FtSgemm:
             alpha: float = 1.0, beta: float = 0.0, opts: Opts | None = None):
         """out = act(alpha * (a @ b) + beta * out + bias) for 3-D float32 CUDA tensors a: (Bt, M, K), b: (Bt, K, N), out:
         (Bt, M, N), an optional bias (N,) shared by all entries or (Bt, N) one per entry, and an optional activation --
-        torch.baddbmm plus a bias and an activation -- as ONE run_batched (run_batched_act) call; returns out.
+        torch.baddbmm plus a bias and an activation -- as ONE run_batched_typed call; returns out.
 
         Every matrix may be row- or column-major with any leading stride that keeps 16-byte rows, and is read in place when
         its batch stride is a multiple of 4 floats: contiguous bmm operands and q @ k.transpose(-1, -2) copy nothing.  An
@@ -563,8 +563,7 @@ class FtSgemm:
 
         activation = "relu" | "gelu" stores act(z) with z the value above, in the same store pass, and z into preact when
         given (preact must have out's shape and strides; out and preact must be writable in place, else ValueError), as
-        matmul does.  A per-entry bias (bmm_plan: stride_bias) or an activation runs run_batched_act; anything else the
-        run_batched call.
+        matmul does.
 
         Autograd: with out=None, grad mode on and any of a, b, bias requiring grad, bmm is differentiable.  The forward is
         the same single call; z is written for GELU only (ReLU's backward reads out > 0).  Backward: grad_z =
@@ -576,20 +575,22 @@ class FtSgemm:
         torch.cuda.make_graphed_callables.
 
         c: a (Bt, M, N) tensor read in place of out's old values and never written -- out = act(alpha * (a @ b) + beta * c
-        + bias), bit for bit what the call gives with out holding a copy of c (one run_batched_out call).  beta must not be
-        0 (c would not be read: ValueError).  With out=None, out is allocated with c's strides (c dense) and the call is
-        differentiable in c as well: grad_c = beta * grad_z.  The kernels read c with out's geometry: a c with other strides
-        (or a base that is not 16-byte aligned) is copied once into that geometry first.
+        + bias), bit for bit what the call gives with out holding a copy of c (the same call with C = c and D = out; without
+        c, C = D = out).  beta must not be 0 (c would not be read: ValueError).  With out=None, out is allocated with c's
+        strides (c dense) and the call is differentiable in c as well: grad_c = beta * grad_z.  The kernels read c with out's
+        geometry: a c with other strides (or a base that is not 16-byte aligned) is copied once into that geometry first.
 
-        a and b may also both be bfloat16 (mixed with float32: TypeError): one run_batched_typed call on the BF16 kernels,
+        a and b may also both be bfloat16 (mixed with float32: TypeError): the same call with TYPE_BF16, on the BF16 kernels,
         FP32 accumulate, with out, c and preact float32 as above and a bfloat16 bias upcast (exactly) into a float32
         temporary; copies pad rows to 8 elements (bmm_plan with bf16).  Autograd as above, with grad_z rounded to bfloat16
         once for the two gradient products (the rounding of torch autocast's BF16 backward), which run on the BF16 kernels;
         grad_a, grad_b and grad_bias come back in the dtypes of a, b and the bias."""
         import torch
         for name, t in (("a", a), ("b", b)):
-            if t.dim() != 3 or t.dtype not in (torch.float32, torch.bfloat16) or not t.is_cuda:
-                raise TypeError(f"{name} must be a 3-D float32 or bfloat16 CUDA tensor")
+            if t.dtype not in (torch.float32, torch.bfloat16) or not t.is_cuda:
+                raise TypeError(f"{name} must be a float32 or bfloat16 CUDA tensor")
+            if t.dim() != 3:
+                raise TypeError(f"{name} must be 3-D")
         if a.dtype != b.dtype:
             raise TypeError(f"a and b must both be float32 or both bfloat16, not {a.dtype} and {b.dtype}")
         bf16 = a.dtype == torch.bfloat16
@@ -606,21 +607,17 @@ class FtSgemm:
                 raise ValueError("c is not read with beta = 0")
             if c.shape != (Bt, M, N) or c.dtype != torch.float32 or c.device != a.device:
                 raise ValueError(f"c must be a float32 ({Bt}, {M}, {N}) tensor on {a.device}")
+        if out is None and c is None and beta != 0.0:
+            raise ValueError("beta != 0 needs an out tensor or c")
         if out is None and torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (a, b, bias, c)):
             # (a bfloat16 bias is upcast inside the forward, which runs without grad: autograd sees the caller's tensor)
-            if beta != 0.0 and c is None:
-                raise ValueError("beta != 0 needs an out tensor or c")
             fwd = Opts.from_buffer_copy(opts) if opts is not None else make_opts()
             if not fwd.stream:
                 fwd.stream = torch.cuda.current_stream(a.device).cuda_stream
             return _bmm_fn().apply(a, b, bias, preact, c, self, kernel_id, alpha, beta, fwd, activation)
         if out is None:
-            if c is not None:
-                out = torch.empty_like(c, memory_format=torch.preserve_format)
-            elif beta != 0.0:
-                raise ValueError("beta != 0 needs an out tensor or c")
-            else:
-                out = torch.empty(Bt, M, N, device=a.device, dtype=torch.float32)
+            out = (torch.empty_like(c, memory_format=torch.preserve_format) if c is not None else
+                   torch.empty(Bt, M, N, device=a.device, dtype=torch.float32))
         if out.shape != (Bt, M, N) or out.dtype != torch.float32 or out.device != a.device:
             raise ValueError(f"out must be a float32 ({Bt}, {M}, {N}) tensor on {a.device}")
         if bf16 and bias is not None and bias.dtype == torch.bfloat16:
@@ -637,7 +634,6 @@ class FtSgemm:
         plan = bmm_plan(tuple(a.shape), a.stride(), tuple(b.shape), b.stride(), out.stride(), a.data_ptr(), b.data_ptr(),
                         out.data_ptr(), bias_stride, bias.data_ptr() if bias is not None else 0,
                         bias.stride(0) if per_entry else None, bf16)
-        fused = activation is not None or plan["stride_bias"] != 0
         if activation is not None and plan["copy_out"]:
             raise ValueError("out (and so preact) must be writable in place with an activation: 16-byte rows and entries")
         if plan["copy_bias"]:
@@ -659,23 +655,10 @@ class FtSgemm:
         if opts is None:
             opts = make_opts(stream=torch.cuda.current_stream(a.device).cuda_stream)
         kA, kB = (b, a) if plan["swap"] else (a, b)
-        if bf16:
-            self.run_batched_typed(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], plan["stride_a"],
-                                   kB, plan["layout_b"], plan["ldb"], plan["stride_b"], TYPE_BF16, c if c is not None else dst,
-                                   plan["ldc"], plan["stride_c"], dst, Bt, alpha, beta, bias, plan["bias_mode"],
-                                   plan["stride_bias"], ACTIVATIONS[activation], preact, opts)
-        elif c is not None:
-            self.run_batched_out(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], plan["stride_a"],
-                                 kB, plan["layout_b"], plan["ldb"], plan["stride_b"], c, plan["ldc"], plan["stride_c"], dst, Bt,
-                                 alpha, beta, bias, plan["bias_mode"], plan["stride_bias"], ACTIVATIONS[activation], preact, opts)
-        elif fused:
-            self.run_batched_act(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], plan["stride_a"],
-                                 kB, plan["layout_b"], plan["ldb"], plan["stride_b"], dst, plan["ldc"], plan["stride_c"], Bt, alpha,
-                                 beta, bias, plan["bias_mode"], plan["stride_bias"], ACTIVATIONS[activation], preact, opts)
-        else:
-            self.run_batched(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], plan["stride_a"], kB,
-                             plan["layout_b"], plan["ldb"], plan["stride_b"], dst, plan["ldc"], plan["stride_c"], Bt, alpha, beta,
-                             bias, plan["bias_mode"], opts)
+        self.run_batched_typed(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], plan["stride_a"],
+                               kB, plan["layout_b"], plan["ldb"], plan["stride_b"], TYPE_BF16 if bf16 else TYPE_F32,
+                               c if c is not None else dst, plan["ldc"], plan["stride_c"], dst, Bt, alpha, beta, bias,
+                               plan["bias_mode"], plan["stride_bias"], ACTIVATIONS[activation], preact, opts)
         if dst is not out:
             out.copy_(dst)
         return out
@@ -695,38 +678,28 @@ class FtSgemm:
         injected faults (opts) and of stats() events are the kernel's, transposed against out in that case.  A kernel M or
         N (after the mapping) that is not a multiple of 4 raises FtsgemmError(-2) for the tensor-core ids, as run does.
         Runs on the current torch stream unless opts.stream says otherwise.  No autograd: linear() is the differentiable
-        F.linear.  This is bmm on a batch of one entry (a run_batched call with batch = 1, which is run_bias).  Capturable in a
+        F.linear.  Every call is bmm on a batch of one entry, so one run_batched_typed call with batch = 1.  Capturable in a
         CUDA graph (see the class docstring).
 
-        activation = "relu" | "gelu" stores act(z) with z the value above, in the same store pass (one run_act call), and z
+        activation = "relu" | "gelu" stores act(z) with z the value above, in the same store pass of the same call, and z
         into preact when given.  preact must have out's shape and strides, and out and preact must both be writable in place
         (else ValueError: there is no copy path for them); a, b and the bias are copied as above when needed.
 
         c: an (M, N) tensor read in place of out's old values and never written -- out = act(alpha * (a @ b) + beta * c +
-        bias), bit for bit what the call gives with out holding a copy of c (one run_out / run_batched_out call).  beta must
-        not be 0 (c would not be read: ValueError).  With out=None, out is allocated with c's strides (c dense).  The kernels
-        read c with out's geometry: a c with other strides (or a base that is not 16-byte aligned) is copied once into that
-        geometry first.
+        bias), bit for bit what the call gives with out holding a copy of c (the same call with C = c and D = out).  beta
+        must not be 0 (c would not be read: ValueError).  With out=None, out is allocated with c's strides (c dense).  The
+        kernels read c with out's geometry: a c with other strides (or a base that is not 16-byte aligned) is copied once
+        into that geometry first.
 
-        a and b may also both be bfloat16 (float32 and bfloat16 mixed raise TypeError): bmm on a batch of one entry, one
-        run_batched_typed call on the BF16 kernels, FP32 accumulate, with out, c and preact float32 as above; a bfloat16 bias
-        is upcast (exactly) into a float32 temporary.  Their copies pad rows to 8 elements (matmul_plan with bf16)."""
+        a and b may also both be bfloat16 (float32 and bfloat16 mixed raise TypeError): the same call on the BF16 kernels,
+        FP32 accumulate, with out, c and preact float32 as above; a bfloat16 bias is upcast (exactly) into a float32
+        temporary.  Their copies pad rows to 8 elements (matmul_plan with bf16)."""
         import torch
+        # (bmm checks everything else on the batch-of-one views)
         for name, t in (("a", a), ("b", b)):
-            if t.dim() != 2 or t.dtype not in (torch.float32, torch.bfloat16) or not t.is_cuda:
-                raise TypeError(f"{name} must be a 2-D float32 or bfloat16 CUDA tensor")
-        if a.dtype != b.dtype:
-            raise TypeError(f"a and b must both be float32 or both bfloat16, not {a.dtype} and {b.dtype}")
-        bf16 = a.dtype == torch.bfloat16
-        if bf16 and bias is not None and bias.dtype == torch.bfloat16:
-            bias = bias.float()
-        M, K = a.shape
-        K2, N = b.shape
-        if c is not None:
-            if beta == 0.0:
-                raise ValueError("c is not read with beta = 0")
-            if c.shape != (M, N) or c.dtype != torch.float32 or c.device != a.device:
-                raise ValueError(f"c must be a float32 ({M}, {N}) tensor on {a.device}")
+            if t.dim() != 2:
+                raise TypeError(f"{name} must be 2-D")
+        M, N = a.shape[0], b.shape[1]
         if out is None:
             if c is not None:
                 out = torch.empty_like(c, memory_format=torch.preserve_format)
@@ -734,48 +707,13 @@ class FtSgemm:
                 raise ValueError("beta != 0 needs an out tensor or c")
             else:
                 out = torch.empty(M, N, device=a.device, dtype=torch.float32)
-        if out.shape != (M, N) or out.dtype != torch.float32 or out.device != a.device or b.device != a.device:
-            raise ValueError(f"out must be a float32 ({M}, {N}) tensor on {a.device}")
-        if bias is not None and (bias.shape != (N,) or bias.dtype != torch.float32 or bias.device != a.device):
-            raise ValueError(f"bias must be a float32 ({N},) tensor on {a.device}")
-        if K != K2:
-            raise ValueError(f"inner dimensions differ: {tuple(a.shape)} @ {tuple(b.shape)}")
-        if bf16:  # (one run_batched_typed call: bmm on a batch of one entry)
-            self.bmm(a.unsqueeze(0), b.unsqueeze(0), out.unsqueeze(0), c=c.unsqueeze(0) if c is not None else None, bias=bias,
-                     activation=activation, preact=preact.unsqueeze(0) if preact is not None else None, kernel_id=kernel_id,
-                     alpha=alpha, beta=beta, opts=opts)
-            return out
-        if activation is None and preact is None:
-            self.bmm(a.unsqueeze(0), b.unsqueeze(0), out.unsqueeze(0), c=c.unsqueeze(0) if c is not None else None, bias=bias,
-                     kernel_id=kernel_id, alpha=alpha, beta=beta, opts=opts)
-            return out
-        if activation not in ("relu", "gelu"):
-            raise ValueError(f"activation must be None, 'relu' or 'gelu' (preact needs one), not {activation!r}")
-        if preact is not None and (preact.shape != out.shape or preact.stride() != out.stride() or
-                                   preact.dtype != torch.float32 or preact.device != a.device):
-            raise ValueError("preact must be a float32 tensor with out's shape and strides on out's device")
-        plan = matmul_plan((M, K), a.stride(), (K, N), b.stride(), out.stride(), a.data_ptr(), b.data_ptr(), out.data_ptr(),
-                           bias.stride(0) if bias is not None else None, bias.data_ptr() if bias is not None else 0)
-        if plan["copy_out"]:
-            raise ValueError("out (and so preact) must be writable in place with an activation: unit stride, 16-byte aligned")
-        if plan["copy_bias"]:
-            bias = torch.empty(N, device=a.device, dtype=torch.float32).copy_(bias)
-        if plan["copy_a"]:
-            a = torch.empty(M, _pad4(K), device=a.device, dtype=torch.float32)[:, :K].copy_(a)
-        if plan["copy_b"]:
-            b = torch.empty(N, _pad4(K), device=a.device, dtype=torch.float32)[:, :K].copy_(b.t()).t()
-        if opts is None:
-            opts = make_opts(stream=torch.cuda.current_stream(a.device).cuda_stream)
-        kA, kB = (b, a) if plan["swap"] else (a, b)
-        if c is not None:
-            if c.stride() != out.stride() or c.data_ptr() % 16 != 0:
-                c = torch.empty_strided(out.shape, out.stride(), device=a.device, dtype=torch.float32).copy_(c)
-            self.run_out(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], kB, plan["layout_b"],
-                         plan["ldb"], c, plan["ldc"], out, alpha, beta, bias, plan["bias_mode"], ACTIVATIONS[activation], preact,
-                         opts)
-            return out
-        self.run_act(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], kB, plan["layout_b"],
-                     plan["ldb"], out, plan["ldc"], alpha, beta, bias, plan["bias_mode"], ACTIVATIONS[activation], preact, opts)
+        for name, t in (("c", c), ("out", out), ("preact", preact)):
+            if t is not None and t.shape != (M, N):
+                raise ValueError(f"{name} must be an ({M}, {N}) tensor")
+        if bias is not None and bias.dim() != 1:  # (bmm would take a (1, N) bias as one bias per entry)
+            raise ValueError(f"bias must be a ({N},) tensor")
+        self.bmm(a[None], b[None], out[None], c=c[None] if c is not None else None, bias=bias, activation=activation,
+                 preact=preact[None] if preact is not None else None, kernel_id=kernel_id, alpha=alpha, beta=beta, opts=opts)
         return out
 
     def linear(self, x, weight, bias=None, *, activation=None, residual=None, kernel_id: int = ID_ABFT_AUTO,
@@ -783,7 +721,8 @@ class FtSgemm:
         """F.linear(x, weight, bias) = x @ weight.T + bias under ABFT protection, differentiable: x (..., K), weight (N, K),
         bias (N,) or None, all float32 CUDA tensors; returns (..., N).
 
-        The forward is one matmul with the bias fused into the store pass; x's leading dimensions are flattened as a view
+        The forward is one matmul, so one run_batched_typed call, with the bias fused into the store pass, whatever the
+        activation and residual (one autograd Function, _linear_fn); x's leading dimensions are flattened as a view
         where the strides allow it (linear_plan) and copied otherwise.  Backward: grad_x = grad_y @ weight and
         grad_weight = grad_y^T @ x through matmul with the same kernel id and opts (both read in place), grad_bias =
         grad_y.sum(0) in torch.  Faults injected through opts land in the forward product only; faults detected in any of
@@ -826,13 +765,8 @@ class FtSgemm:
         fwd = Opts.from_buffer_copy(opts) if opts is not None else make_opts()
         if not fwd.stream:
             fwd.stream = torch.cuda.current_stream(x.device).cuda_stream
-        if activation is None:
-            y = _linear_fn().apply(x2, weight, bias, r2, self, kernel_id, fwd)
-        else:
-            if activation not in ("relu", "gelu"):
-                raise ValueError(f"activation must be None, 'relu' or 'gelu', not {activation!r}")
-            grad = torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x, weight, bias))
-            y = _linear_act_fn().apply(x2, weight, bias, self, kernel_id, fwd, activation, grad)
+        grad = torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x, weight, bias))
+        y = _linear_fn().apply(x2, weight, bias, r2, self, kernel_id, fwd, activation, grad)
         return y.view(lp["out_shape"])
 
     def run_host(self, kernel_id: int, M: int, N: int, K: int, hA, hB, hC, alpha: float = 1.0, beta: float = 0.0,
@@ -915,32 +849,57 @@ _LINEAR_FN = None
 
 
 def _linear_fn():
-    """The torch.autograd.Function behind FtSgemm.linear (built on first use: torch is imported lazily)."""
+    """The torch.autograd.Function behind FtSgemm.linear (built on first use: torch is imported lazily): one matmul
+    forward (so one run_batched_typed call), the activation's backward in torch, then the products of _linear_grads."""
     global _LINEAR_FN
     if _LINEAR_FN is None:
         import torch
 
         class LinearFn(torch.autograd.Function):
             @staticmethod
-            def forward(ctx, x2, weight, bias, residual, dev, kernel_id, opts):
-                ctx.save_for_backward(x2, weight)
-                ctx.dev, ctx.kernel_id, ctx.opts = dev, kernel_id, opts
+            def forward(ctx, x2, weight, bias, residual, dev, kernel_id, opts, activation, grad):
+                # (grad: grad mode was on and an input requires grad -- forward itself runs with grad mode off.  z is
+                # written for GELU's backward only: ReLU's reads y > 0, and without an activation grad_z is grad_y)
+                z = None
+                if grad and activation == "gelu":
+                    z = torch.empty(x2.shape[0], weight.shape[0], device=x2.device, dtype=torch.float32)
+                y = dev.matmul(x2, weight.t(), c=residual, bias=bias, activation=activation, preact=z, kernel_id=kernel_id,
+                               beta=0.0 if residual is None else 1.0, opts=opts)
+                ctx.save_for_backward(x2, weight, y if activation == "relu" else z)
+                ctx.dev, ctx.kernel_id, ctx.opts, ctx.activation = dev, kernel_id, opts, activation
                 ctx.bias_dtype = bias.dtype if bias is not None else None
-                if residual is None:
-                    return dev.matmul(x2, weight.t(), bias=bias, kernel_id=kernel_id, opts=opts)
-                return dev.matmul(x2, weight.t(), c=residual, bias=bias, kernel_id=kernel_id, beta=1.0, opts=opts)
+                return y
 
             @staticmethod
             def backward(ctx, gy):
-                x2, weight = ctx.saved_tensors
-                bwd = Opts.from_buffer_copy(ctx.opts)
-                bwd.inject_mode, bwd.n_faults = 0, 0
-                bwd.stream = torch.cuda.current_stream(gy.device).cuda_stream
-                gx, gw, gb = _linear_grads(ctx, gy, x2, weight, bwd)
-                return gx, gw, gb, gy if ctx.needs_input_grad[3] else None, None, None, None
+                x2, weight, saved = ctx.saved_tensors
+                gz = _grad_z(gy, ctx.activation, saved)
+                gx, gw, gb = _linear_grads(ctx, gz, x2, weight, _backward_opts(ctx.opts, gy.device))
+                return gx, gw, gb, gy if ctx.needs_input_grad[3] else None, None, None, None, None, None
 
         _LINEAR_FN = LinearFn
     return _LINEAR_FN
+
+
+def _backward_opts(opts, device):
+    """The forward's opts for the gradient products: a copy with the injected faults stripped, on the stream autograd runs
+    the backward on."""
+    import torch
+    bwd = Opts.from_buffer_copy(opts)
+    bwd.inject_mode, bwd.n_faults = 0, 0
+    bwd.stream = torch.cuda.current_stream(device).cuda_stream
+    return bwd
+
+
+def _grad_z(gy, activation, saved):
+    """grad_z from grad_y: threshold_backward on the saved output y (ReLU) or gelu_backward on the saved z (GELU) in torch,
+    grad_y itself without an activation."""
+    import torch
+    if activation == "relu":
+        return torch.ops.aten.threshold_backward(gy, saved, 0)
+    if activation == "gelu":
+        return torch.ops.aten.gelu_backward(gy, saved)
+    return gy
 
 
 def _linear_grads(ctx, gz, x2, weight, bwd):
@@ -959,52 +918,12 @@ def _linear_grads(ctx, gz, x2, weight, bwd):
     return gx, gw, gb
 
 
-_LINEAR_ACT_FN = None
-
-
-def _linear_act_fn():
-    """The torch.autograd.Function behind FtSgemm.linear(activation=...): one run_act forward, the activation's backward in
-    torch, then the products of _linear_fn's backward."""
-    global _LINEAR_ACT_FN
-    if _LINEAR_ACT_FN is None:
-        import torch
-
-        class LinearActFn(torch.autograd.Function):
-            @staticmethod
-            def forward(ctx, x2, weight, bias, dev, kernel_id, opts, activation, grad):
-                # (grad: grad mode was on and an input requires grad -- forward itself runs with grad mode off)
-                z = None
-                if grad and activation == "gelu":
-                    z = torch.empty(x2.shape[0], weight.shape[0], device=x2.device, dtype=torch.float32)
-                y = dev.matmul(x2, weight.t(), bias=bias, activation=activation, preact=z, kernel_id=kernel_id, opts=opts)
-                ctx.save_for_backward(x2, weight, y if activation == "relu" else z)
-                ctx.dev, ctx.kernel_id, ctx.opts, ctx.activation = dev, kernel_id, opts, activation
-                ctx.bias_dtype = bias.dtype if bias is not None else None
-                return y
-
-            @staticmethod
-            def backward(ctx, gy):
-                x2, weight, saved = ctx.saved_tensors
-                if ctx.activation == "relu":
-                    gz = torch.ops.aten.threshold_backward(gy, saved, 0)
-                else:
-                    gz = torch.ops.aten.gelu_backward(gy, saved)
-                bwd = Opts.from_buffer_copy(ctx.opts)
-                bwd.inject_mode, bwd.n_faults = 0, 0
-                bwd.stream = torch.cuda.current_stream(gy.device).cuda_stream
-                gx, gw, gb = _linear_grads(ctx, gz, x2, weight, bwd)
-                return gx, gw, gb, None, None, None, None, None
-
-        _LINEAR_ACT_FN = LinearActFn
-    return _LINEAR_ACT_FN
-
-
 _BMM_FN = None
 
 
 def _bmm_fn():
-    """The torch.autograd.Function behind a differentiable FtSgemm.bmm: one run_batched / run_batched_act forward, the
-    activation's backward in torch, then the two gradient products through bmm."""
+    """The torch.autograd.Function behind a differentiable FtSgemm.bmm: one bmm forward (so one run_batched_typed call),
+    the activation's backward in torch, then the two gradient products through bmm."""
     global _BMM_FN
     if _BMM_FN is None:
         import torch
@@ -1026,15 +945,8 @@ def _bmm_fn():
             @staticmethod
             def backward(ctx, gy):
                 a, b, saved = ctx.saved_tensors
-                if ctx.activation == "relu":
-                    gz = torch.ops.aten.threshold_backward(gy, saved, 0)
-                elif ctx.activation == "gelu":
-                    gz = torch.ops.aten.gelu_backward(gy, saved)
-                else:
-                    gz = gy
-                bwd = Opts.from_buffer_copy(ctx.opts)
-                bwd.inject_mode, bwd.n_faults = 0, 0
-                bwd.stream = torch.cuda.current_stream(gy.device).cuda_stream
+                gz = _grad_z(gy, ctx.activation, saved)
+                bwd = _backward_opts(ctx.opts, gy.device)
                 ga = gb = gbias = gc = None
                 # (BF16 operands: grad_z rounded to bfloat16 once for the products, gradients in the inputs' dtypes)
                 g = gz.to(torch.bfloat16) if a.dtype == torch.bfloat16 else gz
