@@ -99,9 +99,10 @@ EXPORTED_SYMBOLS = [
     "ftsgemm_verify_bad_count", "ftsgemm_debug_trace", "ftsgemm_stats_device", "ftsgemm_select_kernel", "ftsgemm_launch_count", "ftsgemm_peer_export", "ftsgemm_peer_connect",
     "ftsgemm_peer_verdict", "ftsgemm_run_batched", "ftsgemm_debug_schedule_batched", "ftsgemm_run_act",
     "ftsgemm_run_batched_act", "ftsgemm_run_out", "ftsgemm_run_batched_out", "ftsgemm_run_typed", "ftsgemm_run_batched_typed",
+    "ftsgemm_run_batched_mixed",
 ]
 
-# operand element types of run_typed / run_batched_typed (include/ftsgemm.h: FTSGEMM_TYPE_*)
+# element types of run_typed / run_batched_typed / run_batched_mixed (include/ftsgemm.h: FTSGEMM_TYPE_*)
 TYPE_F32, TYPE_BF16 = 0, 1
 
 _lib = None
@@ -151,6 +152,8 @@ def lib():
                                         C.POINTER(Opts)]
         L.ftsgemm_run_batched_typed.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, ll, vp, ip, ip, ll, ip, vp, ip, ll, vp, ip, fp,
                                                 fp, vp, ip, ll, ip, vp, C.POINTER(Opts)]
+        L.ftsgemm_run_batched_mixed.argtypes = [vp, ip, ip, ip, ip, vp, ip, ip, ll, vp, ip, ip, ll, ip, vp, ip, ll, vp, ip, ip,
+                                                fp, fp, vp, ip, ll, ip, vp, C.POINTER(Opts)]
         L.ftsgemm_get_stats.argtypes = [vp, C.POINTER(Stats)]
         L.ftsgemm_run_host.argtypes = [vp, ip, ip, ip, ip, vp, vp, vp, fp, fp, C.POINTER(Opts)]
         L.ftsgemm_stats_device.argtypes = [vp, vp, vp]
@@ -295,7 +298,7 @@ def _view(shape, stride, ptr: int, ld4: bool, elems16: int = 4):
 
 
 def matmul_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0, b_ptr: int = 0, out_ptr: int = 0,
-                bias_stride=None, bias_ptr: int = 0, bf16: bool = False) -> dict:
+                bias_stride=None, bias_ptr: int = 0, bf16: bool = False, out_bf16: bool = False) -> dict:
     """run_ex arguments for out = a @ b with a: (M, K), b: (K, N), out: (M, N), from shapes, element strides and addresses.
 
     Column-major out: C = out, kernel A = a, kernel B = b^T.  Row-major out: C = out^T = b^T a^T (swap = True), so the
@@ -306,7 +309,9 @@ def matmul_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0
     row-major matrix.  bias_stride (the element stride of a length-N bias, None without a bias) gives bias_mode: a bias
     over out's columns is one per kernel column (BIAS_COL), or per kernel row (BIAS_ROW) when swapped; copy_bias marks a
     bias without unit stride or with a base that is not 4-byte aligned.  bf16: a and b are BF16 (run_typed), whose 16-byte
-    rows are 8 elements: leading strides and the copies' padded rows are multiples of 8."""
+    rows are 8 elements: leading strides and the copies' padded rows are multiples of 8.  out_bf16: out is BF16 too
+    (run_batched_mixed), written in place only with a leading stride that is a multiple of 8, and its copy is row-major
+    with rows padded to a multiple of 8 elements."""
     M, K = a_shape
     K2, N = b_shape
     if K != K2:
@@ -314,11 +319,11 @@ def matmul_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0
     e16, pad = (8, _pad8) if bf16 else (4, _pad4)
     va = _view(a_shape, a_stride, a_ptr, True, e16)
     vb = _view(b_shape, b_stride, b_ptr, True, e16)
-    vo = _view((M, N), out_stride, out_ptr, False)
+    vo = _view((M, N), out_stride, out_ptr, True, 8) if out_bf16 else _view((M, N), out_stride, out_ptr, False)
     copies = {"copy_a": va is None, "copy_b": vb is None, "copy_out": vo is None}
     va = va or ("row", pad(K))
     vb = vb or ("col", pad(K))
-    vo = vo or ("row", N)
+    vo = vo or ("row", _pad8(N) if out_bf16 else N)
     a_kmajor, b_kmajor = va[0] == "row", vb[0] == "col"  # a(m, k) along k / b(k, n) along k
     lay = {True: LAYOUT_K_MAJOR, False: LAYOUT_MN_MAJOR}
     if vo[0] == "col":
@@ -334,7 +339,7 @@ def matmul_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0
 
 
 def bmm_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0, b_ptr: int = 0, out_ptr: int = 0,
-             bias_stride=None, bias_ptr: int = 0, bias_entry_stride=None, bf16: bool = False) -> dict:
+             bias_stride=None, bias_ptr: int = 0, bias_entry_stride=None, bf16: bool = False, out_bf16: bool = False) -> dict:
     """run_batched arguments for out = a @ b with a: (Bt, M, K), b: (Bt, K, N), out: (Bt, M, N), from shapes, element strides
     and addresses.  Each matrix is mapped as in matmul_plan (layouts, lds, swap, bias_mode); stride_a / stride_b / stride_c
     are the batch strides of the kernel's A, B and C (b's and a's when swapped).  With more than one entry a tensor is also
@@ -346,13 +351,14 @@ def bmm_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0, b
     stride_bias is the entry stride run_batched_act takes: 0 for a shared bias, an expanded one (entry stride 0) or a single
     entry.  copy_bias also marks a per-entry bias with a negative entry stride; the copy bmm makes of a per-entry bias is
     (Bt, N) contiguous (stride_bias = N), of a shared one (N,).  bf16: a and b are BF16 (run_batched_typed): their rows,
-    batch strides and copies' padded rows are multiples of 8 elements (16 bytes) instead of 4."""
+    batch strides and copies' padded rows are multiples of 8 elements (16 bytes) instead of 4.  out_bf16: the same for out
+    (run_batched_mixed): its rows and batch stride are multiples of 8 elements or it is copied, the copy (Bt, M, pad8(N))."""
     Bt, M, K = a_shape
     Bt2, K2, N = b_shape
     if Bt != Bt2:
         raise ValueError(f"batch sizes differ: {tuple(a_shape)} @ {tuple(b_shape)}")
     mp = matmul_plan((M, K), tuple(a_stride[1:]), (K2, N), tuple(b_stride[1:]), tuple(out_stride[1:]), a_ptr, b_ptr, out_ptr,
-                     bias_stride, bias_ptr, bf16)
+                     bias_stride, bias_ptr, bf16, out_bf16)
     sa, sb, so = a_stride[0], b_stride[0], out_stride[0]
     e16, pad = (8, _pad8) if bf16 else (4, _pad4)
     if Bt > 1:
@@ -360,15 +366,18 @@ def bmm_plan(a_shape, a_stride, b_shape, b_stride, out_stride, a_ptr: int = 0, b
             return st <= 0 or st % e != 0
         mp["copy_a"] = mp["copy_a"] or bad(sa, e16)
         mp["copy_b"] = mp["copy_b"] or bad(sb, e16)
-        mp["copy_out"] = mp["copy_out"] or bad(so) or so < mp["ldc"] * mp["N"]
+        mp["copy_out"] = mp["copy_out"] or bad(so, 8 if out_bf16 else 4) or so < mp["ldc"] * mp["N"]
     if mp["copy_a"] or mp["copy_b"] or mp["copy_out"]:
-        # the copies: a (Bt, M, pad4(K)) row-major, b as (Bt, N, pad4(K)) transposed, out (Bt, M, N) contiguous (pad8: BF16)
+        # the copies: a (Bt, M, pad4(K)) row-major, b as (Bt, N, pad4(K)) transposed, out (Bt, M, N) contiguous (pad8: BF16;
+        # a BF16 out: (Bt, M, pad8(N)))
+        on = _pad8(N) if out_bf16 else N
         a_st = (M * pad(K), pad(K), 1) if mp["copy_a"] else tuple(a_stride)
         b_st = (N * pad(K), 1, pad(K)) if mp["copy_b"] else tuple(b_stride)
-        o_st = (M * N, N, 1) if mp["copy_out"] else tuple(out_stride)
+        o_st = (M * on, on, 1) if mp["copy_out"] else tuple(out_stride)
         copies = {k: mp[k] for k in ("copy_a", "copy_b", "copy_out", "copy_bias")}
         mp = matmul_plan((M, K), a_st[1:], (K, N), b_st[1:], o_st[1:], 0 if copies["copy_a"] else a_ptr,
-                         0 if copies["copy_b"] else b_ptr, 0 if copies["copy_out"] else out_ptr, bias_stride, bias_ptr, bf16)
+                         0 if copies["copy_b"] else b_ptr, 0 if copies["copy_out"] else out_ptr, bias_stride, bias_ptr, bf16,
+                         out_bf16)
         mp.update(copies)
         sa, sb, so = a_st[0], b_st[0], o_st[0]
     mp["batch"] = Bt
@@ -538,6 +547,21 @@ class FtSgemm:
                                                           stride_bias, activation, _ptr(dZ) if dZ is not None else None,
                                                           C.byref(opts) if opts is not None else None))
 
+    def run_batched_mixed(self, kernel_id: int, M: int, N: int, K: int, dA, layout_a: int, lda: int, stride_a: int, dB,
+                          layout_b: int, ldb: int, stride_b: int, ab_type: int, dC, ldc: int, stride_c: int, dD, cd_type: int,
+                          batch: int, alpha: float = 1.0, beta: float = 0.0, bias=None, bias_mode: int = BIAS_NONE,
+                          stride_bias: int = 0, activation: int = ACT_NONE, dZ=None, opts: Opts | None = None) -> None:
+        """run_batched_typed with C, D and Z of element type cd_type (TYPE_F32: run_batched_typed itself; TYPE_BF16: BF16 C,
+        D and Z, BF16 operands only, ldc and stride_c in elements, everything up to the store FP32 and the stored values
+        rounded to nearest even; include/ftsgemm.h: ftsgemm_run_batched_mixed)."""
+        self._run_checked(lib().ftsgemm_run_batched_mixed(self._h, kernel_id, M, N, K, _ptr(dA), layout_a, lda, stride_a,
+                                                          _ptr(dB), layout_b, ldb, stride_b, ab_type,
+                                                          _ptr(dC) if dC is not None else None, ldc, stride_c, _ptr(dD), cd_type,
+                                                          batch, alpha, beta, _ptr(bias) if bias is not None else None,
+                                                          bias_mode, stride_bias, activation,
+                                                          _ptr(dZ) if dZ is not None else None,
+                                                          C.byref(opts) if opts is not None else None))
+
     def run_typed(self, kernel_id: int, M: int, N: int, K: int, dA, layout_a: int, lda: int, dB, layout_b: int, ldb: int,
                   ab_type: int, dC, ldc: int, dD, alpha: float = 1.0, beta: float = 0.0, bias=None, bias_mode: int = BIAS_NONE,
                   activation: int = ACT_NONE, dZ=None, opts: Opts | None = None) -> None:
@@ -548,10 +572,10 @@ class FtSgemm:
                                                   _ptr(dZ) if dZ is not None else None, C.byref(opts) if opts is not None else None))
 
     def bmm(self, a, b, out=None, *, c=None, bias=None, activation=None, preact=None, kernel_id: int = ID_ABFT_AUTO,
-            alpha: float = 1.0, beta: float = 0.0, opts: Opts | None = None):
+            alpha: float = 1.0, beta: float = 0.0, opts: Opts | None = None, out_dtype=None):
         """out = act(alpha * (a @ b) + beta * out + bias) for 3-D float32 CUDA tensors a: (Bt, M, K), b: (Bt, K, N), out:
         (Bt, M, N), an optional bias (N,) shared by all entries or (Bt, N) one per entry, and an optional activation --
-        torch.baddbmm plus a bias and an activation -- as ONE run_batched_typed call; returns out.
+        torch.baddbmm plus a bias and an activation -- as ONE run_batched_mixed call; returns out.
 
         Every matrix may be row- or column-major with any leading stride that keeps 16-byte rows, and is read in place when
         its batch stride is a multiple of 4 floats: contiguous bmm operands and q @ k.transpose(-1, -2) copy nothing.  An
@@ -583,8 +607,15 @@ class FtSgemm:
         a and b may also both be bfloat16 (mixed with float32: TypeError): the same call with TYPE_BF16, on the BF16 kernels,
         FP32 accumulate, with out, c and preact float32 as above and a bfloat16 bias upcast (exactly) into a float32
         temporary; copies pad rows to 8 elements (bmm_plan with bf16).  Autograd as above, with grad_z rounded to bfloat16
-        once for the two gradient products (the rounding of torch autocast's BF16 backward), which run on the BF16 kernels;
-        grad_a, grad_b and grad_bias come back in the dtypes of a, b and the bias."""
+        once for the two gradient products (the rounding of torch autocast's BF16 backward), which run on the BF16 kernels
+        and write bfloat16 directly; grad_a, grad_b, grad_bias and grad_c come back in the dtypes of a, b, the bias and c.
+
+        The result dtype is out.dtype when out is given, else c.dtype when c is, else out_dtype (None: float32).  A bfloat16
+        result needs bfloat16 a and b (else TypeError) and is one run_batched_mixed call with BF16 C / D / Z: the float32
+        result of the same call rounded to nearest even, as .to(torch.bfloat16) rounds it, with no separate cast pass.  c
+        and preact must have the result dtype, and an out_dtype that contradicts out or c raises ValueError.  A bfloat16 out
+        is written in place when its rows and batch stride are multiples of 8 elements; otherwise through a copy with rows
+        padded to 8 (bmm_plan with out_bf16).  Autograd: grad_out arrives in the result dtype."""
         import torch
         for name, t in (("a", a), ("b", b)):
             if t.dtype not in (torch.float32, torch.bfloat16) or not t.is_cuda:
@@ -594,6 +625,15 @@ class FtSgemm:
         if a.dtype != b.dtype:
             raise TypeError(f"a and b must both be float32 or both bfloat16, not {a.dtype} and {b.dtype}")
         bf16 = a.dtype == torch.bfloat16
+        rdt = out.dtype if out is not None else c.dtype if c is not None else out_dtype or torch.float32  # result dtype
+        if out_dtype is not None and out_dtype != rdt:
+            raise ValueError(f"out_dtype {out_dtype} contradicts the {rdt} of {'out' if out is not None else 'c'}")
+        if rdt not in (torch.float32, torch.bfloat16):
+            raise ValueError(f"the result must be float32 or bfloat16, not {rdt}")
+        out16 = rdt == torch.bfloat16
+        if out16 and not bf16:
+            raise TypeError("a bfloat16 result needs bfloat16 a and b")
+        rname = "bfloat16" if out16 else "float32"
         Bt, M, K = a.shape
         N = b.shape[2]
         if b.shape[0] != Bt or b.shape[1] != K or b.device != a.device:
@@ -605,8 +645,8 @@ class FtSgemm:
         if c is not None:
             if beta == 0.0:
                 raise ValueError("c is not read with beta = 0")
-            if c.shape != (Bt, M, N) or c.dtype != torch.float32 or c.device != a.device:
-                raise ValueError(f"c must be a float32 ({Bt}, {M}, {N}) tensor on {a.device}")
+            if c.shape != (Bt, M, N) or c.dtype != rdt or c.device != a.device:
+                raise ValueError(f"c must be a {rname} ({Bt}, {M}, {N}) tensor on {a.device}")
         if out is None and c is None and beta != 0.0:
             raise ValueError("beta != 0 needs an out tensor or c")
         if out is None and torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (a, b, bias, c)):
@@ -614,26 +654,26 @@ class FtSgemm:
             fwd = Opts.from_buffer_copy(opts) if opts is not None else make_opts()
             if not fwd.stream:
                 fwd.stream = torch.cuda.current_stream(a.device).cuda_stream
-            return _bmm_fn().apply(a, b, bias, preact, c, self, kernel_id, alpha, beta, fwd, activation)
+            return _bmm_fn().apply(a, b, bias, preact, c, self, kernel_id, alpha, beta, fwd, activation, rdt)
         if out is None:
             out = (torch.empty_like(c, memory_format=torch.preserve_format) if c is not None else
-                   torch.empty(Bt, M, N, device=a.device, dtype=torch.float32))
-        if out.shape != (Bt, M, N) or out.dtype != torch.float32 or out.device != a.device:
-            raise ValueError(f"out must be a float32 ({Bt}, {M}, {N}) tensor on {a.device}")
+                   torch.empty(Bt, M, N, device=a.device, dtype=rdt))
+        if out.shape != (Bt, M, N) or out.device != a.device:
+            raise ValueError(f"out must be a {rname} ({Bt}, {M}, {N}) tensor on {a.device}")
         if bf16 and bias is not None and bias.dtype == torch.bfloat16:
             bias = bias.float()
         if bias is not None and (bias.shape not in ((N,), (Bt, N)) or bias.dtype != torch.float32 or bias.device != a.device):
             raise ValueError(f"bias must be a float32 ({N},) or ({Bt}, {N}) tensor on {a.device}")
         if preact is not None and (preact.shape != out.shape or preact.stride() != out.stride() or
-                                   preact.dtype != torch.float32 or preact.device != a.device):
-            raise ValueError("preact must be a float32 tensor with out's shape and strides on out's device")
+                                   preact.dtype != rdt or preact.device != a.device):
+            raise ValueError(f"preact must be a {rname} tensor with out's shape and strides on out's device")
         if Bt == 0:  # an empty batch (torch.bmm accepts it): nothing to compute
             return out
         per_entry = bias is not None and bias.dim() == 2
         bias_stride = bias.stride(-1) if bias is not None else None
         plan = bmm_plan(tuple(a.shape), a.stride(), tuple(b.shape), b.stride(), out.stride(), a.data_ptr(), b.data_ptr(),
                         out.data_ptr(), bias_stride, bias.data_ptr() if bias is not None else 0,
-                        bias.stride(0) if per_entry else None, bf16)
+                        bias.stride(0) if per_entry else None, bf16, out16)
         if activation is not None and plan["copy_out"]:
             raise ValueError("out (and so preact) must be writable in place with an activation: 16-byte rows and entries")
         if plan["copy_bias"]:
@@ -645,26 +685,31 @@ class FtSgemm:
         if plan["copy_b"]:
             b = torch.empty(Bt, N, pad(K), device=a.device, dtype=b.dtype)[:, :, :K].copy_(b.transpose(1, 2)).transpose(1, 2)
         dst = out
-        if plan["copy_out"]:
+        if plan["copy_out"] and out16:  # (rows padded to 8 elements, plan["ldc"])
+            dst = torch.empty(Bt, M, _pad8(N), device=a.device, dtype=rdt)[:, :, :N]
+            if beta != 0.0 and c is None:
+                dst.copy_(out)
+        elif plan["copy_out"]:
             dst = (out.contiguous() if beta != 0.0 and c is None else
                    torch.empty(Bt, M, N, device=a.device, dtype=torch.float32))
             if dst is out:
                 dst = out.clone()
         if c is not None and (c.stride() != dst.stride() or c.data_ptr() % 16 != 0):
-            c = torch.empty_strided(dst.shape, dst.stride(), device=a.device, dtype=torch.float32).copy_(c)
+            c = torch.empty_strided(dst.shape, dst.stride(), device=a.device, dtype=rdt).copy_(c)
         if opts is None:
             opts = make_opts(stream=torch.cuda.current_stream(a.device).cuda_stream)
         kA, kB = (b, a) if plan["swap"] else (a, b)
-        self.run_batched_typed(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], plan["stride_a"],
+        self.run_batched_mixed(kernel_id, plan["M"], plan["N"], plan["K"], kA, plan["layout_a"], plan["lda"], plan["stride_a"],
                                kB, plan["layout_b"], plan["ldb"], plan["stride_b"], TYPE_BF16 if bf16 else TYPE_F32,
-                               c if c is not None else dst, plan["ldc"], plan["stride_c"], dst, Bt, alpha, beta, bias,
-                               plan["bias_mode"], plan["stride_bias"], ACTIVATIONS[activation], preact, opts)
+                               c if c is not None else dst, plan["ldc"], plan["stride_c"], dst, TYPE_BF16 if out16 else TYPE_F32,
+                               Bt, alpha, beta, bias, plan["bias_mode"], plan["stride_bias"], ACTIVATIONS[activation], preact,
+                               opts)
         if dst is not out:
             out.copy_(dst)
         return out
 
     def matmul(self, a, b, out=None, *, c=None, bias=None, activation=None, preact=None, kernel_id: int = ID_ABFT_AUTO,
-               alpha: float = 1.0, beta: float = 0.0, opts: Opts | None = None):
+               alpha: float = 1.0, beta: float = 0.0, opts: Opts | None = None, out_dtype=None):
         """out = alpha * (a @ b) + beta * out + bias for 2-D float32 CUDA tensors a: (M, K), b: (K, N) and an optional 1-D
         float32 bias of length N (one value per column of out, added in the fused store pass); returns out.
 
@@ -678,7 +723,7 @@ class FtSgemm:
         injected faults (opts) and of stats() events are the kernel's, transposed against out in that case.  A kernel M or
         N (after the mapping) that is not a multiple of 4 raises FtsgemmError(-2) for the tensor-core ids, as run does.
         Runs on the current torch stream unless opts.stream says otherwise.  No autograd: linear() is the differentiable
-        F.linear.  Every call is bmm on a batch of one entry, so one run_batched_typed call with batch = 1.  Capturable in a
+        F.linear.  Every call is bmm on a batch of one entry, so one run_batched_mixed call with batch = 1.  Capturable in a
         CUDA graph (see the class docstring).
 
         activation = "relu" | "gelu" stores act(z) with z the value above, in the same store pass of the same call, and z
@@ -693,7 +738,10 @@ class FtSgemm:
 
         a and b may also both be bfloat16 (float32 and bfloat16 mixed raise TypeError): the same call on the BF16 kernels,
         FP32 accumulate, with out, c and preact float32 as above; a bfloat16 bias is upcast (exactly) into a float32
-        temporary.  Their copies pad rows to 8 elements (matmul_plan with bf16)."""
+        temporary.  Their copies pad rows to 8 elements (matmul_plan with bf16).
+
+        The result dtype is chosen as in bmm: out.dtype, else c.dtype, else out_dtype (None: float32); a bfloat16 result
+        needs bfloat16 a and b and is the float32 result rounded to nearest even in the same store pass."""
         import torch
         # (bmm checks everything else on the batch-of-one views)
         for name, t in (("a", a), ("b", b)):
@@ -706,22 +754,23 @@ class FtSgemm:
             elif beta != 0.0:
                 raise ValueError("beta != 0 needs an out tensor or c")
             else:
-                out = torch.empty(M, N, device=a.device, dtype=torch.float32)
+                out = torch.empty(M, N, device=a.device, dtype=out_dtype or torch.float32)
         for name, t in (("c", c), ("out", out), ("preact", preact)):
             if t is not None and t.shape != (M, N):
                 raise ValueError(f"{name} must be an ({M}, {N}) tensor")
         if bias is not None and bias.dim() != 1:  # (bmm would take a (1, N) bias as one bias per entry)
             raise ValueError(f"bias must be a ({N},) tensor")
         self.bmm(a[None], b[None], out[None], c=c[None] if c is not None else None, bias=bias, activation=activation,
-                 preact=preact[None] if preact is not None else None, kernel_id=kernel_id, alpha=alpha, beta=beta, opts=opts)
+                 preact=preact[None] if preact is not None else None, kernel_id=kernel_id, alpha=alpha, beta=beta, opts=opts,
+                 out_dtype=out_dtype)
         return out
 
     def linear(self, x, weight, bias=None, *, activation=None, residual=None, kernel_id: int = ID_ABFT_AUTO,
-               opts: Opts | None = None):
+               opts: Opts | None = None, out_dtype=None):
         """F.linear(x, weight, bias) = x @ weight.T + bias under ABFT protection, differentiable: x (..., K), weight (N, K),
         bias (N,) or None, all float32 CUDA tensors; returns (..., N).
 
-        The forward is one matmul, so one run_batched_typed call, with the bias fused into the store pass, whatever the
+        The forward is one matmul, so one run_batched_mixed call, with the bias fused into the store pass, whatever the
         activation and residual (one autograd Function, _linear_fn); x's leading dimensions are flattened as a view
         where the strides allow it (linear_plan) and copied otherwise.  Backward: grad_x = grad_y @ weight and
         grad_weight = grad_y^T @ x through matmul with the same kernel id and opts (both read in place), grad_bias =
@@ -744,7 +793,13 @@ class FtSgemm:
         x and weight may also both be bfloat16 (mixed with float32: TypeError): the product runs on the BF16 kernels (FP32
         accumulate) and y is float32, as are the residual and the pre-activation value; a bfloat16 bias is upcast exactly.
         The backward rounds grad_z to bfloat16 once (the rounding of torch autocast's BF16 backward) and runs grad_x and
-        grad_weight on the BF16 kernels; the gradients come back in the dtypes of x, weight and the bias."""
+        grad_weight on the BF16 kernels, which write them as bfloat16; the gradients come back in the dtypes of x, weight
+        and the bias.
+
+        out_dtype=torch.bfloat16 (bfloat16 x and weight only, else TypeError) makes y bfloat16: the float32 y above rounded
+        to nearest even in the same store pass, as F.linear on bfloat16 tensors returns it.  The residual must then be
+        bfloat16 and the saved pre-activation value is bfloat16; grad_y arrives as bfloat16, grad_z is formed from it in
+        torch (rounded to bfloat16 once) and grad_r is grad_y."""
         import torch
         if x.dtype not in (torch.float32, torch.bfloat16) or not x.is_cuda or x.dim() < 1:
             raise TypeError("x must be a float32 or bfloat16 CUDA tensor with at least one dimension")
@@ -752,6 +807,11 @@ class FtSgemm:
             raise TypeError("weight must be 2-D (out_features, in_features)")
         if weight.dtype != x.dtype:
             raise TypeError(f"x and weight must both be float32 or both bfloat16, not {x.dtype} and {weight.dtype}")
+        ydt = out_dtype or torch.float32
+        if ydt not in (torch.float32, torch.bfloat16):
+            raise ValueError(f"out_dtype must be float32 or bfloat16, not {ydt}")
+        if ydt == torch.bfloat16 and x.dtype != torch.bfloat16:
+            raise TypeError("out_dtype=torch.bfloat16 needs bfloat16 x and weight")
         lp = linear_plan(tuple(x.shape), x.stride(), tuple(weight.shape))
         x2 = (x.as_strided((lp["M"], lp["K"]), lp["view"], x.storage_offset()) if lp["view"] is not None
               else x.reshape(lp["M"], lp["K"]).contiguous())
@@ -759,14 +819,14 @@ class FtSgemm:
         if residual is not None:
             if activation is not None:
                 raise ValueError("a residual cannot be combined with an activation")
-            if tuple(residual.shape) != lp["out_shape"] or residual.dtype != torch.float32 or residual.device != x.device:
-                raise ValueError(f"residual must be a float32 {lp['out_shape']} tensor on {x.device}")
+            if tuple(residual.shape) != lp["out_shape"] or residual.dtype != ydt or residual.device != x.device:
+                raise ValueError(f"residual must be a {ydt} {lp['out_shape']} tensor on {x.device}")
             r2 = residual.reshape(lp["M"], lp["N"])
         fwd = Opts.from_buffer_copy(opts) if opts is not None else make_opts()
         if not fwd.stream:
             fwd.stream = torch.cuda.current_stream(x.device).cuda_stream
         grad = torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in (x, weight, bias))
-        y = _linear_fn().apply(x2, weight, bias, r2, self, kernel_id, fwd, activation, grad)
+        y = _linear_fn().apply(x2, weight, bias, r2, self, kernel_id, fwd, activation, grad, ydt)
         return y.view(lp["out_shape"])
 
     def run_host(self, kernel_id: int, M: int, N: int, K: int, hA, hB, hC, alpha: float = 1.0, beta: float = 0.0,
@@ -850,21 +910,22 @@ _LINEAR_FN = None
 
 def _linear_fn():
     """The torch.autograd.Function behind FtSgemm.linear (built on first use: torch is imported lazily): one matmul
-    forward (so one run_batched_typed call), the activation's backward in torch, then the products of _linear_grads."""
+    forward (so one run_batched_mixed call), the activation's backward in torch, then the products of _linear_grads."""
     global _LINEAR_FN
     if _LINEAR_FN is None:
         import torch
 
         class LinearFn(torch.autograd.Function):
             @staticmethod
-            def forward(ctx, x2, weight, bias, residual, dev, kernel_id, opts, activation, grad):
+            def forward(ctx, x2, weight, bias, residual, dev, kernel_id, opts, activation, grad, ydt):
                 # (grad: grad mode was on and an input requires grad -- forward itself runs with grad mode off.  z is
-                # written for GELU's backward only: ReLU's reads y > 0, and without an activation grad_z is grad_y)
+                # written for GELU's backward only: ReLU's reads y > 0, and without an activation grad_z is grad_y.
+                # ydt: the dtype of y, and of z)
                 z = None
                 if grad and activation == "gelu":
-                    z = torch.empty(x2.shape[0], weight.shape[0], device=x2.device, dtype=torch.float32)
+                    z = torch.empty(x2.shape[0], weight.shape[0], device=x2.device, dtype=ydt)
                 y = dev.matmul(x2, weight.t(), c=residual, bias=bias, activation=activation, preact=z, kernel_id=kernel_id,
-                               beta=0.0 if residual is None else 1.0, opts=opts)
+                               beta=0.0 if residual is None else 1.0, opts=opts, out_dtype=ydt)
                 ctx.save_for_backward(x2, weight, y if activation == "relu" else z)
                 ctx.dev, ctx.kernel_id, ctx.opts, ctx.activation = dev, kernel_id, opts, activation
                 ctx.bias_dtype = bias.dtype if bias is not None else None
@@ -875,7 +936,7 @@ def _linear_fn():
                 x2, weight, saved = ctx.saved_tensors
                 gz = _grad_z(gy, ctx.activation, saved)
                 gx, gw, gb = _linear_grads(ctx, gz, x2, weight, _backward_opts(ctx.opts, gy.device))
-                return gx, gw, gb, gy if ctx.needs_input_grad[3] else None, None, None, None, None, None
+                return gx, gw, gb, gy if ctx.needs_input_grad[3] else None, None, None, None, None, None, None
 
         _LINEAR_FN = LinearFn
     return _LINEAR_FN
@@ -905,14 +966,15 @@ def _grad_z(gy, activation, saved):
 def _linear_grads(ctx, gz, x2, weight, bwd):
     """grad_x = grad_z @ weight, grad_weight = grad_z^T @ x through matmul, grad_bias = grad_z summed over the rows (the
     needed ones, None otherwise).  BF16 x and weight: grad_z is rounded to bfloat16 once and the products run on the BF16
-    kernels; every gradient is returned in its input's dtype."""
+    kernels, which write bfloat16 gradients directly (the float32 products rounded once, bit for bit); every gradient is
+    returned in its input's dtype."""
     import torch
     gx = gw = gb = None
     g = gz.to(torch.bfloat16) if x2.dtype == torch.bfloat16 else gz
     if ctx.needs_input_grad[0]:
-        gx = ctx.dev.matmul(g, weight, kernel_id=ctx.kernel_id, opts=bwd).to(x2.dtype)
+        gx = ctx.dev.matmul(g, weight, kernel_id=ctx.kernel_id, opts=bwd, out_dtype=x2.dtype)
     if ctx.needs_input_grad[1]:
-        gw = ctx.dev.matmul(g.t(), x2, kernel_id=ctx.kernel_id, opts=bwd).to(weight.dtype)
+        gw = ctx.dev.matmul(g.t(), x2, kernel_id=ctx.kernel_id, opts=bwd, out_dtype=weight.dtype)
     if ctx.needs_input_grad[2]:
         gb = g.float().sum(0).to(ctx.bias_dtype)
     return gx, gw, gb
@@ -922,7 +984,7 @@ _BMM_FN = None
 
 
 def _bmm_fn():
-    """The torch.autograd.Function behind a differentiable FtSgemm.bmm: one bmm forward (so one run_batched_typed call),
+    """The torch.autograd.Function behind a differentiable FtSgemm.bmm: one bmm forward (so one run_batched_mixed call),
     the activation's backward in torch, then the two gradient products through bmm."""
     global _BMM_FN
     if _BMM_FN is None:
@@ -930,12 +992,13 @@ def _bmm_fn():
 
         class BmmFn(torch.autograd.Function):
             @staticmethod
-            def forward(ctx, a, b, bias, preact, c, dev, kernel_id, alpha, beta, opts, activation):
+            def forward(ctx, a, b, bias, preact, c, dev, kernel_id, alpha, beta, opts, activation, rdt):
+                # (rdt: the result dtype, which z has too)
                 z = preact
                 if z is None and activation == "gelu":
-                    z = torch.empty(a.shape[0], a.shape[1], b.shape[2], device=a.device, dtype=torch.float32)
+                    z = torch.empty(a.shape[0], a.shape[1], b.shape[2], device=a.device, dtype=rdt)
                 y = dev.bmm(a, b, c=c, bias=bias, activation=activation, preact=z, kernel_id=kernel_id, alpha=alpha,
-                            beta=beta if c is not None else 0.0, opts=opts)
+                            beta=beta if c is not None else 0.0, opts=opts, out_dtype=rdt)
                 ctx.save_for_backward(a, b, y if activation == "relu" else z)
                 ctx.dev, ctx.kernel_id, ctx.alpha, ctx.beta, ctx.opts, ctx.activation = dev, kernel_id, alpha, beta, opts, activation
                 ctx.per_entry_bias = bias is not None and bias.dim() == 2
@@ -948,18 +1011,19 @@ def _bmm_fn():
                 gz = _grad_z(gy, ctx.activation, saved)
                 bwd = _backward_opts(ctx.opts, gy.device)
                 ga = gb = gbias = gc = None
-                # (BF16 operands: grad_z rounded to bfloat16 once for the products, gradients in the inputs' dtypes)
+                # (BF16 operands: grad_z rounded to bfloat16 once for the products, which write the gradients in the inputs'
+                # dtypes directly)
                 g = gz.to(torch.bfloat16) if a.dtype == torch.bfloat16 else gz
                 if ctx.needs_input_grad[0]:
-                    ga = ctx.dev.bmm(g, b.transpose(1, 2), kernel_id=ctx.kernel_id, alpha=ctx.alpha, opts=bwd).to(a.dtype)
+                    ga = ctx.dev.bmm(g, b.transpose(1, 2), kernel_id=ctx.kernel_id, alpha=ctx.alpha, opts=bwd, out_dtype=a.dtype)
                 if ctx.needs_input_grad[1]:
-                    gb = ctx.dev.bmm(a.transpose(1, 2), g, kernel_id=ctx.kernel_id, alpha=ctx.alpha, opts=bwd).to(b.dtype)
+                    gb = ctx.dev.bmm(a.transpose(1, 2), g, kernel_id=ctx.kernel_id, alpha=ctx.alpha, opts=bwd, out_dtype=b.dtype)
                 if ctx.needs_input_grad[2]:
                     gf = g.float() if a.dtype == torch.bfloat16 else gz
                     gbias = (gf.sum(1) if ctx.per_entry_bias else gf.sum((0, 1))).to(ctx.bias_dtype)
                 if ctx.needs_input_grad[4]:
                     gc = ctx.beta * gz
-                return ga, gb, gbias, None, gc, None, None, None, None, None, None
+                return ga, gb, gbias, None, gc, None, None, None, None, None, None, None
 
         _BMM_FN = BmmFn
     return _BMM_FN

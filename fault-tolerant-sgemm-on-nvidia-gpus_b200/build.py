@@ -13,9 +13,10 @@ ROOT = HERE.parent
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-ccbin", "/usr/bin/g++"]
-# ptxas compiles the library's ~230 kernels on up to 8 threads: the same machine code as a serial run (SASS identical),
-# in about half the build time; the cap bounds its memory (~1 GB per thread)
-PTXAS_THREADS = ["-Xptxas", f"--split-compile={max(1, min(8, os.cpu_count() or 1))}"]
+# ptxas compiles the library's kernels on several threads: the same machine code as a serial run (SASS identical), in about
+# half the build time.  The units compiled at the same time share one budget of threads, which bounds the build's memory
+# (~1 GB per thread): 3 x min(8, CPUs) in all, what three units of 8 threads took before the fourth unit existed.
+PTXAS_BUDGET = 3 * max(1, min(8, os.cpu_count() or 1))
 
 LIB = HERE / "libftsgemm.so"
 CLI = HERE / "ft_sgemm"
@@ -29,18 +30,25 @@ def _stale(target: Path, sources) -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> None:
-    # three translation units compiled at the same time (their device compilation is single-threaded up to ptxas): the
-    # library, the OUT kernels of ftsgemm_run_batched_out (ftsgemm_out.cu) and the BF16 kernels of ftsgemm_run_batched_typed
-    # (ftsgemm_bf16.cu); then one link
-    lib_src = [CSRC / "ftsgemm.cu", CSRC / "ftsgemm_out.cu", CSRC / "ftsgemm_bf16.cu"]
+    # four translation units compiled at the same time (their device compilation is single-threaded up to ptxas): the
+    # library, the OUT kernels of ftsgemm_run_batched_out (ftsgemm_out.cu), the BF16 kernels of ftsgemm_run_batched_typed
+    # (ftsgemm_bf16.cu) and their BF16-output twins of ftsgemm_run_batched_mixed (ftsgemm_bf16_cd.cu); then one link
+    lib_src = [CSRC / "ftsgemm.cu", CSRC / "ftsgemm_out.cu", CSRC / "ftsgemm_bf16.cu", CSRC / "ftsgemm_bf16_cd.cu"]
     lib_dep = lib_src + sorted(CSRC.glob("*.cuh")) + sorted(CSRC.glob("*.h")) + [ROOT / "include" / "ftsgemm.h"]
     if force or _stale(LIB, lib_dep):
+        threads = ["-Xptxas", f"--split-compile={max(1, PTXAS_BUDGET // len(lib_src))}"]
         with tempfile.TemporaryDirectory() as tmp:
             objs = [Path(tmp) / (src.stem + ".o") for src in lib_src]
-            procs = [subprocess.Popen([NVCC, *ARCH, *COMMON, *PTXAS_THREADS, "-c", "-Xptxas", "-v", str(src), "-o", str(obj)],
-                                      stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True)
-                     for src, obj in zip(lib_src, objs)]
-            outs = [p.communicate() for p in procs]
+            # (each unit's output goes to files: a full pipe would stall a unit until the slowest one is read)
+            logs = [(Path(tmp) / (src.stem + ".out"), Path(tmp) / (src.stem + ".err")) for src in lib_src]
+            procs = []
+            for src, obj, (lo, le) in zip(lib_src, objs, logs):
+                with open(lo, "w") as fo, open(le, "w") as fe:
+                    procs.append(subprocess.Popen([NVCC, *ARCH, *COMMON, *threads, "-c", "-Xptxas", "-v", str(src), "-o", str(obj)],
+                                                  stdout=fo, stderr=fe))
+            for p in procs:
+                p.wait()
+            outs = [(lo.read_text(), le.read_text()) for lo, le in logs]
             err = "".join(e for _, e in outs)
             rc = max(p.returncode for p in procs)
             if rc == 0:

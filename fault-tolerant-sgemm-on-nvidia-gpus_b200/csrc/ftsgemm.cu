@@ -144,6 +144,7 @@ struct ftsgemm_handle_s {
   DeviceStats *d_stats = nullptr;
   bool out_launched = false;    // an OUT kernel (ftsgemm_out.cu: its own abort flag) has run through the handle
   bool bf16_launched = false;   // a BF16 kernel (ftsgemm_bf16.cu: its own abort flag) has run through the handle
+  bool bf16_cd_launched = false;  // a BF16-output kernel (ftsgemm_bf16_cd.cu: its own abort flag) has run through the handle
   DevBuf d_chk;                 // encoded checksum vectors [K][tiles_n*8]  (extra "rows" of B)
   DevBuf d_chk_out;             // slab flags, then the expected checksums M x (tiles_n*8), column-major
   size_t chk_flag_bytes = kChkFlagBytes;  // bytes of d_chk_out in front of the expected checksums: the slab flags
@@ -240,12 +241,14 @@ struct DeviceGuard {
 
 // The kernels' watchdog (ptx.cuh) raises a device-wide flag instead of trapping; reported once, then cleared.
 int check_abort_flag(ftsgemm_handle_t h) {
-  int flag = 0, out_flag = 0, bf16_flag = 0;
+  int flag = 0, out_flag = 0, bf16_flag = 0, bf16_cd_flag = 0;
   FT_CUDA(h, cudaMemcpyFromSymbol(&flag, ptx::g_abort_flag, sizeof(int)));
-  // (the OUT and BF16 kernels' translation units have their own copies, read once one of them has run through this handle)
+  // (the OUT, BF16 and BF16-output kernels' translation units have their own copies, read once one of them has run through
+  // this handle)
   if (h->out_launched) FT_CUDA(h, tc_out_abort_flag(&out_flag));
   if (h->bf16_launched) FT_CUDA(h, tc_bf16_abort_flag(&bf16_flag));
-  if (flag == 0) return (out_flag == 0 && bf16_flag == 0) ? FTSGEMM_OK : FTSGEMM_ERR_TIMEOUT;
+  if (h->bf16_cd_launched) FT_CUDA(h, tc_bf16_cd_abort_flag(&bf16_cd_flag));
+  if (flag == 0) return (out_flag == 0 && bf16_flag == 0 && bf16_cd_flag == 0) ? FTSGEMM_OK : FTSGEMM_ERR_TIMEOUT;
   flag = 0;
   FT_CUDA(h, cudaMemcpyToSymbol(ptx::g_abort_flag, &flag, sizeof(int)));
   return FTSGEMM_ERR_TIMEOUT;
@@ -340,13 +343,14 @@ template <int BN, int CG>
 int launch_kernel(ftsgemm_handle_t h, TcKernel kern, int resident, const CUtensorMap &tmA, const CUtensorMap &tmB,
                   const CUtensorMap &tmC, const KernelParams &p, int units, cudaStream_t stream);
 
-// query_max_units of the BF16 kernel of a tile, flags and layouts (ftsgemm_bf16.cu), cached under its own key
+// query_max_units of the BF16 kernel of a tile, flags, layouts and output type (ftsgemm_bf16.cu, ftsgemm_bf16_cd.cu), cached
+// under its own key
 template <int BN, int CG>
-int query_bf16_units(ftsgemm_handle_t h, bool ft, bool seed, bool a_kmajor, bool b_kmajor, int *out) {
-  const TcKernel kern = tc_bf16_kernel(BN, ft, seed, a_kmajor, b_kmajor);
+int query_bf16_units(ftsgemm_handle_t h, bool ft, bool seed, bool a_kmajor, bool b_kmajor, int *out, bool cd_bf16 = false) {
+  const TcKernel kern = tc_bf16_kernel(BN, ft, seed, a_kmajor, b_kmajor, cd_bf16);
   if (!kern || CG != 2) return FTSGEMM_ERR_UNSUPPORTED;
-  const int key = (1 << 20) | (BN << 8) | ((ft ? 1 : 0) << 4) | ((seed ? 1 : 0) << 3) | ((a_kmajor ? 1 : 0) << 2) |
-                  ((b_kmajor ? 1 : 0) << 1) | (CG - 1);
+  const int key = (1 << 20) | ((cd_bf16 ? 1 : 0) << 5) | (BN << 8) | ((ft ? 1 : 0) << 4) | ((seed ? 1 : 0) << 3) |
+                  ((a_kmajor ? 1 : 0) << 2) | ((b_kmajor ? 1 : 0) << 1) | (CG - 1);
   return query_max_units<BN, true, CG>(h, out, kern, key);
 }
 
@@ -425,17 +429,19 @@ int with_flag(bool b, F &&f) {
 // ftsgemm_tc_kernel), BATCH for a batch of more than one entry, PROT (fault-tolerant kernels only) for opts.protect_epilogue.
 // An activation (the bias mode is then a run-time field) selects the ACT kernels instead of BIAS: with BATCH for a batch of
 // more than one entry.  A separate output D (p.d, with or without an activation) selects the OUT form of the ACT kernels.
-// bf16: the BF16 kernels (ftsgemm_bf16.cu), which take the bias, the activation, D and the protection level at run time.
+// bf16: the BF16 kernels (ftsgemm_bf16.cu), which take the bias, the activation, D and the protection level at run time;
+// with cd_bf16 their twins with BF16 C, D and Z (ftsgemm_bf16_cd.cu).
 template <int BN, int CG>
 int launch_variant(ftsgemm_handle_t h, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
-                   const KernelParams &p, int units, cudaStream_t stream, bool ft, bool prot, bool bf16 = false) {
+                   const KernelParams &p, int units, cudaStream_t stream, bool ft, bool prot, bool bf16 = false,
+                   bool cd_bf16 = false) {
   if (bf16) {
-    const TcKernel kern = tc_bf16_kernel(BN, ft, p.sk_tiles > 0, p.a_kmajor != 0, p.b_kmajor != 0);
+    const TcKernel kern = tc_bf16_kernel(BN, ft, p.sk_tiles > 0, p.a_kmajor != 0, p.b_kmajor != 0, cd_bf16);
     if (!kern || CG != 2) return FTSGEMM_ERR_UNSUPPORTED;
     int resident = 0;
-    const int qrc = query_bf16_units<BN, CG>(h, ft, p.sk_tiles > 0, p.a_kmajor != 0, p.b_kmajor != 0, &resident);
+    const int qrc = query_bf16_units<BN, CG>(h, ft, p.sk_tiles > 0, p.a_kmajor != 0, p.b_kmajor != 0, &resident, cd_bf16);
     if (qrc) return qrc;
-    h->bf16_launched = true;
+    (cd_bf16 ? h->bf16_cd_launched : h->bf16_launched) = true;
     return launch_kernel<BN, CG>(h, kern, resident, tmA, tmB, tmC, p, units, stream);
   }
   if (p.act != kActNone || p.d != nullptr) {
@@ -749,11 +755,13 @@ int bind_operands(ftsgemm_handle_t h, const Variant &v, KernelParams &p, CUtenso
 }
 
 // The launch plan for as many work units as the device holds at once.
-int plan_on_device(ftsgemm_handle_t h, const Variant &v, KernelParams &p, PlanInput *pin, bool bf16 = false) {
+int plan_on_device(ftsgemm_handle_t h, const Variant &v, KernelParams &p, PlanInput *pin, bool bf16 = false,
+                   bool cd_bf16 = false) {
   int max_units = 0;
   const int rc = with_tile(v.bn, v.cg, [&](auto bn, auto cg) {
     if (bf16)  // (the BF16 kernel the launch runs; its SEED twin has the same resources and is checked at the launch)
-      return query_bf16_units<bn, cg>(h, v.info.fault_tolerant != 0, false, p.a_kmajor != 0, p.b_kmajor != 0, &max_units);
+      return query_bf16_units<bn, cg>(h, v.info.fault_tolerant != 0, false, p.a_kmajor != 0, p.b_kmajor != 0, &max_units,
+                                      cd_bf16);
     return v.info.fault_tolerant ? query_max_units<bn, true, cg>(h, &max_units) : query_max_units<bn, false, cg>(h, &max_units);
   });
   if (rc) return rc;
@@ -962,10 +970,11 @@ int bind_plan(ftsgemm_handle_t h, const Variant &v, KernelParams &p, const PlanI
 }
 
 // One product on the wgmma kernels, in stages: argument checks, kernel parameters, operands, launch plan, checksums, cached
-// work plan, per-plan workspaces, launch.  dD: a separate output (C read-only), null in place.
+// work plan, per-plan workspaces, launch.  dD: a separate output (C read-only), null in place.  cd_bf16: C, D and Z are
+// BF16 (BF16 operands only).
 int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC, int ldc,
            float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o, cudaStream_t stream,
-           const BatchArg &bt = kSingle, const ActArg &act = kNoAct, float *dD = nullptr) {
+           const BatchArg &bt = kSingle, const ActArg &act = kNoAct, float *dD = nullptr, bool cd_bf16 = false) {
   int rc = check_tc_args(v, M, N, K, A, B, dC, bt.count);
   if (rc) return rc;
   const bool bf16 = A.bf16;
@@ -973,7 +982,7 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
   KernelParams p = make_params(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, bt, act, bf16 && !dD ? dC : dD);
   CUtensorMap tmA, tmB, tmC;
   PlanInput pin;
-  if ((rc = bind_operands(h, v, p, &tmA, &tmB, bf16)) || (rc = plan_on_device(h, v, p, &pin, bf16))) return rc;
+  if ((rc = bind_operands(h, v, p, &tmA, &tmB, bf16)) || (rc = plan_on_device(h, v, p, &pin, bf16, cd_bf16))) return rc;
   tmC = tmB;
   if (v.info.fault_tolerant && (rc = bind_checksums(h, v, p, o, stream, &tmC, bf16))) return rc;
   CachedPlan *cp = nullptr;
@@ -985,19 +994,20 @@ int run_tc(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Oper
   ++h->launch_count;
   return with_tile(v.bn, v.cg, [&](auto bn, auto cg) {
     return launch_variant<bn, cg>(h, tmA, tmB, tmC, p, cp->plan.units, stream, v.info.fault_tolerant != 0,
-                                  o.protect_epilogue != 0, bf16);
+                                  o.protect_epilogue != 0, bf16, cd_bf16);
   });
 }
 
 int run_cublas(ftsgemm_handle_t h, bool tf32, int M, int N, int K, const Operand &A, const Operand &B, float *dC, int ldc,
-               float alpha, float beta, cudaStream_t stream, const BatchArg &bt = kSingle) {
+               float alpha, float beta, cudaStream_t stream, const BatchArg &bt = kSingle, bool cd_bf16 = false) {
   FT_CUBLAS(h, cublasSetStream(h->cublas, stream));
   FT_CUBLAS(h, cublasSetPointerMode(h->cublas, CUBLAS_POINTER_MODE_HOST));
   FT_CUBLAS(h, cublasSetMathMode(h->cublas, tf32 ? CUBLAS_TF32_TENSOR_OP_MATH : CUBLAS_DEFAULT_MATH));
-  if (A.bf16) {  // BF16 A and B, FP32 C, FP32 compute (ids 0 and 7 alike); one entry: strides 0
+  if (A.bf16) {  // BF16 A and B, FP32 (cd_bf16: BF16) C, FP32 compute (ids 0 and 7 alike); one entry: strides 0
     FT_CUBLAS(h, cublasGemmStridedBatchedEx(h->cublas, A.kmajor ? CUBLAS_OP_T : CUBLAS_OP_N, B.kmajor ? CUBLAS_OP_N : CUBLAS_OP_T, M,
                                             N, K, &alpha, A.p, CUDA_R_16BF, A.ld, bt.sa, B.p, CUDA_R_16BF, B.ld, bt.sb, &beta, dC,
-                                            CUDA_R_32F, ldc, bt.sc, bt.count, CUBLAS_COMPUTE_32F, CUBLAS_GEMM_DEFAULT));
+                                            cd_bf16 ? CUDA_R_16BF : CUDA_R_32F, ldc, bt.sc, bt.count, CUBLAS_COMPUTE_32F,
+                                            CUBLAS_GEMM_DEFAULT));
     h->last_stream = stream;
     return FTSGEMM_OK;
   }
@@ -1222,7 +1232,7 @@ int run_3xtf32(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const 
 
 int run_resolved(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC,
                  int ldc, float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o,
-                 cudaStream_t stream, const BatchArg &bt, const ActArg &act = kNoAct, float *dD = nullptr);
+                 cudaStream_t stream, const BatchArg &bt, const ActArg &act = kNoAct, float *dD = nullptr, bool cd_bf16 = false);
 
 // Intra-K checking (ftsgemm_opts::check_segments): S consecutive K-segments, each a complete fault-tolerant GEMM.  A
 // segment of an operand is a pointer offset: k0 * ld for an MN-major operand (k is the slow index), k0 for a K-major one;
@@ -1255,18 +1265,19 @@ int run_segments(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, cons
 }
 
 // One call of ftsgemm_run_batched after validation: its variant resolved (ids 20 / 40 chosen per shape), its options
-// loaded and h->capturing set.  dD (a separate output, wgmma ids only) is null in place.
+// loaded and h->capturing set.  dD (a separate output, wgmma ids only) is null in place.  cd_bf16: C, D and Z are BF16
+// (run_call has refused the segmented and 3xTF32 forms for them).
 int run_resolved(ftsgemm_handle_t h, const Variant &v, int M, int N, int K, const Operand &A, const Operand &B, float *dC,
                  int ldc, float alpha, float beta, const float *bias, int bias_mode, const ftsgemm_opts &o,
-                 cudaStream_t stream, const BatchArg &bt, const ActArg &act, float *dD) {
+                 cudaStream_t stream, const BatchArg &bt, const ActArg &act, float *dD, bool cd_bf16) {
   const bool tc = v.info.engine == 1;
   if (tc && o.check_segments > 1 && v.info.fault_tolerant)
     return run_segments(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt, act, dD);
   if (tc && o.precision == 1)
     return run_3xtf32(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt, act, dD);
   switch (v.info.engine) {
-    case 0: return run_cublas(h, v.info.id == 7, M, N, K, A, B, dC, ldc, alpha, beta, stream, bt);
-    case 1: return run_tc(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt, act, dD);
+    case 0: return run_cublas(h, v.info.id == 7, M, N, K, A, B, dC, ldc, alpha, beta, stream, bt, cd_bf16);
+    case 1: return run_tc(h, v, M, N, K, A, B, dC, ldc, alpha, beta, bias, bias_mode, o, stream, bt, act, dD, cd_bf16);
     case 2:
       // the non-fused baseline keeps the reference's call sequence, on the reference layout only
       if (A.kmajor || B.kmajor || A.ld != M || B.ld != N || ldc != M) return FTSGEMM_ERR_UNSUPPORTED;
@@ -1489,19 +1500,21 @@ int ftsgemm_run_bias(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, con
                              bias_mode, opts);
 }
 
-// [p, p + n floats) and [q, q + n floats) share an address
-static bool overlaps(const float *p, const float *q, long long n) {
-  const uintptr_t a = reinterpret_cast<uintptr_t>(p), b = reinterpret_cast<uintptr_t>(q), bytes = static_cast<uintptr_t>(n) * 4u;
+// [p, p + n elements) and [q, q + n elements) share an address (elem: bytes per element, 4 for FP32, 2 for BF16)
+static bool overlaps(const float *p, const float *q, long long n, int elem = 4) {
+  const uintptr_t a = reinterpret_cast<uintptr_t>(p), b = reinterpret_cast<uintptr_t>(q),
+                  bytes = static_cast<uintptr_t>(n) * static_cast<uintptr_t>(elem);
   return a < b + bytes && b < a + bytes;
 }
 
 // ftsgemm_run_batched_out (and through it every run entry point): validation, options, capture state, variant; then
 // run_resolved.  dD == dC is the in-place call.
-// (bf16: A and B are BF16, ftsgemm_run_batched_typed)
+// (bf16: A and B are BF16, ftsgemm_run_batched_typed; cd_bf16: C, D and Z are BF16 too, ftsgemm_run_batched_mixed)
 static int run_call(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
                     long long stride_a, const float *dB, int layout_b, int ldb, long long stride_b, const float *dC, int ldc,
                     long long stride_c, float *dD, int batch, float alpha, float beta, const float *bias, int bias_mode,
-                    long long stride_bias, const ActArg &act, const ftsgemm_opts *opts, bool bf16 = false) {
+                    long long stride_bias, const ActArg &act, const ftsgemm_opts *opts, bool bf16 = false,
+                    bool cd_bf16 = false) {
   if (!h) return FTSGEMM_ERR_NO_DEVICE;
   const bool sep = dD != dC;  // a separate output: C is read-only, and not read at all with beta == 0 (may be null)
   if (!dA || !dB || !dD || (!dC && !(sep && beta == 0.0f)) || M <= 0 || N <= 0 || K <= 0 || batch < 1)
@@ -1519,6 +1532,12 @@ static int run_call(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, cons
     if ((lda % 8) || (ldb % 8) || ((reinterpret_cast<uintptr_t>(dA) | reinterpret_cast<uintptr_t>(dB)) & 15))
       return FTSGEMM_ERR_INVALID_ARG;
     if (batch > 1 && ((stride_a % 8) || (stride_b % 8))) return FTSGEMM_ERR_INVALID_ARG;
+  }
+  // BF16 C / D / Z: the operand rules of BF16 A and B -- 16-byte rows and entry strides, 16-byte aligned C (when read), D and Z
+  if (cd_bf16) {
+    if ((ldc % 8) || (batch > 1 && (stride_c % 8))) return FTSGEMM_ERR_INVALID_ARG;
+    const uintptr_t c_read = (dC && beta != 0.0f) ? reinterpret_cast<uintptr_t>(dC) : 0u;
+    if ((reinterpret_cast<uintptr_t>(dD) | reinterpret_cast<uintptr_t>(act.z) | c_read) & 15) return FTSGEMM_ERR_INVALID_ARG;
   }
   if (lda < (A.kmajor ? K : M) || ldb < (B.kmajor ? K : N) || ldc < M) return FTSGEMM_ERR_INVALID_ARG;
   if (bias_mode < FTSGEMM_BIAS_NONE || bias_mode > FTSGEMM_BIAS_COL) return FTSGEMM_ERR_INVALID_ARG;
@@ -1543,8 +1562,9 @@ static int run_call(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, cons
     if (v->info.engine != 1) return FTSGEMM_ERR_UNSUPPORTED;  // only the wgmma kernels store to a separate output
     if (reinterpret_cast<uintptr_t>(dD) & 15) return FTSGEMM_ERR_INVALID_ARG;
     const long long span = (batch > 1 ? (batch - 1) * stride_c : 0) + static_cast<long long>(N - 1) * ldc + M;
-    if (dC && overlaps(dC, dD, span)) return FTSGEMM_ERR_INVALID_ARG;
-    if (act.z && (overlaps(act.z, dD, span) || (dC && overlaps(act.z, dC, span)))) return FTSGEMM_ERR_INVALID_ARG;
+    const int elem = cd_bf16 ? 2 : 4;  // (footprints in bytes of the output type)
+    if (dC && overlaps(dC, dD, span, elem)) return FTSGEMM_ERR_INVALID_ARG;
+    if (act.z && (overlaps(act.z, dD, span, elem) || (dC && overlaps(act.z, dC, span, elem)))) return FTSGEMM_ERR_INVALID_ARG;
     if (beta != 0.0f) {  // (beta == 0: the in-place call on D)
       dOld = const_cast<float *>(dC);  // (read only: the kernels store to dSep)
       dSep = dD;
@@ -1554,6 +1574,8 @@ static int run_call(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, cons
   const int orc = load_opts(opts, &o);
   if (orc) return orc;
   if (bf16 && o.precision == 1) return FTSGEMM_ERR_INVALID_ARG;  // BF16 products are exact in FP32: nothing to split
+  // segments 2..S accumulate into D in place: a BF16 D would be rounded once per segment
+  if (cd_bf16 && o.check_segments > 1) return FTSGEMM_ERR_UNSUPPORTED;
   DeviceGuard guard(h);
   cudaStream_t stream = static_cast<cudaStream_t>(o.stream);
   {
@@ -1568,7 +1590,7 @@ static int run_call(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, cons
     v = find_variant(select_variant(M, N, v->info.fault_tolerant != 0, bt.count));
     if (!v) return FTSGEMM_ERR_UNSUPPORTED;
   }
-  return run_resolved(h, *v, M, N, K, A, B, dOld, ldc, alpha, beta, bias, bias_mode, o, stream, bt, act, dSep);
+  return run_resolved(h, *v, M, N, K, A, B, dOld, ldc, alpha, beta, bias, bias_mode, o, stream, bt, act, dSep, cd_bf16);
 }
 
 int ftsgemm_run_batched(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const float *dA, int layout_a, int lda,
@@ -1622,14 +1644,28 @@ int ftsgemm_run_batched_typed(ftsgemm_handle_t h, int kernel_id, int M, int N, i
                               const float *dC, int ldc, long long stride_c, float *dD, int batch, float alpha, float beta,
                               const float *bias, int bias_mode, long long stride_bias, int activation, float *dZ,
                               const ftsgemm_opts *opts) {
+  return ftsgemm_run_batched_mixed(h, kernel_id, M, N, K, dA, layout_a, lda, stride_a, dB, layout_b, ldb, stride_b, ab_type, dC,
+                                   ldc, stride_c, dD, FTSGEMM_TYPE_F32, batch, alpha, beta, bias, bias_mode, stride_bias,
+                                   activation, dZ, opts);
+}
+
+int ftsgemm_run_batched_mixed(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const void *dA, int layout_a, int lda,
+                              long long stride_a, const void *dB, int layout_b, int ldb, long long stride_b, int ab_type,
+                              const void *dC, int ldc, long long stride_c, void *dD, int cd_type, int batch, float alpha,
+                              float beta, const float *bias, int bias_mode, long long stride_bias, int activation, void *dZ,
+                              const ftsgemm_opts *opts) {
   if (!h) return FTSGEMM_ERR_NO_DEVICE;
   if (ab_type != FTSGEMM_TYPE_F32 && ab_type != FTSGEMM_TYPE_BF16) return FTSGEMM_ERR_INVALID_ARG;
+  if (cd_type != FTSGEMM_TYPE_F32 && cd_type != FTSGEMM_TYPE_BF16) return FTSGEMM_ERR_INVALID_ARG;
   if (activation < FTSGEMM_ACT_NONE || activation > FTSGEMM_ACT_GELU) return FTSGEMM_ERR_INVALID_ARG;
   if (dZ && (activation == FTSGEMM_ACT_NONE || dZ == dC || dZ == dD || (reinterpret_cast<uintptr_t>(dZ) & 3)))
     return FTSGEMM_ERR_INVALID_ARG;
+  // BF16 output needs BF16 operands: the TF32 kernels have no BF16-output form
+  if (cd_type == FTSGEMM_TYPE_BF16 && ab_type != FTSGEMM_TYPE_BF16) return FTSGEMM_ERR_UNSUPPORTED;
   return run_call(h, kernel_id, M, N, K, static_cast<const float *>(dA), layout_a, lda, stride_a, static_cast<const float *>(dB),
-                  layout_b, ldb, stride_b, dC, ldc, stride_c, dD, batch, alpha, beta, bias, bias_mode, stride_bias,
-                  ActArg{activation, dZ}, opts, ab_type == FTSGEMM_TYPE_BF16);
+                  layout_b, ldb, stride_b, static_cast<const float *>(dC), ldc, stride_c, static_cast<float *>(dD), batch, alpha,
+                  beta, bias, bias_mode, stride_bias, ActArg{activation, static_cast<float *>(dZ)}, opts,
+                  ab_type == FTSGEMM_TYPE_BF16, cd_type == FTSGEMM_TYPE_BF16);
 }
 
 int ftsgemm_get_stats(ftsgemm_handle_t h, ftsgemm_stats *out) {

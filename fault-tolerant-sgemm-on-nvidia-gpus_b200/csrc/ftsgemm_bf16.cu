@@ -3,24 +3,14 @@
 // tc_bf16_kernel, launch_encode_bf16 and tc_bf16_abort_flag only.  With B of 8 MB or more the fault-tolerant kernels encode
 // B in their front phase (front_encode_bf16), otherwise the pre-pass below does.
 //
-// Instantiations: the OUT x BATCH form of ftsgemm_tc_kernel (bias mode, activation, Z and D at run time; a single product is
-// a batch of one on 3-D tensor maps) for the two-CTA tiles 256 x 256 and 256 x 128, plain and fault-tolerant (with PROT: the
-// protection level is read at run time), with and without SEED, for the four layout pairs: 32 kernels.
+// Instantiations (tc_bf16_select<0>): the OUT x BATCH form of ftsgemm_tc_kernel (bias mode, activation, Z and D at run time;
+// a single product is a batch of one on 3-D tensor maps) for the two-CTA tiles 256 x 256 and 256 x 128, plain and
+// fault-tolerant (with PROT: the protection level is read at run time), with and without SEED, for the four layout pairs:
+// 32 kernels.  Their twins with BF16 C, D and Z are compiled in ftsgemm_bf16_cd.cu; tc_bf16_kernel hands them out too.
 #include "ftsgemm_kernel.cuh"
 
 namespace ftsgemm {
 namespace {
-template <int BN, bool FT, int AB>
-TcKernel bf16_kernel(bool seed) {
-  return seed ? ftsgemm_tc_kernel<BN, FT, 2, FT, true, false, true, true, true, AB>
-              : ftsgemm_tc_kernel<BN, FT, 2, FT, false, false, true, true, true, AB>;
-}
-template <int BN, bool FT>
-TcKernel bf16_kernel_of_layouts(bool seed, bool a_kmajor, bool b_kmajor) {
-  constexpr int a = kAbBf16 | kAbAMn, b = kAbBf16 | kAbBMn;
-  if (a_kmajor) return b_kmajor ? bf16_kernel<BN, FT, kAbBf16>(seed) : bf16_kernel<BN, FT, b>(seed);
-  return b_kmajor ? bf16_kernel<BN, FT, a>(seed) : bf16_kernel<BN, FT, a | b>(seed);
-}
 
 // The stand-alone encode pre-pass (B below 8 MB; encode_bf16_mn_items / encode_bf16_k_items in ftsgemm_kernel.cuh): entry
 // e = blockIdx.y, blockIdx.y + gridDim.y, ...
@@ -48,12 +38,8 @@ encode_bf16_k_kernel(const __nv_bfloat16 *__restrict__ B, int N, int K, int ldb,
 }
 }  // namespace
 
-TcKernel tc_bf16_kernel(int bn, bool ft, bool seed, bool a_kmajor, bool b_kmajor) {
-  if (bn == 256)
-    return ft ? bf16_kernel_of_layouts<256, true>(seed, a_kmajor, b_kmajor) : bf16_kernel_of_layouts<256, false>(seed, a_kmajor, b_kmajor);
-  if (bn == 128)
-    return ft ? bf16_kernel_of_layouts<128, true>(seed, a_kmajor, b_kmajor) : bf16_kernel_of_layouts<128, false>(seed, a_kmajor, b_kmajor);
-  return nullptr;
+TcKernel tc_bf16_kernel(int bn, bool ft, bool seed, bool a_kmajor, bool b_kmajor, bool cd_bf16) {
+  return cd_bf16 ? tc_bf16_cd_kernel(bn, ft, seed, a_kmajor, b_kmajor) : tc_bf16_select<0>(bn, ft, seed, a_kmajor, b_kmajor);
 }
 
 cudaError_t launch_encode_bf16(int bn, bool b_kmajor, const void *B, int N, int K, int ldb, long long stride_b, int batch,

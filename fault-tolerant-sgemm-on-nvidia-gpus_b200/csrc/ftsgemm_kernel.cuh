@@ -407,12 +407,24 @@ __device__ __forceinline__ BiasRef make_bias(const float *p, int mode, int m, bo
 // set (Z + m: the pre-activation value the GELU backward needs).
 // OUT (the ACT code with a separate output D): the value is stored to drow (D + m), its old value read from C + m, and
 // NONE is the identity -- a call with D and no activation runs these kernels too.
+// CT: the element type of C, D and Z -- float, or __nv_bfloat16 for the kCdBf16 kernels (ftsgemm_run_batched_mixed), which
+// read an old value as its exact FP32 upcast and round a stored FP32 value to nearest even (cvt.rn.bf16.f32) as the last
+// step, after every check.  Overloads, so that the float code is the code it was.
+__device__ __forceinline__ float cd_load(const float *p) { return *p; }
+__device__ __forceinline__ float cd_load(const __nv_bfloat16 *p) { return __bfloat162float(*p); }
+__device__ __forceinline__ void cd_store(float *p, float x) { *p = x; }
+__device__ __forceinline__ void cd_store(__nv_bfloat16 *p, float x) { *p = __float2bfloat16_rn(x); }
+// the caller's C / D / Z pointer as the kernel's output type (the identity for FP32)
+template <typename CT>
+__device__ __forceinline__ CT *cd_ptr(float *p) { return reinterpret_cast<CT *>(p); }
 constexpr int kActNone = 0, kActRelu = 1, kActGelu = 2;
-struct ActRef {
+template <typename CT = float>
+struct ActRefT {
   int kind;
-  float *zrow;  // Z + m, or null
-  float *drow;  // D + m (OUT only)
+  CT *zrow;  // Z + m, or null
+  CT *drow;  // D + m (OUT only)
 };
+using ActRef = ActRefT<float>;
 template <bool OUT = false>
 __device__ __forceinline__ float act_apply(int kind, float z) {
   if (OUT && kind == kActNone) return z;
@@ -420,22 +432,22 @@ __device__ __forceinline__ float act_apply(int kind, float z) {
   return z * 0.5f * (1.0f + erff(z * 0.707106781186547524f));  // (float)M_SQRT1_2
 }
 // z = x (+ b), stored to Z when requested; returns act(z)  (one element: the ragged-N and recompute paths)
-template <bool OUT = false>
-__device__ __forceinline__ float act_value(float x, const BiasRef &bias, int n, const ActRef &act, size_t off) {
+template <bool OUT = false, typename CT = float>
+__device__ __forceinline__ float act_value(float x, const BiasRef &bias, int n, const ActRefT<CT> &act, size_t off) {
   if (bias.mode != kBiasNone) x = __fadd_rn(x, bias.at(n));
-  if (act.zrow != nullptr) act.zrow[off] = x;
+  if (act.zrow != nullptr) cd_store(act.zrow + off, x);
   return act_apply<OUT>(act.kind, x);
 }
 // the same for the 32 columns [nb, nb + 32) of one chunk, the warp-uniform branches taken once per chunk, not per element
-template <bool OUT = false>
-__device__ __forceinline__ void act_chunk(uint32_t (&v)[32], const BiasRef &bias, int nb, const ActRef &act, int ldc) {
+template <bool OUT = false, typename CT = float>
+__device__ __forceinline__ void act_chunk(uint32_t (&v)[32], const BiasRef &bias, int nb, const ActRefT<CT> &act, int ldc) {
   if (bias.mode != kBiasNone) {
 #pragma unroll
     for (int i = 0; i < 32; ++i) v[i] = f2u(__fadd_rn(u2f(v[i]), bias.at(nb + i)));
   }
   if (act.zrow != nullptr) {
 #pragma unroll
-    for (int i = 0; i < 32; ++i) act.zrow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
+    for (int i = 0; i < 32; ++i) cd_store(act.zrow + static_cast<size_t>(nb + i) * ldc, u2f(v[i]));
   }
   if (act.kind == kActRelu) {
 #pragma unroll
@@ -445,29 +457,29 @@ __device__ __forceinline__ void act_chunk(uint32_t (&v)[32], const BiasRef &bias
     for (int i = 0; i < 32; ++i) v[i] = f2u(act_apply(kActGelu, u2f(v[i])));
   }
 }
-template <bool ACT>
-__device__ __forceinline__ ActRef act_of(const KernelParams &p, int m) {
-  if constexpr (ACT) return ActRef{p.act, p.z != nullptr ? p.z + m : nullptr, nullptr};
-  else return ActRef{kActNone, nullptr, nullptr};
+template <bool ACT, typename CT = float>
+__device__ __forceinline__ ActRefT<CT> act_of(const KernelParams &p, int m) {
+  if constexpr (ACT) return ActRefT<CT>{p.act, p.z != nullptr ? cd_ptr<CT>(p.z) + m : nullptr, nullptr};
+  else return ActRefT<CT>{kActNone, nullptr, nullptr};
 }
 // (strided batch: Z is the entry's, null when not written)
-template <bool ACT>
-__device__ __forceinline__ ActRef act_of_entry(const KernelParams &p, float *Z, int m) {
-  if constexpr (ACT) return ActRef{p.act, Z != nullptr ? Z + m : nullptr, nullptr};
-  else return ActRef{kActNone, nullptr, nullptr};
+template <bool ACT, typename CT = float>
+__device__ __forceinline__ ActRefT<CT> act_of_entry(const KernelParams &p, CT *Z, int m) {
+  if constexpr (ACT) return ActRefT<CT>{p.act, Z != nullptr ? Z + m : nullptr, nullptr};
+  else return ActRefT<CT>{kActNone, nullptr, nullptr};
 }
 // (OUT: the output row D + m as well)
-template <bool OUT>
-__device__ __forceinline__ ActRef with_out(ActRef a, float *D, int m) {
+template <bool OUT, typename CT = float>
+__device__ __forceinline__ ActRefT<CT> with_out(ActRefT<CT> a, CT *D, int m) {
   if constexpr (OUT) a.drow = D + m;
   return a;
 }
 
-template <int BN, bool BIAS = false, bool ACT = false, bool OUT = false>
-__device__ __forceinline__ void store_tile(uint32_t taddr, float *crow, bool row_ok, int n0, int n_limit, int ldc,
+template <int BN, bool BIAS = false, bool ACT = false, bool OUT = false, typename CT = float>
+__device__ __forceinline__ void store_tile(uint32_t taddr, CT *crow, bool row_ok, int n0, int n_limit, int ldc,
                                            float alpha, float beta, int c_begin = 0, int c_end = BN / 32, BiasRef bias = {},
-                                           ActRef act = {}) {
-  float *const drow = OUT ? act.drow : crow;  // (OUT: the old values come from C, the results go to D)
+                                           ActRefT<CT> act = {}) {
+  CT *const drow = OUT ? act.drow : crow;  // (OUT: the old values come from C, the results go to D)
   const bool full_n = (n0 + BN <= n_limit);
   if (full_n && beta != 0.0f) {
     // Software pipeline: the old values of chunk c + 1 are fetched while chunk c is stored (a chunk's 32 loads would
@@ -475,7 +487,7 @@ __device__ __forceinline__ void store_tile(uint32_t taddr, float *crow, bool row
     float old[32];
     if (row_ok) {
 #pragma unroll
-      for (int i = 0; i < 32; ++i) old[i] = crow[static_cast<size_t>(n0 + c_begin * 32 + i) * ldc];
+      for (int i = 0; i < 32; ++i) old[i] = cd_load(crow + static_cast<size_t>(n0 + c_begin * 32 + i) * ldc);
     }
 #pragma unroll 1
     for (int c = c_begin; c < c_end; ++c) {
@@ -492,10 +504,10 @@ __device__ __forceinline__ void store_tile(uint32_t taddr, float *crow, bool row
         if constexpr (ACT) act_chunk<OUT>(v, bias, nb, act, ldc);
         if (c + 1 < c_end) {
 #pragma unroll
-          for (int i = 0; i < 32; ++i) old[i] = crow[static_cast<size_t>(nb + 32 + i) * ldc];
+          for (int i = 0; i < 32; ++i) old[i] = cd_load(crow + static_cast<size_t>(nb + 32 + i) * ldc);
         }
 #pragma unroll
-        for (int i = 0; i < 32; ++i) drow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
+        for (int i = 0; i < 32; ++i) cd_store(drow + static_cast<size_t>(nb + i) * ldc, u2f(v[i]));
       }
     }
     return;
@@ -512,26 +524,26 @@ __device__ __forceinline__ void store_tile(uint32_t taddr, float *crow, bool row
         for (int i = 0; i < 32; ++i) v[i] = f2u(alpha * u2f(v[i]));
         act_chunk<OUT>(v, bias, nb, act, ldc);
 #pragma unroll
-        for (int i = 0; i < 32; ++i) drow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
+        for (int i = 0; i < 32; ++i) cd_store(drow + static_cast<size_t>(nb + i) * ldc, u2f(v[i]));
       } else {
 #pragma unroll
         for (int i = 0; i < 32; ++i) {
           float x = alpha * u2f(v[i]);
           if constexpr (BIAS) x = __fadd_rn(x, bias.at(nb + i));
-          crow[static_cast<size_t>(nb + i) * ldc] = x;
+          cd_store(crow + static_cast<size_t>(nb + i) * ldc, x);
         }
       }
     } else {
 #pragma unroll
       for (int i = 0; i < 32; ++i) {
         if (nb + i < n_limit) {
-          float *dst = crow + static_cast<size_t>(nb + i) * ldc;
-          const float o = (beta == 0.0f) ? 0.0f : beta * (*dst);
+          CT *dst = crow + static_cast<size_t>(nb + i) * ldc;
+          const float o = (beta == 0.0f) ? 0.0f : beta * cd_load(dst);
           float x = alpha * u2f(v[i]) + o;
           if constexpr (BIAS) x = __fadd_rn(x, bias.at(nb + i));
           if constexpr (ACT) x = act_value<OUT>(x, bias, nb + i, act, static_cast<size_t>(nb + i) * ldc);
           if constexpr (OUT) dst = drow + static_cast<size_t>(nb + i) * ldc;
-          *dst = x;
+          cd_store(dst, x);
         }
       }
     }
@@ -849,17 +861,19 @@ struct StoreVerdict {
 // ACT: the pass verifies z -- the values it sums are the pre-activation values, with the run-time bias in sum(b) as above
 // -- and then stores act(z) to C and z to Z.  The activation's own arithmetic is elementwise and nonlinear: no linear
 // checksum covers it, so an upset inside it or after it is not detected.
-template <int BN, bool BIAS, bool ACT = false, bool OUT = false>
-__device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, float *crow, bool row_ok, int n0, int ldc, float alpha,
+// (a BF16 output, CT = __nv_bfloat16: the old values are summed as their exact FP32 upcasts, and the verified z is rounded
+// to BF16 only as it is stored -- like the activation, an elementwise step after the check that no checksum covers)
+template <int BN, bool BIAS, bool ACT = false, bool OUT = false, typename CT = float>
+__device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, CT *crow, bool row_ok, int n0, int ldc, float alpha,
                                                           float beta, int c_begin, int c_end, float chk_s1, bool chk_s1_valid,
-                                                          int bad_col, uint32_t bad_mask, const BiasRef &bias, ActRef act = {}) {
+                                                          int bad_col, uint32_t bad_mask, const BiasRef &bias, ActRefT<CT> act = {}) {
   float s1 = 0.0f, s2 = 0.0f, sabs = 0.0f, so0 = 0.0f, so1 = 0.0f, sold0 = 0.0f, sold1 = 0.0f, aold0 = 0.0f, aold1 = 0.0f;
   float sb = 0.0f, ab = 0.0f;  // sum(b), sum|b| of the segment
   const bool rmw = beta != 0.0f;
   float old[32];
   if (row_ok && rmw) {
 #pragma unroll
-    for (int i = 0; i < 32; ++i) old[i] = crow[static_cast<size_t>(n0 + c_begin * 32 + i) * ldc];
+    for (int i = 0; i < 32; ++i) old[i] = cd_load(crow + static_cast<size_t>(n0 + c_begin * 32 + i) * ldc);
   }
 #pragma unroll 1
   for (int c = c_begin; c < c_end; ++c) {
@@ -881,7 +895,7 @@ __device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, flo
         for (int i = 0; i < 32; ++i) v[i] = f2u(alpha * u2f(v[i]) + beta * old[i]);
         if (c + 1 < c_end) {
 #pragma unroll
-          for (int i = 0; i < 32; ++i) old[i] = crow[static_cast<size_t>(nb + 32 + i) * ldc];
+          for (int i = 0; i < 32; ++i) old[i] = cd_load(crow + static_cast<size_t>(nb + 32 + i) * ldc);
         }
       } else {
 #pragma unroll
@@ -920,7 +934,7 @@ __device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, flo
       if constexpr (ACT) {
         if (act.zrow != nullptr) {
 #pragma unroll
-          for (int i = 0; i < 32; ++i) act.zrow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
+          for (int i = 0; i < 32; ++i) cd_store(act.zrow + static_cast<size_t>(nb + i) * ldc, u2f(v[i]));
         }
         if (act.kind == kActRelu) {
 #pragma unroll
@@ -930,9 +944,9 @@ __device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, flo
           for (int i = 0; i < 32; ++i) v[i] = f2u(act_apply(kActGelu, u2f(v[i])));
         }
       }
-      float *const drow = OUT ? act.drow : crow;
+      CT *const drow = OUT ? act.drow : crow;
 #pragma unroll
-      for (int i = 0; i < 32; ++i) drow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
+      for (int i = 0; i < 32; ++i) cd_store(drow + static_cast<size_t>(nb + i) * ldc, u2f(v[i]));
     }
   }
   float ref = alpha * s1 + beta * (sold0 + sold1);
@@ -961,10 +975,11 @@ __device__ __forceinline__ StoreVerdict store_tile_protected(uint32_t taddr, flo
 // An operand element as the tensor core reads it: FP32 truncated to TF32, BF16 exactly (ftsgemm_run_batched_typed).
 __device__ __forceinline__ float op_load(const float *p) { return u2f(f2u(__ldg(p)) & 0xFFFFE000u); }
 __device__ __forceinline__ float op_load(const __nv_bfloat16 *p) { return __bfloat162float(__ldg(p)); }
-template <int BN, bool BIAS, bool ACT = false, bool OUT = false, typename T = float>
-__device__ __forceinline__ void recompute_row_body(const T *A, const T *B, float *C, int lda, int ldb, int kmajor, int ldc,
+// (CT: the element type of C, Z and D)
+template <int BN, bool BIAS, bool ACT = false, bool OUT = false, typename T = float, typename CT = float>
+__device__ __forceinline__ void recompute_row_body(const T *A, const T *B, CT *C, int lda, int ldb, int kmajor, int ldc,
                                                    int N, int K, float alpha, float beta, int m, int n0, int lane, const float *bias,
-                                                   int bias_mode, int act_kind = kActNone, float *Z = nullptr, float *D = nullptr) {
+                                                   int bias_mode, int act_kind = kActNone, CT *Z = nullptr, CT *D = nullptr) {
   constexpr int J = BN / 32;
   float acc[J];
 #pragma unroll
@@ -988,17 +1003,17 @@ __device__ __forceinline__ void recompute_row_body(const T *A, const T *B, float
   for (int j = 0; j < J; ++j) {
     const int n = n0 + lane + 32 * j;
     if (n < N) {
-      float *dst = C + m + static_cast<size_t>(n) * ldc;
-      const float o = (beta == 0.0f) ? 0.0f : beta * (*dst);
+      CT *dst = C + m + static_cast<size_t>(n) * ldc;
+      const float o = (beta == 0.0f) ? 0.0f : beta * cd_load(dst);
       float x = alpha * acc[j] + o;
       if constexpr (BIAS) x = __fadd_rn(x, __ldg(bias + (bias_mode == kBiasRow ? m : n)));
       if constexpr (ACT) {
         if (bias_mode != kBiasNone) x = __fadd_rn(x, __ldg(bias + (bias_mode == kBiasRow ? m : n)));
-        if (Z != nullptr) Z[m + static_cast<size_t>(n) * ldc] = x;
+        if (Z != nullptr) cd_store(Z + m + static_cast<size_t>(n) * ldc, x);
         x = act_apply<OUT>(act_kind, x);
         if constexpr (OUT) dst = D + m + static_cast<size_t>(n) * ldc;
       }
-      *dst = x;
+      cd_store(dst, x);
     }
   }
 }
@@ -1032,9 +1047,17 @@ __device__ __noinline__ void recompute_row_out(const T *A, const T *B, float *C,
   recompute_row_body<BN, false, true, true, T>(A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, m, n0, lane, bias, bias_mode, act_kind,
                                             Z, D);
 }
-// (D: OUT only, the output the row is stored to)
-template <int BN, bool BIAS, bool ACT = false, bool ENTRY = false, bool OUT = false, typename... Args>
-__device__ __forceinline__ void recompute(const float *bias, int bias_mode, int act_kind, float *Z, float *D, Args... args) {
+// (the BF16-output kernels: C, Z and D are BF16; an overload, so that the FP32-output entry above keeps its name)
+template <int BN, bool ENTRY, typename T>
+__device__ __noinline__ void recompute_row_out(const T *A, const T *B, __nv_bfloat16 *C, int lda, int ldb, int kmajor, int ldc,
+                                               int N, int K, float alpha, float beta, int m, int n0, int lane, const float *bias,
+                                               int bias_mode, int act_kind, __nv_bfloat16 *Z, __nv_bfloat16 *D) {
+  recompute_row_body<BN, false, true, true, T>(A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, m, n0, lane, bias, bias_mode, act_kind,
+                                            Z, D);
+}
+// (D: OUT only, the output the row is stored to; CT: the element type of Z and D)
+template <int BN, bool BIAS, bool ACT = false, bool ENTRY = false, bool OUT = false, typename CT = float, typename... Args>
+__device__ __forceinline__ void recompute(const float *bias, int bias_mode, int act_kind, CT *Z, CT *D, Args... args) {
   if constexpr (OUT) recompute_row_out<BN, ENTRY>(args..., bias, bias_mode, act_kind, Z, D);
   else if constexpr (ACT) recompute_row_act<BN, ENTRY>(args..., bias, bias_mode, act_kind, Z);
   else if constexpr (BIAS) recompute_row_bias<BN>(args..., bias, bias_mode);
@@ -1046,17 +1069,17 @@ __device__ __forceinline__ void recompute(const float *bias, int bias_mode, int 
 // block would force a local copy of all of it.  Row segments that fail are counted and, with beta == 0, recomputed from A
 // and B (with beta != 0 the old values of C are already overwritten: reported as uncorrectable -- unless the results go
 // to a separate output D (OUT), which leaves C intact: then the segment is recomputed into D whatever beta is).
-template <int BN, bool BIAS, bool ACT = false, bool ENTRY = false, bool OUT = false, typename T = float>
-__device__ __forceinline__ void protected_store_body(uint32_t taddr, const T *A, const T *B, float *C, int lda, int ldb,
+template <int BN, bool BIAS, bool ACT = false, bool ENTRY = false, bool OUT = false, typename T = float, typename CT = float>
+__device__ __forceinline__ void protected_store_body(uint32_t taddr, const T *A, const T *B, CT *C, int lda, int ldb,
                                                      int kmajor, int ldc, int N, int K, float alpha, float beta, DeviceStats *stats,
                                                      bool can_recompute, int m, int row0, bool row_ok, int n0, int c_begin, int c_end,
                                                      float chk_s1, bool chk_s1_valid, int bad_col, uint32_t bad_mask, int lane,
                                                      const float *bias, int bias_mode, int row_ofs, int act_kind = kActNone,
-                                                     float *Z = nullptr, float *D = nullptr) {
+                                                     CT *Z = nullptr, CT *D = nullptr) {
   const StoreVerdict sv = store_tile_protected<BN, BIAS, ACT, OUT>(
       taddr, C + m, row_ok, n0, ldc, alpha, beta, c_begin, c_end, chk_s1, chk_s1_valid, bad_col, bad_mask,
       make_bias(bias, bias_mode, m, (BIAS || ACT) && row_ok),
-      ActRef{act_kind, (ACT && Z != nullptr) ? Z + m : nullptr, OUT ? D + m : nullptr});
+      ActRefT<CT>{act_kind, (ACT && Z != nullptr) ? Z + m : nullptr, OUT ? D + m : nullptr});
   unsigned mask = __ballot_sync(0xffffffffu, sv.bad);
   if (mask == 0u) return;
   const bool can_fix = (beta == 0.0f || (OUT && D != C)) && can_recompute;
@@ -1089,8 +1112,9 @@ __device__ __forceinline__ void protected_store_body(uint32_t taddr, const T *A,
   }
 }
 #define FT_PROT_PARAMS FT_PROT_PARAMS_T(float)
-#define FT_PROT_PARAMS_T(T)                                                                                                   \
-  uint32_t taddr, const T *A, const T *B, float *C, int lda, int ldb, int kmajor, int ldc, int N, int K, float alpha, \
+#define FT_PROT_PARAMS_T(T) FT_PROT_PARAMS_TC(T, float)
+#define FT_PROT_PARAMS_TC(T, CT)                                                                                           \
+  uint32_t taddr, const T *A, const T *B, CT *C, int lda, int ldb, int kmajor, int ldc, int N, int K, float alpha,    \
       float beta, DeviceStats *stats, bool can_recompute, int m, int row0, bool row_ok, int n0, int c_begin, int c_end,        \
       float chk_s1, bool chk_s1_valid, int bad_col, uint32_t bad_mask, int lane
 #define FT_PROT_ARGS                                                                                                            \
@@ -1129,11 +1153,18 @@ __device__ __noinline__ void protected_store_pass_out(FT_PROT_PARAMS_T(T), const
                                                       float *Z, float *D) {
   protected_store_body<BN, false, true, ENTRY, true, T>(FT_PROT_ARGS, bias, bias_mode, row_ofs, act_kind, Z, D);
 }
+// (the BF16-output kernels: C, Z and D are BF16; an overload, so that the FP32-output entry above keeps its name)
+template <int BN, bool ENTRY, typename T>
+__device__ __noinline__ void protected_store_pass_out(FT_PROT_PARAMS_TC(T, __nv_bfloat16), const float *bias, int bias_mode, int row_ofs,
+                                                      int act_kind, __nv_bfloat16 *Z, __nv_bfloat16 *D) {
+  protected_store_body<BN, false, true, ENTRY, true, T>(FT_PROT_ARGS, bias, bias_mode, row_ofs, act_kind, Z, D);
+}
 #undef FT_PROT_PARAMS
 #undef FT_PROT_PARAMS_T
+#undef FT_PROT_PARAMS_TC
 #undef FT_PROT_ARGS
-template <int BN, bool BIAS, bool BATCH, bool ACT, bool OUT, typename... Args>
-__device__ __forceinline__ void protected_store(const float *bias, int bias_mode, int row_ofs, int act_kind, float *Z, float *D,
+template <int BN, bool BIAS, bool BATCH, bool ACT, bool OUT, typename CT, typename... Args>
+__device__ __forceinline__ void protected_store(const float *bias, int bias_mode, int row_ofs, int act_kind, CT *Z, CT *D,
                                                 Args... args) {
   if constexpr (OUT) protected_store_pass_out<BN, BATCH>(args..., bias, bias_mode, row_ofs, act_kind, Z, D);
   else if constexpr (ACT && BATCH) protected_store_pass_act_batched<BN>(args..., bias, bias_mode, row_ofs, act_kind, Z);
@@ -1233,16 +1264,18 @@ __device__ __forceinline__ float chunk_sum(const uint32_t (&v)[32], float &sabs)
 }
 // The old values are read from C + m and the outputs stored to D + m (D = C but in the OUT kernels' entry).
 #define FT_PROT_V2_PARAMS FT_PROT_V2_PARAMS_T(float)
-#define FT_PROT_V2_PARAMS_T(T)                                                                                                  \
-  uint32_t taddr, const T *A, const T *B, float *C, int lda, int ldb, int kmajor, int ldc, int N, int K, float alpha,  \
+#define FT_PROT_V2_PARAMS_T(T) FT_PROT_V2_PARAMS_TC(T, float)
+#define FT_PROT_V2_PARAMS_TC(T, CT)                                                                                          \
+  uint32_t taddr, const T *A, const T *B, CT *C, int lda, int ldb, int kmajor, int ldc, int N, int K, float alpha,     \
       float beta, DeviceStats *stats, bool can_recompute, int m, int row0, bool row_ok, int n0, bool ragged_n, int c_begin,    \
       int c_end, float chk_s1, bool chk_s1_valid, StoreUpsets up, int lane, const float *bias, int bias_mode, int row_ofs,     \
-      int act_kind, float *Z
+      int act_kind, CT *Z
 #define FT_PROT_V2_ARGS                                                                                                          \
   taddr, A, B, C, lda, ldb, kmajor, ldc, N, K, alpha, beta, stats, can_recompute, m, row0, row_ok, n0, ragged_n, c_begin, c_end, \
       chk_s1, chk_s1_valid, up, lane, bias, bias_mode, row_ofs, act_kind, Z
-template <bool BIAS, bool ACT, bool ENTRY, bool OUT, typename T = float>
-__device__ __forceinline__ void protected_store_v2_body(FT_PROT_V2_PARAMS_T(T), float *D) {
+// (CT: the element type of C, Z and D; a BF16 output rounds the verified chunk as it stores it)
+template <bool BIAS, bool ACT, bool ENTRY, bool OUT, typename T = float, typename CT = float>
+__device__ __forceinline__ void protected_store_v2_body(FT_PROT_V2_PARAMS_TC(T, CT), CT *D) {
   // ---- pass 1: the chunk sums, and their running sum against the check's ----
   float sc[kMaxChunks];
   float s1 = 0.0f;
@@ -1263,16 +1296,16 @@ __device__ __forceinline__ void protected_store_v2_body(FT_PROT_V2_PARAMS_T(T), 
   // ---- pass 2: verify each chunk, then store it ----
   const bool has_bias = BIAS || (ACT && bias_mode != kBiasNone);
   const BiasRef b = make_bias(bias, bias_mode, m, has_bias && row_ok);
-  float *crow = C + m;
-  float *drow = D + m;
-  float *zrow = (ACT && Z != nullptr) ? Z + m : nullptr;
+  CT *crow = C + m;
+  CT *drow = D + m;
+  CT *zrow = (ACT && Z != nullptr) ? Z + m : nullptr;
   const bool rmw = beta != 0.0f;
   const int c_stop = min(c_end, (N - n0 + 31) / 32);  // chunks wholly past N are skipped
   uint32_t bad_chunks = reread_differs ? (1u << (c_end - c_begin)) - 1u : 0u;
   float old[32];
   auto load_old = [&](int nb) {
 #pragma unroll
-    for (int i = 0; i < 32; ++i) old[i] = (nb + i < N) ? crow[static_cast<size_t>(nb + i) * ldc] : 0.0f;
+    for (int i = 0; i < 32; ++i) old[i] = (nb + i < N) ? cd_load(crow + static_cast<size_t>(nb + i) * ldc) : 0.0f;
   };
   if (row_ok && rmw && c_begin < c_stop) load_old(n0 + c_begin * 32);
 #pragma unroll 1
@@ -1340,7 +1373,7 @@ __device__ __forceinline__ void protected_store_v2_body(FT_PROT_V2_PARAMS_T(T), 
       if (zrow != nullptr) {
 #pragma unroll
         for (int i = 0; i < 32; ++i)
-          if (full || nb + i < N) zrow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
+          if (full || nb + i < N) cd_store(zrow + static_cast<size_t>(nb + i) * ldc, u2f(v[i]));
       }
       if (act_kind == kActRelu) {
 #pragma unroll
@@ -1352,7 +1385,7 @@ __device__ __forceinline__ void protected_store_v2_body(FT_PROT_V2_PARAMS_T(T), 
     }
 #pragma unroll
     for (int i = 0; i < 32; ++i)
-      if (full || nb + i < N) drow[static_cast<size_t>(nb + i) * ldc] = u2f(v[i]);
+      if (full || nb + i < N) cd_store(drow + static_cast<size_t>(nb + i) * ldc, u2f(v[i]));
   }
   // chunks of a segment that failed pass 1 but lie wholly past N hold nothing to repair
   if (c_stop < c_end) bad_chunks &= (c_stop > c_begin) ? (1u << (c_stop - c_begin)) - 1u : 0u;
@@ -1396,11 +1429,17 @@ template <bool ENTRY, typename T = float>
 __device__ __noinline__ void protected_store_pass_v2_out(FT_PROT_V2_PARAMS_T(T), float *D) {
   protected_store_v2_body<false, true, ENTRY, true, T>(FT_PROT_V2_ARGS, D);
 }
+// (the BF16-output kernels: C, Z and D are BF16; an overload, so that the FP32-output entry above keeps its name)
+template <bool ENTRY, typename T>
+__device__ __noinline__ void protected_store_pass_v2_out(FT_PROT_V2_PARAMS_TC(T, __nv_bfloat16), __nv_bfloat16 *D) {
+  protected_store_v2_body<false, true, ENTRY, true, T>(FT_PROT_V2_ARGS, D);
+}
 #undef FT_PROT_V2_PARAMS
 #undef FT_PROT_V2_PARAMS_T
+#undef FT_PROT_V2_PARAMS_TC
 #undef FT_PROT_V2_ARGS
-template <bool BIAS, bool ACT, bool ENTRY, bool OUT, typename... Args>
-__device__ __forceinline__ void protected_store_v2(float *D, Args... args) {
+template <bool BIAS, bool ACT, bool ENTRY, bool OUT, typename CT, typename... Args>
+__device__ __forceinline__ void protected_store_v2(CT *D, Args... args) {
   if constexpr (OUT) protected_store_pass_v2_out<ENTRY>(args..., D);
   else protected_store_pass_v2<BIAS, ACT, ENTRY>(args...);
 }
@@ -1972,8 +2011,8 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[BN / 2], uint64_t a_desc, 
 }
 // The operand form of an instantiation (ftsgemm_tc_kernel's AB): 0 = FP32 operands; BF16 operands with the layout of A and
 // of B in shared memory as compile-time bits, so that the transpose immediates are constants (wgmmas chosen by a run-time
-// branch are serialised by ptxas)
-constexpr int kAbBf16 = 1, kAbAMn = 2, kAbBMn = 4;
+// branch are serialised by ptxas); kAbCdBf16 (with kAbBf16 only): C, D and Z are BF16 (ftsgemm_run_batched_mixed)
+constexpr int kAbBf16 = 1, kAbAMn = 2, kAbBMn = 4, kAbCdBf16 = 8;
 // Whether a PROT kernel runs the level-1 protected store pass: the BF16 kernels take the level at run time (0: the plain
 // store pass), the FP32 PROT kernels are only launched with a level.  (A helper: the same test written as
 // `!BF16 || p.protect != 0` in the kernel moved the spills of the FP32 PROT kernels.)
@@ -2012,16 +2051,21 @@ __device__ __forceinline__ const T *op_ptr(const float *p) { return reinterpret_
 // is BF16 with three terms per checksum (kChkPerTileBf16), in the layout of B.  The layouts of A and B are template bits
 // (kAbAMn, kAbBMn).  Only the OUT x BATCH form of the two-CTA tiles exists: bias mode, activation, Z and D (D == C in place)
 // are run-time fields, and with PROT the protection level is read at run time too (0: the plain store pass).
+// AB & kAbCdBf16: the same kernels with BF16 C, D and Z (ftsgemm_run_batched_mixed; compiled in ftsgemm_bf16_cd.cu).  Every
+// value is formed and checked in FP32 as above; the old value is read as its exact FP32 upcast, and the value stored to D
+// and Z is rounded to nearest even as the last step.  The checksum tile-columns and the parked accumulators stay FP32.
 template <int BN, bool FT, int CG, bool PROT = false, bool SEED = false, bool BIAS = false, bool BATCH = false, bool ACT = false,
           bool OUT = false, int AB = 0>
 __global__ void __launch_bounds__(kThreads, 1)
 ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmChk, const KernelParams p) {
-  constexpr bool BF16 = AB != 0, A_MN = (AB & kAbAMn) != 0, B_MN = (AB & kAbBMn) != 0;
+  constexpr bool BF16 = AB != 0, A_MN = (AB & kAbAMn) != 0, B_MN = (AB & kAbBMn) != 0, CD_BF16 = (AB & kAbCdBf16) != 0;
   static_assert(!(ACT && BIAS), "the ACT kernels take the bias mode at run time");
   static_assert(!OUT || ACT, "the OUT kernels are ACT kernels");
   static_assert(!BF16 || (OUT && BATCH && CG == 2 && BN >= 128), "BF16: the OUT x BATCH form of the two-CTA tiles");
-  using OpT = std::conditional_t<BF16, __nv_bfloat16, float>;  // operand element type
+  static_assert(!CD_BF16 || (AB & kAbBf16) != 0, "BF16 C / D / Z: BF16 operands only");
+  using OpT = std::conditional_t<BF16, __nv_bfloat16, float>;      // operand element type
+  using CdT = std::conditional_t<CD_BF16, __nv_bfloat16, float>;  // element type of C, D and Z
   using Cfg = TileCfg<BN, FT, CG>;
   constexpr int kStages = Cfg::kStages;
   constexpr int kAccRegs = BN / 2;  // per thread of a consumer warpgroup: 64 x BN FP32
@@ -2221,10 +2265,10 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       // register allocation of the biased fault-tolerant kernels)
       const OpT *const Ab = BATCH ? reinterpret_cast<const OpT *>(p.A) + bt * p.stride_a : nullptr;
       const OpT *const Bb = BATCH ? reinterpret_cast<const OpT *>(p.B) + bt * p.stride_b : nullptr;
-      float *const Cb = BATCH ? p.C + bt * p.stride_c : nullptr;
+      CdT *const Cb = BATCH ? cd_ptr<CdT>(p.C) + bt * p.stride_c : nullptr;
       const float *const biasb = BATCH ? p.bias + ((BIAS || ACT) ? bt * p.stride_bias : 0) : nullptr;  // (the entry's bias)
-      float *const Zb = (BATCH && ACT && p.z != nullptr) ? p.z + bt * p.stride_c : nullptr;          // (Z: C's geometry)
-      float *const Db = OUT ? p.d + (BATCH ? bt * p.stride_c : 0) : nullptr;  // (OUT: the entry's D, C's geometry)
+      CdT *const Zb = (BATCH && ACT && p.z != nullptr) ? cd_ptr<CdT>(p.z) + bt * p.stride_c : nullptr;  // (Z: C's geometry)
+      CdT *const Db = OUT ? cd_ptr<CdT>(p.d) + (BATCH ? bt * p.stride_c : 0) : nullptr;  // (OUT: the entry's D, C's geometry)
       const int row_ofs = bt * p.M;                           // stacked rows: fault list and events
       const int slab_ofs = bt * (p.tiles_m * CG * (kBM / 32));  // the entry's checksum flags
       const size_t chk_ofs = static_cast<size_t>(bt) * p.M * p.n_chk_cols * (p.chk_slices > 1 ? p.chk_slices : 1);
@@ -2325,22 +2369,22 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             if constexpr (PROT) stale = (ptx::ld_acquire_shared_u32(xchg_base(q) + 4) >> lane) & 1u;  // rows it repaired
           }
           if (PROT && FT && !(p.dbg_flags & 1) && p.protect == 2) {
-            protected_store_v2<BIAS, ACT, ACT && BATCH, OUT>(Db, taddr, BATCH ? Ab : op_ptr<OpT>(p.A), BATCH ? Bb : op_ptr<OpT>(p.B), BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1),
+            protected_store_v2<BIAS, ACT, ACT && BATCH, OUT>(Db, taddr, BATCH ? Ab : op_ptr<OpT>(p.A), BATCH ? Bb : op_ptr<OpT>(p.B), BATCH ? Cb : cd_ptr<CdT>(p.C), p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1),
                                                p.ldc, p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m,
                                                m0_cta + q * 32, m < p.M && !skip, n0, n0 + BN > p.N, kMid, BN / 32, s1, stale == 0u,
                                                stored_value_upsets<BN, BATCH>(p, q, lane, m0_cta, n0, kMid, BN / 32, row_ofs), lane,
                                                (BIAS || ACT) ? (BATCH ? biasb : p.bias) : nullptr, p.bias_mode, row_ofs, ACT ? p.act : 0,
-                                               ACT ? (BATCH ? Zb : p.z) : nullptr);
+                                               ACT ? (BATCH ? Zb : cd_ptr<CdT>(p.z)) : nullptr);
           } else if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N && level1_on<BF16>(p)) {
             uint32_t bad_bits = 0u;
             const int bad_col = stored_value_fault<BN, BATCH>(p, q, lane, m0_cta, n0, kMid, BN / 32, bad_bits, row_ofs);
-            protected_store<BN, BIAS, BATCH, ACT, OUT>(BATCH ? biasb : p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? (BATCH ? Zb : p.z) : nullptr, Db, taddr, BATCH ? Ab : op_ptr<OpT>(p.A), BATCH ? Bb : op_ptr<OpT>(p.B), BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
+            protected_store<BN, BIAS, BATCH, ACT, OUT>(BATCH ? biasb : p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? (BATCH ? Zb : cd_ptr<CdT>(p.z)) : nullptr, Db, taddr, BATCH ? Ab : op_ptr<OpT>(p.A), BATCH ? Bb : op_ptr<OpT>(p.B), BATCH ? Cb : cd_ptr<CdT>(p.C), p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
                                       p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32,
                                       m < p.M && !skip, n0, kMid, BN / 32, s1, stale == 0u, bad_col, bad_bits, lane);
           } else {
-            store_tile<BN, BIAS, ACT, OUT>(taddr, (BATCH ? Cb : p.C) + m, m < p.M && !skip, n0, p.N, p.ldc, p.alpha, p.beta, kMid, BN / 32,
+            store_tile<BN, BIAS, ACT, OUT>(taddr, (BATCH ? Cb : cd_ptr<CdT>(p.C)) + m, m < p.M && !skip, n0, p.N, p.ldc, p.alpha, p.beta, kMid, BN / 32,
                                       make_bias(BATCH ? biasb : p.bias, p.bias_mode, m, (BIAS || ACT) && m < p.M && !skip),
-                                      with_out<OUT>(BATCH ? act_of_entry<ACT>(p, Zb, m) : act_of<ACT>(p, m), Db, m));
+                                      with_out<OUT>(BATCH ? act_of_entry<ACT>(p, Zb, m) : act_of<ACT, CdT>(p, m), Db, m));
           }
           ptx::named_bar_sync(4 + q, 64);  // both halves are out of the accumulator
         }
@@ -2396,30 +2440,30 @@ ftsgemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
         if (assist_on && FT && !(p.dbg_flags & 1)) ptx::named_bar_sync(4 + q, 64);  // corrections are in place
         if (PROT && FT && !(p.dbg_flags & 1) && p.protect == 2) {
-          protected_store_v2<BIAS, ACT, ACT && BATCH, OUT>(Db, taddr, BATCH ? Ab : op_ptr<OpT>(p.A), BATCH ? Bb : op_ptr<OpT>(p.B), BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1),
+          protected_store_v2<BIAS, ACT, ACT && BATCH, OUT>(Db, taddr, BATCH ? Ab : op_ptr<OpT>(p.A), BATCH ? Bb : op_ptr<OpT>(p.B), BATCH ? Cb : cd_ptr<CdT>(p.C), p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1),
                                              p.ldc, p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m,
                                              m0_cta + q * 32, m < p.M && !redo, n0, n0 + BN > p.N, 0, c_mid, own_s1,
                                              ((stale_mask >> lane) & 1u) == 0u,
                                              stored_value_upsets<BN, BATCH>(p, q, lane, m0_cta, n0, 0, c_mid, row_ofs), lane,
                                              (BIAS || ACT) ? (BATCH ? biasb : p.bias) : nullptr, p.bias_mode, row_ofs, ACT ? p.act : 0,
-                                             ACT ? (BATCH ? Zb : p.z) : nullptr);
+                                             ACT ? (BATCH ? Zb : cd_ptr<CdT>(p.z)) : nullptr);
         } else if (PROT && FT && !(p.dbg_flags & 1) && n0 + BN <= p.N && level1_on<BF16>(p)) {
           uint32_t bad_bits = 0u;
           const int bad_col = stored_value_fault<BN, BATCH>(p, q, lane, m0_cta, n0, 0, c_mid, bad_bits, row_ofs);
-          protected_store<BN, BIAS, BATCH, ACT, OUT>(BATCH ? biasb : p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? (BATCH ? Zb : p.z) : nullptr, Db, taddr, BATCH ? Ab : op_ptr<OpT>(p.A), BATCH ? Bb : op_ptr<OpT>(p.B), BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
+          protected_store<BN, BIAS, BATCH, ACT, OUT>(BATCH ? biasb : p.bias, p.bias_mode, row_ofs, ACT ? p.act : 0, ACT ? (BATCH ? Zb : cd_ptr<CdT>(p.z)) : nullptr, Db, taddr, BATCH ? Ab : op_ptr<OpT>(p.A), BATCH ? Bb : op_ptr<OpT>(p.B), BATCH ? Cb : cd_ptr<CdT>(p.C), p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc,
                                     p.N, p.K, p.alpha, p.beta, p.stats, p.recompute != 0 && p.detect_only == 0, m, m0_cta + q * 32,
                                     m < p.M && !redo, n0, 0, c_mid, own_s1, ((stale_mask >> lane) & 1u) == 0u, bad_col, bad_bits, lane);
         } else {
-          store_tile<BN, BIAS, ACT, OUT>(taddr, (BATCH ? Cb : p.C) + m, m < p.M && !redo, n0, p.N, p.ldc, p.alpha, p.beta, 0, c_mid,
+          store_tile<BN, BIAS, ACT, OUT>(taddr, (BATCH ? Cb : cd_ptr<CdT>(p.C)) + m, m < p.M && !redo, n0, p.N, p.ldc, p.alpha, p.beta, 0, c_mid,
                                     make_bias(BATCH ? biasb : p.bias, p.bias_mode, m, (BIAS || ACT) && m < p.M && !redo),
-                                    with_out<OUT>(BATCH ? act_of_entry<ACT>(p, Zb, m) : act_of<ACT>(p, m), Db, m));
+                                    with_out<OUT>(BATCH ? act_of_entry<ACT>(p, Zb, m) : act_of<ACT, CdT>(p, m), Db, m));
         }
         if (FT && redo_mask != 0u) {  // rare, warp-uniform: recompute the flagged rows from global memory
           unsigned rm = redo_mask;
           while (rm != 0u) {
             const int r = __ffs(rm) - 1;
             rm &= rm - 1u;
-            recompute<BN, BIAS, ACT, ACT && BATCH, OUT>(BATCH ? biasb : p.bias, p.bias_mode, ACT ? p.act : 0, ACT ? (BATCH ? Zb : p.z) : nullptr, Db, BATCH ? Ab : op_ptr<OpT>(p.A), BATCH ? Bb : op_ptr<OpT>(p.B), BATCH ? Cb : p.C, p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K,
+            recompute<BN, BIAS, ACT, ACT && BATCH, OUT>(BATCH ? biasb : p.bias, p.bias_mode, ACT ? p.act : 0, ACT ? (BATCH ? Zb : cd_ptr<CdT>(p.z)) : nullptr, Db, BATCH ? Ab : op_ptr<OpT>(p.A), BATCH ? Bb : op_ptr<OpT>(p.B), BATCH ? Cb : cd_ptr<CdT>(p.C), p.lda, p.ldb, p.a_kmajor | (p.b_kmajor << 1), p.ldc, p.N, p.K,
                                 p.alpha, p.beta, m0_cta + q * 32 + r, n0, lane);
           }
         }
@@ -2517,9 +2561,35 @@ cudaError_t tc_out_abort_flag(int *flag);
 // The BF16 kernels (ftsgemm_bf16.cu): the two-CTA tile of width bn (128 or 256) for A and B in the given layouts, fault-
 // tolerant or not, or null; the encode pre-pass of a BF16 B (both layouts, `batch` entries stride_b elements apart) into its
 // BF16 checksum operand, in B's layout (K-major: [checksum column][chk_ld]; MN-major: [k][chk_ld]); the unit's abort flag.
-TcKernel tc_bf16_kernel(int bn, bool ft, bool seed, bool a_kmajor, bool b_kmajor);
+// cd_bf16: the kernel with BF16 C, D and Z (kAbCdBf16), which tc_bf16_kernel takes from ftsgemm_bf16_cd.cu: tc_bf16_cd_kernel
+// and that unit's own abort flag.
+TcKernel tc_bf16_kernel(int bn, bool ft, bool seed, bool a_kmajor, bool b_kmajor, bool cd_bf16);
 cudaError_t launch_encode_bf16(int bn, bool b_kmajor, const void *B, int N, int K, int ldb, long long stride_b, int batch,
                                void *chk, int chk_ld, long long chk_stride, int tiles_n, int blocks, cudaStream_t stream);
 cudaError_t tc_bf16_abort_flag(int *flag);
+TcKernel tc_bf16_cd_kernel(int bn, bool ft, bool seed, bool a_kmajor, bool b_kmajor);
+cudaError_t tc_bf16_cd_abort_flag(int *flag);
+
+// The BF16-operand instantiations of one output type (CD: 0 for FP32, kAbCdBf16 for BF16 C / D / Z): the OUT x BATCH form of
+// the two-CTA tile of width bn (256 or 128), plain or fault-tolerant (with PROT), with or without SEED, for the layouts of A
+// and B; null for another width.  Called only by the translation unit that compiles that output type's kernels.
+template <int CD>
+TcKernel tc_bf16_select(int bn, bool ft, bool seed, bool a_kmajor, bool b_kmajor) {
+  auto of_tile = [&](auto bn_c, auto ft_c) -> TcKernel {
+    constexpr int BN = decltype(bn_c)::value;
+    constexpr bool FT = decltype(ft_c)::value;
+    auto pick = [&](auto ab_c) -> TcKernel {
+      constexpr int AB = decltype(ab_c)::value;
+      return seed ? ftsgemm_tc_kernel<BN, FT, 2, FT, true, false, true, true, true, AB>
+                  : ftsgemm_tc_kernel<BN, FT, 2, FT, false, false, true, true, true, AB>;
+    };
+    constexpr int a = kAbBf16 | CD | kAbAMn, b = kAbBf16 | CD | kAbBMn, ab = kAbBf16 | CD | kAbAMn | kAbBMn;
+    if (a_kmajor) return b_kmajor ? pick(std::integral_constant<int, kAbBf16 | CD>()) : pick(std::integral_constant<int, b>());
+    return b_kmajor ? pick(std::integral_constant<int, a>()) : pick(std::integral_constant<int, ab>());
+  };
+  if (bn == 256) return ft ? of_tile(std::integral_constant<int, 256>(), std::true_type()) : of_tile(std::integral_constant<int, 256>(), std::false_type());
+  if (bn == 128) return ft ? of_tile(std::integral_constant<int, 128>(), std::true_type()) : of_tile(std::integral_constant<int, 128>(), std::false_type());
+  return nullptr;
+}
 
 }  // namespace ftsgemm

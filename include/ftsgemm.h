@@ -400,11 +400,35 @@ int ftsgemm_run_out(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, cons
  *    the other element type) and for the plain ids.
  *  - Every other option applies as for FP32; opts.precision = 1 (3xTF32) is FTSGEMM_ERR_INVALID_ARG: the products of BF16
  *    values are exact in FP32.
- * ab_type outside 0..1: FTSGEMM_ERR_INVALID_ARG.  Capturable into a CUDA graph like the other compute calls. */
+ * ab_type outside 0..1: FTSGEMM_ERR_INVALID_ARG.  Capturable into a CUDA graph like the other compute calls.
+ * (The wrapper of ftsgemm_run_batched_mixed with cd_type = FTSGEMM_TYPE_F32.) */
 int ftsgemm_run_batched_typed(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const void *A, int layout_a, int lda,
                               long long stride_a, const void *B, int layout_b, int ldb, long long stride_b, int ab_type,
                               const float *C, int ldc, long long stride_c, float *D, int batch, float alpha, float beta,
                               const float *bias, int bias_mode, long long stride_bias, int activation, float *dZ,
+                              const ftsgemm_opts *opts);
+/* ftsgemm_run_batched_typed with C, D and Z of element type cd_type (all three the same).  FTSGEMM_TYPE_F32 is
+ * ftsgemm_run_batched_typed, bit for bit (which is this call's wrapper).
+ * BF16 (FTSGEMM_TYPE_BF16) is defined as: upcast C to FP32 (exact); run the FTSGEMM_TYPE_F32 call with every other argument
+ * unchanged; round D and Z to BF16, to nearest even (cvt.rn.bf16.f32, as torch's .to(torch.bfloat16) on CUDA).  D and Z equal
+ * that bit for bit, except that a NaN is stored as some NaN; FP32 values past the BF16 range round to +-Inf.
+ *  - Accumulation, the checksums, alpha, beta, the bias (still const float *), the activation and every check stay FP32.
+ *    protect_epilogue 1 and 2 verify the FP32 values z, summing the old values as their exact FP32 upcasts.  The rounding is
+ *    the last step: like the activation it is elementwise, after the verified value, and NO checksum covers it.  Every
+ *    repair (the row recompute, level 1's segment recompute, level 2's chunk recompute) stores the same BF16 bits as a
+ *    fault-free call.  D == C is the in-place call (C read as BF16 and overwritten); with beta == 0 C is not read.
+ *  - BF16 operands only: ab_type = FTSGEMM_TYPE_F32 with BF16 output is FTSGEMM_ERR_UNSUPPORTED.  Kernel ids as for BF16
+ *    operands; cuBLAS (0 / 7) runs in place with CUDA_R_16BF C (a bias, an activation or D != C stay unsupported there).
+ *  - ldc % 8 == 0 and, for batch > 1, stride_c % 8 == 0 (elements); C (when read), D and Z 16-byte aligned; or
+ *    FTSGEMM_ERR_INVALID_ARG.  C, D and Z must not overlap, counted in bytes (2 per element).
+ *  - opts.check_segments > 1: FTSGEMM_ERR_UNSUPPORTED (segments 2..S accumulate into D, which would be rounded once per
+ *    segment).  opts.precision = 1: FTSGEMM_ERR_INVALID_ARG, as for BF16 operands.
+ *  - Launch counts are those of the FP32-output BF16 call: 1 from 8 MB of B, 2 below.
+ * cd_type outside 0..1: FTSGEMM_ERR_INVALID_ARG.  Capturable into a CUDA graph like the other compute calls. */
+int ftsgemm_run_batched_mixed(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const void *A, int layout_a, int lda,
+                              long long stride_a, const void *B, int layout_b, int ldb, long long stride_b, int ab_type,
+                              const void *C, int ldc, long long stride_c, void *D, int cd_type, int batch, float alpha,
+                              float beta, const float *bias, int bias_mode, long long stride_bias, int activation, void *dZ,
                               const ftsgemm_opts *opts);
 /* ftsgemm_run_batched_typed with batch = 1 (the strides are ignored). */
 int ftsgemm_run_typed(ftsgemm_handle_t h, int kernel_id, int M, int N, int K, const void *A, int layout_a, int lda,
