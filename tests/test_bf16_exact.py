@@ -11,11 +11,15 @@ CTAs), more than one checksum tile-column (six checksum columns per N-tile strad
 production sizes, the planner knobs, batches past the encode's 65535 grid rows, the row and chunk recomputes in every
 layout pair, and the BF16 value range (full 8-bit mantissas, wide exponent spreads, subnormals, column-block sums that
 round to Inf in BF16).
+
+With BF16 C, D and Z (ftsgemm_run_batched_mixed) the same checks hold against the float64 result rounded once to nearest
+even (round_bf16, mismatch16); the tests that can take the output type do, and each of their BF16-output cases asserts that
+its data needs that rounding (Rounding).  What only a BF16 output has is in tests/test_bf16_out_exact.py.
 """
 import numpy as np
 import pytest
 
-from test_bf16 import exact, exact_budget_ok, ld_bf16, pack16, run16, zero_residual
+from test_bf16 import exact_budget_ok, ld_bf16, pack16, pad8, run16, zero_residual
 from test_exact import DYADIC, LIMIT, TOL_MODEL, _free, _upset, budget, knobs, mismatch, odd_ints, tiles
 
 MN, KM = 0, 1
@@ -23,8 +27,11 @@ NONE, ROW, COL = 0, 1, 2
 RELU = 1
 PAIRS = {"256": (21, 31), "128": (3, 13), "128s": (22, 32), "auto": (20, 40)}   # plain and ABFT id of each BF16 tile
 CUBLAS_BF16 = 7
+F32, BF16 = 0, 1          # FTSGEMM_TYPE_*: the element type of C, D and Z
 SENTINEL = -12345.5
 Z_SENTINEL = 7777.25
+SENTINEL16 = -12352.0     # the sentinels of a BF16 output: BF16 values (8 significant bits)
+Z_SENTINEL16 = 7776.0
 BF16_MAX = 2.0 ** 128 - 2.0 ** 120
 CHK_PER_TILE = 6          # checksum columns per N-tile: e hi, mid, lo, w hi, mid, lo (DESIGN.md §3.1)
 
@@ -79,6 +86,139 @@ def chk_geometry(BN, N):
     return tiles_n, tiles_c, straddle
 
 
+# ------------------------------------------------------------------ BF16 output: the reference rounded once (no GPU)
+def _u32(x):
+    """the FP32 bit patterns of float32 x as int64 in [0, 2^32)"""
+    t = _t()
+    return x.contiguous().view(t.int32).to(t.int64) & 0xFFFFFFFF
+
+
+def round_bf16(want, double_round=False):
+    """The BF16 bits (int64 in [0, 0xFFFF]) of float64 values rounded to nearest even from their FP32 bits u:
+    (u + 0x7FFF + ((u >> 16) & 1)) >> 16, NaN as 0x7FC0 -- integer arithmetic, independent of torch's own cast, on want's
+    device.  Every finite value must be an FP32 value: on exact data the kernels round once, at the store.  double_round
+    declares a case whose results are not FP32 values (FP32 subnormals that lose bits): there the defined value is float64 ->
+    FP32 (nearest even) -> BF16, the order the kernel rounds in."""
+    t = _t()
+    f = want.float()
+    if not double_round:
+        inexact = t.isfinite(want) & (f.double() != want)
+        assert not bool(inexact.any()), f"{int(inexact.sum())} finite values are not FP32 values"
+    u = _u32(f)
+    r = (u + 0x7FFF + ((u >> 16) & 1)) >> 16
+    return t.where(t.isnan(f), t.full_like(r, 0x7FC0), r)
+
+
+def bits16(x):
+    """the bits of a bfloat16 tensor as int64 in [0, 0xFFFF]"""
+    t = _t()
+    return x.contiguous().view(t.int16).to(t.int64) & 0xFFFF
+
+
+def mismatch16(got, want_bits, show=4):
+    """'' when the bfloat16 tensor got has the bits want_bits (round_bf16) at every element, with +0 == -0 and NaN == NaN
+    (any payload); otherwise the count and the first few (index, got, want)"""
+    if tuple(got.shape) != tuple(want_bits.shape):
+        return f"shape {tuple(got.shape)} != {tuple(want_bits.shape)}"
+    g, w = bits16(got), want_bits
+    ng, nw = (g & 0x7FFF) > 0x7F80, (w & 0x7FFF) > 0x7F80
+    zero = ((g | w) & 0x7FFF) == 0
+    bad = (ng != nw) | (~ng & ~zero & (g != w))
+    n = int(bad.sum())
+    if n == 0:
+        return ""
+    val = lambda b: float(np.array([b << 16], np.uint32).view(np.float32)[0])
+    out = []
+    for i in bad.nonzero()[:show].tolist():
+        gb, wb = int(g[tuple(i)]), int(w[tuple(i)])
+        out.append(f"{tuple(i)}: got {val(gb)!r} (0x{gb:04x}) want {val(wb)!r} (0x{wb:04x})")
+    return f"{n} elements differ, e.g. " + ", ".join(out)
+
+
+class Rounding:
+    """What the float64 references of one BF16-output test case asked of the rounding: elements that need more than 8
+    significant bits, and exact ties rounded down (the even neighbour has the smaller magnitude) and up.  Data that needs no
+    rounding proves nothing about it, so check() requires all three."""
+
+    def __init__(self):
+        self.wide = self.down = self.up = 0
+
+    def add(self, want):
+        t = _t()
+        u = _u32(want[t.isfinite(want)].float())
+        low, odd = u & 0xFFFF, ((u >> 16) & 1) == 1
+        tie = low == 0x8000
+        self.wide += int((low != 0).sum())
+        self.down += int((tie & ~odd).sum())
+        self.up += int((tie & odd).sum())
+
+    def check(self, tag):
+        assert self.wide > 0 and self.down > 0 and self.up > 0, (tag, "the data needs no rounding", vars(self))
+
+
+def exact(got, want, tag, seen=None, double_round=False):
+    """got equals the float64 want at every element: float32 bit for bit (NaN == NaN, +0 == -0), bfloat16 as want rounded
+    once (round_bf16); seen (a Rounding) tallies what the rounding had to do"""
+    if got.dtype == _t().bfloat16:
+        msg = mismatch16(got, round_bf16(want, double_round))
+        if seen is not None:
+            seen.add(want)
+    else:
+        msg = mismatch(got, want)
+    assert not msg, f"{tag}: {msg}"
+
+
+TIE_A = 17.0
+
+
+def tie_factors(alpha, most=63):
+    """(v_down, v_up): the smallest integers v <= most for which alpha * 17 * v is an exact BF16 tie that rounds down, and
+    one that rounds up"""
+    t = _t()
+    v = t.arange(1, most + 1, dtype=t.float64)
+    u = _u32((alpha * TIE_A * v).float())
+    tie, odd = (u & 0xFFFF) == 0x8000, ((u >> 16) & 1) == 1
+    return float(v[tie & ~odd][0]), float(v[tie & odd][0])
+
+
+def plant_ties(A, B, alpha, C0=None, bias=None, mode=NONE):
+    """For the BF16-output cases whose small data would need no rounding: row 0 of A (of every entry) becomes 17 e_0 and four
+    rows n of B become +-v e_0, so D(0, n) = alpha * 17 * (+-v) are exact ties of both signs, one pair rounded down and one
+    up (tie_factors); C0 and the bias are zeroed where they are added to those four elements.  In place; returns the four
+    columns.  The exactness budget holds: these rows only shrink, and a column-block sum grows by at most 4 * 63
+    (plant_budget_ok)."""
+    N = B.shape[-2]
+    cols = sorted({0, N // 3, (2 * N) // 3, N - 1})
+    assert len(cols) == 4, N
+    vd, vu = tie_factors(alpha)
+    A[..., 0, :] = 0.0
+    A[..., 0, 0] = TIE_A
+    for n, v in zip(cols, (vd, -vd, vu, -vu)):
+        B[..., n, :] = 0.0
+        B[..., n, 0] = v
+    if C0 is not None:
+        C0[..., 0, cols] = 0.0
+    if bias is not None and mode == ROW:
+        bias[..., 0] = 0.0
+    elif bias is not None and mode == COL:
+        bias[..., cols] = 0.0
+    return cols
+
+
+def plant_budget_ok(K, amax, BN=256):
+    """bf16_budget_ok's checksum and weighted column-block sums with plant_ties' four rows of B (|v| <= 63) in one N-tile:
+    only the k = 0 sums grow"""
+    return K * amax * BN * amax + amax * 4 * 63 <= LIMIT and BN * (BN + 1) // 2 * amax + 4 * BN * 63 <= LIMIT
+
+
+def with_cd(values, ids=None):
+    """pytest params (value, F32) with the ids the F32 cases always had, then (value, BF16) with '-bf16' appended"""
+    tup = lambda v: v if isinstance(v, tuple) else (v,)
+    ids = ids or ["-".join(map(str, tup(v))) for v in values]
+    return ([pytest.param(*tup(v), F32, id=i) for v, i in zip(values, ids)] +
+            [pytest.param(*tup(v), BF16, id=f"{i}-bf16") for v, i in zip(values, ids)])
+
+
 MULTI = ((128, 2816, 21), (128, 2944, 21), (256, 11008, 42))   # (BN, N, the straddling N-tile)
 
 SWEEP_K = (1, 7, 8, 15, 16, 17, 63, 64, 65, 127, 129, 1000, 2088)
@@ -109,8 +249,9 @@ def sweep16(BN, seed):
 FUZZ_ENTRIES = ("plain", "bias_row", "bias_col", "relu_z", "out_of_place", "batched")
 
 
-def fuzz16(seed):
-    """the parameters of one seeded BF16 fuzz case (no GPU): shape, tile, layouts, padding, alpha / beta, entry point, knobs"""
+def fuzz16(seed, cd=F32):
+    """the parameters of one seeded BF16 fuzz case (no GPU): shape, tile, layouts, padding, alpha / beta, entry point, knobs.
+    With a BF16 output an alpha of 0 becomes 1 (the result must have ties to round: plant_ties)."""
     rng = np.random.default_rng(17000 + seed)
     p = {"seed": seed, "M": int(rng.integers(1, 200)) * 4, "N": int(rng.integers(1, 200)) * 4,
          "K": int(rng.choice([int(rng.integers(1, 130)), int(rng.integers(1, 1500))])),
@@ -120,6 +261,8 @@ def fuzz16(seed):
          "knobs": {"splitk": int(rng.choice([-1, 0, 2, 3])), "wave_sync": int(rng.choice([0, 1])), "pdl": int(rng.choice([0, 1])),
                    "epi_assist": int(rng.choice([0, 1])), "chk_slices": int(rng.choice([1, 2, 3])),
                    "enc_front": int(rng.choice([0, 1]))}}
+    if cd == BF16 and p["alpha"] == 0.0:
+        p["alpha"] = 1.0
     p["cmax"] = 0 if p["beta"] == 0.0 else 64
     p["bias_max"] = 64 if p["entry"] in ("bias_row", "bias_col", "batched") else 0
     p["amax"] = pick_amax16(p["K"], p["alpha"], p["beta"], p["cmax"], p["bias_max"])
@@ -139,6 +282,13 @@ def test_budgets_of_every_parameter_set():
         for alpha, beta in SWEEP_AB:
             assert bf16_budget_ok(K, pick_amax16(K, alpha, beta, 64), pick_amax16(K, alpha, beta, 64), alpha, beta, 64)
     assert pick_amax16(2088) == 4 and pick_amax16(256) == 8
+    # the ties planted in the BF16-output sets keep them exact
+    for K in SWEEP_K:
+        for alpha, beta in SWEEP_AB:
+            assert plant_budget_ok(K, pick_amax16(K, alpha, beta, 64))
+            if alpha != 0.0:
+                assert max(tie_factors(alpha)) <= 63
+    assert plant_budget_ok(200, 2) and plant_budget_ok(129, 4) and tie_factors(-1.0) == tie_factors(1.0) == (17.0, 19.0)
     assert bf16_budget_ok(200, 4, 4) and bf16_budget_ok(201, 2, 2, -0.5, 1.0, 64) and bf16_budget_ok(201, 2, 2, 1.0, -2.0, 64)
     assert bf16_budget_ok(6, 8, 8, bias_max=64) and bf16_budget_ok(201, 4, 4, -1.0, 0.5, 64, 64)
     assert bf16_budget_ok(301, 8, 8, -0.5) and bf16_budget_ok(256, 4, 4) and bf16_budget_ok(256, 8, 8)
@@ -200,9 +350,14 @@ def test_sweep_covers_every_value():
 
 def test_fuzz_cases_are_within_budget():
     for seed in range(40):
-        p = fuzz16(seed)
-        assert bf16_budget_ok(p["K"], p["amax"], p["amax"], p["alpha"], p["beta"], p["cmax"], p["bias_max"]), p
-        assert p["M"] % 4 == 0 and p["N"] % 4 == 0 and p["K"] >= 1
+        for cd in (F32, BF16):
+            p = fuzz16(seed, cd)
+            assert bf16_budget_ok(p["K"], p["amax"], p["amax"], p["alpha"], p["beta"], p["cmax"], p["bias_max"]), p
+            assert p["M"] % 4 == 0 and p["N"] % 4 == 0 and p["K"] >= 1
+            if cd == BF16:
+                assert plant_budget_ok(p["K"], p["amax"]) and p["alpha"] != 0.0, p
+                vd, vu = tie_factors(p["alpha"])
+                assert max(vd, vu) <= 63
     cases = [fuzz16(s) for s in range(40)]
     assert {c["entry"] for c in cases} == set(FUZZ_ENTRIES) and {c["pair"] for c in cases} == set(PAIRS)
     for knob in ("splitk", "wave_sync", "pdl", "epi_assist", "chk_slices", "enc_front"):
@@ -235,26 +390,41 @@ def reference(A, B, alpha=1.0, beta=0.0, C0=None, bias=None, mode=NONE):
     return out
 
 
+def out_buffers(t, cd):
+    """(dtype, D sentinel, Z sentinel) of an output of type cd"""
+    return (t.bfloat16, SENTINEL16, Z_SENTINEL16) if cd == BF16 else (t.float32, SENTINEL, Z_SENTINEL)
+
+
 def run1(t, ft, dev, kid, A, B, la=KM, lb=KM, pad=False, ldc=None, alpha=1.0, beta=0.0, C0=None, bias=None, mode=NONE,
-         act=0, z=False, out_of_place=False, opts=None):
-    """run16 with Z's padding checked too: one run_typed call; returns (D, Z) as M x N views"""
+         act=0, z=False, out_of_place=False, opts=None, cd=F32):
+    """run16 with Z's padding checked too: one run_typed call (cd = BF16: one run_batched_mixed call with BF16 C, D and Z,
+    ldc rounded up to a multiple of 8; C0 must hold BF16 values); returns (D, Z) as M x N views"""
     M, K = A.shape
     N = B.shape[0]
     lda, ldb, ldc = ld_bf16(la, M, K, pad), ld_bf16(lb, N, K, pad), ldc or M
-    cbuf = t.full((N, ldc), SENTINEL, device="cuda")
+    typ, sent, zsent = out_buffers(t, cd)
+    if cd == BF16:
+        ldc = pad8(ldc)
+        assert C0 is None or t.equal(C0.to(t.bfloat16).float(), C0.float())
+    cbuf = t.full((N, ldc), sent, device="cuda", dtype=typ)
     cbuf[:, :M] = 0.0 if C0 is None else C0.T
     c_before = cbuf.clone()
-    dbuf = t.full((N, ldc), SENTINEL, device="cuda") if out_of_place else cbuf
-    zbuf = t.full((N, ldc), Z_SENTINEL, device="cuda") if z else None
-    dev.run_typed(kid, M, N, K, pack16(t, A, la, lda), la, lda, pack16(t, B, lb, ldb), lb, ldb, ft.TYPE_BF16, cbuf, ldc, dbuf,
-                  alpha, beta, bias, mode, act, zbuf, opts)
+    dbuf = t.full((N, ldc), sent, device="cuda", dtype=typ) if out_of_place else cbuf
+    zbuf = t.full((N, ldc), zsent, device="cuda", dtype=typ) if z else None
+    dA, dB = pack16(t, A, la, lda), pack16(t, B, lb, ldb)
+    if cd == BF16:
+        dev.run_batched_mixed(kid, M, N, K, dA, la, lda, 0, dB, lb, ldb, 0, ft.TYPE_BF16, cbuf, ldc, 0, dbuf, ft.TYPE_BF16, 1,
+                              alpha, beta, bias, mode, 0, act, zbuf, opts)
+    else:
+        dev.run_typed(kid, M, N, K, dA, la, lda, dB, lb, ldb, ft.TYPE_BF16, cbuf, ldc, dbuf, alpha, beta, bias, mode, act, zbuf,
+                      opts)
     t.cuda.synchronize()
     if out_of_place:
-        assert t.equal(cbuf.view(t.int32), c_before.view(t.int32)), "C was written"
+        assert t.equal(cbuf.view(t.int16), c_before.view(t.int16)), "C was written"
     if ldc > M:
-        assert bool((dbuf[:, M:] == SENTINEL).all()), "D's padding was written"
+        assert bool((dbuf[:, M:].float() == sent).all()), "D's padding was written"
         if z:
-            assert bool((zbuf[:, M:] == Z_SENTINEL).all()), "Z's padding was written"
+            assert bool((zbuf[:, M:].float() == zsent).all()), "Z's padding was written"
     return dbuf[:, :M].t(), (zbuf[:, :M].t() if z else None)
 
 
@@ -270,25 +440,38 @@ def pack_batch16(t, X, layout, ld, gap=0):
 
 
 def batch16(t, ft, dev, kid, A, B, la=KM, lb=KM, pad=False, gap=0, alpha=1.0, beta=0.0, C0=None, bias=None, mode=NONE,
-            act=0, z=False, out_of_place=False, opts=None):
+            act=0, z=False, out_of_place=False, opts=None, cd=F32):
     """one run_batched_typed call: A (Bt, M, K), B (Bt, N, K), C column-major per entry, one bias per entry (Bt, len) or
-    None.  Returns (D, Z) as (Bt, M, N) views; checks that C kept its bytes when D != C."""
+    None (cd = BF16: one run_batched_mixed call with BF16 C, D and Z, each entry's columns padded to pad8(M) with the
+    sentinel).  Returns (D, Z) as (Bt, M, N) views; checks that C kept its bytes when D != C and that no padding was
+    written."""
     Bt, M, K = A.shape
     N = B.shape[1]
     lda, ldb = ld_bf16(la, M, K, pad), ld_bf16(lb, N, K, pad)
     dA, sa = pack_batch16(t, A, la, lda, gap)
     dB, sb = pack_batch16(t, B, lb, ldb, gap)
-    dC = t.zeros(Bt, N, M, device="cuda") if C0 is None else C0.transpose(1, 2).contiguous()
+    typ, sent, zsent = out_buffers(t, cd)
+    ldc = pad8(M) if cd == BF16 else M
+    dC = t.full((Bt, N, ldc), sent, device="cuda", dtype=typ)
+    dC[:, :, :M] = 0.0 if C0 is None else C0.transpose(1, 2)
     c_before = dC.clone()
-    dD = t.full((Bt, N, M), SENTINEL, device="cuda") if out_of_place else dC
-    dZ = t.full((Bt, N, M), Z_SENTINEL, device="cuda") if z else None
+    dD = t.full((Bt, N, ldc), sent, device="cuda", dtype=typ) if out_of_place else dC
+    dZ = t.full((Bt, N, ldc), zsent, device="cuda", dtype=typ) if z else None
     sbias = 0 if bias is None else bias.shape[1]
-    dev.run_batched_typed(kid, M, N, K, dA, la, lda, sa, dB, lb, ldb, sb, ft.TYPE_BF16, dC, M, M * N, dD, Bt, alpha, beta, bias,
-                          mode, sbias, act, dZ, opts)
+    if cd == BF16:
+        dev.run_batched_mixed(kid, M, N, K, dA, la, lda, sa, dB, lb, ldb, sb, ft.TYPE_BF16, dC, ldc, ldc * N, dD, ft.TYPE_BF16,
+                              Bt, alpha, beta, bias, mode, sbias, act, dZ, opts)
+    else:
+        dev.run_batched_typed(kid, M, N, K, dA, la, lda, sa, dB, lb, ldb, sb, ft.TYPE_BF16, dC, M, M * N, dD, Bt, alpha, beta,
+                              bias, mode, sbias, act, dZ, opts)
     t.cuda.synchronize()
     if out_of_place:
-        assert t.equal(dC.view(t.int32), c_before.view(t.int32)), "C was written"
-    return dD.transpose(1, 2), (dZ.transpose(1, 2) if z else None)
+        assert t.equal(dC.view(t.int16), c_before.view(t.int16)), "C was written"
+    if ldc > M:
+        assert bool((dD[:, :, M:].float() == sent).all()), "D's padding was written"
+        if z:
+            assert bool((dZ[:, :, M:].float() == zsent).all()), "Z's padding was written"
+    return dD[:, :, :M].transpose(1, 2), (dZ[:, :, :M].transpose(1, 2) if z else None)
 
 
 def events(st):
@@ -301,13 +484,16 @@ def statuses(st):
 
 # ------------------------------------------------------------------ GPU 1: tile and stage edges
 @pytest.mark.gpu
-@pytest.mark.parametrize("name", list(PAIRS))
-def test_tile_edges_exact(cuda, ft, dev, name):
+@pytest.mark.parametrize("name,cd", with_cd(list(PAIRS)))
+def test_tile_edges_exact(cuda, ft, dev, name, cd):
     """Ids 21 / 31, 3 / 13, 22 / 32 and 20 / 40 at K around the 16-k wgmma step and the 64-k stage, M around the 64-row A
     boxes and the tile, N around the BN/2 halves the two CTAs multicast and the tile: all four layout pairs, NaN-padded
     leading dimensions, ldc > M (sentinel untouched), D != C in half the cases (C untouched), splitk -1 / 0 / 2, dyadic
-    alpha / beta with an integer C0.  D equals the float64 product at every element, every row check closes exactly."""
+    alpha / beta with an integer C0.  D equals the float64 product at every element, every row check closes exactly.  With
+    BF16 C / D: D equals the float64 product rounded once, the BF16 padding sentinel (rows of M % 8 = 4 end mid-sector)
+    untouched; ties are planted where alpha != 0."""
     t = cuda
+    seen = Rounding()
     plain, abft = PAIRS[name]
     BN = tiles(ft)[31 if name == "auto" else abft][1]
     g = t.Generator(device="cuda").manual_seed(300 + list(PAIRS).index(name))
@@ -316,35 +502,44 @@ def test_tile_edges_exact(cuda, ft, dev, name):
         amax = pick_amax16(K, alpha, beta, 64)
         A, B = ints(t, g, (M, K), amax), ints(t, g, (N, K), amax)
         C0 = ints(t, g, (M, N), 64)
+        if cd == BF16 and alpha != 0.0:
+            plant_ties(A, B, alpha, C0)
         want = reference(A, B, alpha, beta, C0)
         for kid in (plain, abft):
-            tag = (kid, c)
+            tag = (kid, cd, c)
             with knobs(ft, splitk=c["splitk"]):
                 dev.stats()
                 got, _ = run1(t, ft, dev, kid, A, B, c["la"], c["lb"], c["pad"], M + 8 if c["ldc"] else None, alpha, beta, C0,
-                              out_of_place=c["out_of_place"])
+                              out_of_place=c["out_of_place"], cd=cd)
                 st = dev.stats()
-            exact(got, want, tag)
+            exact(got, want, tag, seen)
             zero_residual(st, kid, tag)
+    if cd == BF16:
+        seen.check(name)
 
 
 # ------------------------------------------------------------------ GPU 2: more than one checksum tile-column
 @pytest.mark.gpu
-@pytest.mark.parametrize("BN,N,tile", MULTI)
-def test_multi_column_checksums(cuda, ft, dev, BN, N, tile):
+@pytest.mark.parametrize("BN,N,tile,cd", with_cd(MULTI))
+def test_multi_column_checksums(cuda, ft, dev, BN, N, tile, cd):
     """N wide enough for two checksum tile-columns, where the six checksum columns of one N-tile straddle both (BN = 128,
     tile 21: e hi / mid in columns 126..127, e lo and w in 128..131; BN = 256, tile 42: e and w hi in 252..255, w mid / lo in
     256..257).  Both layouts of B, the encode in the front phase and in the pre-pass, a single product and a 2-entry batch:
     exact with zero residuals, and single upsets in several rows and columns of the straddling tile are each corrected
-    exactly, the event naming that element."""
+    exactly, the event naming that element.  With BF16 C / D the same, each corrected element rounded once (ties planted in
+    row 0)."""
     t = cuda
+    seen = Rounding()
     pairs = [(p, a) for p, a in (PAIRS["256"], PAIRS["128"], PAIRS["128s"]) if tiles(ft)[a][1] == BN]
     assert pairs and chk_geometry(BN, N)[1] >= 2
     M, K = 260, 200
     g = t.Generator(device="cuda").manual_seed(N)
     A, B = odd_ints(g, M, N, K, 2)     # (|acc| small enough that an upset of 1 is located: 6 thr < 1)
-    want = reference(A, B)
     Ab, Bb = odd_ints(g, M, N, K, 2, (2,))
+    if cd == BF16:
+        plant_ties(A, B, 1.0)
+        plant_ties(Ab, Bb, 1.0)
+    want = reference(A, B)
     wantb = reference(Ab, Bb)
     n0 = tile * BN
     cols = [n0, n0 + 1, n0 + BN // 2 - 1, n0 + BN // 2, n0 + BN - 2, n0 + BN - 1]
@@ -358,13 +553,13 @@ def test_multi_column_checksums(cuda, ft, dev, BN, N, tile):
                 with knobs(ft, enc_front=front):
                     for kid in (plain, abft):
                         dev.stats()
-                        got, _ = run1(t, ft, dev, kid, A, B, la, lb, pad=True)
-                        exact(got, want, (kid,) + tag)
+                        got, _ = run1(t, ft, dev, kid, A, B, la, lb, pad=True, cd=cd)
+                        exact(got, want, (kid,) + tag, seen)
                         zero_residual(dev.stats(), kid, (kid,) + tag)
                     for shift in range(2):
                         faults = [{"row": rows[i], "col": cols[(i + shift) % 6], "add": adds[i]} for i in range(6)]
                         dev.stats()
-                        got, _ = run1(t, ft, dev, abft, A, B, la, lb, pad=True, opts=ft.make_opts(faults=faults))
+                        got, _ = run1(t, ft, dev, abft, A, B, la, lb, pad=True, opts=ft.make_opts(faults=faults), cd=cd)
                         st = dev.stats()
                         exact(got, want, tag + (faults,))
                         assert st["detected"] == st["corrected"] == 6 and st["recomputed"] == 0, (tag, st)
@@ -373,18 +568,27 @@ def test_multi_column_checksums(cuda, ft, dev, BN, N, tile):
                     faults = [{"row": M + rows[i], "col": cols[i], "add": adds[i]} for i in range(0, 6, 2)]
                     for kid, opts in ((plain, None), (abft, None), (abft, ft.make_opts(faults=faults))):
                         dev.stats()
-                        got, _ = batch16(t, ft, dev, kid, Ab, Bb, la, lb, pad=True, opts=opts)
+                        got, _ = batch16(t, ft, dev, kid, Ab, Bb, la, lb, pad=True, opts=opts, cd=cd)
                         st = dev.stats()
-                        exact(got, wantb, (kid, "batch") + tag)
+                        exact(got, wantb, (kid, "batch") + tag, seen)
                         if opts is None:
                             zero_residual(st, kid, (kid, "batch") + tag)
                         else:
                             assert st["detected"] == st["corrected"] == 3, (tag, st)
                             assert events(st) == {(f["row"], f["col"]) for f in faults}, (tag, st)
+    if cd == BF16:
+        seen.check((BN, N))
 
 
 # ------------------------------------------------------------------ GPU 3: production sizes, whole output
-def _whole16(t, ft, dev, M, N, K, ids, amax, seed, layouts=((MN, MN),), beta=0.0, saturate=False):
+def within_one_ulp16(t, got, want):
+    """bfloat16 got within one BF16 ulp of want rounded once (cuBLAS sums in another order and may round partial sums)"""
+    w = (round_bf16(want) << 16).to(t.int32).view(t.float32).double()
+    ulp = (w.abs() * 2.0 ** -7).clamp_min(2.0 ** -133)
+    return bool(((got.double() - w).abs() <= ulp).all())
+
+
+def _whole16(t, ft, dev, M, N, K, ids, amax, seed, layouts=((MN, MN),), beta=0.0, saturate=False, cd=F32, seen=None):
     g = t.Generator(device="cuda").manual_seed(seed)
     A, B = ints(t, g, (M, K), amax), ints(t, g, (N, K), amax)
     if saturate:  # row 0 of A and the first 256 rows of B all amax: acc(0, n < 256) = K * amax^2, r1 = s1 = 2^24 there
@@ -400,17 +604,32 @@ def _whole16(t, ft, dev, M, N, K, ids, amax, seed, layouts=((MN, MN),), beta=0.0
         dB = (B.T if lb == MN else B).contiguous().to(t.bfloat16)
         lda, ldb = (M if la == MN else K), (N if lb == MN else K)
         for kid in ids:
-            dD = t.full((N, M), SENTINEL, device="cuda")
-            c_before = None if C0 is None else C0.clone()
+            tag = (kid, M, N, K, la, lb, beta, cd)
             dev.stats()
-            dev.run_typed(kid, M, N, K, dA, la, lda, dB, lb, ldb, ft.TYPE_BF16, C0 if C0 is not None else dD, M, dD, 1.0, beta)
-            t.cuda.synchronize()
+            if cd == BF16:
+                dD = t.full((N, M), SENTINEL16, device="cuda", dtype=t.bfloat16)
+                c16 = None if C0 is None else C0.to(t.bfloat16)
+                c_before = None if C0 is None else c16.clone()
+                dev.run_batched_mixed(kid, M, N, K, dA, la, lda, 0, dB, lb, ldb, 0, ft.TYPE_BF16, c16 if C0 is not None else dD,
+                                      M, 0, dD, ft.TYPE_BF16, 1, 1.0, beta)
+                t.cuda.synchronize()
+                if kid == CUBLAS_BF16:
+                    assert within_one_ulp16(t, dD, want), tag
+                else:
+                    exact(dD, want, tag, seen)
+                if C0 is not None:
+                    assert t.equal(c16.view(t.int16), c_before.view(t.int16)), tag
+            else:
+                dD = t.full((N, M), SENTINEL, device="cuda")
+                c_before = None if C0 is None else C0.clone()
+                dev.run_typed(kid, M, N, K, dA, la, lda, dB, lb, ldb, ft.TYPE_BF16, C0 if C0 is not None else dD, M, dD, 1.0,
+                              beta)
+                t.cuda.synchronize()
+                bad = int((dD.double() != want).sum())
+                assert bad == 0, (tag, mismatch(dD.T, want.T))
+                if C0 is not None:
+                    assert t.equal(C0.view(t.int32), c_before.view(t.int32)), tag
             st = dev.stats()
-            tag = (kid, M, N, K, la, lb, beta)
-            bad = int((dD.double() != want).sum())
-            assert bad == 0, (tag, mismatch(dD.T, want.T))
-            if C0 is not None:
-                assert t.equal(C0.view(t.int32), c_before.view(t.int32)), tag
             zero_residual(st, kid, tag)
             del dD, c_before
         del dA, dB
@@ -425,23 +644,36 @@ def test_production_sizes_whole_output(cuda, ft, dev):
     """Every output element against float64 at the sizes the project is measured at: 4096^3 (ids 21, 31, 13, 32, 40, with
     cuBLAS BF16 as witness), 8192^3 (21 and 31 in MN,MN and K,K, and beta = -1 with D != C), 16384^3 (id 31: the wave
     re-synchronisation), 256 x 256 x 65536 (1024 k-blocks of 64) with a row checksum of exactly 2^24 (31, 40, cuBLAS BF16)
-    and 512 x 1024 x 32768.  Peak device memory ~8 GB."""
+    and 512 x 1024 x 32768.  Then all of it again with BF16 C and D: every element the float64 product rounded once (values
+    up to 2^24, ties of both kinds by the million), cuBLAS with BF16 C in place within one BF16 ulp.  Peak device memory
+    ~12 GB."""
     t = cuda
     both = ((MN, MN), (KM, KM))
-    _whole16(t, ft, dev, 4096, 4096, 4096, (21, 31, 13, 32, 40, CUBLAS_BF16), 2, 1, both)
-    _whole16(t, ft, dev, 8192, 8192, 8192, (21, 31), 2, 3, both)
-    _whole16(t, ft, dev, 8192, 8192, 8192, (31,), 2, 4, ((MN, KM),), beta=-1.0)
-    _whole16(t, ft, dev, 16384, 16384, 16384, (31,), 2, 5)
-    _whole16(t, ft, dev, 256, 256, 65536, (31, 40, CUBLAS_BF16), 1, 6, both, saturate=True)
-    _whole16(t, ft, dev, 512, 1024, 32768, (31, 40), 1, 7, ((KM, MN),))
+    for cd in (F32, BF16):
+        seen = Rounding()
+        _whole16(t, ft, dev, 4096, 4096, 4096, (21, 31, 13, 32, 40, CUBLAS_BF16), 2, 1, both, cd=cd, seen=seen)
+        _whole16(t, ft, dev, 8192, 8192, 8192, (21, 31), 2, 3, both, cd=cd, seen=seen)
+        _whole16(t, ft, dev, 8192, 8192, 8192, (31,), 2, 4, ((MN, KM),), beta=-1.0, cd=cd, seen=seen)
+        _whole16(t, ft, dev, 16384, 16384, 16384, (31,), 2, 5, cd=cd, seen=seen)
+        _whole16(t, ft, dev, 256, 256, 65536, (31, 40, CUBLAS_BF16), 1, 6, both, saturate=True, cd=cd, seen=seen)
+        _whole16(t, ft, dev, 512, 1024, 32768, (31, 40), 1, 7, ((KM, MN),), cd=cd, seen=seen)
+        if cd == BF16:
+            seen.check("production sizes")
 
 
 # ------------------------------------------------------------------ GPU 4: batch edges
 @pytest.mark.gpu
 def test_batched_ragged_entries_exact(cuda, ft, dev):
     """Strided BF16 batches with M not a multiple of the tile (rows past M must not leak into the next entry), a per-entry
-    ROW / COL bias, ReLU with Z, NaN gaps between entries, every layout pair: every entry exact."""
+    ROW / COL bias, ReLU with Z, NaN gaps between entries, every layout pair: every entry exact.  Then the same with BF16 C,
+    D and Z (entries' columns padded to 8 with the sentinel, ties planted in row 0 of every entry): rounded once."""
     t = cuda
+    for cd in (F32, BF16):
+        _batched_ragged(t, ft, dev, cd)
+
+
+def _batched_ragged(t, ft, dev, cd):
+    seen = Rounding()
     g = t.Generator(device="cuda").manual_seed(23)
     i = 0
     for kid in (31, 13, 32):
@@ -452,14 +684,19 @@ def test_batched_ragged_entries_exact(cuda, ft, dev):
                 la, lb = i % 2, (i // 2) % 2
                 i += 1
                 bias = ints(t, g, (Bt, L), 64)
+                if cd == BF16:
+                    A, B, C0 = A.clone(), B.clone(), C0.clone()
+                    plant_ties(A, B, -1.0, C0, bias, mode)
                 want = reference(A, B, -1.0, 0.5, C0, bias, mode)
                 dev.stats()
                 c, z = batch16(t, ft, dev, kid, A, B, la, lb, pad=True, gap=8, alpha=-1.0, beta=0.5, C0=C0, bias=bias,
-                               mode=mode, act=RELU, z=True, out_of_place=i % 2 == 0)
-                tag = (kid, Bt, M, N, K, mode, la, lb)
+                               mode=mode, act=RELU, z=True, out_of_place=i % 2 == 0, cd=cd)
+                tag = (kid, Bt, M, N, K, mode, la, lb, cd)
                 zero_residual(dev.stats(), kid, tag)
-                exact(z, want, tag + ("Z",))
+                exact(z, want, tag + ("Z",), seen)
                 exact(c, t.relu(want), tag + ("D",))
+    if cd == BF16:
+        seen.check("batched ragged")
 
 
 @pytest.mark.gpu
@@ -467,7 +704,8 @@ def test_batched_ragged_entries_exact(cuda, ft, dev):
 def test_batch_of_65537_entries(cuda, ft, dev):
     """65537 tiny entries (4 x 4 x 6, NaN padding inside and between entries), past the 65535 grid rows of the BF16 encode
     pre-pass (B below 8 MB, enc_front = 0) and through the front-phase encode (enc_front = 1): every entry exact in both
-    layouts of B, every row of every entry checked with zero residual."""
+    layouts of B, every row of every entry checked with zero residual.  Then with BF16 C / D (each entry's 4 rows padded to
+    8 with the sentinel): every entry rounded once -- results up to 448 with a bias, ties of both kinds among them."""
     t = cuda
     g = t.Generator(device="cuda").manual_seed(65537)
     Bt, M, N, K = 65537, 4, 4, 6
@@ -475,30 +713,36 @@ def test_batch_of_65537_entries(cuda, ft, dev):
     A, B = ints(t, g, (Bt, M, K), 8), ints(t, g, (Bt, N, K), 8)
     bias = ints(t, g, (Bt, N), 64)
     want = reference(A, B, 1.0, 0.0, None, bias, COL)
-    for kid in (31, 13):
-        for la, lb in ((KM, KM), (MN, MN), (KM, MN)):
-            for front in (0, 1):
-                tag = (kid, la, lb, front)
-                with knobs(ft, enc_front=front):
-                    dev.stats()
-                    c, _ = batch16(t, ft, dev, kid, A, B, la, lb, pad=True, gap=8, bias=bias, mode=COL)
-                    st = dev.stats()
-                zero_residual(st, kid, tag)
-                assert st["rows_checked"] >= Bt * M, (tag, st)
-                exact(c, want, tag)
+    for cd in (F32, BF16):
+        seen = Rounding()
+        for kid in (31, 13):
+            for la, lb in ((KM, KM), (MN, MN), (KM, MN)):
+                for front in (0, 1):
+                    tag = (kid, la, lb, front, cd)
+                    with knobs(ft, enc_front=front):
+                        dev.stats()
+                        c, _ = batch16(t, ft, dev, kid, A, B, la, lb, pad=True, gap=8, bias=bias, mode=COL, cd=cd)
+                        st = dev.stats()
+                    zero_residual(st, kid, tag)
+                    assert st["rows_checked"] >= Bt * M, (tag, st)
+                    exact(c, want, tag, seen)
+        if cd == BF16:
+            seen.check("65537 entries")
     del A, B, bias, want
     _free(t)
 
 
 # ------------------------------------------------------------------ GPU 5: seeded exact fuzz
 @pytest.mark.gpu
-@pytest.mark.parametrize("seed", range(40))
-def test_exact_fuzz(cuda, ft, dev, seed):
+@pytest.mark.parametrize("seed,cd", with_cd(list(range(40))))
+def test_exact_fuzz(cuda, ft, dev, seed, cd):
     """Random shapes, BF16 tiles, layouts, padding, dyadic alpha / beta, entry points (plain, ROW / COL bias, ReLU with Z,
     D != C, batched with a per-entry bias) and planner knobs (splitk, wave_sync, pdl, epi_assist, chk_slices, enc_front): the
-    plain and the ABFT id of the tile are exact, the ABFT checks close with zero residual."""
+    plain and the ABFT id of the tile are exact, the ABFT checks close with zero residual.  With BF16 C / D / Z (fuzz16 with
+    BF16, ties planted in row 0): rounded once."""
     t = cuda
-    p = fuzz16(seed)
+    seen = Rounding()
+    p = fuzz16(seed, cd)
     M, N, K, amax = p["M"], p["N"], p["K"], p["amax"]
     g = t.Generator(device="cuda").manual_seed(19000 + seed)
     tag = str(p)
@@ -515,24 +759,28 @@ def test_exact_fuzz(cuda, ft, dev, seed):
             C0 = ints(t, g, (M, N), p["cmax"])
             mode = {"bias_row": ROW, "bias_col": COL}.get(entry, NONE)
             bias = ints(t, g, (M if mode == ROW else N,), p["bias_max"]) if mode else None
+        if cd == BF16:
+            plant_ties(A, B, p["alpha"], C0, bias, mode)
         want = reference(A, B, p["alpha"], p["beta"], C0, bias, mode)
         for kid in PAIRS[p["pair"]]:
             dev.stats()
             z = None
             if entry == "batched":
                 got, _ = batch16(t, ft, dev, kid, A, B, p["la"], p["lb"], p["pad"], 8 if p["pad"] else 0, p["alpha"], p["beta"],
-                                 C0, bias, mode)
+                                 C0, bias, mode, cd=cd)
             else:
                 got, z = run1(t, ft, dev, kid, A, B, p["la"], p["lb"], p["pad"], M + 4 if p["pad"] else None, p["alpha"],
                               p["beta"], C0, bias, mode, RELU if entry == "relu_z" else 0, entry == "relu_z",
-                              entry == "out_of_place")
+                              entry == "out_of_place", cd=cd)
             st = dev.stats()
             if entry == "relu_z":
-                exact(z, want, (kid, tag, "Z"))
+                exact(z, want, (kid, tag, "Z"), seen)
                 exact(got, t.relu(want), (kid, tag))
             else:
-                exact(got, want, (kid, tag))
+                exact(got, want, (kid, tag), seen)
             zero_residual(st, kid, (kid, tag))
+    if cd == BF16:
+        seen.check(tag)
 
 
 # ------------------------------------------------------------------ GPU 6: exact repairs in every layout pair
@@ -544,23 +792,26 @@ def _apart(bn):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("la,lb", [(MN, MN), (MN, KM), (KM, MN), (KM, KM)])
-@pytest.mark.parametrize("kid", [31, 32])
-def test_repairs_are_exact(cuda, ft, dev, kid, la, lb):
+@pytest.mark.parametrize("kid,cd", with_cd([31, 32]))
+def test_repairs_are_exact(cuda, ft, dev, kid, cd, la, lb):
     """test_exact.test_repairs_are_exact on BF16 operands, in every layout pair with padded leading dimensions.  Single upsets
     at columns 0, 31 / 32, BN/2 - 1 / BN/2, BN - 1 and N - 1 of a ragged tile and rows around the 32-row slabs and the row
     tile: each corrected exactly.  Two upsets in one row: the BF16 row recompute (status 5) is exact.  Level 2 with beta != 0
     and an upset of the value about to be stored: the chunk recompute (status 6) is exact.  Level 1 with D != C and beta != 0:
     the segment is recomputed into D (status 6), exactly.  Two upsets in entry 2 of a batch: recomputed exactly there (the
-    entry offset in BF16 elements)."""
+    entry offset in BF16 elements).  With BF16 C / D every repaired element is stored rounded once; C0 is then 16 times as
+    large (BF16 values up to 512), so the recomputed rows hold ties at half-integers and the level 1 / 2 results at odd
+    integers."""
     t = cuda
+    seen = Rounding()
     tm, bn = tiles(ft)[kid]
     M, N, K = 2 * tm + 4, 2 * bn + 4 if bn < 256 else bn + 132, 201
     g = t.Generator(device="cuda").manual_seed(41 + kid + 2 * la + lb)
     A, B = odd_ints(g, M, N, K, 2)
-    C0 = 2 * ints(t, g, (M, N), 32)
+    C0 = (16 if cd == BF16 else 2) * ints(t, g, (M, N), 32)
     want = reference(A, B)
     assert bool((want.remainder(2) == 1).all())
-    kw = dict(la=la, lb=lb, pad=True, ldc=M + 8)
+    kw = dict(la=la, lb=lb, pad=True, ldc=M + 8, cd=cd)
     cols = [0, 31, 32, bn // 2 - 1, bn // 2, bn - 1, N - 1, min(63, bn - 1)]
     rows = [0, 31, 32, 127, 128, M - 1, tm - 1, tm]
     kinds = [1, -1, 7, -7, 1000, -1000, "exp", "sign"]
@@ -574,7 +825,7 @@ def test_repairs_are_exact(cuda, ft, dev, kid, la, lb):
             dev.stats()
             got, _ = run1(t, ft, dev, kid, A, B, opts=ft.make_opts(faults=faults, **opts), **kw)
             st = dev.stats()
-            exact(got, want, (kid, la, lb, shift, faults, opts))
+            exact(got, want, (kid, la, lb, shift, faults, opts), seen)
             assert st["detected"] == st["corrected"] == 8 and st["recomputed"] == 0, (kid, la, lb, faults, st)
             assert events(st) == where and set(statuses(st)) == {1}, st
     # two upsets in one row: the row recompute, from A and B in BF16
@@ -584,7 +835,7 @@ def test_repairs_are_exact(cuda, ft, dev, kid, la, lb):
         dev.stats()
         got, _ = run1(t, ft, dev, kid, A, B, alpha=-0.5, beta=1.0, C0=C0, opts=ft.make_opts(faults=two, **opts), **kw)
         st = dev.stats()
-        exact(got, reference(A, B, -0.5, 1.0, C0), (kid, la, lb, "two in a row", opts))
+        exact(got, reference(A, B, -0.5, 1.0, C0), (kid, la, lb, "two in a row", opts), seen)
         assert st["detected"] == 1 and st["recomputed"] == 1 and statuses(st) == [5], st
     # level 2: an upset of the value about to be stored, beta != 0, at the last column of the ragged corner tile (the chunk
     # recompute)
@@ -593,24 +844,26 @@ def test_repairs_are_exact(cuda, ft, dev, kid, la, lb):
     got, _ = run1(t, ft, dev, kid, A, B, alpha=1.0, beta=-2.0, C0=C0, opts=ft.make_opts(
         faults=[{"row": M - 1, "col": N - 1, "xor": 1 << 22, "where": "epilogue_value"}], protect_epilogue=2), **kw)
     st = dev.stats()
-    exact(got, w2, (kid, la, lb, "level 2"))
+    exact(got, w2, (kid, la, lb, "level 2"), seen)
     assert st["epilogue_faults"] == 1 and st["recomputed"] == 1 and statuses(st) == [6], st
     # level 1 with D != C and beta != 0: the failed segment is recomputed into D from A, B and the intact C
     dev.stats()
     got, _ = run1(t, ft, dev, kid, A, B, alpha=1.0, beta=-2.0, C0=C0, out_of_place=True, opts=ft.make_opts(
         faults=[{"row": 37, "col": 40, "xor": 1 << 27, "where": "epilogue_value"}], protect_epilogue=1), **kw)
     st = dev.stats()
-    exact(got, w2, (kid, la, lb, "level 1, D != C"))
+    exact(got, w2, (kid, la, lb, "level 1, D != C"), seen)
     assert st["epilogue_faults"] == 1 and st["recomputed"] == 1 and statuses(st) == [6], st
     # two upsets in one row of entry 2 of a batch
     Ab, Bb = odd_ints(g, M, N, K, 2, (3,))
     r = 5
     dev.stats()
     got, _ = batch16(t, ft, dev, kid, Ab, Bb, la, lb, pad=True, gap=8, opts=ft.make_opts(
-        faults=[{"row": 2 * M + r, "col": 3, "add": 7.0}, {"row": 2 * M + r, "col": bn - 2, "add": v2}]))
+        faults=[{"row": 2 * M + r, "col": 3, "add": 7.0}, {"row": 2 * M + r, "col": bn - 2, "add": v2}]), cd=cd)
     st = dev.stats()
-    exact(got, reference(Ab, Bb), (kid, la, lb, "batch"))
+    exact(got, reference(Ab, Bb), (kid, la, lb, "batch"), seen)
     assert st["recomputed"] == 1 and [(e["row"], e["status"]) for e in st["events"]] == [(2 * M + r, 5)], st
+    if cd == BF16:
+        seen.check((kid, la, lb))
 
 
 # ------------------------------------------------------------------ GPU 7: the BF16 value range
@@ -649,8 +902,14 @@ def test_power_of_two_scaling_exact(cuda, ft, dev):
     Rows of A and of B scaled together (2^(r_m + s_n), r, s in [-40, 40]): D is still exact, but the encode's FP32 groups of 8
     mix scales and round, and so does a tile row's sum.  The plain ids and detect_only are exact; the rows the check flags
     with mixed-sign operands are counted and printed, and with repairs on nothing but flagged rows may change (at most one
-    element each).  With operands of one sign nothing is flagged."""
+    element each).  With operands of one sign nothing is flagged.  All of it again with BF16 C / D: rounded once."""
     t = cuda
+    for cd in (F32, BF16):
+        _power_of_two_scaling(t, ft, dev, cd)
+
+
+def _power_of_two_scaling(t, ft, dev, cd):
+    seen = Rounding()
     g = t.Generator(device="cuda").manual_seed(52)
     M, N, K = 516, 388, 301
     A = scale_rows(t, g, ints(t, g, (M, K), 8), 60)
@@ -659,8 +918,8 @@ def test_power_of_two_scaling_exact(cuda, ft, dev):
     for kid in (21, 31, 3, 13, 32):
         for la, lb in ((MN, KM), (KM, MN)):
             dev.stats()
-            got, _ = run1(t, ft, dev, kid, A, B, la, lb, alpha=-0.5)
-            exact(got, want, (kid, la, lb, "2^r"))
+            got, _ = run1(t, ft, dev, kid, A, B, la, lb, alpha=-0.5, cd=cd)
+            exact(got, want, (kid, la, lb, "2^r", cd), seen)
             zero_residual(dev.stats(), kid, (kid, la, lb, "2^r"))
     A2 = scale_rows(t, g, ints(t, g, (M, K), 2), 40)
     B2 = scale_rows(t, g, ints(t, g, (N, K), 2), 40)
@@ -668,39 +927,43 @@ def test_power_of_two_scaling_exact(cuda, ft, dev):
     flagged, changed = {}, {}
     for plain, kid in ((21, 31), (3, 13), (22, 32)):
         for la, lb in ((MN, MN), (KM, KM)):
-            got, _ = run1(t, ft, dev, plain, A2, B2, la, lb)
-            exact(got, want, (plain, la, lb, "2^r 2^s"))
+            got, _ = run1(t, ft, dev, plain, A2, B2, la, lb, cd=cd)
+            exact(got, want, (plain, la, lb, "2^r 2^s", cd), seen)
             dev.stats()
-            got, _ = run1(t, ft, dev, kid, A2, B2, la, lb, opts=ft.make_opts(detect_only=True))
+            got, _ = run1(t, ft, dev, kid, A2, B2, la, lb, opts=ft.make_opts(detect_only=True), cd=cd)
             st = dev.stats()
-            exact(got, want, (kid, la, lb, "2^r 2^s, detect_only"))
+            exact(got, want, (kid, la, lb, "2^r 2^s, detect_only", cd))
             flagged[kid] = flagged.get(kid, 0) + st["detected"]
-            got, _ = run1(t, ft, dev, kid, A2, B2, la, lb)
+            got, _ = run1(t, ft, dev, kid, A2, B2, la, lb, cd=cd)
             st2 = dev.stats()
-            bad = int((got.double() != want).sum())
+            bad = int((bits16(got) != round_bf16(want)).sum() if cd == BF16 else (got.double() != want).sum())
             assert st2["detected"] == st["detected"] and bad <= st2["detected"], (kid, la, lb, bad, st2)
             changed[kid] = changed.get(kid, 0) + bad
-    print("bf16 2^r 2^s scaling, mixed signs: rows flagged", flagged, "elements changed by a repair", changed)
+    print("bf16 2^r 2^s scaling, mixed signs, output", ("F32", "BF16")[cd], ": rows flagged", flagged,
+          "elements changed by a repair", changed)
     A3 = scale_rows(t, g, ints(t, g, (M, K), 2).abs() + 1.0, 40)
     B3 = scale_rows(t, g, ints(t, g, (N, K), 2).abs() + 1.0, 40)
     want = reference(A3, B3)
     for kid in (31, 13, 32):
         for la, lb in ((MN, MN), (KM, KM)):
             dev.stats()
-            got, _ = run1(t, ft, dev, kid, A3, B3, la, lb)
+            got, _ = run1(t, ft, dev, kid, A3, B3, la, lb, cd=cd)
             st = dev.stats()
-            exact(got, want, (kid, la, lb, "2^r 2^s, one sign"))
+            exact(got, want, (kid, la, lb, "2^r 2^s, one sign", cd), seen)
             assert st["detected"] == 0 and st["rows_checked"] > 0, (kid, la, lb, st)
+    if cd == BF16:
+        seen.check("power-of-two scaling")
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("role", ["a", "b"])
-def test_subnormal_operands_exact(cuda, ft, dev, role):
+@pytest.mark.parametrize("role,cd", with_cd(["a", "b"]))
+def test_subnormal_operands_exact(cuda, ft, dev, role, cd):
     """BF16 subnormals (2^-130 times integers of at most 15) in one operand against integers scaled by 2^40 in the other, so
     every product is a normal FP32 value: the tensor core keeps the subnormals, and D equals the float64 product in every
     layout pair (cuBLAS BF16 witnesses it), with zero residuals.  The CUDA-core row recompute (two upsets in a row) reads the
-    same values and is exact too."""
+    same values and is exact too.  With BF16 C / D (cuBLAS: BF16 C in place, within one BF16 ulp): rounded once."""
     t = cuda
+    seen = Rounding()
     g = t.Generator(device="cuda").manual_seed(130 + (role == "b"))
     M, N, K = 260, 388, 201
     tiny = lambda shape: ints(t, g, shape, 15) * 2.0 ** -130
@@ -713,19 +976,24 @@ def test_subnormal_operands_exact(cuda, ft, dev, role):
     for la, lb in ((MN, MN), (MN, KM), (KM, MN), (KM, KM)):
         for kid in (21, 31, 13, CUBLAS_BF16):
             dev.stats()
-            got, _ = run1(t, ft, dev, kid, A, B, la, lb, pad=True)
+            got, _ = run1(t, ft, dev, kid, A, B, la, lb, pad=True, cd=cd)
             assert bool((got != 0).any()), (kid, role, la, lb, "the tensor core flushed the BF16 subnormals")
-            exact(got, want, (kid, role, la, lb))
+            if kid == CUBLAS_BF16 and cd == BF16:
+                assert within_one_ulp16(t, got, want), (kid, role, la, lb)
+            else:
+                exact(got, want, (kid, role, la, lb, cd), seen)
             zero_residual(dev.stats(), kid, (kid, role, la, lb))
         for kid in (31, 13):
             # (upsets far above the data: the threshold's absolute term, tau_abs = 1e-3, dwarfs these products)
             bn = tiles(ft)[kid][1]
             two = [{"row": 33, "col": 3, "add": 7.0}, {"row": 33, "col": bn - 2, "add": _apart(bn)}]
             dev.stats()
-            got, _ = run1(t, ft, dev, kid, A, B, la, lb, pad=True, opts=ft.make_opts(faults=two))
+            got, _ = run1(t, ft, dev, kid, A, B, la, lb, pad=True, opts=ft.make_opts(faults=two), cd=cd)
             st = dev.stats()
-            exact(got, want, (kid, role, la, lb, "recompute"))
+            exact(got, want, (kid, role, la, lb, "recompute", cd), seen)
             assert st["detected"] == 1 and st["recomputed"] == 1 and statuses(st) == [5], (kid, role, st)
+    if cd == BF16:
+        seen.check(role)
 
 
 @pytest.mark.gpu

@@ -192,7 +192,10 @@ def test_definition_every_id_layout_and_option(cuda, ft, dev, kid):
 
 @pytest.mark.gpu
 def test_comparator_catches_one_ulp(cuda, ft, dev):
-    """The comparator of these tests fails on a one-ulp change of one BF16 element of D."""
+    """The comparator of these tests fails on a one-ulp change of one BF16 element of D, and so does the float64 one of
+    tests/test_bf16_exact.py (round_bf16 / mismatch16), which names that element; on integer data whose results need
+    rounding D meets both.  (Its sensitivity to the rounding mode is test_bf16_out_exact.test_rounding_edge_data.)"""
+    from test_bf16_exact import mismatch16, round_bf16
     t = cuda
     g = t.Generator(device="cuda").manual_seed(1)
     A, B = bf(t, g, (1, 128, 64)), bf(t, g, (1, 256, 64))
@@ -202,6 +205,13 @@ def test_comparator_catches_one_ulp(cuda, ft, dev):
     bad = d16.clone()
     bad.view(t.int16)[0, 17, 33] ^= 1
     assert not same16(t, bad, want)
+    Ai, Bi = _ints(t, g, (1, 128, 64), 15).to(t.bfloat16), _ints(t, g, (1, 256, 64), 15).to(t.bfloat16)
+    d16, _, _, _ = mixed_pair(t, dev, 31, Ai, Bi)
+    bits = round_bf16(Ai[0].double() @ Bi[0].double().T)
+    assert mismatch16(d16[0], bits) == ""
+    bad = d16.clone()
+    bad.view(t.int16)[0, 17, 33] ^= 1
+    assert mismatch16(bad[0], bits).startswith("1 elements differ, e.g. (17, 33)")
 
 
 # ------------------------------------------------------------------ GPU: exactness
